@@ -1,11 +1,11 @@
-"""In-tree build of the native code (sm_100a only).
+"""In-tree build of the native code (sm_90a: H100).
 
   libgs_b200.so                      hand-written CUDA kernels + the C ABI of include/gs_b200.h
                                      (no libtorch dependency; links cudart statically)
   gaussian.cpython-*.so              torch/pybind11 shim == the reference's `gaussian` module
                                      surface (reference setup.py:33-52 builds the equivalent)
 
-Both land next to this file so that they travel with the gpurun snapshot; objects go to
+Both land next to this file, so the package imports from the source tree; objects go to
 `build/` (git-ignored).  Usage:  python build.py [--force] [-v]
 """
 from __future__ import annotations
@@ -22,7 +22,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CU_SOURCES = ["project.cu", "binning.cu", "blend.cu", "blend_sh.cu", "blend_sh_tc.cu", "render.cu", "optim.cu", "collective.cu", "loss.cu", "densify.cu"]
 HEADERS = ["gs_common.cuh", "sh_common.cuh", "tc_common.cuh", "project.cuh", "internal.h", os.path.join(ROOT, "include", "gs_b200.h")]
 LIB = os.path.join(HERE, "libgs_b200.so")

@@ -557,7 +557,7 @@ void allreduce_push_finish_mc(int64_t bucket_multicast, int64_t bucket_local, in
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   using namespace gsb200;
-  m.doc() = "B200-native drop-in for the reference `gaussian` extension (libgs_b200 C ABI underneath)";
+  m.doc() = "H100-native (sm_90a) drop-in for the reference `gaussian` extension (libgs_b200 C ABI underneath)";
   m.def("culling", &culling, "gaussian culling (no-op stub, as in the reference)");
   m.def("world2camera", &world2camera, "world to camera (CUDA)");
   m.def("world2camera_backward", &world2camera_backward, "world to camera backward (CUDA)");

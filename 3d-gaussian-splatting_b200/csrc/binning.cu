@@ -97,7 +97,7 @@ __global__ void gather_kernel(const int* __restrict__ accum, const int* __restri
 // The backward writes an instance's gradient record to row ("slot") offsets_g[g] + rank, where
 // offsets_g is the exclusive scan of the tile counts in Gaussian-id order: the records of one
 // Gaussian are contiguous, and nothing in the pipeline needs a scattered store (scattered
-// 4-byte stores cost 0.5 ms at C3 when tried: partial-sector read-modify-write in L2).
+// 4-byte stores are partial-sector read-modify-writes in L2).
 // One warp emits the instances of 32 depth-consecutive Gaussians - a CONTIGUOUS range of the key / value arrays -
 // cooperatively: lane L writes entries first + L, first + L + 32, ... and finds the owning Gaussian of its entry
 // by a 5-step binary search over the warp's offsets (shuffles).  Every store instruction of the warp covers 128

@@ -4,7 +4,7 @@
 // The reference evaluates SH PER PIXEL RAY inside the blend: colour_c(pixel, instance) =
 // sigmoid(sum_k SH_k(dir_pixel) * coef[c*K + k]) with K = 9 (degree 2, D = 27).  K = 16
 // (degree 3, D = 48; svox2's C3 constants, defined but unused in the reference :395-403) is the
-// extension BASELINE.json's configs[2] asks for.  Same staging / early-exit / reduction design
+// extension (bench.py --colour 48).  Same staging / early-exit / reduction design
 // as blend.cu; the third stream carries the 3K coefficients + the gradient slot per instance.
 #include <type_traits>
 
@@ -483,6 +483,12 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
 int gs_sh_basis_count(int d) { return d == 27 ? 9 : (d == 48 ? 16 : 0); }
 int gs_sh_stream_width(int d) { return d == 27 ? sh_sw(9) : sh_sw(16); }
 int gs_sh_grad_width(int d) { return d == 27 ? (sh_nv(9) + 3) / 4 * 4 : (sh_nv(16) + 3) / 4 * 4; }
+// Default (sh_tc < 0): on the H100 the tensor-core kernels win at degree 3 (K = 16: frame 8.5 vs 11.3 ms at C3) and
+// lose at degree 2 (K = 9: 8.3 vs 7.6 ms), where the scalar kernels' FMAs cost less than the hi/lo operand traffic.
+int gs_sh_tc_mode(int d) {
+  const int t = gs_tuning().sh_tc;
+  return t >= 0 ? t : (d == 48 ? 3 : 0);
+}
 
 cudaError_t gs_launch_blend_sh_fwd(const float4* pA, const float2* pB, const float* pS, const GsRec* grec,
                                    const float* rgb, const uint32_t* ids, const uint32_t* goff, int d,
@@ -493,7 +499,7 @@ cudaError_t gs_launch_blend_sh_fwd(const float4* pA, const float2* pB, const flo
   blend_sh_fwd_kernel<K, GA><<<g.n_tiles, 64, 0, st>>>(pA, pB, pS, grec, rgb, ids, goff, tile_accum, g.wp, g.hp, g.ntx,   \
                                                        g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image, tile_neff, \
                                                        final_img, crop)
-  if (grec && (gs_tuning().sh_tc & 1))
+  if (grec && (gs_sh_tc_mode(d) & 1))
     return gs_launch_blend_sh_fwd_tc(grec, rgb, ids, d, tile_accum, g, r, image, tile_neff, final_img, crop, st);
   if (grec) {
     if (d == 27) GS_SHF(9, true); else GS_SHF(16, true);
@@ -511,7 +517,7 @@ cudaError_t gs_launch_blend_sh_bwd(const float4* pA, const float2* pB, const flo
                                    const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
                                    uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st) {
   if (grec && !row_epoch) return cudaErrorInvalidValue;
-  if (grec && (gs_tuning().sh_tc & 2))
+  if (grec && (gs_sh_tc_mode(d) & 2))
     return gs_launch_blend_sh_bwd_tc(grec, rgb, ids, goff, d, tile_accum, g, r, image, grad_image, grad_inst, grad_is_final,
                                      crop, row_epoch, epoch, tile_neff_b, st);
 #define GS_SHB(K, GA)                                                                                               \

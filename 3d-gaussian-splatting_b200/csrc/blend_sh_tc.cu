@@ -1,23 +1,23 @@
-// Tile blend with per-pixel SH colour on the 5th-generation tensor cores (tcgen05, accumulators in TMEM).
+// Tile blend with per-pixel SH colour on the Hopper tensor cores (wgmma, fp32 accumulators in registers).
 //
 // The two dense contractions of the SH path (reference gaussian.cu:936-948 forward colour, :665-689 backward)
 //   logit[pixel, (instance, channel)] = sum_q SH_q(pixel) * coef[instance, channel, q]                  (forward + backward)
 //   d coef[(instance, channel), q]    = sum_pixel d logit[pixel, (instance, channel)] * SH_q(pixel)     (backward)
-// are the only GEMM-shaped work of the rasterizer: 3K (forward) / 2 * 3K (backward) FMAs per (pixel, instance), i.e.
-// 27 of the 57 and 54 of the 137 instructions the scalar kernels (blend_sh.cu) issue per warp and 32 pairs at K = 9.
+// are the only GEMM-shaped work of the rasterizer: 3K (forward) / 2 * 3K (backward) FMAs per (pixel, instance).
 // Here ONE THREAD OWNS ONE PIXEL:
-//   * a tile is 256 pixels = two M = 128 accumulator blocks; the SH basis of the tile is written once to shared
+//   * a tile is 256 pixels = four M = 64 accumulator blocks; the SH basis of the tile is written once to shared
 //     memory as bf16 hi + lo parts (x = hi + lo to 2^-17) in the no-swizzle canonical layout, whose image is at the
 //     same time the K-major A operand of the first and the MN-major B operand of the second contraction;
+//   * pixel p sits in accumulator row tc_row(p), chosen so that the fragment rows a warp receives from wgmma are
+//     the pixels of that same warp: logits go registers -> shared memory -> registers without a CTA barrier;
 //   * per round of 16 instances the raw coefficients (gathered by cp.async, as in blend_sh.cu) are split into
-//     bf16 hi / lo K-major B operands [48 x 16] (pre-multiplied by -log2 e), three MMAs per block
-//     (hi*hi + hi*lo + lo*hi, fp32 accumulate: logits to ~2e-5 relative) leave the logits of 16 instances x 3
-//     channels in 48 TMEM columns of the lane (= pixel) that blends them: tcgen05.ld 32x32b hands every thread
-//     its own pixel's row, so the front-to-back recurrence stays a plain sequential loop;
+//     bf16 hi / lo K-major B operands [48 x 16] (pre-multiplied by -log2 e); per half round (8 instances x 3
+//     channels = N 24) three MMAs per block (hi*hi + hi*lo + lo*hi, fp32 accumulate: logits to ~2e-5 relative);
 //   * backward: the per-(pixel, instance) logit gradients are written back to shared memory as the MN-major A
 //     operand [96 rows = (hi | lo) x 3 channels x 16 instances, K = 256 pixels] and contracted with the basis
-//     image (N = 32 = hi | lo) by 16 K = 16 MMAs; the six geometry sums per instance keep the warp-shuffle reduction.
-// Layouts / descriptor encodings: tc_common.cuh (validated by profiles/r2_micro/umma_probe.cu).
+//     image (N = 32 = hi | lo) by 16 K = 16 MMAs per M = 64 block; the six geometry sums per instance keep the
+//     warp-shuffle reduction.
+// Layouts / descriptor encodings: tc_common.cuh.
 #include <cstddef>
 
 #include "internal.h"
@@ -31,6 +31,21 @@ using namespace gs_tc;
 
 constexpr int TC_J = 16;     // instances per round
 constexpr int TC_NT = 256;   // threads per CTA = pixels per tile
+constexpr int TC_LGS = 24;   // floats per row of the logit staging buffer: 3 channels x 8 instances
+
+// float offset of logit column col (c * 8 + jj) of accumulator row `row` in the staging buffer: the six 16-byte
+// chunks of a row are swapped in pairs on rows with bit 2 set, so that the eight rows a quarter warp reads (and
+// the four a half warp writes) fall into different banks despite the 96-byte row stride
+__device__ __forceinline__ int tc_lgs_off(int row, int col) {
+  return row * TC_LGS + (((col >> 2) ^ ((row >> 2) & 1)) << 2) + (col & 3);
+}
+
+// accumulator row (= K index of the backward contraction) of tile pixel p: warp w of warpgroup g owns pixels
+// 128 g + 32 w .. + 31, which are rows 16 w .. 16 w + 15 of blocks 2 g and 2 g + 1 - exactly the fragment rows
+// of that warp when warpgroup g issues those two blocks (and of the same warp of a single warpgroup issuing all four)
+__device__ __forceinline__ int tc_row(int p) {
+  return (p >> 7) * 128 + ((p >> 4) & 1) * 64 + ((p >> 5) & 3) * 16 + (p & 15);
+}
 
 template <int K, int STAGES>
 struct TcStage {
@@ -90,10 +105,11 @@ __device__ __forceinline__ void tc_split_coefs(const float* __restrict__ S, uint
   }
 }
 
-// SH basis of this thread's pixel -> bf16 hi / lo operand image: 16-byte unit (q / 8) * 256 + pixel
+// SH basis of tile pixel p -> bf16 hi / lo operand image: 16-byte unit (q / 8) * 256 + tc_row(p)
 template <int K>
 __device__ __forceinline__ void tc_store_basis(const float* sh, uint4* __restrict__ img_hi, uint4* __restrict__ img_lo,
-                                               int pixel) {
+                                               int p) {
+  const int row = tc_row(p);
 #pragma unroll
   for (int g = 0; g < 2; ++g) {
     uint32_t h[4], l[4];
@@ -103,25 +119,64 @@ __device__ __forceinline__ void tc_store_basis(const float* sh, uint4* __restric
       const float v1 = (g * 8 + 2 * w + 1 < K) ? sh[g * 8 + 2 * w + 1] : 0.f;
       split_bf16x2(v0, v1, h[w], l[w]);
     }
-    img_hi[g * 256 + pixel] = make_uint4(h[0], h[1], h[2], h[3]);
-    img_lo[g * 256 + pixel] = make_uint4(l[0], l[1], l[2], l[3]);
+    img_hi[g * 256 + row] = make_uint4(h[0], h[1], h[2], h[3]);
+    img_lo[g * 256 + row] = make_uint4(l[0], l[1], l[2], l[3]);
   }
 }
 
-// logits of one round: D[block][pixel, n] = basis[pixel, :] . coef[n, :]   (3 MMAs per 128-pixel block)
-__device__ __forceinline__ void tc_issue_logits(uint32_t tm, const uint4* img_hi, const uint4* img_lo, const uint4* bc_hi,
-                                                const uint4* bc_lo, uint64_t* bar) {
-  constexpr uint32_t idesc = idesc_bf16(0, 0, 128, 48);
-  const uint64_t b_hi = smem_desc(gs_smem_u32(bc_hi), 768, 128), b_lo = smem_desc(gs_smem_u32(bc_lo), 768, 128);
+// logits of half round h (instances 8h .. 8h + 7, all three channels) for accumulator blocks b0 .. b0 + NB - 1,
+// issued by the calling warpgroup: D[row, c * 8 + jj] = basis[row, :] . coef[c * 16 + 8h + jj, :], left in
+// lgs[row * TC_LGS + c * 8 + jj] for the rows of the calling warp (which only that warp reads).
+template <int NB>
+__device__ __forceinline__ void tc_logits_half(int b0, int h, const uint4* img_hi, const uint4* img_lo, const uint4* bc_hi,
+                                               const uint4* bc_lo, float* lgs, int wq, int lane) {
+  float acc[NB][12];
 #pragma unroll
-  for (int b = 0; b < 2; ++b) {
-    const uint64_t a_hi = smem_desc(gs_smem_u32(img_hi) + b * 2048, 4096, 128);
-    const uint64_t a_lo = smem_desc(gs_smem_u32(img_lo) + b * 2048, 4096, 128);
-    mma_bf16(tm + b * 48, a_hi, b_hi, idesc, 0);
-    mma_bf16(tm + b * 48, a_hi, b_lo, idesc, 1);
-    mma_bf16(tm + b * 48, a_lo, b_hi, idesc, 1);
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int i = 0; i < 12; ++i) acc[b][i] = 0.f;
+  // N = 24 selects the 8-row groups h, h + 2, h + 4 of the [48 x 16] coefficient operand
+  const uint64_t b_hi = smem_desc(gs_smem_u32(bc_hi) + h * 128, 768, 256);
+  const uint64_t b_lo = smem_desc(gs_smem_u32(bc_lo) + h * 128, 768, 256);
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc_fence(acc[b]);
+  wg_fence();
+#pragma unroll
+  for (int b = 0; b < NB; ++b) {
+    const uint64_t a_hi = smem_desc(gs_smem_u32(img_hi) + (b0 + b) * 1024, 4096, 128);
+    const uint64_t a_lo = smem_desc(gs_smem_u32(img_lo) + (b0 + b) * 1024, 4096, 128);
+    mma_n24_kk(acc[b], a_hi, b_hi, 0);
+    mma_n24_kk(acc[b], a_hi, b_lo, 1);
+    mma_n24_kk(acc[b], a_lo, b_hi, 1);
   }
-  mma_commit(bar);
+  wg_commit();
+  wg_wait_all();
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc_fence(acc[b]);
+  __syncwarp();                                             // the warp's reads of the previous half are done
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = (b0 + b) * 64 + wq * 16 + (lane >> 2) + 8 * r;
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        *reinterpret_cast<float2*>(lgs + tc_lgs_off(row, c * 8 + 2 * (lane & 3))) =
+            make_float2(acc[b][4 * c + 2 * r], acc[b][4 * c + 2 * r + 1]);
+    }
+  __syncwarp();
+}
+
+// the 24 logits of half round of the pixel in accumulator row `row`
+__device__ __forceinline__ void tc_read_logits(const float* lgs, int row, float* lr, float* lg, float* lb) {
+  float* dst[3] = {lr, lg, lb};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float4 u = *reinterpret_cast<const float4*>(lgs + tc_lgs_off(row, c * 8));
+    const float4 v = *reinterpret_cast<const float4*>(lgs + tc_lgs_off(row, c * 8 + 4));
+    dst[c][0] = u.x; dst[c][1] = u.y; dst[c][2] = u.z; dst[c][3] = u.w;
+    dst[c][4] = v.x; dst[c][5] = v.y; dst[c][6] = v.z; dst[c][7] = v.w;
+  }
 }
 
 // three sigmoids from v_c = -logit_c * log2 e with ONE reciprocal (see blend_sh.cu)
@@ -142,11 +197,12 @@ template <int K>
 struct TcFwdSmem {
   uint4 img_hi[2 * 256];
   uint4 img_lo[2 * 256];
-  uint4 bc_hi[2 * 48];
-  uint4 bc_lo[2 * 48];
+  // by round parity: with one CTA barrier per round, a warpgroup may split round k + 1 while the other one still
+  // runs the logit MMAs of round k
+  uint4 bc_hi[2][2 * 48];
+  uint4 bc_lo[2][2 * 48];
+  float lgs[256 * TC_LGS];
   TcStage<K, 4> st;
-  uint64_t mma_bar;
-  uint32_t tmem_base;
 };
 
 template <int K>
@@ -158,9 +214,10 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
                                                                 const float* __restrict__ vdx, const float* __restrict__ vdy,
                                                                 float* __restrict__ image, int* __restrict__ tile_neff,
                                                                 float* __restrict__ final_img, GsCrop crop) {
-  constexpr int STAGES = 4, TCOLS = 128;
-  __shared__ __align__(128) TcFwdSmem<K> sm;
-  const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5;
+  constexpr int STAGES = 4;
+  extern __shared__ __align__(128) uint8_t tc_smem_raw[];
+  TcFwdSmem<K>& sm = *reinterpret_cast<TcFwdSmem<K>*>(tc_smem_raw);
+  const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tx = tile % ntx, ty = tile / ntx;
   const int ix = tx * GS_TILE + (tid & 15), iy = ty * GS_TILE + (tid >> 4);
   const int start = tile_accum[tile];
@@ -171,24 +228,19 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
     const int nchunks = (cnt + TC_J - 1) / TC_J;
     if (tid == 0) {
       for (int s = 0; s < STAGES; ++s) gs_mbar_init(&sm.st.full[s], TC_NT);
-      gs_mbar_init(&sm.mma_bar, 1);
       gs_fence_barrier_init();
     }
-    if (warp == 0) tmem_alloc<TCOLS>(&sm.tmem_base);
     {
       float sh[16];
       pixel_sh<K>(ix, iy, rays_o, lefttop, vdx, vdy, sh);
       tc_store_basis<K>(sh, sm.img_hi, sm.img_lo, tid);
     }
-    if (tid < 96) {                                           // q >= K columns of the coefficient operand stay zero
-      sm.bc_hi[tid] = make_uint4(0, 0, 0, 0);
-      sm.bc_lo[tid] = make_uint4(0, 0, 0, 0);
+    if (tid < 192) {                                          // q >= K columns of the coefficient operand stay zero
+      sm.bc_hi[tid / 96][tid % 96] = make_uint4(0, 0, 0, 0);
+      sm.bc_lo[tid / 96][tid % 96] = make_uint4(0, 0, 0, 0);
     }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tm = sm.tmem_base;
-    const uint32_t trow = tm + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(warp >> 2) * 48u;
+    const int row = tc_row(tid);
     const float px = gs_pixel_coord(ix, wp, fx), py = gs_pixel_coord(iy, hp, fy);
     for (int k = 0; k < STAGES - 1 && k < nchunks; ++k)
       tc_gather<K, STAGES, false>(sm.st, k, grec, rgb, ids, nullptr, start + k * TC_J, min(TC_J, cnt - k * TC_J), tid);
@@ -197,35 +249,28 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
       const int stage = k % STAGES;
       gs_mbar_wait(&sm.st.full[stage], (uint32_t)((k / STAGES) & 1));
       const int n = min(TC_J, cnt - k * TC_J);
-      tc_split_coefs<K>(sm.st.S[stage], sm.bc_hi, sm.bc_lo, tid);
+      uint4* bc_hi = sm.bc_hi[k & 1];
+      uint4* bc_lo = sm.bc_lo[k & 1];
+      tc_split_coefs<K>(sm.st.S[stage], bc_hi, bc_lo, tid);
       fence_smem_to_async();
-      fence_before_sync();
-      // every thread has finished round k - 1 (its TMEM reads, its staged rows); all pixels saturated -> done
+      // every thread has finished round k - 1 (its logit MMAs, its staged rows); all pixels saturated -> done
       if (__syncthreads_and(!(T > GS_T_STOP))) {
         consumed = k * TC_J;
         break;
-      }
-      if (warp == 0) {
-        if (elect_one()) {
-          fence_after_sync();
-          tc_issue_logits(tm, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, &sm.mma_bar);
-        }
-        __syncwarp();
       }
       if (k + STAGES - 1 < nchunks) {
         const int kn = k + STAGES - 1;
         tc_gather<K, STAGES, false>(sm.st, kn % STAGES, grec, rgb, ids, nullptr, start + kn * TC_J,
                                     min(TC_J, cnt - kn * TC_J), tid);
       }
-      gs_mbar_wait(&sm.mma_bar, (uint32_t)(k & 1));
-      fence_after_sync();
       const float4* R = sm.st.R[stage];
 #pragma unroll 1
       for (int h = 0; h < 2; ++h) {
-        if (h * 8 >= n) break;
-        if (__all_sync(0xffffffffu, !(T > GS_T_STOP))) break;
+        if (h * 8 >= n) break;                                // uniform
+        tc_logits_half<2>(2 * (warp >> 2), h, sm.img_hi, sm.img_lo, bc_hi, bc_lo, sm.lgs, warp & 3, lane);
+        if (__all_sync(0xffffffffu, !(T > GS_T_STOP))) continue;
         float lr[8], lg[8], lb[8];
-        tmem_ld8x3(trow + h * 8, trow + 16 + h * 8, trow + 32 + h * 8, lr, lg, lb);
+        tc_read_logits(sm.lgs, row, lr, lg, lb);
         const float4* Rh = R + 32 * h;
         // one (pixel, instance) pair; a saturated pixel blends nothing (w = 0), without a divergent branch
         auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2) {
@@ -252,9 +297,6 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
       }
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<TCOLS>(tm);
   }
   float* o = image + ((size_t)iy * wp + ix) * 3;
   o[0] = cr;
@@ -270,23 +312,143 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
 // ---------------------------------------------------------------------------------------
 template <int K>
 struct TcBwdSmem {
-  // A operand of the coefficient-gradient contraction, MN-major: 16-byte unit G * 256 + pixel holds the 8 rows
-  // (instances 8h .. 8h+7 of channel c, hi or lo part) G = part * 6 + c * 2 + h of that pixel.  The M = 128
-  // instruction reads 16 groups: the last four fall into img_hi / img_lo, which MUST follow (their rows are unused).
+  // A operand of the coefficient-gradient contraction, MN-major: 16-byte unit G * 256 + row holds the 8 rows
+  // (instances 8h .. 8h+7 of channel c, hi or lo part) G = part * 6 + c * 2 + h of that pixel row.  The second
+  // M = 64 block reads 8 groups: the last four fall into img_hi / img_lo, which MUST follow (their rows are unused).
   uint4 dct[12 * 256];
   uint4 img_hi[2 * 256];
   uint4 img_lo[2 * 256];
   uint4 bc_hi[2 * 48];
   uint4 bc_lo[2 * 48];
-  TcStage<K, 4> st;
-  float part[2][8][TC_J][8];   // per-warp sums of the six geometry values (by round parity)
-  float epi[48][17];           // (lo part) . basis, staged for the thread that owns the hi row
-  uint64_t mma_bar, mma2_bar;
-  uint32_t tmem_base;
+  float lgs[256 * TC_LGS];
+  TcStage<K, 3> st;            // three stages (not four): with them the CTA fits twice into an SM's shared memory
+  float part[8][TC_J][8];      // per-warp sums of the six geometry values
+  float epi[48][17];           // (lo part) . basis hi, staged for the thread that owns the hi row
 };
 
+// Coefficient-gradient contraction of one round, M = 64 blocks mb0 .. mb0 + NB - 1 issued by the calling warpgroup:
+// D[row, n] = sum_pixel dct[pixel, row] * basis[pixel, n], rows = part * 48 + channel * 16 + instance,
+// n = (hi | lo) x q.  Returns after issuing; tc_contract_finish waits.
+template <int NB>
+__device__ __forceinline__ void tc_contract_issue(int mb0, const uint4* dct, const uint4* img_hi, float (&acc)[NB][16]) {
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[b][i] = 0.f;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc_fence(acc[b]);
+  wg_fence();
+  const uint32_t a0 = gs_smem_u32(dct), b0 = gs_smem_u32(img_hi);
+#pragma unroll
+  for (int s = 0; s < 16; ++s)
+#pragma unroll
+    for (int b = 0; b < NB; ++b)
+      mma_n32_mn(acc[b], smem_desc(a0 + (mb0 + b) * 8 * 4096 + s * 256, 128, 4096), smem_desc(b0 + s * 256, 128, 4096),
+                 s > 0);
+  wg_commit();
+}
+
+// Waits for the contraction, then: rows 48 .. 95 (lo part, basis hi columns) -> epi; rows 0 .. 47 (hi part) keep
+// basis hi + basis lo in hs[r][2 i + e] = column q = 8 i + 2 (lane % 4) + e of row 16 wq + lane / 4 + 8 r.
+// Only block 0 holds hi rows (warps wq 0 .. 2 of the warpgroup that issued it).
+template <int NB>
+__device__ __forceinline__ void tc_contract_finish(int mb0, float (&acc)[NB][16], float (*epi)[17], float (&hs)[2][4],
+                                                   int wq, int lane) {
+  wg_wait_all();
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc_fence(acc[b]);
+#pragma unroll
+  for (int b = 0; b < NB; ++b)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = (mb0 + b) * 64 + wq * 16 + (lane >> 2) + 8 * r;
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float bh = acc[b][4 * i + 2 * r + e], bl = acc[b][4 * (i + 2) + 2 * r + e];   // basis hi | lo columns
+          if (row < 48) {
+            hs[r][2 * i + e] = bh + bl;
+          } else if (row < 96) {
+            epi[row - 48][8 * i + 2 * (lane & 3) + e] = bh;
+          }
+        }
+    }
+}
+
+// coefficient-gradient rows of the previous round (after a CTA barrier behind tc_contract_finish): threads of
+// warps 0 .. 2 of the warpgroup that issued block 0 own rows 16 wq + lane / 4 (+ 8) = channel * 16 + instance.
+// (np, Rp: instance count and staged records of THAT round - its stage is not refilled before the next barrier)
+template <int K, int GREC>
+__device__ __forceinline__ void tc_coef_rows(int np, const float4* Rp, const float (*epi)[17], const float (&hs)[2][4],
+                                             int wq, int lane, int tx, int ty, float* __restrict__ grad_inst) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = wq * 16 + (lane >> 2) + 8 * r;
+    const int c = row >> 4, j = row & 15;
+    if (j < np) {
+      const float4 cc = Rp[4 * j + 2];
+      const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
+      const uint32_t slot = __float_as_uint(Rp[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
+                            ((uint32_t)tx - (rxy & 0xffffu));
+      float* out = grad_inst + (size_t)slot * GREC + 6 + c * K;
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int q = 8 * i + 2 * (lane & 3) + e;
+          if (q < K) out[q] = hs[r][2 * i + e] + epi[row][q];
+        }
+    }
+  }
+}
+
+// geometry row of instance j of a round from the per-warp partial sums (NW warps)
+template <int NW, int GREC>
+__device__ __forceinline__ void tc_geom_row(int j, const float (*part)[TC_J][8], const float4* Rr, int tx, int ty,
+                                            float* __restrict__ grad_inst, uint32_t* __restrict__ row_epoch,
+                                            uint32_t epoch) {
+  float s[6];
+#pragma unroll
+  for (int u = 0; u < 6; ++u) {
+    float t = 0.f;
+#pragma unroll
+    for (int w8 = 0; w8 < NW; ++w8) t += part[w8][j][u];
+    s[u] = t;
+  }
+  const float4 a = Rr[4 * j];
+  const float4 b4 = Rr[4 * j + 1];
+  const float4 cc = Rr[4 * j + 2];
+  const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
+  const uint32_t slot = __float_as_uint(Rr[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
+                        ((uint32_t)tx - (rxy & 0xffffu));
+  float* out = grad_inst + (size_t)slot * GREC;
+  out[0] = GS_LN2 * (2.f * a.z * s[0] - a.w * s[1]);
+  out[1] = GS_LN2 * (2.f * b4.x * s[1] - a.w * s[0]);
+  out[2] = -GS_LN2 * s[2];
+  out[3] = GS_LN2 * s[3];
+  out[4] = -GS_LN2 * s[4];
+  out[5] = GS_LN2 * s[5];
+  row_epoch[slot] = epoch;
+}
+
+// Schedule of round k (two CTA-wide barriers per round):
+//   wait records(k)  ->  [96 threads: split the coefficients of round k]  ->  B1(k)  ->  [warps 0-2: coefficient rows
+//   of round k - 1]  ->  per half: logits (wgmma, waited), blend, store the dct rows  ->  B2(k) + "all pixels saturated"
+//   vote  ->  issue contraction(k)  ->  [geometry rows of round k]  ->  gather round k + 2  ->  wait contraction(k),
+//   stage its lo rows in epi / keep its hi rows in registers.
+// What orders every producer / consumer pair:
+//   staged records / coefficients   cp.async -> stage mbarrier (full[s]) -> every reader waits on it; a stage is refilled
+//                                   (round k + 2 into the stage of round k - 1) after B2(k), its last readers (blend of
+//                                   k - 1, geometry rows of k - 1, coefficient rows of k - 1) all run before B2(k)
+//   bc_hi / bc_lo                   written before B1(k); read by the logit MMAs of round k, waited before B2(k)
+//   lgs                             rows of a warp are written and read by that warp only (__syncwarp between)
+//   sm.dct                          written between B1(k) and B2(k); read by contraction(k), waited before B1(k + 1)
+//   sm.part                         written between B1(k) and B2(k); read by the geometry rows before B1(k + 1)
+//   sm.epi                          written after contraction(k), before B1(k + 1); read between B1(k + 1) and B2(k + 1)
+
 template <int K>
-__global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __restrict__ grec, const float* __restrict__ rgb,
+__global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* __restrict__ grec, const float* __restrict__ rgb,
                                                                 const uint32_t* __restrict__ ids,
                                                                 const uint32_t* __restrict__ goff,
                                                                 const int* __restrict__ tile_accum, int wp, int hp, int ntx,
@@ -298,13 +460,12 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
                                                                 float* __restrict__ grad_inst, int grad_is_final, GsCrop crop,
                                                                 uint32_t* __restrict__ row_epoch, uint32_t epoch,
                                                                 int* __restrict__ tile_neff_b) {
-  constexpr int STAGES = 4, TCOLS = 256, NV = sh_nv(K), GREC = (NV + 3) / 4 * 4;
-  constexpr uint32_t D2COL = 96;                            // logits: columns [0, 96); gradient accumulators: 2 x 32
+  constexpr int STAGES = 3, NV = sh_nv(K), GREC = (NV + 3) / 4 * 4;
   static_assert(offsetof(TcBwdSmem<K>, img_hi) == 12 * 256 * 16 && offsetof(TcBwdSmem<K>, img_lo) == 14 * 256 * 16,
                 "the basis image must follow the gradient operand: descriptors address both as one region");
   extern __shared__ __align__(128) uint8_t tc_smem_raw[];
   TcBwdSmem<K>& sm = *reinterpret_cast<TcBwdSmem<K>*>(tc_smem_raw);
-  const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
   const int tx = tile % ntx, ty = tile / ntx;
   const int ix = tx * GS_TILE + (tid & 15), iy = ty * GS_TILE + (tid >> 4);
   const int start = tile_accum[tile];
@@ -313,11 +474,8 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
   const int nchunks = (cnt + TC_J - 1) / TC_J;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) gs_mbar_init(&sm.st.full[s], TC_NT);
-    gs_mbar_init(&sm.mma_bar, 1);
-    gs_mbar_init(&sm.mma2_bar, 1);
     gs_fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc<TCOLS>(&sm.tmem_base);
   {
     float sh[16];
     pixel_sh<K>(ix, iy, rays_o, lefttop, vdx, vdy, sh);
@@ -340,44 +498,11 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
     }
     R = gr * raw[0] + gg * raw[1] + gb * raw[2];
   }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tm = sm.tmem_base;
-  const uint32_t tlane = (uint32_t)((warp & 3) * 32) << 16;
-  const uint32_t trow = tm + tlane + (uint32_t)(warp >> 2) * 48u;
+  const int row = tc_row(tid);
   const float px = gs_pixel_coord(ix, wp, fx), py = gs_pixel_coord(iy, hp, fy);
   for (int k = 0; k < STAGES - 1 && k < nchunks; ++k)
     tc_gather<K, STAGES, true>(sm.st, k, grec, rgb, ids, goff, start + k * TC_J, min(TC_J, cnt - k * TC_J), tid);
-
-  // coefficient-gradient rows of the previous round: its contraction ran while this round's operands were prepared.
-  // Rows 0 .. 95 of the accumulators live in TMEM lanes 0 .. 95 (warps 0 .. 2): (hi part) x (basis hi | lo) in rows
-  // 0 .. 47, (lo part) x basis hi in rows 48 .. 95, summed by the thread that owns the hi row.
-  // (np, Rp: instance count and staged records of THAT round - its stage is not refilled before the next barrier)
-  auto epilogue = [&](int np, const float4* Rp) {
-    if (warp < 3) {
-      float a[32], b[32];
-      tmem_ld32(tm + tlane + D2COL, a);
-      tmem_ld32(tm + tlane + D2COL + 32, b);
-      if (tid >= 48) {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) sm.epi[tid - 48][q] = a[q] + b[q];
-      }
-      gs_bar_sync(1, 96);
-      if (tid < 48) {
-        const int c = tid >> 4, j = tid & 15;
-        if (j < np) {
-          const float4 cc = Rp[4 * j + 2];
-          const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
-          const uint32_t slot = __float_as_uint(Rp[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
-                                ((uint32_t)tx - (rxy & 0xffffu));
-          float* out = grad_inst + (size_t)slot * GREC + 6 + c * K;
-#pragma unroll
-          for (int q = 0; q < K; ++q) out[q] = ((a[q] + b[q]) + (a[16 + q] + b[16 + q])) + sm.epi[tid][q];
-        }
-      }
-    }
-  };
 
   // one (pixel, instance) pair: blend state update, logit gradients dc[3], geometry values v[0..5]
   auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2, float* dc, float* v) {
@@ -410,56 +535,27 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
     dc[2] = gb * w * col[2] * (1.f - col[2]);
   };
 
-  // Schedule of round k (ONE CTA-wide barrier per round; the tensor core works one step ahead / behind):
-  //   wait logits(k)  ->  [96 threads: split the coefficients of round k + 1]  ->  first 8 instances  ->
-  //   wait contraction(k - 1) (it read sm.dct)  ->  store their rows  ->  [warps 0-2: coefficient rows of round k - 1]
-  //   ->  second 8 instances  ->  barrier + "all pixels saturated" vote  ->  issue logits(k + 1), then contraction(k)
-  //   ->  [warp 4: geometry rows of round k]  ->  gather round k + 3.
-  // What orders every producer / consumer pair (B(k) = the barrier of round k):
-  //   staged records / coefficients   cp.async -> stage mbarrier (full[s]) -> every reader waits on it; a stage is refilled
-  //                                   (round k + 3 into the stage of round k - 1) after B(k), its last readers (blend of
-  //                                   k - 1, geometry rows, coefficient rows of k - 1) all run before B(k)
-  //   bc_hi / bc_lo                   written (warps 5-7) after their wait on logits(k); read by logits(k + 1), issued after B(k)
-  //   TMEM logits                     written by logits(k + 1) after B(k); all tcgen05.ld of round k precede B(k)
-  //   sm.dct                          written after the wait on contraction(k - 1); read by contraction(k), issued after B(k)
-  //   TMEM gradient accumulators      written by contraction(k) after B(k); read (warps 0-2) in round k + 1 after its mbarrier,
-  //                                   before B(k + 1), after which contraction(k + 1) overwrites them
-  //   sm.part[k & 1]                  written in round k; read by warp 4 after B(k); rewritten in round k + 2, after B(k + 1)
-  //   sm.epi                          warps 0-2 only, named barrier 1; the next use lies behind B(k)
   int consumed = cnt, n_prev = 0, st_prev = 0;
-  uint32_t par_prev = 0;
-  gs_mbar_wait(&sm.st.full[0], 0);
-  tc_split_coefs<K>(sm.st.S[0], sm.bc_hi, sm.bc_lo, tid);
-  fence_smem_to_async();
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    if (elect_one()) {
-      fence_after_sync();
-      tc_issue_logits(tm, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, &sm.mma_bar);
-    }
-    __syncwarp();
-  }
+  float hs[2][4];
   for (int k = 0; k < nchunks; ++k) {
     const int stage = k % STAGES;
     const int n = min(TC_J, cnt - k * TC_J);
     gs_mbar_wait(&sm.st.full[stage], (uint32_t)((k / STAGES) & 1));   // records of this round
-    gs_mbar_wait(&sm.mma_bar, (uint32_t)(k & 1));
-    fence_after_sync();
-    if (k + 1 < nchunks) {                                  // logits(k) are complete: the coefficient operand is free
-      gs_mbar_wait(&sm.st.full[(k + 1) % STAGES], (uint32_t)(((k + 1) / STAGES) & 1));
-      tc_split_coefs<K>(sm.st.S[(k + 1) % STAGES], sm.bc_hi, sm.bc_lo, tid - 160);   // warps 5 .. 7
-    }
+    tc_split_coefs<K>(sm.st.S[stage], sm.bc_hi, sm.bc_lo, tid);
+    fence_smem_to_async();
+    __syncthreads();                                        // B1(k)
+    if (n_prev > 0 && tid < 96)
+      tc_coef_rows<K, GREC>(n_prev, sm.st.R[st_prev], sm.epi, hs, wq, lane, tx, ty, grad_inst);
     const float4* Rr = sm.st.R[stage];
-    float(*part)[8] = sm.part[k & 1][warp];
+    float(*part)[8] = sm.part[warp];
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
+      if (h * 8 >= n) break;                                // uniform; rows of a missing half are never read out
+      tc_logits_half<2>(2 * wg, h, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, sm.lgs, wq, lane);
       uint32_t hw[3][4], lw[3][4];
-      const bool have = h * 8 < n;                          // uniform
-      const bool idle = have && __all_sync(0xffffffffu, !(T > GS_T_STOP));
-      if (have && !idle) {
+      if (!__all_sync(0xffffffffu, !(T > GS_T_STOP))) {
         float lr[8], lg[8], lb[8];
-        tmem_ld8x3(trow + h * 8, trow + 16 + h * 8, trow + 32 + h * 8, lr, lg, lb);
+        tc_read_logits(sm.lgs, row, lr, lg, lb);
         const float4* Rh = Rr + 32 * h;
         float* ph = &part[h * 8][(lane >> 2) & 7];
         if (h * 8 + 8 <= n) {                               // all eight instances exist: no per-instance tests
@@ -496,7 +592,7 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
             for (int c = 0; c < 3; ++c) split_bf16x2(dc[0][c], dc[1][c], hw[c][jp], lw[c][jp]);
           }
         }
-      } else if (idle) {
+      } else {
         // nothing left to blend in this warp: the rows of this half round are zeros
 #pragma unroll
         for (int c = 0; c < 3; ++c)
@@ -505,94 +601,43 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_bwd_tc_kernel(const GsRec* __r
         part[h * 8 + (lane >> 2)][lane & 3] = 0.f;
         part[h * 8 + (lane >> 2)][4 + (lane & 3)] = 0.f;
       }
-      if (h == 0 && n_prev > 0) {                           // the previous contraction has read sm.dct
-        gs_mbar_wait(&sm.mma2_bar, par_prev);
-        fence_after_sync();
-      }
-      if (have) {
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          sm.dct[(c * 2 + h) * 256 + tid] = make_uint4(hw[c][0], hw[c][1], hw[c][2], hw[c][3]);
-          sm.dct[(6 + c * 2 + h) * 256 + tid] = make_uint4(lw[c][0], lw[c][1], lw[c][2], lw[c][3]);
-        }
+      for (int c = 0; c < 3; ++c) {
+        sm.dct[(c * 2 + h) * 256 + row] = make_uint4(hw[c][0], hw[c][1], hw[c][2], hw[c][3]);
+        sm.dct[(6 + c * 2 + h) * 256 + row] = make_uint4(lw[c][0], lw[c][1], lw[c][2], lw[c][3]);
       }
-      if (h == 0 && n_prev > 0) epilogue(n_prev, sm.st.R[(k - 1) % STAGES]);
     }
     fence_smem_to_async();
-    fence_before_sync();
-    const bool done = __syncthreads_and(!(T > GS_T_STOP)) != 0;   // operands of both contractions complete
-    const bool more = !done && k + 1 < nchunks;
-    if (warp == 0) {
-      if (elect_one()) {
-        fence_after_sync();
-        if (more) tc_issue_logits(tm, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, &sm.mma_bar);
-        constexpr uint32_t idesc2 = idesc_bf16(1, 1, 128, 32);
-        const uint32_t a0 = gs_smem_u32(sm.dct), b0 = gs_smem_u32(sm.img_hi);
-#pragma unroll
-        for (int s = 0; s < 16; ++s)
-          mma_bf16(tm + D2COL + (uint32_t)(s & 1) * 32u, smem_desc(a0 + s * 256, 128, 4096), smem_desc(b0 + s * 256, 128, 4096),
-                   idesc2, s >= 2);
-        mma_commit(&sm.mma2_bar);
-      }
-      __syncwarp();
-    }
+    const bool done = __syncthreads_and(!(T > GS_T_STOP)) != 0;   // B2(k): operands of the contraction complete
+    float acc[1][16];
+    tc_contract_issue<1>(wg, sm.dct, sm.img_hi, acc);
     // geometry rows (while the tensor core contracts): threads 128 .. 143, one instance each
-    if (tid >= 128 && tid < 128 + n) {
-      const int j = tid - 128;
-      float s[6];
-#pragma unroll
-      for (int u = 0; u < 6; ++u) {
-        float t = 0.f;
-#pragma unroll
-        for (int w8 = 0; w8 < 8; ++w8) t += sm.part[k & 1][w8][j][u];
-        s[u] = t;
-      }
-      const float4 a = Rr[4 * j];
-      const float4 b4 = Rr[4 * j + 1];
-      const float4 cc = Rr[4 * j + 2];
-      const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
-      const uint32_t slot = __float_as_uint(Rr[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
-                            ((uint32_t)tx - (rxy & 0xffffu));
-      float* out = grad_inst + (size_t)slot * GREC;
-      out[0] = GS_LN2 * (2.f * a.z * s[0] - a.w * s[1]);
-      out[1] = GS_LN2 * (2.f * b4.x * s[1] - a.w * s[0]);
-      out[2] = -GS_LN2 * s[2];
-      out[3] = GS_LN2 * s[3];
-      out[4] = -GS_LN2 * s[4];
-      out[5] = GS_LN2 * s[5];
-      row_epoch[slot] = epoch;
-    }
+    if (tid >= 128 && tid < 128 + n)
+      tc_geom_row<8, GREC>(tid - 128, sm.part, Rr, tx, ty, grad_inst, row_epoch, epoch);
     n_prev = n;
-    par_prev = (uint32_t)(k & 1);
     st_prev = stage;
-    if (done) {
-      consumed = min(cnt, (k + 1) * TC_J);
-      break;
-    }
-    // stage (k + 3) % 4 held round k - 1, whose records were last read before this round's barrier
-    if (k + STAGES - 1 < nchunks) {
+    // stage (k + 2) % 3 held round k - 1, whose records were last read before this round's B2
+    if (!done && k + STAGES - 1 < nchunks) {
       const int kn = k + STAGES - 1;
       tc_gather<K, STAGES, true>(sm.st, kn % STAGES, grec, rgb, ids, goff, start + kn * TC_J, min(TC_J, cnt - kn * TC_J),
                                  tid);
     }
+    tc_contract_finish<1>(wg, acc, sm.epi, hs, wq, lane);
+    if (done) {
+      consumed = min(cnt, (k + 1) * TC_J);
+      break;
+    }
   }
   __syncthreads();
-  if (n_prev > 0) {
-    gs_mbar_wait(&sm.mma2_bar, par_prev);
-    fence_after_sync();
-    epilogue(n_prev, sm.st.R[st_prev]);
-  }
+  if (n_prev > 0 && tid < 96) tc_coef_rows<K, GREC>(n_prev, sm.st.R[st_prev], sm.epi, hs, wq, lane, tx, ty, grad_inst);
   asm volatile("cp.async.wait_all;" ::: "memory");
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<TCOLS>(tm);
   if (tile_neff_b && tid == 0) tile_neff_b[tile] = consumed;
 }
 
 
 // ---------------------------------------------------------------------------------------
-// backward, TWO pixels per thread: 128 threads per tile, thread t owns pixels t (accumulator block 0) and t + 128
-// (block 1: same column, 8 rows below) - both in TMEM lane t.  The per-instance work that one pixel per thread
+// backward, TWO pixels per thread: 128 threads (one warpgroup) per tile, thread t owns pixels t and t + 128 (same
+// column, 8 rows below) and issues all four accumulator blocks.  The per-instance work that one pixel per thread
 // repeats for every 32 pixels (record loads, dx, the shuffle reduction of the six geometry sums) is shared by
 // 64 pixels, and every thread carries two independent blend recurrences.  Same operands, schedule and
 // result rows as blend_sh_bwd_tc_kernel.
@@ -610,8 +655,7 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
                                                                float* __restrict__ grad_inst, int grad_is_final, GsCrop crop,
                                                                uint32_t* __restrict__ row_epoch, uint32_t epoch,
                                                                int* __restrict__ tile_neff_b) {
-  constexpr int NT = 128, STAGES = 4, TCOLS = 256, NV = sh_nv(K), GREC = (NV + 3) / 4 * 4;
-  constexpr uint32_t D2COL = 96;
+  constexpr int NT = 128, STAGES = 3, NV = sh_nv(K), GREC = (NV + 3) / 4 * 4;
   extern __shared__ __align__(128) uint8_t tc_smem_raw[];
   TcBwdSmem<K>& sm = *reinterpret_cast<TcBwdSmem<K>*>(tc_smem_raw);
   const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -623,11 +667,8 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
   const int nchunks = (cnt + TC_J - 1) / TC_J;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) gs_mbar_init(&sm.st.full[s], NT);
-    gs_mbar_init(&sm.mma_bar, 1);
-    gs_mbar_init(&sm.mma2_bar, 1);
     gs_fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc<TCOLS>(&sm.tmem_base);
   {
     float sh[16];
     pixel_sh<K>(ix, iy0, rays_o, lefttop, vdx, vdy, sh);
@@ -654,42 +695,12 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
     }
     R[p] = gr[p] * raw[0] + gg[p] * raw[1] + gb[p] * raw[2];
   }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tm = sm.tmem_base;
-  const uint32_t tlane = (uint32_t)(warp * 32) << 16;
-  const uint32_t trow = tm + tlane;                         // block b: + 48 b
+  const int row[2] = {tc_row(tid), tc_row(tid + 128)};
   const float px = gs_pixel_coord(ix, wp, fx);
   const float py[2] = {gs_pixel_coord(iy0, hp, fy), gs_pixel_coord(iy1, hp, fy)};
   for (int k = 0; k < STAGES - 1 && k < nchunks; ++k)
     tc_gather<K, STAGES, true, NT>(sm.st, k, grec, rgb, ids, goff, start + k * TC_J, min(TC_J, cnt - k * TC_J), tid);
-
-  // (np, Rp: instance count and staged records of THAT round - its stage is not refilled before the next barrier)
-  auto epilogue = [&](int np, const float4* Rp) {
-    if (warp < 3) {
-      float a[32], b[32];
-      tmem_ld32(tm + tlane + D2COL, a);
-      tmem_ld32(tm + tlane + D2COL + 32, b);
-      if (tid >= 48) {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) sm.epi[tid - 48][q] = a[q] + b[q];
-      }
-      gs_bar_sync(1, 96);
-      if (tid < 48) {
-        const int c = tid >> 4, j = tid & 15;
-        if (j < np) {
-          const float4 cc = Rp[4 * j + 2];
-          const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
-          const uint32_t slot = __float_as_uint(Rp[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
-                                ((uint32_t)tx - (rxy & 0xffffu));
-          float* out = grad_inst + (size_t)slot * GREC + 6 + c * K;
-#pragma unroll
-          for (int q = 0; q < K; ++q) out[q] = ((a[q] + b[q]) + (a[16 + q] + b[16 + q])) + sm.epi[tid][q];
-        }
-      }
-    }
-  };
 
   // one instance, both pixels: blend state updates, logit gradients dc[pixel][3], summed geometry values v[0..7]
   auto pair2 = [&](const float4 a, const float4 b4, const float* l0, const float* l1, float (*dc)[3], float* v) {
@@ -732,40 +743,27 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
   };
 
   int consumed = cnt, n_prev = 0, st_prev = 0;
-  uint32_t par_prev = 0;
-  gs_mbar_wait(&sm.st.full[0], 0);
-  tc_split_coefs<K>(sm.st.S[0], sm.bc_hi, sm.bc_lo, tid);
-  fence_smem_to_async();
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    if (elect_one()) {
-      fence_after_sync();
-      tc_issue_logits(tm, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, &sm.mma_bar);
-    }
-    __syncwarp();
-  }
+  float hs[2][4];
   for (int k = 0; k < nchunks; ++k) {
     const int stage = k % STAGES;
     const int n = min(TC_J, cnt - k * TC_J);
     gs_mbar_wait(&sm.st.full[stage], (uint32_t)((k / STAGES) & 1));
-    gs_mbar_wait(&sm.mma_bar, (uint32_t)(k & 1));
-    fence_after_sync();
-    if (k + 1 < nchunks) {
-      gs_mbar_wait(&sm.st.full[(k + 1) % STAGES], (uint32_t)(((k + 1) / STAGES) & 1));
-      tc_split_coefs<K>(sm.st.S[(k + 1) % STAGES], sm.bc_hi, sm.bc_lo, tid - 32);   // warps 1 .. 3
-    }
+    tc_split_coefs<K>(sm.st.S[stage], sm.bc_hi, sm.bc_lo, tid);
+    fence_smem_to_async();
+    __syncthreads();                                        // B1(k)
+    if (n_prev > 0 && tid < 96)
+      tc_coef_rows<K, GREC>(n_prev, sm.st.R[st_prev], sm.epi, hs, warp, lane, tx, ty, grad_inst);
     const float4* Rr = sm.st.R[stage];
-    float(*part)[8] = sm.part[k & 1][warp];
+    float(*part)[8] = sm.part[warp];
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
+      if (h * 8 >= n) break;
+      tc_logits_half<4>(0, h, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, sm.lgs, warp, lane);
       uint32_t hw[2][3][4], lw[2][3][4];
-      const bool have = h * 8 < n;
-      const bool idle = have && __all_sync(0xffffffffu, !(T[0] > GS_T_STOP) && !(T[1] > GS_T_STOP));
-      if (have && !idle) {
+      if (!__all_sync(0xffffffffu, !(T[0] > GS_T_STOP) && !(T[1] > GS_T_STOP))) {
         float lr[2][8], lg[2][8], lb[2][8];
-        tmem_ld8x3(trow + h * 8, trow + 16 + h * 8, trow + 32 + h * 8, lr[0], lg[0], lb[0]);
-        tmem_ld8x3(trow + 48 + h * 8, trow + 64 + h * 8, trow + 80 + h * 8, lr[1], lg[1], lb[1]);
+        tc_read_logits(sm.lgs, row[0], lr[0], lg[0], lb[0]);
+        tc_read_logits(sm.lgs, row[1], lr[1], lg[1], lb[1]);
         const float4* Rh = Rr + 32 * h;
         float* ph = &part[h * 8][(lane >> 2) & 7];
         const bool full = h * 8 + 8 <= n;
@@ -790,7 +788,7 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
 #pragma unroll
             for (int c = 0; c < 3; ++c) split_bf16x2(dc[0][p][c], dc[1][p][c], hw[p][c][jp], lw[p][c][jp]);
         }
-      } else if (idle) {
+      } else {
 #pragma unroll
         for (int p = 0; p < 2; ++p)
 #pragma unroll
@@ -800,83 +798,36 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
         part[h * 8 + (lane >> 2)][lane & 3] = 0.f;
         part[h * 8 + (lane >> 2)][4 + (lane & 3)] = 0.f;
       }
-      if (h == 0 && n_prev > 0) {
-        gs_mbar_wait(&sm.mma2_bar, par_prev);
-        fence_after_sync();
-      }
-      if (have) {
 #pragma unroll
-        for (int p = 0; p < 2; ++p)
+      for (int p = 0; p < 2; ++p)
 #pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            sm.dct[(c * 2 + h) * 256 + tid + 128 * p] = make_uint4(hw[p][c][0], hw[p][c][1], hw[p][c][2], hw[p][c][3]);
-            sm.dct[(6 + c * 2 + h) * 256 + tid + 128 * p] = make_uint4(lw[p][c][0], lw[p][c][1], lw[p][c][2], lw[p][c][3]);
-          }
-      }
-      if (h == 0 && n_prev > 0) epilogue(n_prev, sm.st.R[(k - 1) % STAGES]);
+        for (int c = 0; c < 3; ++c) {
+          sm.dct[(c * 2 + h) * 256 + row[p]] = make_uint4(hw[p][c][0], hw[p][c][1], hw[p][c][2], hw[p][c][3]);
+          sm.dct[(6 + c * 2 + h) * 256 + row[p]] = make_uint4(lw[p][c][0], lw[p][c][1], lw[p][c][2], lw[p][c][3]);
+        }
     }
     fence_smem_to_async();
-    fence_before_sync();
-    const bool done = __syncthreads_and(!(T[0] > GS_T_STOP) && !(T[1] > GS_T_STOP)) != 0;
-    const bool more = !done && k + 1 < nchunks;
-    if (warp == 0) {
-      if (elect_one()) {
-        fence_after_sync();
-        if (more) tc_issue_logits(tm, sm.img_hi, sm.img_lo, sm.bc_hi, sm.bc_lo, &sm.mma_bar);
-        constexpr uint32_t idesc2 = idesc_bf16(1, 1, 128, 32);
-        const uint32_t a0 = gs_smem_u32(sm.dct), b0 = gs_smem_u32(sm.img_hi);
-#pragma unroll
-        for (int s = 0; s < 16; ++s)
-          mma_bf16(tm + D2COL + (uint32_t)(s & 1) * 32u, smem_desc(a0 + s * 256, 128, 4096), smem_desc(b0 + s * 256, 128, 4096),
-                   idesc2, s >= 2);
-        mma_commit(&sm.mma2_bar);
-      }
-      __syncwarp();
-    }
+    const bool done = __syncthreads_and(!(T[0] > GS_T_STOP) && !(T[1] > GS_T_STOP)) != 0;   // B2(k)
+    float acc[2][16];
+    tc_contract_issue<2>(0, sm.dct, sm.img_hi, acc);
     // geometry rows: threads 96 .. 111 (warp 3), one instance each
-    if (tid >= 96 && tid < 96 + n) {
-      const int j = tid - 96;
-      float s[6];
-#pragma unroll
-      for (int u = 0; u < 6; ++u) s[u] = (sm.part[k & 1][0][j][u] + sm.part[k & 1][1][j][u]) + (sm.part[k & 1][2][j][u] + sm.part[k & 1][3][j][u]);
-      const float4 a = Rr[4 * j];
-      const float4 b4 = Rr[4 * j + 1];
-      const float4 cc = Rr[4 * j + 2];
-      const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
-      const uint32_t slot = __float_as_uint(Rr[4 * j + 3].x) + ((uint32_t)ty - (rxy >> 16)) * (rwh & 0xffffu) +
-                            ((uint32_t)tx - (rxy & 0xffffu));
-      float* out = grad_inst + (size_t)slot * GREC;
-      out[0] = GS_LN2 * (2.f * a.z * s[0] - a.w * s[1]);
-      out[1] = GS_LN2 * (2.f * b4.x * s[1] - a.w * s[0]);
-      out[2] = -GS_LN2 * s[2];
-      out[3] = GS_LN2 * s[3];
-      out[4] = -GS_LN2 * s[4];
-      out[5] = GS_LN2 * s[5];
-      row_epoch[slot] = epoch;
-    }
+    if (tid >= 96 && tid < 96 + n) tc_geom_row<4, GREC>(tid - 96, sm.part, Rr, tx, ty, grad_inst, row_epoch, epoch);
     n_prev = n;
-    par_prev = (uint32_t)(k & 1);
     st_prev = stage;
-    if (done) {
-      consumed = min(cnt, (k + 1) * TC_J);
-      break;
-    }
-    if (k + STAGES - 1 < nchunks) {
+    if (!done && k + STAGES - 1 < nchunks) {
       const int kn = k + STAGES - 1;
       tc_gather<K, STAGES, true, NT>(sm.st, kn % STAGES, grec, rgb, ids, goff, start + kn * TC_J, min(TC_J, cnt - kn * TC_J),
                                      tid);
     }
+    tc_contract_finish<2>(0, acc, sm.epi, hs, warp, lane);
+    if (done) {
+      consumed = min(cnt, (k + 1) * TC_J);
+      break;
+    }
   }
   __syncthreads();
-  if (n_prev > 0) {
-    gs_mbar_wait(&sm.mma2_bar, par_prev);
-    fence_after_sync();
-    epilogue(n_prev, sm.st.R[st_prev]);
-  }
+  if (n_prev > 0 && tid < 96) tc_coef_rows<K, GREC>(n_prev, sm.st.R[st_prev], sm.epi, hs, warp, lane, tx, ty, grad_inst);
   asm volatile("cp.async.wait_all;" ::: "memory");
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<TCOLS>(tm);
   if (tile_neff_b && tid == 0) tile_neff_b[tile] = consumed;
 }
 
@@ -886,9 +837,15 @@ cudaError_t gs_launch_blend_sh_fwd_tc(const GsRec* grec, const float* rgb, const
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, float* image,
                                       int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st) {
 #define GS_SHF_TC(K)                                                                                                  \
-  blend_sh_fwd_tc_kernel<K><<<g.n_tiles, TC_NT, 0, st>>>(grec, rgb, ids, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy,     \
-                                                         r.rays_o, r.lefttop, r.dx, r.dy, image, tile_neff, final_img, \
-                                                         crop)
+  do {                                                                                                                \
+    /* per device and cheap: set on every launch rather than cached in a process-wide flag */                        \
+    cudaError_t e = cudaFuncSetAttribute(blend_sh_fwd_tc_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
+                                         (int)sizeof(TcFwdSmem<K>));                                                  \
+    if (e != cudaSuccess) return e;                                                                                   \
+    blend_sh_fwd_tc_kernel<K><<<g.n_tiles, TC_NT, sizeof(TcFwdSmem<K>), st>>>(                                         \
+        grec, rgb, ids, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image, tile_neff,  \
+        final_img, crop);                                                                                             \
+  } while (0)
   if (d == 27) GS_SHF_TC(9); else GS_SHF_TC(16);
 #undef GS_SHF_TC
   return cudaGetLastError();
@@ -899,10 +856,9 @@ cudaError_t gs_launch_blend_sh_bwd_tc(const GsRec* grec, const float* rgb, const
                                       const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
                                       uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st) {
   if (!row_epoch) return cudaErrorInvalidValue;   // unprocessed rows are left stale: the consumer needs the epoch tags
-  const bool two_px = (gs_tuning().sh_tc & 4) != 0;   // two pixels per thread (128 threads per tile)
+  const bool two_px = (gs_sh_tc_mode(d) & 4) != 0;   // two pixels per thread (128 threads per tile)
 #define GS_SHB_TC(K)                                                                                                  \
   do {                                                                                                                \
-    /* per device and cheap: set on every launch rather than cached in a process-wide flag */                        \
     cudaError_t e = two_px ? cudaFuncSetAttribute(blend_sh_bwd_tc2_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                                   (int)sizeof(TcBwdSmem<K>))                                          \
                            : cudaFuncSetAttribute(blend_sh_bwd_tc_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, \

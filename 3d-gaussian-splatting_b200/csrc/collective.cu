@@ -124,8 +124,13 @@ __global__ void __launch_bounds__(512) push_finish_mc_kernel(float4* mc_bucket, 
 
 int nvls_max_grid() {
   static const int g = [] {
-    const char* e = getenv("GS_NVLS_GRID");          // tuning knob (CTAs), default 4 per SM
-    return e && atoi(e) > 0 ? atoi(e) : 148 * 4;
+    const char* e = getenv("GS_NVLS_GRID");          // tuning knob (CTAs), default 4 per SM of the current device
+    if (e && atoi(e) > 0) return atoi(e);
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0)
+      sms = 132;                                     // H100 SXM
+    return sms * 4;
   }();
   return g;
 }

@@ -1,4 +1,4 @@
-// Shared device helpers for libgs_b200 (sm_100a only).
+// Shared device helpers for libgs_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

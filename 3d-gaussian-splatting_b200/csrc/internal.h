@@ -27,7 +27,7 @@ struct GsRayPtrs {
   const float *rays_o, *lefttop, *dx, *dy;
 };
 
-// Run-time tuning knobs (A/B experiments and profiles/; the defaults are the shipped configuration).
+// Run-time tuning knobs (A/B experiments; the defaults are the configuration measured fastest on the H100).
 // Set with gs_tune("name", value) or the environment variable GS_TUNE_<NAME> (read once).
 struct GsTuning {
   int fwd_kernel;   // 0 = consumer thread 0 issues the copies, 1 = dedicated producer warp
@@ -43,7 +43,8 @@ struct GsTuning {
   int bwd_ch;       // gather path: instances per staging chunk of the backward (64 or 32)
   int strict;       // 1: an un-instantiated knob combination is an error (sweeps); 0: falls back to the shipped kernel
   int gather;       // fused frame path (RGB and SH): 1 = no pack pass, blend kernels gather records from rec[N]; 0 = packed streams
-  int sh_tc;        // SH blend on the tensor cores (blend_sh_tc.cu, gather path only): bit 0 = forward, bit 1 = backward
+  int sh_tc;        // SH blend on the tensor cores (blend_sh_tc.cu, gather path only): -1 = by colour width (gs_sh_tc_mode),
+                    // else bit 0 = forward, bit 1 = backward, bit 2 = two pixels per thread in the backward
 };
 GsTuning& gs_tuning();
 
@@ -54,6 +55,7 @@ void gs_count_launch(int n = 1);
 int gs_sh_basis_count(int d);      // 27 -> 9, 48 -> 16, else 0
 int gs_sh_stream_width(int d);     // floats per instance row of the SH stream (coefficients + slot, padded)
 int gs_sh_grad_width(int d);       // floats per instance gradient row (6 geometry + d coefficients, padded)
+int gs_sh_tc_mode(int d);          // the sh_tc bits in effect for colour width d
 // grec != nullptr: gather path (records from rec[N], raw coefficients from the parameter tensor rgb[N, d])
 cudaError_t gs_launch_blend_sh_fwd(const float4* pA, const float2* pB, const float* pS, const GsRec* grec,
                                    const float* rgb, const uint32_t* ids, const uint32_t* goff /*offsets_g*/, int d,
@@ -67,7 +69,7 @@ cudaError_t gs_launch_blend_sh_bwd(const float4* pA, const float2* pB, const flo
                                    const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
                                    uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st);
 
-// ---- blend_sh_tc.cu (tcgen05 / TMEM) -----------------------------------------------------
+// ---- blend_sh_tc.cu (wgmma) ---------------------------------------------------------------
 cudaError_t gs_launch_blend_sh_fwd_tc(const GsRec* grec, const float* rgb, const uint32_t* ids, int d,
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, float* image,
                                       int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st);

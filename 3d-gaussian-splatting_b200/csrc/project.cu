@@ -173,8 +173,9 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
       rgb_raw[1] = rgb[3 * i + 1];
       rgb_raw[2] = rgb[3 * i + 2];
     }
-    // (measured slower: loading the tags and rows of 4 instances at once - 0.180 vs 0.168 ms, 80 registers; a
-    //  warp-cooperative version streaming the 32 Gaussians' contiguous row span through shared memory - 0.238 ms)
+    // (one row at a time; alternatives tried on an earlier GPU and found slower: loading the tags and rows of
+    //  4 instances at once (80 registers), a warp-cooperative version streaming the 32 Gaussians' contiguous row
+    //  span through shared memory)
     for (uint32_t r = o0; r < o1; ++r) {
       if (row_epoch[r] != epoch) continue;     // instance not reached by its (saturated) tile: zero gradient
       const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)r * GW);
@@ -227,8 +228,8 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
   if (W == 0) {
     if constexpr (kStagedRgb) {
       // The 32 Gaussians of a warp own 32 * D contiguous floats of g_rgb.  One strided 4-byte store per coefficient
-      // makes every store a partial-sector write (read-modify-write under ECC: 8x the bytes; 0.45 / 0.91 ms at
-      // D = 27 / 48 against 0.17 ms for RGB): the rows go through shared memory and leave as whole sectors.
+      // makes every store a partial-sector write (read-modify-write under ECC: 8x the bytes): the rows go through
+      // shared memory and leave as whole sectors.
       // D = 48: two passes of 24 floats (96-byte, sector-aligned pieces); D = 27: the whole 32 x 108-byte span.
       constexpr int HW = (D % 8 == 0) ? D / 2 : D;
       __shared__ float stage[kBlock / 32][32][HW + 1];

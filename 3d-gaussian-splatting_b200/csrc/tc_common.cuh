@@ -1,19 +1,19 @@
-// tcgen05 / TMEM helpers of the SH blend kernels (sm_100a, cta_group::1, no-swizzle canonical layouts).
+// wgmma helpers of the SH blend kernels (sm_90a, bf16 operands in shared memory, fp32 accumulators in registers,
+// no-swizzle canonical layouts).
 //
 // Shared-memory matrix descriptor (64 bit): start address >> 4 in bits [0,14), leading byte offset >> 4 in
-// [16,30), stride byte offset >> 4 in [32,46), version 1 in [46,48), swizzle mode 0 (none) in [61,64).
+// [16,30), stride byte offset >> 4 in [32,46), base offset 0 in [49,52), layout type 0 (no swizzle) in [62,64).
 // For the no-swizzle layouts a "core matrix" is 8 rows x 16 bytes, stored as 128 contiguous bytes:
 //   K-major  operand (row = M/N index, 16 B = 8 bf16 along K):  LBO = distance between the two core matrices
 //            that one K = 16 instruction spans along K, SBO = distance between groups of 8 rows;
 //   MN-major operand (row = K index, 16 B = 8 bf16 along M/N):  LBO = distance between the two groups of 8 K
 //            rows of one instruction, SBO = distance between groups of 8 M/N elements.
-// (Both checked on the device with profiles/r2_micro/umma_probe.cu.)
-// Instruction descriptor (32 bit): D format f32 (1) in [4,6), A / B format bf16 (1) in [7,10) / [10,13),
-// A / B major (0 = K, 1 = MN) in bits 15 / 16, N >> 3 in [17,23), M >> 4 in [24,29).
 //
-// Every .sync.aligned instruction below is preceded by __syncwarp(): after divergent code (an elected issuing
-// lane, a spin on an mbarrier) the lanes of a warp are not guaranteed to have reconverged, and a split warp
-// executes e.g. tcgen05.dealloc twice.
+// Accumulator fragment of an m64nN instruction issued by a warpgroup: warp w (of the warpgroup), lane L holds
+// d[4 i + 2 r + e] = D[16 w + L / 4 + 8 r][8 i + 2 (L % 4) + e],  i < N / 8, r, e in {0, 1}.
+//
+// Every .sync.aligned instruction below is preceded by __syncwarp(): after divergent code (a subset of threads
+// splitting operands, a spin on an mbarrier) the lanes of a warp are not guaranteed to have reconverged.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -23,80 +23,48 @@ namespace gs_tc {
 
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
   const uint32_t lo = ((addr & 0x3FFFFu) >> 4) | ((lbo >> 4) << 16);
-  const uint32_t hi = (sbo >> 4) | (1u << 14);
+  const uint32_t hi = sbo >> 4;
   return ((uint64_t)hi << 32) | lo;
 }
-__host__ __device__ constexpr uint32_t idesc_bf16(int a_mn, int b_mn, int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// accumulator registers are written by the asynchronous tensor core: keep the compiler from moving accesses
+// across the issue / wait points
+template <int N>
+__device__ __forceinline__ void acc_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void mma_bf16(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               :: "r"(d), "l"(a), "l"(b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on `bar` when all MMAs issued so far by this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(gs_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// whole warp; the base address (lane 0, first column) is written to *dst_smem
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  static_assert(COLS == 32 || COLS == 64 || COLS == 128 || COLS == 256 || COLS == 512, "power of two >= 32");
+__device__ __forceinline__ void wg_fence() {
   __syncwarp();
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(gs_smem_u32(dst_smem)), "r"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() {
   __syncwarp();
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "r"(COLS) : "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 // generic-proxy shared-memory writes -> visible to the tensor core's (async proxy) operand reads
 __device__ __forceinline__ void fence_smem_to_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// tcgen05.ld.32x32b: lane L of the warp reads consecutive columns of TMEM lane (warp % 4) * 32 + L; the helpers block
-// until the data is there (tcgen05.wait::ld).
-// three column blocks of 8 (one per colour channel) with a single wait
-__device__ __forceinline__ void tmem_ld8x3(uint32_t t0, uint32_t t1, uint32_t t2, float* v0, float* v1, float* v2) {
-  uint32_t r[24];
-  __syncwarp();
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%24];\n\t"
-               "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%8,%9,%10,%11,%12,%13,%14,%15}, [%25];\n\t"
-               "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%16,%17,%18,%19,%20,%21,%22,%23}, [%26];\n\t"
-               "tcgen05.wait::ld.sync.aligned;"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                 "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23])
-               : "r"(t0), "r"(t1), "r"(t2) : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    v0[i] = __uint_as_float(r[i]);
-    v1[i] = __uint_as_float(r[8 + i]);
-    v2[i] = __uint_as_float(r[16 + i]);
-  }
+// D[64 x 24] (+)= A[64 x 16] * B[24 x 16]^T, A and B K-major; issued by the whole warpgroup
+__device__ __forceinline__ void mma_n24_kk(float (&d)[12], uint64_t a, uint64_t b, int accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+               : "l"(a), "l"(b), "r"(accumulate)
+               : "memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  __syncwarp();
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-               "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n\t"
-               "tcgen05.wait::ld.sync.aligned;"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                 "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                 "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-               : "r"(taddr) : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32], A and B MN-major; issued by the whole warpgroup
+__device__ __forceinline__ void mma_n32_mn(float (&d)[16], uint64_t a, uint64_t b, int accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(a), "l"(b), "r"(accumulate)
+               : "memory");
 }
 
 // x = hi + lo (+ 2^-17 |x|) with hi, lo in bf16: two values per 32-bit word, the first in the low half

@@ -2,7 +2,7 @@
 replicated, camera views sharded, ONE all-reduce of a flat gradient bucket per step.
 
 The reference is single-process/single-GPU (no collective anywhere); this is the only
-cross-GPU exchange the path needs.  `GradBucket` is backend-agnostic (NCCL on the B200 box,
+cross-GPU exchange the path needs.  `GradBucket` is backend-agnostic (NCCL on GPUs,
 gloo in the CPU tests).  `SymmetricGradBucket` is the NVLink-native version: the fused backward
 writes its gradients straight into a symmetric-memory bucket and one kernel of ours
 (csrc/collective.cu: NVSwitch multimem reduction, or peer loads/stores) sums it in place;
@@ -92,11 +92,8 @@ class SymmetricGradBucket:
       mode "auto":     push (W = 2, 4, 8; GS_DP_PUSH_MC=1 sends its broadcast half through the NVSwitch with
                        multimem.st), else multimem / p2p.
 
-    Measured on B200 for the 134 MB bucket of 2.4 M Gaussians (profiles/r1_exchange.md), exchange
-    alone: W = 2: p2p 0.214 ms, multimem 0.357, NCCL 0.292; W = 8: multimem 0.330, p2p 0.394,
-    NCCL 0.394.  Whole step at W = 2: push 2.30 ms, p2p 2.40, NCCL 2.50 (one GPU: 2.16).
-    `make_grad_bucket("auto")` picks push for W = 2 (validated against NCCL on 2 GPUs) and keeps
-    NCCL for W >= 4, where push measured 2.35 ms vs 2.56 at W = 4 but is not yet parity-tested.
+    The exchange timings of these modes have not been measured on H100; `tests/test_exchange_gpu.py`
+    checks every mode against NCCL on 2 GPUs.
 
     `allocator` must be installed with `renderer.set_flat_grad_allocator` (make_grad_bucket does
     it).  A change of the bucket size (densification changes N on every rank at the same step)
@@ -141,8 +138,7 @@ class SymmetricGradBucket:
             self.mode = "p2p" if (p2p_ok or not has_mc) else "multimem"
         # broadcast half of the pushed exchange: plain peer stores by default; GS_DP_PUSH_MC=1 sends it through
         # the NVSwitch instead (one multimem.st per 16 bytes: each GPU sends its slice once, but the switch also
-        # loops the slice back to its owner) - measured within noise of each other at 4 and 8 GPUs
-        # (profiles/r2_scaling.md), so the simpler one ships
+        # loops the slice back to its owner); the simpler peer stores are the default
         self.push_mc = has_mc and os.environ.get("GS_DP_PUSH_MC") == "1"
         if self.mode == "multimem" and not has_mc:
             raise RuntimeError("symmetric memory has no multicast mapping (NVLS unavailable)")

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Run the reference's `train.py` UNCHANGED on this framework, on 1..8 GPUs (SURVEY.md §8 f-1,
-BASELINE configs[3] "8 views sharded across 8 GPUs, NCCL grad allreduce, train.py loop").
+"8 views sharded across 8 GPUs, NCCL grad allreduce, train.py loop").
 
     python dp_launch.py [--train-py PATH] [--splatter ours|reference] [--torch-adam] -- <train.py arguments>
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 dp_launch.py -- --data ...

@@ -3,7 +3,7 @@
 Same public names, positional argument order, return values and zero-fill/ownership
 conventions as reference renderer.py (`draw` :89, `trunc_exp` :102,
 `world2camera_func` :119, `global_culling` :158), so code written against the
-reference keeps working; underneath, every op calls the sm_100a kernels of
+reference keeps working; underneath, every op calls the sm_90a kernels of
 libgs_b200 through the `gaussian` extension in this directory.  Additive:
 `render_frame`, one autograd node for the whole frame (fused path).
 
@@ -19,7 +19,7 @@ try:
 except ImportError as e:  # pragma: no cover - fail loudly, never fall back
     raise ImportError(
         "the `gaussian` CUDA extension is not built; run "
-        "`python 3d-gaussian-splatting_b200/build.py` (needs nvcc, sm_100a)") from e
+        "`python 3d-gaussian-splatting_b200/build.py` (needs nvcc, sm_90a)") from e
 
 
 def _f32(t):

@@ -1,5 +1,5 @@
 """Scene + per-frame pipeline: host-side mirror of the reference's `Splatter`
-(reference splatter.py:323-655) on top of the fused B200 frame path.
+(reference splatter.py:323-655) on top of the fused frame path.
 
 Same constructor as the reference (`Splatter(colmap_path, image_path, near=..., ...)`,
 splatter.py:324-345) and the surface train.py / visergui.py touch (train.py:57-61,:67,:99,:150,

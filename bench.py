@@ -2,6 +2,7 @@
 """Benchmark of the hot path: render + backward FPS at 1080p, 2.4M Gaussians.
 
   python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload C2|C3|C5] [--colour 3|27|48]
+                  [--dump-outputs DIR]
 
 One "step" = one forward + backward of one 1920x1080 view per GPU: raw parameters ->
 image -> gradients of all five parameter tensors for a fixed upstream image gradient
@@ -14,6 +15,10 @@ from pinned HOST memory and the rendered image read back to the host every step.
 Also on the line: `stage_ms`, `roofline` (HBM fraction as the metric asks + what really binds),
 `gpu_launches` (counted by the library), at N = 1 short legs `sh` (D = 27 / 48) and `opaque_scene`, at
 N > 1 `exchange_check` (active exchange vs NCCL, bit-equality across ranks) and `per_rank`.
+
+--dump-outputs DIR writes what the last timed step computed (rank 0; either arm) as float32 .npy files: `image`
+and the gradients `grad_<param>` of the five parameter tensors (see dump_outputs).  Inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 --impl reference times the reference's own CUDA build (oracle/_ref: unmodified
 gaussian.cu + bindings.cpp + renderer.py) driven with the reference's per-frame call
@@ -73,7 +78,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
@@ -225,22 +230,6 @@ def workload_string(name, n, w, h, colour, fwd_only):
             f"one view per GPU (view k = rank mod 8), seed 0 (SURVEY.md §8d generator)")
 
 
-def ncu_metrics(workload, colour, kernel):
-    """Per-launch counters of `kernel` from the committed `ncu --set full` captures
-    (profiles/*_ncu_metrics.json, written by profiles/summarize.py; latest round wins): DRAM traffic,
-    executed warp instructions, MUFU (XU pipe) and FMA pipe utilisation.  None if not captured."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    for name in sorted(os.listdir(pdir)) if os.path.isdir(pdir) else []:
-        if name.endswith("_ncu_metrics.json"):
-            try:
-                d = json.load(open(os.path.join(pdir, name)))
-                best = d.get(f"{workload}/D{colour}", {}).get(kernel, best)
-            except Exception:
-                pass
-    return best
-
-
 class Scene:
     """One replica of the benchmark scene on this rank's GPU, driven through the public Splatter API."""
 
@@ -274,7 +263,7 @@ class Scene:
 
 
 def exchange_check(sc, view_id, world, dev):
-    """Run on every multi-GPU bench (the driver's GPU-test box has ONE GPU): the gradient bucket summed by the
+    """Run on every multi-GPU bench: the gradient bucket summed by the
     active exchange vs NCCL's all-reduce of the same per-rank gradients (the backward is deterministic, so
     two backwards of the same frame give identical local gradients), and bit-equality across ranks."""
     import torch.distributed as dist
@@ -296,6 +285,38 @@ def exchange_check(sc, view_id, world, dev):
             if sc.symmetric else "nccl",
             "max_rel_err_vs_nccl": float(err), "bit_equal_across_ranks": bool(all(int(d) == int(alld[0]) for d in alld)),
             "floats": int(got.numel())}
+
+
+DUMP_ROWS = 65536        # Gaussians sampled for the gradient dumps
+DUMP_PIXELS = 1 << 21    # image pixels kept when the image is larger (4K)
+
+
+def _sample_rows(n, k, seed):
+    """A fixed, seeded sample of k of n row indices (sorted), or all rows when n <= k."""
+    if n <= k:
+        return torch.arange(n)
+    g = torch.Generator().manual_seed(seed)
+    return torch.randperm(n, generator=g)[:k].sort().values
+
+
+def dump_outputs(out_dir, img, params):
+    """The arrays a caller of the timed path receives from its last step, as float32 .npy files (at most ~40 MB):
+    the rendered image [H, W, 3] (a seeded sample of DUMP_PIXELS pixels [k, 3] above that size) and, per parameter,
+    its gradient on a seeded sample of DUMP_ROWS Gaussians (the same rows for every parameter)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    im = img.detach().float().cpu()
+    if im.shape[0] * im.shape[1] > DUMP_PIXELS:
+        im = im.reshape(-1, im.shape[-1])[_sample_rows(im.shape[0] * im.shape[1], DUMP_PIXELS, 1)]
+    arrays["image"] = im
+    names = ("pos", "rgb", "opa", "quat", "scale")
+    if all(p.grad is not None for p in params):
+        rows = _sample_rows(params[0].shape[0], DUMP_ROWS, 2)
+        for name, p in zip(names, params):
+            arrays["grad_" + name] = p.grad.detach().float().cpu().reshape(p.shape[0], -1)[rows]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy().astype(np.float32))
 
 
 def run_ours(args, world, rank, local):
@@ -320,9 +341,10 @@ def run_ours(args, world, rank, local):
     if rank == 0:
         sampler.start()
     launches0 = None
+    last_img = [None]
 
     def step_resident():
-        sc.step(view_id)
+        last_img[0] = sc.step(view_id)
 
     for _ in range(args.warmup):
         step_resident()
@@ -336,6 +358,8 @@ def run_ours(args, world, rank, local):
     barrier(world)
     launches = gaussian.kernel_launches() - launches0
     ms_local = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_img[0], params)
     ms = max_over_ranks(ms_local, world, dev)
     clocks = sampler.stop() if rank == 0 else {}
 
@@ -431,24 +455,17 @@ def run_ours(args, world, rank, local):
     alg_bytes, k_ms = (bb, blend_b_ms) if not fwd_only else (bf, blend_f_ms)
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9 if k_ms and k_ms > 0 else None
     pairs = (Meff_b if not fwd_only else Meff) * 256
-    ncu = ncu_metrics(args.workload, D, roof_kernel) or {}
-    sm_hz = (clocks.get("sm_mhz") or 1965.0) * 1e6
+    sm_hz = (clocks.get("sm_mhz") or 1980.0) * 1e6
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
     roof = {"bound": "hbm", "kernel": roof_kernel, "achieved": achieved, "peak": peak, "unit": "GB/s",
-            "frac": (achieved / peak) if achieved else None, "traffic": ncu.get("dram_bytes"),
-            "traffic_unit": "bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum, ncu --set full)",
+            "frac": (achieved / peak) if achieved else None,
             "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
             # the roof that actually binds: instruction issue (4 warp-instructions / clk / SM) and MUFU (16 / clk / SM)
             "binding": "issue",
             "pairs_per_launch": pairs, "pairs_per_s": pairs / (k_ms * 1e-3) if k_ms and k_ms > 0 else None,
             "pairs_per_clk_per_sm": pairs / (k_ms * 1e-3 * sm_hz * n_sm) if k_ms and k_ms > 0 else None,
-            "issue_frac": ncu.get("issue_active_frac"), "mufu_frac": ncu.get("xu_pipe_frac"),
-            "fma_pipe_frac": ncu.get("fma_pipe_frac"), "warp_inst_per_launch": ncu.get("warp_inst"),
-            "thread_inst_per_pair": (ncu["warp_inst"] * 32.0 / pairs) if ncu.get("warp_inst") and pairs else None,
-            "ncu_source": ncu.get("source"),
             "note": "blend is instruction-issue / MUFU bound, not HBM bound (SURVEY.md §8d): the HBM fraction is reported "
-                    "because the metric asks for it; issue_frac / mufu_frac come from the committed ncu capture of this "
-                    "workload (null if not captured), pairs_per_s is measured live",
+                    "because the metric asks for it; pairs_per_s is measured live",
             "blend_fwd": {"ms": blend_f_ms, "algorithmic_bytes": bf,
                           "achieved": bf / (blend_f_ms * 1e-3) / 1e9 if blend_f_ms > 0 else None},
             "blend_bwd": {"ms": blend_b_ms, "algorithmic_bytes": bb,
@@ -461,8 +478,9 @@ def run_ours(args, world, rank, local):
         "config": {"workload": workload_string(args.workload, n, w, h, D, fwd_only),
                    "tile_instances_M": M, "tile_instances_consumed_M_eff": Meff, "consumed_by_backward": Meff_b,
                    "max_tile_count": st["max_tile_count"],
-                   "n_visible": st["n_visible"], "l2": "inputs larger than L2 (per-frame working set "
-                                                       f"{(M * 112 + n * 56) / 1e6:.0f} MB >> 126 MB)",
+                   "n_visible": st["n_visible"], "l2": "per-frame working set "
+                                                       f"{(M * 112 + n * 56) / 1e6:.0f} MB, L2 "
+                                                       f"{torch.cuda.get_device_properties(dev).L2_cache_size / 1e6:.0f} MB",
                    "parallelism": f"dp{world} over views, gradient bucket exchange: {exchange}"},
         "clocks": clocks,
         "e2e": {"value": world * 1000.0 / ms_e2e, "unit": "frames/s", "ms_per_step": ms_e2e,
@@ -502,7 +520,7 @@ def _short_leg(sc, steps=10, warmup=3):
 
 
 def sh_legs(dev):
-    """BASELINE configs[2] as written ("SH degree 3") and the reference's own SH (degree 2): short 10-step
+    """Per-pixel SH colour, degree 3 (D = 48) and the reference's own SH (degree 2): short 10-step
     legs of the same C3 scene with per-pixel SH colour; D=27 also times the reference's CUDA build here."""
     import gc
     res = {}
@@ -592,6 +610,8 @@ def run_reference(args, world, rank, local):
     n, w, h, fwd_only = WORKLOADS[args.workload]
     gref, rref = ref_pipeline.load_reference()
     if gref is None:
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs with --impl reference needs the reference's CUDA build (oracle/_ref)")
         cb = cpu_baseline(args.workload)
         return {"impl": "reference", "metric": METRIC, "value": cb["value"], "unit": "frames/s", "n_gpus": 1,
                 "steps": 1, "warmup": 0, "ms_per_step": 1000.0 / cb["value"], "higher_is_better": True,
@@ -608,21 +628,24 @@ def run_reference(args, world, rank, local):
                                      use_sh_coeff=args.colour != 3)
     p = {k: t.to(dev).clone().requires_grad_(True) for k, t in g.items()}
     go = S.make_grad_output(h, w, 0).to(dev)
+    last_img = [None]
 
     def step():
         for t in p.values():
             t.grad = None
         if fwd_only:
             with torch.no_grad():
-                frame(p["pos"], p["rgb"], p["opa"], p["quat"], p["scale"])
+                last_img[0] = frame(p["pos"], p["rgb"], p["opa"], p["quat"], p["scale"])
         else:
-            img = frame(p["pos"], p["rgb"], p["opa"], p["quat"], p["scale"])
-            img.backward(go)
+            last_img[0] = frame(p["pos"], p["rgb"], p["opa"], p["quat"], p["scale"])
+            last_img[0].backward(go)
 
     sampler = ClockSampler(local)
     sampler.start()
     ms = timed_loop(step, args.steps, args.warmup, 1, dev)
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_img[0], [p[k] for k in ("pos", "rgb", "opa", "quat", "scale")])
     fps = 1000.0 / ms
     return {"impl": "reference", "metric": METRIC if args.workload == "C3" else f"FPS ({args.workload})",
             "value": fps, "unit": "frames/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
@@ -648,7 +671,7 @@ def main():
     os.dup2(2, 1)
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="C3", choices=sorted(WORKLOADS))
@@ -661,7 +684,12 @@ def main():
     ap.add_argument("--colour", type=int, default=3, choices=[3, 27, 48],
                     help="3 = RGB (default; the reference's published 2.4M point), 27 = per-pixel SH degree 2 "
                          "(the reference's use_sh_coeff), 48 = SH degree 3 extension")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the image and (sampled) parameter gradients of the last step "
+                         "to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs a CUDA device (the product path has no CPU fallback)")
     if args.impl != "reference":

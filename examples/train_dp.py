@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """View-sharded data-parallel training loop on a synthetic multi-view scene (SURVEY.md §8f-1,
-BASELINE configs[3]): the `train_step` of the reference trainer (train.py:85-201 — zero_grad,
+the multi-view training configuration): the `train_step` of the reference trainer (train.py:85-201 — zero_grad,
 render one training camera, L1 loss, backward, Adam over the five parameter groups with the
 reference's learning-rate factors train.py:21-25,56-64) with the one change multi-GPU needs: each
 rank renders a different view and the gradients are all-reduced (one flat bucket) before the step.

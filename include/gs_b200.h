@@ -1,5 +1,5 @@
 /*
- * gs_b200.h — C ABI of libgs_b200.so: B200-native (sm_100a) differentiable tile rasterizer.
+ * gs_b200.h — C ABI of libgs_b200.so: H100-native (sm_90a) differentiable tile rasterizer.
  *
  * This is the drop-in boundary for the hot path of WangFeng18/3d-gaussian-splatting
  * (projection + 3D->2D covariance, (tile|depth) sort, front-to-back alpha blend, and the
@@ -33,7 +33,7 @@ typedef void* gs_stream_t; /* cudaStream_t */
 int gs_abi_version(void);
 /* Human-readable text of the last error on this host thread ("" if none). */
 const char* gs_last_error(void);
-/* A/B tuning knobs of the blend kernels (profiles/ experiments; defaults = the shipped configuration):
+/* A/B tuning knobs of the blend kernels (A/B experiments; defaults = the configuration measured fastest on the H100):
  * "fwd_kernel", "fwd_ch", "bwd_kernel", "bwd_px", "bwd_ws", "bwd_unroll", "bwd_stages", "bwd_minb"
  * (see csrc/internal.h GsTuning).  An unsupported combination makes the next backward fail with
  * cudaErrorInvalidValue.  Process-wide, not thread-safe. */

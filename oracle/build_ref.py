@@ -1,15 +1,15 @@
 """Build the UNMODIFIED reference CUDA extension into oracle/_ref/ (git-ignored).
 
-TEST INFRASTRUCTURE ONLY.  Compiles /root/reference/src/{gaussian.cu,bindings.cpp}
+TEST INFRASTRUCTURE ONLY.  Compiles <reference>/src/{gaussian.cu,bindings.cpp}
 from where they lie (no source is copied into the repo) into
 ``oracle/_ref/gaussian_ref*.so``.  The only deviation from the reference's own
 setup.py (setup.py:7-13) is build flags: ``-std=c++17`` instead of ``-std=c++14``
-(torch >= 2.1 headers refuse C++14), an explicit sm_100a ``-gencode`` and the module
+(torch >= 2.1 headers refuse C++14), an explicit sm_90a ``-gencode`` and the module
 name ``gaussian_ref`` (``-DTORCH_EXTENSION_NAME``, so that it can be imported
 next to our own ``gaussian`` module in one process).
 
-The built .so travels to the GPU box with the gpurun snapshot; /root/reference itself
-does not exist there, so nothing at test/bench time reads the sources.
+The reference checkout is $GS_REFERENCE_DIR.  Tests and bench.py only load the built .so and the copied Python
+files; nothing at test/bench time reads the sources.
 The reference's pure-python files that the ``bench.py --impl reference`` arm and the drop-in tests
 drive UNCHANGED (renderer.py, splatter.py, utils.py, train.py, visergui.py, transforms/) are copied next
 to the .so at build time as build outputs (also git-ignored), never committed.
@@ -19,6 +19,7 @@ import shutil
 import subprocess
 import sys
 import sysconfig
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF = os.environ.get("GS_REFERENCE_DIR", "/root/reference")
@@ -43,25 +44,28 @@ def build(verbose: bool = False) -> str:
     # bindings.cpp includes "include/common.hpp" relative to its own directory: fine in place.
     common = ["-O3", "-std=c++17", "-DTORCH_EXTENSION_NAME=gaussian_ref",
               "-DTORCH_API_INCLUDE_EXTENSION_H", f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}"]
-    tmp = os.path.join("/tmp", "gs_ref_build")
-    os.makedirs(tmp, exist_ok=True)
-    nvcc = os.path.join(ce.CUDA_HOME, "bin", "nvcc")
-    o_cu = os.path.join(tmp, "gaussian.o")
-    o_cpp = os.path.join(tmp, "bindings.o")
-    cmds = [
-        [nvcc, "-c", srcs[0], "-o", o_cu, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
-         "--compiler-options", "-fPIC", "-w"] + common + inc,
-        ["g++", "-c", srcs[1], "-o", o_cpp, "-fPIC", "-w"] + common + inc,
-    ]
-    procs = [subprocess.Popen(c, stdout=None if verbose else subprocess.DEVNULL) for c in cmds]
-    for p, c in zip(procs, cmds):
-        if p.wait() != 0:
-            raise RuntimeError("reference build failed: " + " ".join(c))
-    libdirs = ce.library_paths("cuda")
-    link = ["g++", "-shared", o_cu, o_cpp, "-o", target] + [f"-L{d}" for d in libdirs] + \
-           [f"-Wl,-rpath,{d}" for d in libdirs] + \
-           ["-lc10", "-ltorch", "-ltorch_cpu", "-ltorch_python", "-lc10_cuda", "-ltorch_cuda", "-lcudart"]
-    subprocess.check_call(link)
+    tmp = tempfile.mkdtemp(prefix="gs_ref_build_")   # private: a shared fixed path may belong to another user
+    try:
+        nvcc = os.path.join(ce.CUDA_HOME, "bin", "nvcc")
+        o_cu = os.path.join(tmp, "gaussian.o")
+        o_cpp = os.path.join(tmp, "bindings.o")
+        cmds = [
+            [nvcc, "-c", srcs[0], "-o", o_cu, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
+             "--compiler-options", "-fPIC", "-w"] + common + inc,
+            ["g++", "-c", srcs[1], "-o", o_cpp, "-fPIC", "-w"] + common + inc,
+        ]
+        procs = [subprocess.Popen(c, stdout=None if verbose else subprocess.DEVNULL) for c in cmds]
+        codes = [p.wait() for p in procs]            # both finish before the directory is removed
+        for code, c in zip(codes, cmds):
+            if code != 0:
+                raise RuntimeError("reference build failed: " + " ".join(c))
+        libdirs = ce.library_paths("cuda")
+        link = ["g++", "-shared", o_cu, o_cpp, "-o", target] + [f"-L{d}" for d in libdirs] + \
+               [f"-Wl,-rpath,{d}" for d in libdirs] + \
+               ["-lc10", "-ltorch", "-ltorch_cpu", "-ltorch_python", "-lc10_cuda", "-ltorch_cuda", "-lcudart"]
+        subprocess.check_call(link)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
     _copy_glue()
     return target
 

@@ -13,7 +13,7 @@ vectorised as  T = exclusive-cumprod(1 - alpha)  with the early-stop mask
 
 Parity pinning: the reference ships no tests/golden vectors (SURVEY.md §4), and its
 kernels are CUDA-only, so this oracle is pinned against outputs of the reference's
-own CUDA build (oracle/_ref, built by oracle/build_ref.py) generated on a B200 by
+own CUDA build (oracle/_ref, built by oracle/build_ref.py) generated on a GPU by
 tests/golden/make_golden.py and committed under tests/golden/*.npz.
 Until those fixtures exist the status is "parity unpinned".
 """

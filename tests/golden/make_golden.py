@@ -1,7 +1,7 @@
 """Generates tests/golden/*.npz by running the REFERENCE's own CUDA build (oracle/_ref,
 built by oracle/build_ref.py from the unmodified sources) on a GPU.
 
-Run on the B200 box:   python tests/golden/make_golden.py gpurun_out/golden
+Run on a GPU:   python tests/golden/make_golden.py <output dir>
 then copy the files into tests/golden/ and commit them.  Nothing of ours (kernels or
 oracle arithmetic) produces the stored outputs; the oracle only prepares the sorted
 per-instance INPUTS of the `draw` case, which are stored alongside.
@@ -103,4 +103,4 @@ def main(out_dir):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden"))
+    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "golden_out"))

@@ -151,7 +151,7 @@ def test_round2_entry_points_validate_without_a_gpu():
     assert lib.gs_tune(b"no_such_knob", 1) == -1 and "unknown knob" in err()
     assert lib.gs_tune(None, 1) == -1
     # every documented knob is accepted (values are validated at launch time); restore the shipped defaults
-    for knob, dflt in ((b"sh_tc", 3), (b"gather", 1), (b"strict", 0), (b"bwd_ch", 32)):
+    for knob, dflt in ((b"sh_tc", -1), (b"gather", 1), (b"strict", 0), (b"bwd_ch", 32)):
         assert lib.gs_tune(knob, dflt) == 0, knob
     lib.gs_allreduce_push_finish_mc_f32.argtypes = [P, P, P, LL, LL, I, I, P]
     assert lib.gs_allreduce_push_finish_mc_f32(None, 0x1000, 0x2000, 64, 32, 0, 2, None) == -1

@@ -1,6 +1,6 @@
 """CPU tests of the oracle itself: internal consistency (analytic properties of the
 reference's algorithm) and agreement with the golden fixtures produced by the reference's
-own CUDA build on a B200 (tests/golden/make_golden.py)."""
+own CUDA build on a GPU (tests/golden/make_golden.py)."""
 import math
 
 import pytest

@@ -1,4 +1,4 @@
-"""SURVEY.md §8 f-1 / BASELINE configs[3]: the reference's own train.py (oracle/_ref/train.py, the
+"""SURVEY.md §8 f-1: the reference's own train.py (oracle/_ref/train.py, the
 byte-identical copy oracle/build_ref.py makes) runs UNCHANGED through 3d-gaussian-splatting_b200/dp_launch.py
 on a synthetic COLMAP dataset:
   * on OUR splatter.py (fused frame path, fused SSIM through shims/torchmetrics, fused flat Adam);
@@ -96,7 +96,7 @@ def test_reference_train_py_runs_unchanged(gs, cuda, tmp_path, which):
 
 def test_reference_train_py_data_parallel(gs, cuda, tmp_path):
     """2 (4, 8: GS_TEST_TRAIN_WORLD) ranks under torchrun: different views per rank, averaged gradient bucket,
-    identical replicas (BASELINE configs[3] at test size)."""
+    identical replicas (the multi-view training configuration at test size)."""
     world = int(os.environ.get("GS_TEST_TRAIN_WORLD", "2"))          # 2 (default), 4 or 8
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")

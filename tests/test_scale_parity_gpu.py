@@ -1,4 +1,4 @@
-"""Parity at BASELINE.json's FULL sizes (SURVEY.md §8c P4@C2 and P6), where tiles hold up to
+"""Parity at the benchmark's FULL sizes (SURVEY.md §8c P4@C2 and P6), where tiles hold up to
 ~2,000 instances, the staging pipeline runs 8-31 chunks per tile, whole tiles saturate and the
 epoch-tagged tails of the gradient rows are skipped:
 

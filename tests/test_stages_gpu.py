@@ -2,7 +2,7 @@
 against the CPU oracle and, when oracle/_ref is present, against the reference's own CUDA
 build on identical inputs.  Protocol P1/P2/P4 of SURVEY.md §8c.
 
-Tolerances (BASELINE.json north_star): image <= 1e-4 abs per pixel; gradients <= 1e-3
+Tolerances: image <= 1e-4 abs per pixel; gradients <= 1e-3
 relative (max |delta| / max |reference| per tensor); projection 1e-5 relative.
 """
 import pytest

@@ -396,6 +396,79 @@ struct RenderContext {
              "gs_render_backward");
   }
 
+  // depth / alpha maps and a background colour (gs_render_forward_aux): returns
+  // (final[H,W,3] or None, raw padded[Hp,Wp,3], aux padded[Hp,Wp,2], aux_final[H,W,2] or None, mask)
+  py::tuple forward_aux(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                        torch::Tensor scale, int width, int height, float fx, float fy, torch::Tensor rot,
+                        torch::Tensor tran, float near, float thresh, int scale_activation,
+                        std::optional<std::vector<double>> background, bool final) {
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    int64_t n = pos.size(0);
+    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
+                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
+                "RenderContext.forward_aux: bad shapes");
+    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
+    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_aux: background must have 3 values");
+    c10::cuda::CUDAGuard guard(pos.device());
+    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
+    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
+    auto raw = torch::empty({hp, wp, 3}, pos.options());
+    auto aux = torch::empty({hp, wp, 2}, pos.options());
+    torch::Tensor fin, aux_fin;
+    if (final) {
+      fin = torch::empty({height, width, 3}, pos.options());
+      aux_fin = torch::empty({height, width, 2}, pos.options());
+    }
+    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
+    float bg[3] = {0.f, 0.f, 0.f};
+    if (background)
+      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
+    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
+    check_rc(gs_render_forward_aux(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                   scale_activation, &cam, fpm(raw), final ? fpm(fin) : nullptr,
+                                   mask.data_ptr<int64_t>(), &ax, cur_stream()),
+             "gs_render_forward_aux");
+    ++frame;
+    py::object none = py::none();
+    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, mask);
+  }
+
+  // backward of forward_aux; grad_aux = None: the plain backward kernels (zero depth / alpha gradient)
+  void backward_aux_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                         torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_image, bool grad_is_final,
+                         torch::Tensor aux, std::optional<torch::Tensor> grad_aux, torch::Tensor g_pos,
+                         torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
+                         int64_t expected_frame) {
+    check_frame(expected_frame, "RenderContext.backward_aux_into");
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa);
+    GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale);
+    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3 && aux.dim() == 3 && aux.size(0) == raw.size(0) &&
+                    aux.size(1) == raw.size(1) && aux.size(2) == 2,
+                "RenderContext.backward_aux_into: raw must be [Hp,Wp,3] and aux [Hp,Wp,2]");
+    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
+                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
+                "RenderContext.backward_aux_into: grad_image must be [H,W,3] (final) or match raw");
+    if (grad_aux) {
+      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
+                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
+                      grad_aux->size(2) == 2,
+                  "RenderContext.backward_aux_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
+    }
+    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
+                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
+                "RenderContext.backward_aux_into: gradient buffers must match their parameters");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor ga;
+    if (grad_aux) ga = grad_aux->contiguous();
+    check_rc(gs_render_backward_aux(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
+                                    grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fpm(g_pos),
+                                    fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
+             "gs_render_backward_aux");
+  }
+
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
   py::dict stats() {
@@ -598,6 +671,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_final"),
            py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"), py::arg("g_quat"), py::arg("g_scale"),
            py::arg("expected_frame") = -1)
+      .def("forward_aux", &RenderContext::forward_aux, py::arg("pos"), py::arg("rgb"), py::arg("opa"), py::arg("quat"),
+           py::arg("scale"), py::arg("width"), py::arg("height"), py::arg("fx"), py::arg("fy"), py::arg("rot"),
+           py::arg("tran"), py::arg("near"), py::arg("thresh"), py::arg("scale_activation"),
+           py::arg("background") = py::none(), py::arg("final") = true)
+      .def("backward_aux_into", &RenderContext::backward_aux_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
+           py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
+           py::arg("g_quat"), py::arg("g_scale"), py::arg("expected_frame") = -1)
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
       .def("stats", &RenderContext::stats)

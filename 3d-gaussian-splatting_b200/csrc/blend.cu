@@ -81,6 +81,7 @@ struct StageView<true> {
     const float4 t = R[j * recw + 1];
     return make_float4(t.z, t.w, R[j * recw + 2].x, 0.f);
   }
+  __device__ __forceinline__ float depth(int j) const { return R[j * recw + 2].y; }   // |p_c|
   // gradient row of this (Gaussian, tile) instance: first row of the Gaussian + rank of the tile in its rectangle
   __device__ __forceinline__ uint32_t slot(int j, int tx, int ty) const {
     const float4 cc = R[j * recw + 2];
@@ -138,7 +139,9 @@ __device__ __forceinline__ void gather_issue(SM& sm, int stage, const GsRec* __r
 // Per (thread, instance): 3 broadcast LDS + 4 row-shared FP32 ops (dy, cb*dy, cc*dy, l2o-cc*dy^2)
 // + 4 pixels x (dx, u, exponent, MUFU.EX2, setp, mul, sel, 3 FFMA colour, T update) = 12.75
 // issue slots per (pixel, instance) instead of 17-18 with one pixel per thread.
-template <int FWD_CH, int PX, bool GATHER>
+// AUX (gather only): one more FFMA per (pixel, instance) accumulates the depth sum w t; at the end the background
+// T_f bg is added to the colour and (depth, 1 - T_f) is stored to aux / aux_final.
+template <int FWD_CH, int PX, bool GATHER, bool AUX = false>
 __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __restrict__ pA,
                                                                  const float2* __restrict__ pB,
                                                                  const float4* __restrict__ pC,
@@ -148,7 +151,9 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
                                                                  int ntx, float fx, float fy,
                                                                  float* __restrict__ image,
                                                                  int* __restrict__ tile_neff,
-                                                                 float* __restrict__ final_img, GsCrop crop) {
+                                                                 float* __restrict__ final_img, GsCrop crop,
+                                                                 GsAuxOut aux) {
+  static_assert(!AUX || GATHER, "the aux outputs read |p_c| from the gathered records");
   using Smem = typename std::conditional<GATHER, GatherRing<FWD_CH, FWD_STAGES, 3>, FwdSmem<FWD_CH>>::type;
   __shared__ __align__(16) Smem sm;
   const int tile = blockIdx.x;
@@ -185,11 +190,12 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
       issue_chunk<Smem, FWD_CH>(sm, k, pA, pB, pC, start + k * FWD_CH, min(FWD_CH, cnt - k * FWD_CH), shift);
   }
 
-  float T[FWD_PX], cr[FWD_PX], cg[FWD_PX], cb[FWD_PX];
+  float T[FWD_PX], cr[FWD_PX], cg[FWD_PX], cb[FWD_PX], dep[FWD_PX];
 #pragma unroll
   for (int p = 0; p < FWD_PX; ++p) {
     T[p] = 1.f;
     cr[p] = cg[p] = cb[p] = 0.f;
+    dep[p] = 0.f;
   }
   int consumed = cnt;
   int k = 0;
@@ -215,6 +221,8 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
     const float dy = py - a.y;                                                              \
     const float m1 = a.w * dy;                                                              \
     const float ev = fmaf(-b.x * dy, dy, b.y);                                              \
+    float t = 0.f;                                                                          \
+    if constexpr (AUX) t = sv.depth(J);                                                     \
     _Pragma("unroll") for (int p = 0; p < FWD_PX; ++p) {                                    \
       const float dx = px[p] - a.x;                                                         \
       const float eu = fmaf(a.z, dx, -m1);                                                  \
@@ -223,6 +231,7 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
       cr[p] = fmaf(c.x, w, cr[p]);                                                          \
       cg[p] = fmaf(c.y, w, cg[p]);                                                          \
       cb[p] = fmaf(c.z, w, cb[p]);                                                          \
+      if constexpr (AUX) dep[p] = fmaf(t, w, dep[p]);                                       \
       T[p] -= w;                                                                            \
     }                                                                                       \
   }
@@ -265,6 +274,33 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
   if (tid == 0 && k < nchunks) {
     for (int kk = k + 1; kk < nchunks && kk < k + FWD_STAGES; ++kk)
       gs_mbar_wait(&sm.full[kk % FWD_STAGES], (uint32_t)((kk / FWD_STAGES) & 1));
+  }
+  if constexpr (AUX) {
+#pragma unroll
+    for (int p = 0; p < FWD_PX; ++p) {
+      cr[p] = fmaf(T[p], aux.bg[0], cr[p]);
+      cg[p] = fmaf(T[p], aux.bg[1], cg[p]);
+      cb[p] = fmaf(T[p], aux.bg[2], cb[p]);
+    }
+    float ab[FWD_PX * 2];   // (depth, alpha) x PX = PX * 8 contiguous, 16-byte aligned bytes
+#pragma unroll
+    for (int p = 0; p < FWD_PX; ++p) {
+      ab[2 * p] = dep[p];
+      ab[2 * p + 1] = 1.f - T[p];
+    }
+    if (aux.aux) {
+      float4* o = reinterpret_cast<float4*>(aux.aux + ((size_t)iy * wp + ix0) * 2);
+#pragma unroll
+      for (int q = 0; q < FWD_PX / 2; ++q) o[q] = make_float4(ab[4 * q], ab[4 * q + 1], ab[4 * q + 2], ab[4 * q + 3]);
+    }
+    if (aux.aux_final) {
+#pragma unroll
+      for (int p = 0; p < FWD_PX; ++p) {
+        const int x = ix0 + p - crop.left, y = iy - crop.top;
+        if (x >= 0 && x < crop.width && y >= 0 && y < crop.height)
+          *reinterpret_cast<float2*>(aux.aux_final + ((size_t)y * crop.width + x) * 2) = make_float2(ab[2 * p], ab[2 * p + 1]);
+      }
+    }
   }
   // PX pixels x 3 channels = PX * 12 contiguous, 16-byte aligned bytes
   {
@@ -717,12 +753,27 @@ struct Bwd2Smem : std::conditional<GATHER, GatherRing<CH, STAGES, 4>, WsRing<STA
   int valid[2];
 };
 
+// AUX backward: the 7th per-(thread, instance) partial sum, d_t = sum g_D w, lives in a plane of its own,
+// [instance][part][source thread] with part stride SQ and instance stride NT + 1.  With NT == 32 (one consumer warp)
+// a warp's 4-byte stores cover the 32 banks once, and the reducers' loads (32 / RQ instances x RQ parts, all at the
+// same source) hit bank ri + (32 / RQ) rq: distinct as well.  The six other sums keep their buffer and strides.
+template <int PX, int STAGES, int RQ, bool GATHER, int CH>
+struct Bwd2SmemAux : Bwd2Smem<PX, STAGES, RQ, GATHER, CH> {
+  static constexpr int TQS = Bwd2Cfg<PX, STAGES, RQ>::SQ, TIS = Bwd2Cfg<PX, STAGES, RQ>::NT + 1;
+  static_assert(Bwd2Cfg<PX, STAGES, RQ>::NT == 32 && TQS * RQ == 32 && TIS % 32 == 1,
+                "d_t plane strides are conflict free for one consumer warp only");
+  float part_t[Bwd2Cfg<PX, STAGES, RQ>::R * TIS];
+};
+
 // one instance x this thread's row of PX pixels: recompute alpha, analytic d/d alpha, six partial sums
-template <int PX>
+// (AUX: gc and R carry the depth / alpha terms, and d_t = sum g_D w goes to *dst_t)
+template <int PX, bool AUX = false>
 __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const float4 c, const float (&px)[PX],
                                         const float py, float (&T)[PX], float (&Rr)[PX], const float (&gr)[PX],
-                                        const float (&gg)[PX], const float (&gb)[PX], float2* __restrict__ dst) {
-  float s0 = 0.f, sx = 0.f, sxx = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
+                                        const float (&gg)[PX], const float (&gb)[PX], float2* __restrict__ dst,
+                                        const float t = 0.f, const float (*gD)[PX] = nullptr,
+                                        const float (*gA)[PX] = nullptr, float* __restrict__ dst_t = nullptr) {
+  float s0 = 0.f, sx = 0.f, sxx = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, dt = 0.f;
   const float dy = py - a.y;
   const float m1 = a.w * dy;
   const float ev = fmaf(-b.x * dy, dy, b.y);
@@ -733,7 +784,8 @@ __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const fl
     float alpha = gs_ex2(fmaf(-dx, eu, ev));                     // l2o - (ca dx^2 - cb dx dy + cc dy^2)
     alpha = (T[p] > GS_T_STOP) ? alpha : 0.f;                    // early stop (:578): no weight, no gradient
     const float w = alpha * T[p];
-    const float gc = fmaf(gr[p], c.x, fmaf(gg[p], c.y, gb[p] * c.z));
+    float gc = fmaf(gr[p], c.x, fmaf(gg[p], c.y, gb[p] * c.z));
+    if constexpr (AUX) gc = fmaf((*gD)[p], t, gc + (*gA)[p]);   // + g_D t_i + g_A
     Rr[p] = fmaf(-gc, w, Rr[p]);                                 // sum_c g_c (out_c - C_c^{<=i})
     const float rc = gs_rcp(1.0000001f - alpha);                 // 1/(1 - alpha + 1e-7)  (:721)
     const float dal = fmaf(T[p], gc, -Rr[p] * rc);               // d L / d alpha            (:710-722)
@@ -746,28 +798,36 @@ __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const fl
     c0 = fmaf(gr[p], w, c0);
     c1 = fmaf(gg[p], w, c1);
     c2 = fmaf(gb[p], w, c2);
+    if constexpr (AUX) dt = fmaf((*gD)[p], w, dt);
   }
   dst[0] = make_float2(s0, sx);
   dst[1] = make_float2(sxx, c0);
   dst[2] = make_float2(c1, c2);
+  if constexpr (AUX) *dst_t = dt;
 }
 
 // WS: dedicated producer warp (full / empty mbarrier ring); !WS: consumer thread 0 issues the copies at the
 // chunk boundaries (no extra warp holding registers).  UNR: instances per unrolled step of the first phase.
-template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH>
+// AUX (gather only): the upstream gradient also has (g_D, g_A) per pixel (grad_aux, padded or cropped like
+// grad_image); gc and R gain g_D t + g_A and g_D depth + g_A alpha (depth / alpha from the forward's aux), and
+// the 7th sum d_t = sum g_D w lands in column 6 + 3 of the gradient row.
+template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false>
 __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     blend_bwd2_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB, const float4* __restrict__ pC,
                       const GsRec* __restrict__ grec, const uint32_t* __restrict__ ids,
                       const uint32_t* __restrict__ goff, const int* __restrict__ tile_accum, int wp, int hp, int ntx, float fx, float fy,
                       const float* __restrict__ image, const float* __restrict__ grad_image,
                       float* __restrict__ grad_inst, int grad_is_final, GsCrop crop, uint32_t* __restrict__ row_epoch,
-                      uint32_t epoch, int* __restrict__ tile_neff_b) {
+                      uint32_t epoch, int* __restrict__ tile_neff_b, const float* __restrict__ aux,
+                      const float* __restrict__ grad_aux) {
   using Cfg = Bwd2Cfg<PX, STAGES, RQ>;
   constexpr int NT = Cfg::NT, TPR = Cfg::TPR, R = Cfg::R, SQ = Cfg::SQ, QS = Cfg::QS, IS = Cfg::IS, ROWS = Cfg::ROWS;
   static_assert(IS % 2 == 0 && QS % 2 == 0 && IS % 32 == 2 && QS % 32 == 32 / RQ, "partial buffer strides");
   static_assert(!(WS && GATHER), "the gather path issues its copies from all consumer threads");
   static_assert(GATHER || CH == WS_CH, "the packed ring is sized for CH instances per stage");
-  using Smem = Bwd2Smem<PX, STAGES, RQ, GATHER, CH>;
+  static_assert(!AUX || GATHER, "the aux terms read |p_c| from the gathered records");
+  using Smem = typename std::conditional<AUX, Bwd2SmemAux<PX, STAGES, RQ, GATHER, CH>,
+                                         Bwd2Smem<PX, STAGES, RQ, GATHER, CH>>::type;
   __shared__ __align__(16) Smem sm;
   const int tile = blockIdx.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -843,8 +903,44 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
       T[p] = 1.f;
     }
   }
+  float gD[PX], gA[PX];
+  if constexpr (AUX) {
+    // R = sum_c g_c image_c + g_D depth + g_A alpha (forward outputs); (depth, alpha) x PX = PX * 8 aligned bytes
+    const size_t off = ((size_t)iy * wp + ix0) * 2;
+    float abuf[PX * 2], gbuf[PX * 2];
+#pragma unroll
+    for (int q = 0; q < PX / 2; ++q) {
+      const float4 v = reinterpret_cast<const float4*>(aux + off)[q];
+      abuf[4 * q] = v.x; abuf[4 * q + 1] = v.y; abuf[4 * q + 2] = v.z; abuf[4 * q + 3] = v.w;
+    }
+    if (!grad_is_final) {
+#pragma unroll
+      for (int q = 0; q < PX / 2; ++q) {
+        const float4 v = reinterpret_cast<const float4*>(grad_aux + off)[q];
+        gbuf[4 * q] = v.x; gbuf[4 * q + 1] = v.y; gbuf[4 * q + 2] = v.z; gbuf[4 * q + 3] = v.w;
+      }
+    } else {
+#pragma unroll
+      for (int p = 0; p < PX; ++p) {   // depth / alpha are not clamped: only the crop masks their gradient
+        const int x = ix0 + p - crop.left, y = iy - crop.top;
+        float2 v = make_float2(0.f, 0.f);
+        if (x >= 0 && x < crop.width && y >= 0 && y < crop.height)
+          v = *reinterpret_cast<const float2*>(grad_aux + ((size_t)y * crop.width + x) * 2);
+        gbuf[2 * p] = v.x;
+        gbuf[2 * p + 1] = v.y;
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < PX; ++p) {
+      gD[p] = gbuf[2 * p];
+      gA[p] = gbuf[2 * p + 1];
+      Rr[p] = fmaf(gD[p], abuf[2 * p], fmaf(gA[p], abuf[2 * p + 1], Rr[p]));
+    }
+  }
   // this thread's slot in the partial buffer: quarter tid / SQ, position tid % SQ
   float2* const my_part = reinterpret_cast<float2*>(sm.part + (tid / SQ) * QS + (tid % SQ) * 6);
+  float* my_part_t = nullptr;   // AUX: this thread's slot in the d_t plane
+  if constexpr (AUX) my_part_t = sm.part_t + (tid / SQ) * Smem::TQS + (tid % SQ);
   // second-phase role: instance ri of the round, quarter rq of the source threads
   const int ri = tid / RQ, rq = tid % RQ;
   const float2* const red_src = reinterpret_cast<const float2*>(sm.part + ri * IS + rq * QS);
@@ -882,13 +978,24 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
           }
         }
 #pragma unroll
-        for (int u = 0; u < UNR; ++u)
-          bwd_row<PX>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg, gb,
-                      my_part + (j + u) * (IS / 2));
+        for (int u = 0; u < UNR; ++u) {
+          if constexpr (AUX)
+            bwd_row<PX, true>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg, gb,
+                              my_part + (j + u) * (IS / 2), sv.depth(sub + j + u), &gD, &gA,
+                              my_part_t + (j + u) * Smem::TIS);
+          else
+            bwd_row<PX>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg, gb,
+                        my_part + (j + u) * (IS / 2));
+        }
       }
       if (UNR > 1 && !wdead)
-        for (; j < nr; ++j)
-          bwd_row<PX>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb, my_part + j * (IS / 2));
+        for (; j < nr; ++j) {
+          if constexpr (AUX)
+            bwd_row<PX, true>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
+                              my_part + j * (IS / 2), sv.depth(sub + j), &gD, &gA, my_part_t + j * Smem::TIS);
+          else
+            bwd_row<PX>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb, my_part + j * (IS / 2));
+        }
       bool dead = true;
 #pragma unroll
       for (int p = 0; p < PX; ++p) dead = dead && !(T[p] > GS_T_STOP);
@@ -937,11 +1044,20 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
             Syy = fmaf(dyr * dyr, u0.x, Syy);
           }
         }
+        float Dt = 0.f;
+        if constexpr (AUX) {
+          if (act && ri < vq) {
+            const float* src = sm.part_t + ri * Smem::TIS + rq * Smem::TQS;
+#pragma unroll
+            for (int s = 0; s < SQ; ++s) Dt += src[s];
+          }
+        }
 #define GS_RED4(V)                                   \
   V += __shfl_xor_sync(0xffffffffu, V, 1);           \
   V += __shfl_xor_sync(0xffffffffu, V, 2);           \
   if (RQ == 8) V += __shfl_xor_sync(0xffffffffu, V, 4);
         GS_RED4(S0) GS_RED4(Sx) GS_RED4(Sxx) GS_RED4(Sy) GS_RED4(Sxy) GS_RED4(Syy) GS_RED4(C0) GS_RED4(C1) GS_RED4(C2)
+        if constexpr (AUX) { GS_RED4(Dt) }
 #undef GS_RED4
         if (act) {
           const uint32_t slot = sv.slot(sub + ri, tx, ty);
@@ -953,7 +1069,7 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
           else if (rq == 1)
             out[1] = make_float4(-GS_LN2 * Syy, GS_LN2 * S0, C0, C1);
           else if (rq == 2)
-            out[2] = make_float4(C2, 0.f, 0.f, 0.f);
+            out[2] = make_float4(C2, Dt, 0.f, 0.f);   // | d/db, d/dt (AUX; 0 otherwise)
           else if (rq == 3 && row_epoch)
             row_epoch[slot] = epoch;               // marks the row as written in this frame
         }
@@ -1125,9 +1241,15 @@ inline size_t legacy_ws_layout(int m, int d, LegacyWs* ws, char* base) {
 
 cudaError_t gs_launch_blend_fwd(const float4* pA, const float2* pB, const float4* pC, const GsRec* grec,
                                 const uint32_t* ids, const int* tile_accum, const GsFrameGeom& g, float* image,
-                                int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st) {
+                                int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st,
+                                const GsAuxOut* aux) {
   const GsTuning& tn = gs_tuning();
   const bool gather = grec != nullptr;
+  if (aux) {   // the caller has checked gs_blend_aux_supported(true, ...); grec is null only when N == 0 (no instances)
+    blend_fwd_kernel<128, 4, true, true><<<g.n_tiles, 64, 0, st>>>(pA, pB, pC, grec, ids, tile_accum, g.wp, g.hp, g.ntx,
+                                                                  g.fx, g.fy, image, tile_neff, final_img, crop, *aux);
+    return cudaGetLastError();
+  }
   if (!gather && tn.fwd_kernel != 0) {
     blend_fwd_ws_kernel<<<g.n_tiles, WSF_CONS + 32, 0, st>>>(pA, pB, pC, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image,
                                                              tile_neff, final_img, crop);
@@ -1136,7 +1258,7 @@ cudaError_t gs_launch_blend_fwd(const float4* pA, const float2* pB, const float4
   const int ch = tn.fwd_ch;   // staging chunk
 #define GS_FWD_LAUNCH(CH, PX, GA)                                                                                   \
   blend_fwd_kernel<CH, PX, GA><<<g.n_tiles, 256 / PX, 0, st>>>(pA, pB, pC, grec, ids, tile_accum, g.wp, g.hp, g.ntx, \
-                                                               g.fx, g.fy, image, tile_neff, final_img, crop)
+                                                               g.fx, g.fy, image, tile_neff, final_img, crop, GsAuxOut{})
 #define GS_FWD_CH(PX, GA)                     \
   if (ch == 64) GS_FWD_LAUNCH(64, PX, GA);    \
   else if (ch == 256) GS_FWD_LAUNCH(256, PX, GA); \
@@ -1155,16 +1277,24 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
                                 const uint32_t* ids, const uint32_t* goff, const int* tile_accum, const GsFrameGeom& g,
                                 const float* image,
                                 const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
-                                uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st) {
+                                uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
+                                const float* aux, const float* grad_aux) {
   const GsTuning& tn = gs_tuning();
   const bool gather = grec != nullptr;
   if (gather && !row_epoch) return cudaErrorInvalidValue;
+  if (grad_aux) {   // the caller has checked gs_blend_aux_supported(..., true)
+    if (!gather || !aux) return cudaErrorInvalidValue;
+    blend_bwd2_kernel<8, false, 4, 3, 10, 4, true, 32, true><<<g.n_tiles, 32, 0, st>>>(
+        pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,
+        grad_is_final, crop, row_epoch, epoch, tile_neff_b, aux, grad_aux);
+    return cudaGetLastError();
+  }
   if (tn.bwd_kernel != 0 || gather) {
 #define GS_BWD2C(PX, WS, UNR, ST, MINB, RQ, GA, CH)                                                                 \
   blend_bwd2_kernel<PX, WS, UNR, ST, MINB, RQ, GA, CH><<<g.n_tiles, 256 / PX + (WS ? 32 : 0), 0, st>>>(              \
       pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,          \
       grad_is_final,                                                                                                 \
-      crop, row_epoch, epoch, tile_neff_b)
+      crop, row_epoch, epoch, tile_neff_b, nullptr, nullptr)
 #define GS_BWD2(PX, WS, UNR, ST, MINB, RQ, GA) GS_BWD2C(PX, WS, UNR, ST, MINB, RQ, GA, 64)
     // key: px | producer warp | unroll | stages | reducers per instance | min blocks (2 digits)
     const int key = ((((tn.bwd_px * 10 + tn.bwd_ws) * 10 + tn.bwd_unroll) * 10 + tn.bwd_stages) * 10 + tn.bwd_rq) * 100 +
@@ -1234,6 +1364,26 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
   else GS_BWD_LAUNCH(2, 64);
 #undef GS_BWD_LAUNCH
   return cudaGetLastError();
+}
+
+int gs_blend_aux_supported(int d, bool forward, bool backward) {
+  const GsTuning& tn = gs_tuning();
+  if (!tn.gather)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "depth / alpha / background: the packed path (gs_tune(\"gather\", 0)) has no aux kernel");
+  if (d != 3) {   // SH: scalar and one-pixel-per-thread tensor-core kernels both have aux variants
+    if (backward && (gs_sh_tc_mode(d) & 6) == 6)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                              "depth / alpha gradients: the two-pixel tensor-core SH backward (sh_tc bit 2) has no aux kernel");
+    return 0;
+  }
+  if (forward && (tn.fwd_kernel != 0 || tn.fwd_ch != 128 || tn.fwd_px != 4))
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "depth / alpha / background: only the shipped forward blend knobs (fwd_kernel 0, fwd_ch 128, fwd_px 4) have an aux kernel");
+  if (backward && (tn.bwd_kernel == 0 || tn.bwd_px != 8 || tn.bwd_ws != 0 || tn.bwd_unroll != 4 || tn.bwd_stages != 3 ||
+                   tn.bwd_rq != 4 || tn.bwd_minb != 10 || tn.bwd_ch != 32))
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "depth / alpha gradients: only the shipped backward blend knobs have an aux kernel");
+  return 0;
 }
 
 extern "C" size_t gs_draw_workspace_bytes(int m, int d) {

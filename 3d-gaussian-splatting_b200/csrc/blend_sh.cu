@@ -101,6 +101,7 @@ struct ShView<K, true> {
     return make_float2(t.x, t.y);
   }
   __device__ __forceinline__ const float* coef(int j) const { return S + j * sh_sw(K); }
+  __device__ __forceinline__ float depth(int j) const { return R[4 * j + 2].y; }   // |p_c|
   __device__ __forceinline__ uint32_t slot(int j, int tx, int ty) const {
     const float4 cc = R[4 * j + 2];
     const uint32_t rxy = __float_as_uint(cc.z), rwh = __float_as_uint(cc.w);
@@ -110,8 +111,9 @@ struct ShView<K, true> {
 
 // ---------------------------------------------------------------------------------------
 // forward: 64 threads per tile, a row of 4 pixels per thread
+// AUX (gather only): depth sum w t per pixel, T_f bg added, (depth, alpha) stored as in blend.cu
 // ---------------------------------------------------------------------------------------
-template <int K, bool GATHER>
+template <int K, bool GATHER, bool AUX = false>
 __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB,
                                                            const float* __restrict__ pS,
                                                            const GsRec* __restrict__ grec, const float* __restrict__ rgb,
@@ -123,8 +125,9 @@ __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restri
                                                            const float* __restrict__ vdx,
                                                            const float* __restrict__ vdy, float* __restrict__ image,
                                                            int* __restrict__ tile_neff,
-                                                           float* __restrict__ final_img, GsCrop crop) {
+                                                           float* __restrict__ final_img, GsCrop crop, GsAuxOut aux) {
   constexpr int CH = 64, STAGES = 2, PX = 4, SW = sh_sw(K), NT = 64;
+  static_assert(!AUX || GATHER, "the aux outputs read |p_c| from the gathered records");
   using SM = typename std::conditional<GATHER, ShGatherStage<K, CH, STAGES>, ShStage<K, CH, STAGES>>::type;
   __shared__ __align__(16) SM sm;
   const int tile = blockIdx.x, tid = threadIdx.x;
@@ -155,11 +158,12 @@ __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restri
       issue_sh<K>(sm, k, pA, pB, pS, start + k * CH, min(CH, cnt - k * CH), shift);
   }
 
-  float T[PX], cr[PX], cg[PX], cb[PX];
+  float T[PX], cr[PX], cg[PX], cb[PX], dep[PX];
 #pragma unroll
   for (int p = 0; p < PX; ++p) {
     T[p] = 1.f;
     cr[p] = cg[p] = cb[p] = 0.f;
+    dep[p] = 0.f;
   }
   int consumed = cnt, k = 0;
   for (; k < nchunks; ++k) {
@@ -196,6 +200,8 @@ __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restri
       const float dy = py - a.y;
       const float m1 = a.w * dy;
       const float ev = fmaf(-b.x * dy, dy, b.y);
+      float t = 0.f;
+      if constexpr (AUX) t = sv.depth(j);
 #pragma unroll
       for (int p = 0; p < PX; ++p) {
         const float dx = px[p] - a.x;
@@ -226,6 +232,7 @@ __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restri
           cr[p] = fmaf(col[0], w, cr[p]);
           cg[p] = fmaf(col[1], w, cg[p]);
           cb[p] = fmaf(col[2], w, cb[p]);
+          if constexpr (AUX) dep[p] = fmaf(t, w, dep[p]);
           T[p] -= w;
         }
       }
@@ -246,6 +253,15 @@ __global__ void __launch_bounds__(64) blend_sh_fwd_kernel(const float4* __restri
   if (tid == 0 && k < nchunks)
     for (int kk = k + 1; kk < nchunks && kk < k + STAGES; ++kk)
       gs_mbar_wait(&sm.full[kk % STAGES], (uint32_t)((kk / STAGES) & 1));
+  if constexpr (AUX) {
+#pragma unroll
+    for (int p = 0; p < PX; ++p) {
+      cr[p] = fmaf(T[p], aux.bg[0], cr[p]);
+      cg[p] = fmaf(T[p], aux.bg[1], cg[p]);
+      cb[p] = fmaf(T[p], aux.bg[2], cb[p]);
+      gs_store_aux(aux, ix0 + p, iy, wp, crop, dep[p], 1.f - T[p]);
+    }
+  }
   float4* o = reinterpret_cast<float4*>(image + ((size_t)iy * wp + ix0) * 3);
   o[0] = make_float4(cr[0], cg[0], cb[0], cr[1]);
   o[1] = make_float4(cg[1], cb[1], cr[2], cg[2]);
@@ -268,7 +284,9 @@ struct ShBwdSmem {
   float partial[2][32 * sh_nvp(K)];
 };
 
-template <int K, bool GATHER>
+// AUX (gather only): gc += g_D t + g_A, R += g_D depth + g_A alpha, and d_t = sum g_D w is reduced in value slot NV
+// (the first pad value of the NVP-wide partial row) into column 6 + 3K of the gradient row.
+template <int K, bool GATHER, bool AUX = false>
 __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB,
                                                            const float* __restrict__ pS,
                                                            const GsRec* __restrict__ grec, const float* __restrict__ rgb,
@@ -283,9 +301,12 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
                                                            const float* __restrict__ grad_image,
                                                            float* __restrict__ grad_inst, int grad_is_final,
                                                            GsCrop crop, uint32_t* __restrict__ row_epoch,
-                                                           uint32_t epoch, int* __restrict__ tile_neff_b) {
+                                                           uint32_t epoch, int* __restrict__ tile_neff_b,
+                                                           const float* __restrict__ aux,
+                                                           const float* __restrict__ grad_aux) {
   constexpr int CH = 32, STAGES = 2, PX = 4, SW = sh_sw(K), NV = sh_nv(K), NVP = sh_nvp(K), THREADS = 64;
   constexpr int GREC = (NV + 3) / 4 * 4;
+  static_assert(!AUX || (GATHER && NV < NVP && NV < GREC), "d_t needs a pad slot in the partial and gradient rows");
   __shared__ __align__(16) ShBwdSmem<K, GATHER> smem;
   auto& sm = smem.st;
   const int tile = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -329,6 +350,8 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
 #pragma unroll
     for (int p = 0; p < PX; ++p) T[p] = 1.f;
   }
+  float gD[PX], gA[PX];
+  if constexpr (AUX) gs_load_aux_grad<PX>(aux, grad_aux, grad_is_final, ix0, iy, wp, crop, gD, gA, R);
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) gs_mbar_init(&sm.full[s], GATHER ? THREADS : 1);
     gs_fence_barrier_init();
@@ -383,6 +406,8 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
       const float dy = py - a.y;
       const float m1 = a.w * dy;
       const float ev = fmaf(-b.x * dy, dy, b.y);
+      float t = 0.f;
+      if constexpr (AUX) t = sv.depth(j);
 #pragma unroll
       for (int p = 0; p < PX; ++p) {
         const float dx = px[p] - a.x;
@@ -398,7 +423,8 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
             for (int q = 0; q < K; ++q) t = fmaf(sh[p][q], cf[c * K + q], t);
             col[c] = sh_sigmoid(t);
           }
-          const float gc = fmaf(gr[p], col[0], fmaf(gg[p], col[1], gb[p] * col[2]));
+          float gc = fmaf(gr[p], col[0], fmaf(gg[p], col[1], gb[p] * col[2]));
+          if constexpr (AUX) gc = fmaf(gD[p], t, gc + gA[p]);
           R[p] = fmaf(-gc, w, R[p]);
           const float rc = gs_rcp(1.0000001f - alpha);
           const float dal = fmaf(T[p], gc, -R[p] * rc);
@@ -408,6 +434,7 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
           s0 += e;
           sx += ex;
           sxx = fmaf(ex, dx, sxx);
+          if constexpr (AUX) acc[NV] = fmaf(gD[p], w, acc[NV]);
           // d colour_c / d coef[c*K+q] = sigma'(.) * SH_q      (gaussian.cu:666-674)
           const float d0 = gr[p] * w * col[0] * (1.f - col[0]);
           const float d1 = gg[p] * w * col[1] * (1.f - col[1]);
@@ -451,6 +478,7 @@ __global__ void __launch_bounds__(64) blend_sh_bwd_kernel(const float4* __restri
       out[4] = -GS_LN2 * s[4];
       out[5] = GS_LN2 * s[5];
       for (int u = 6; u < NV; ++u) out[u] = p0[u] + p1[u];
+      if constexpr (AUX) out[NV] = p0[NV] + p1[NV];   // d/dt, column 6 + 3K
       if (row_epoch) row_epoch[slot] = epoch;
     }
     const bool dead = !(T[0] > GS_T_STOP) && !(T[1] > GS_T_STOP) && !(T[2] > GS_T_STOP) && !(T[3] > GS_T_STOP);
@@ -494,19 +522,24 @@ cudaError_t gs_launch_blend_sh_fwd(const float4* pA, const float2* pB, const flo
                                    const float* rgb, const uint32_t* ids, const uint32_t* goff, int d,
                                    const int* tile_accum,
                                    const GsFrameGeom& g, const GsRayPtrs& r, float* image, int* tile_neff,
-                                   float* final_img, const GsCrop& crop, cudaStream_t st) {
-#define GS_SHF(K, GA)                                                                                               \
-  blend_sh_fwd_kernel<K, GA><<<g.n_tiles, 64, 0, st>>>(pA, pB, pS, grec, rgb, ids, goff, tile_accum, g.wp, g.hp, g.ntx,   \
-                                                       g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image, tile_neff, \
-                                                       final_img, crop)
-  if (grec && (gs_sh_tc_mode(d) & 1))
-    return gs_launch_blend_sh_fwd_tc(grec, rgb, ids, d, tile_accum, g, r, image, tile_neff, final_img, crop, st);
-  if (grec) {
+                                   float* final_img, const GsCrop& crop, cudaStream_t st, const GsAuxOut* aux) {
+#define GS_SHF_A(K, GA, AX, AV)                                                                                     \
+  blend_sh_fwd_kernel<K, GA, AX><<<g.n_tiles, 64, 0, st>>>(pA, pB, pS, grec, rgb, ids, goff, tile_accum, g.wp, g.hp,   \
+                                                           g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image,  \
+                                                           tile_neff, final_img, crop, AV)
+#define GS_SHF(K, GA) GS_SHF_A(K, GA, false, GsAuxOut{})
+  // aux: the gather instantiations also serve a frame without instances (grec == nullptr when N == 0)
+  if ((grec || aux) && (gs_sh_tc_mode(d) & 1))
+    return gs_launch_blend_sh_fwd_tc(grec, rgb, ids, d, tile_accum, g, r, image, tile_neff, final_img, crop, st, aux);
+  if (aux) {
+    if (d == 27) GS_SHF_A(9, true, true, *aux); else GS_SHF_A(16, true, true, *aux);
+  } else if (grec) {
     if (d == 27) GS_SHF(9, true); else GS_SHF(16, true);
   } else {
     if (d == 27) GS_SHF(9, false); else GS_SHF(16, false);
   }
 #undef GS_SHF
+#undef GS_SHF_A
   return cudaGetLastError();
 }
 
@@ -515,20 +548,27 @@ cudaError_t gs_launch_blend_sh_bwd(const float4* pA, const float2* pB, const flo
                                    const int* tile_accum,
                                    const GsFrameGeom& g, const GsRayPtrs& r, const float* image,
                                    const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
-                                   uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st) {
+                                   uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
+                                   const float* aux, const float* grad_aux) {
   if (grec && !row_epoch) return cudaErrorInvalidValue;
+  if (grad_aux && (!grec || !aux)) return cudaErrorInvalidValue;
   if (grec && (gs_sh_tc_mode(d) & 2))
     return gs_launch_blend_sh_bwd_tc(grec, rgb, ids, goff, d, tile_accum, g, r, image, grad_image, grad_inst, grad_is_final,
-                                     crop, row_epoch, epoch, tile_neff_b, st);
-#define GS_SHB(K, GA)                                                                                               \
-  blend_sh_bwd_kernel<K, GA><<<g.n_tiles, 64, 0, st>>>(pA, pB, pS, grec, rgb, ids, goff, tile_accum, g.wp, g.hp, g.ntx,   \
-                                                       g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image, grad_image, \
-                                                       grad_inst, grad_is_final, crop, row_epoch, epoch, tile_neff_b)
-  if (grec) {
+                                     crop, row_epoch, epoch, tile_neff_b, st, aux, grad_aux);
+#define GS_SHB_A(K, GA, AX)                                                                                         \
+  blend_sh_bwd_kernel<K, GA, AX><<<g.n_tiles, 64, 0, st>>>(pA, pB, pS, grec, rgb, ids, goff, tile_accum, g.wp, g.hp,   \
+                                                           g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image,  \
+                                                           grad_image, grad_inst, grad_is_final, crop, row_epoch,      \
+                                                           epoch, tile_neff_b, aux, grad_aux)
+#define GS_SHB(K, GA) GS_SHB_A(K, GA, false)
+  if (grad_aux) {
+    if (d == 27) GS_SHB_A(9, true, true); else GS_SHB_A(16, true, true);
+  } else if (grec) {
     if (d == 27) GS_SHB(9, true); else GS_SHB(16, true);
   } else {
     if (d == 27) GS_SHB(9, false); else GS_SHB(16, false);
   }
 #undef GS_SHB
+#undef GS_SHB_A
   return cudaGetLastError();
 }

@@ -205,7 +205,8 @@ struct TcFwdSmem {
   TcStage<K, 4> st;
 };
 
-template <int K>
+// AUX: depth sum w t per pixel, T_f bg added, (depth, alpha) stored (gs_store_aux)
+template <int K, bool AUX = false>
 __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __restrict__ grec, const float* __restrict__ rgb,
                                                                 const uint32_t* __restrict__ ids,
                                                                 const int* __restrict__ tile_accum, int wp, int hp, int ntx,
@@ -213,7 +214,8 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
                                                                 const float* __restrict__ lefttop,
                                                                 const float* __restrict__ vdx, const float* __restrict__ vdy,
                                                                 float* __restrict__ image, int* __restrict__ tile_neff,
-                                                                float* __restrict__ final_img, GsCrop crop) {
+                                                                float* __restrict__ final_img, GsCrop crop,
+                                                                GsAuxOut aux) {
   constexpr int STAGES = 4;
   extern __shared__ __align__(128) uint8_t tc_smem_raw[];
   TcFwdSmem<K>& sm = *reinterpret_cast<TcFwdSmem<K>*>(tc_smem_raw);
@@ -222,7 +224,7 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
   const int ix = tx * GS_TILE + (tid & 15), iy = ty * GS_TILE + (tid >> 4);
   const int start = tile_accum[tile];
   const int cnt = tile_accum[tile + 1] - start;
-  float T = 1.f, cr = 0.f, cg = 0.f, cb = 0.f;
+  float T = 1.f, cr = 0.f, cg = 0.f, cb = 0.f, dep = 0.f;
   int consumed = cnt;
   if (cnt > 0) {                                              // uniform over the CTA
     const int nchunks = (cnt + TC_J - 1) / TC_J;
@@ -273,7 +275,7 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
         tc_read_logits(sm.lgs, row, lr, lg, lb);
         const float4* Rh = R + 32 * h;
         // one (pixel, instance) pair; a saturated pixel blends nothing (w = 0), without a divergent branch
-        auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2) {
+        auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2, float t) {
           const float dx = px - a.x, dy = py - a.y;
           const float eu = fmaf(a.z, dx, -a.w * dy);
           const float ev = fmaf(-b4.x * dy, dy, b4.y);
@@ -284,19 +286,27 @@ __global__ void __launch_bounds__(TC_NT) blend_sh_fwd_tc_kernel(const GsRec* __r
           cr = fmaf(col[0], w, cr);
           cg = fmaf(col[1], w, cg);
           cb = fmaf(col[2], w, cb);
+          if constexpr (AUX) dep = fmaf(t, w, dep);
           T -= w;
         };
         if (h * 8 + 8 <= n) {
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj]);
+          for (int jj = 0; jj < 8; ++jj)
+            pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], AUX ? Rh[4 * jj + 2].y : 0.f);
         } else {
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj)
-            if (h * 8 + jj < n) pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj]);
+            if (h * 8 + jj < n) pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], AUX ? Rh[4 * jj + 2].y : 0.f);
         }
       }
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
+  }
+  if constexpr (AUX) {
+    cr = fmaf(T, aux.bg[0], cr);
+    cg = fmaf(T, aux.bg[1], cg);
+    cb = fmaf(T, aux.bg[2], cb);
+    gs_store_aux(aux, ix, iy, wp, crop, dep, 1.f - T);
   }
   float* o = image + ((size_t)iy * wp + ix) * 3;
   o[0] = cr;
@@ -404,7 +414,8 @@ __device__ __forceinline__ void tc_coef_rows(int np, const float4* Rp, const flo
 }
 
 // geometry row of instance j of a round from the per-warp partial sums (NW warps)
-template <int NW, int GREC>
+// DT: value 6 of the partial sums is d_t = sum g_D w (AUX backward), written to column DT (= 6 + 3K)
+template <int NW, int GREC, int DT = 0>
 __device__ __forceinline__ void tc_geom_row(int j, const float (*part)[TC_J][8], const float4* Rr, int tx, int ty,
                                             float* __restrict__ grad_inst, uint32_t* __restrict__ row_epoch,
                                             uint32_t epoch) {
@@ -429,6 +440,13 @@ __device__ __forceinline__ void tc_geom_row(int j, const float (*part)[TC_J][8],
   out[3] = GS_LN2 * s[3];
   out[4] = -GS_LN2 * s[4];
   out[5] = GS_LN2 * s[5];
+  if constexpr (DT > 0) {
+    static_assert(DT < GREC, "d_t needs a pad column");
+    float t = 0.f;
+#pragma unroll
+    for (int w8 = 0; w8 < NW; ++w8) t += part[w8][j][6];
+    out[DT] = t;
+  }
   row_epoch[slot] = epoch;
 }
 
@@ -447,7 +465,9 @@ __device__ __forceinline__ void tc_geom_row(int j, const float (*part)[TC_J][8],
 //   sm.part                         written between B1(k) and B2(k); read by the geometry rows before B1(k + 1)
 //   sm.epi                          written after contraction(k), before B1(k + 1); read between B1(k + 1) and B2(k + 1)
 
-template <int K>
+// AUX: gc += g_D t + g_A, R += g_D depth + g_A alpha, and v[6] = g_D w is reduced with the geometry values into
+// column 6 + 3K of the gradient row
+template <int K, bool AUX = false>
 __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* __restrict__ grec, const float* __restrict__ rgb,
                                                                 const uint32_t* __restrict__ ids,
                                                                 const uint32_t* __restrict__ goff,
@@ -459,7 +479,8 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
                                                                 const float* __restrict__ grad_image,
                                                                 float* __restrict__ grad_inst, int grad_is_final, GsCrop crop,
                                                                 uint32_t* __restrict__ row_epoch, uint32_t epoch,
-                                                                int* __restrict__ tile_neff_b) {
+                                                                int* __restrict__ tile_neff_b, const float* __restrict__ aux,
+                                                                const float* __restrict__ grad_aux) {
   constexpr int STAGES = 3, NV = sh_nv(K), GREC = (NV + 3) / 4 * 4;
   static_assert(offsetof(TcBwdSmem<K>, img_hi) == 12 * 256 * 16 && offsetof(TcBwdSmem<K>, img_lo) == 14 * 256 * 16,
                 "the basis image must follow the gradient operand: descriptors address both as one region");
@@ -498,14 +519,22 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
     }
     R = gr * raw[0] + gg * raw[1] + gb * raw[2];
   }
+  float gD = 0.f, gA = 0.f;
+  if constexpr (AUX) {
+    float gd1[1], ga1[1], r1[1] = {R};
+    gs_load_aux_grad<1>(aux, grad_aux, grad_is_final, ix, iy, wp, crop, gd1, ga1, r1);
+    gD = gd1[0];
+    gA = ga1[0];
+    R = r1[0];
+  }
   __syncthreads();
   const int row = tc_row(tid);
   const float px = gs_pixel_coord(ix, wp, fx), py = gs_pixel_coord(iy, hp, fy);
   for (int k = 0; k < STAGES - 1 && k < nchunks; ++k)
     tc_gather<K, STAGES, true>(sm.st, k, grec, rgb, ids, goff, start + k * TC_J, min(TC_J, cnt - k * TC_J), tid);
 
-  // one (pixel, instance) pair: blend state update, logit gradients dc[3], geometry values v[0..5]
-  auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2, float* dc, float* v) {
+  // one (pixel, instance) pair: blend state update, logit gradients dc[3], geometry values v[0..5] (+ v[6] = g_D w)
+  auto pair = [&](const float4 a, const float4 b4, float l0, float l1, float l2, float* dc, float* v, float t) {
     const float dx = px - a.x, dy = py - a.y;
     const float eu = fmaf(a.z, dx, -a.w * dy);
     const float ev = fmaf(-b4.x * dy, dy, b4.y);
@@ -514,7 +543,8 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
     const float w = live ? alpha * T : 0.f;
     float col[3];
     tc_colours(l0, l1, l2, col);
-    const float gc = fmaf(gr, col[0], fmaf(gg, col[1], gb * col[2]));
+    float gc = fmaf(gr, col[0], fmaf(gg, col[1], gb * col[2]));
+    if constexpr (AUX) gc = fmaf(gD, t, gc + gA);
     R = fmaf(-gc, w, R);
     const float rc = gs_rcp(1.0000001f - alpha);
     const float dal = fmaf(T, gc, -R * rc);
@@ -527,7 +557,7 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
     v[3] = ex * dy;
     v[4] = ey * dy;
     v[5] = e;
-    v[6] = 0.f;
+    v[6] = AUX ? gD * w : 0.f;
     v[7] = 0.f;
     // d colour_c / d logit_c = sigma'(.)      (gaussian.cu:666-674)
     dc[0] = gr * w * col[0] * (1.f - col[0]);
@@ -566,7 +596,7 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
             for (int u = 0; u < 2; ++u) {
               const int jj = 2 * jp + u;
               float v[8];
-              pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], dc[u], v);
+              pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], dc[u], v, AUX ? Rh[4 * jj + 2].y : 0.f);
               const float r = reduce8(v, lane);
               if ((lane & 3) == 0) ph[jj * 8] = r;
             }
@@ -583,7 +613,7 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
               dc[u][0] = dc[u][1] = dc[u][2] = 0.f;
               if (h * 8 + jj < n) {
                 float v[8];
-                pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], dc[u], v);
+                pair(Rh[4 * jj], Rh[4 * jj + 1], lr[jj], lg[jj], lb[jj], dc[u], v, AUX ? Rh[4 * jj + 2].y : 0.f);
                 const float r = reduce8(v, lane);
                 if ((lane & 3) == 0) ph[jj * 8] = r;
               }
@@ -613,7 +643,7 @@ __global__ void __launch_bounds__(TC_NT, 2) blend_sh_bwd_tc_kernel(const GsRec* 
     tc_contract_issue<1>(wg, sm.dct, sm.img_hi, acc);
     // geometry rows (while the tensor core contracts): threads 128 .. 143, one instance each
     if (tid >= 128 && tid < 128 + n)
-      tc_geom_row<8, GREC>(tid - 128, sm.part, Rr, tx, ty, grad_inst, row_epoch, epoch);
+      tc_geom_row<8, GREC, AUX ? NV : 0>(tid - 128, sm.part, Rr, tx, ty, grad_inst, row_epoch, epoch);
     n_prev = n;
     st_prev = stage;
     // stage (k + 2) % 3 held round k - 1, whose records were last read before this round's B2
@@ -835,18 +865,23 @@ __global__ void __launch_bounds__(128) blend_sh_bwd_tc2_kernel(const GsRec* __re
 
 cudaError_t gs_launch_blend_sh_fwd_tc(const GsRec* grec, const float* rgb, const uint32_t* ids, int d,
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, float* image,
-                                      int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st) {
-#define GS_SHF_TC(K)                                                                                                  \
+                                      int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st,
+                                      const GsAuxOut* aux) {
+#define GS_SHF_TC(K, AX)                                                                                              \
   do {                                                                                                                \
     /* per device and cheap: set on every launch rather than cached in a process-wide flag */                        \
-    cudaError_t e = cudaFuncSetAttribute(blend_sh_fwd_tc_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
+    cudaError_t e = cudaFuncSetAttribute(blend_sh_fwd_tc_kernel<K, AX>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
                                          (int)sizeof(TcFwdSmem<K>));                                                  \
     if (e != cudaSuccess) return e;                                                                                   \
-    blend_sh_fwd_tc_kernel<K><<<g.n_tiles, TC_NT, sizeof(TcFwdSmem<K>), st>>>(                                         \
+    blend_sh_fwd_tc_kernel<K, AX><<<g.n_tiles, TC_NT, sizeof(TcFwdSmem<K>), st>>>(                                     \
         grec, rgb, ids, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image, tile_neff,  \
-        final_img, crop);                                                                                             \
+        final_img, crop, aux ? *aux : GsAuxOut{});                                                                    \
   } while (0)
-  if (d == 27) GS_SHF_TC(9); else GS_SHF_TC(16);
+  if (aux) {
+    if (d == 27) GS_SHF_TC(9, true); else GS_SHF_TC(16, true);
+  } else {
+    if (d == 27) GS_SHF_TC(9, false); else GS_SHF_TC(16, false);
+  }
 #undef GS_SHF_TC
   return cudaGetLastError();
 }
@@ -854,9 +889,25 @@ cudaError_t gs_launch_blend_sh_fwd_tc(const GsRec* grec, const float* rgb, const
 cudaError_t gs_launch_blend_sh_bwd_tc(const GsRec* grec, const float* rgb, const uint32_t* ids, const uint32_t* goff, int d,
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, const float* image,
                                       const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
-                                      uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st) {
+                                      uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
+                                      const float* aux, const float* grad_aux) {
   if (!row_epoch) return cudaErrorInvalidValue;   // unprocessed rows are left stale: the consumer needs the epoch tags
   const bool two_px = (gs_sh_tc_mode(d) & 4) != 0;   // two pixels per thread (128 threads per tile)
+  if (grad_aux) {                                    // the two-pixel kernel has no aux variant (checked by the caller)
+    if (two_px || !aux) return cudaErrorInvalidValue;
+#define GS_SHB_TC_AUX(K)                                                                                              \
+  do {                                                                                                                \
+    cudaError_t e = cudaFuncSetAttribute(blend_sh_bwd_tc_kernel<K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                         (int)sizeof(TcBwdSmem<K>));                                                  \
+    if (e != cudaSuccess) return e;                                                                                   \
+    blend_sh_bwd_tc_kernel<K, true><<<g.n_tiles, TC_NT, sizeof(TcBwdSmem<K>), st>>>(                                   \
+        grec, rgb, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image,       \
+        grad_image, grad_inst, grad_is_final, crop, row_epoch, epoch, tile_neff_b, aux, grad_aux);                    \
+  } while (0)
+    if (d == 27) GS_SHB_TC_AUX(9); else GS_SHB_TC_AUX(16);
+#undef GS_SHB_TC_AUX
+    return cudaGetLastError();
+  }
 #define GS_SHB_TC(K)                                                                                                  \
   do {                                                                                                                \
     cudaError_t e = two_px ? cudaFuncSetAttribute(blend_sh_bwd_tc2_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
@@ -871,7 +922,7 @@ cudaError_t gs_launch_blend_sh_bwd_tc(const GsRec* grec, const float* rgb, const
     else                                                                                                              \
       blend_sh_bwd_tc_kernel<K><<<g.n_tiles, TC_NT, sizeof(TcBwdSmem<K>), st>>>(                                        \
           grec, rgb, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, r.rays_o, r.lefttop, r.dx, r.dy, image,     \
-          grad_image, grad_inst, grad_is_final, crop, row_epoch, epoch, tile_neff_b);                                 \
+          grad_image, grad_inst, grad_is_final, crop, row_epoch, epoch, tile_neff_b, nullptr, nullptr);               \
   } while (0)
   if (d == 27) GS_SHB_TC(9); else GS_SHB_TC(16);
 #undef GS_SHB_TC

@@ -22,6 +22,49 @@ struct GsCrop {
   int left, top, width, height;
 };
 
+// Optional per-pixel outputs of the gather blend kernels (gs_render_forward_aux): the image gets T_f * bg added, and
+// aux[Hp,Wp,2] / aux_final[height,width,2] (either nullable) receive (depth = sum w t, alpha = 1 - T_f) per pixel,
+// t = |p_c| (GsRec c.y).  Only read by the AUX instantiations of the blend forward kernels.
+struct GsAuxOut {
+  float bg[3];
+  float* aux;
+  float* aux_final;
+};
+
+#ifdef __CUDACC__
+// (depth, alpha) of padded pixel (ix, iy) to aux[Hp,Wp,2] and, inside the crop, to aux_final[height,width,2]
+__device__ __forceinline__ void gs_store_aux(const GsAuxOut& ax, int ix, int iy, int wp, const GsCrop& crop,
+                                             float depth, float alpha) {
+  if (ax.aux) *reinterpret_cast<float2*>(ax.aux + ((size_t)iy * wp + ix) * 2) = make_float2(depth, alpha);
+  const int x = ix - crop.left, y = iy - crop.top;
+  if (ax.aux_final && x >= 0 && x < crop.width && y >= 0 && y < crop.height)
+    *reinterpret_cast<float2*>(ax.aux_final + ((size_t)y * crop.width + x) * 2) = make_float2(depth, alpha);
+}
+// (g_D, g_A) of PX pixels ix0 .. ix0 + PX - 1 of row iy (padded grad_aux, or the cropped one when grad_is_final:
+// depth / alpha are not clamped, only the crop masks their gradient); R += g_D depth + g_A alpha (forward's aux)
+template <int PX>
+__device__ __forceinline__ void gs_load_aux_grad(const float* __restrict__ aux, const float* __restrict__ grad_aux,
+                                                 int grad_is_final, int ix0, int iy, int wp, const GsCrop& crop,
+                                                 float (&gD)[PX], float (&gA)[PX], float (&R)[PX]) {
+#pragma unroll
+  for (int p = 0; p < PX; ++p) {
+    const size_t off = ((size_t)iy * wp + ix0 + p) * 2;
+    const float2 da = *reinterpret_cast<const float2*>(aux + off);
+    float2 g = make_float2(0.f, 0.f);
+    if (!grad_is_final) {
+      g = *reinterpret_cast<const float2*>(grad_aux + off);
+    } else {
+      const int x = ix0 + p - crop.left, y = iy - crop.top;
+      if (x >= 0 && x < crop.width && y >= 0 && y < crop.height)
+        g = *reinterpret_cast<const float2*>(grad_aux + ((size_t)y * crop.width + x) * 2);
+    }
+    gD[p] = g.x;
+    gA[p] = g.y;
+    R[p] = fmaf(g.x, da.x, fmaf(g.y, da.y, R[p]));
+  }
+}
+#endif
+
 // world-space ray setup for per-pixel SH (reference splatter.py:305-321), DEVICE pointers to 3 floats each
 struct GsRayPtrs {
   const float *rays_o, *lefttop, *dx, *dy;
@@ -61,22 +104,26 @@ cudaError_t gs_launch_blend_sh_fwd(const float4* pA, const float2* pB, const flo
                                    const float* rgb, const uint32_t* ids, const uint32_t* goff /*offsets_g*/, int d,
                                    const int* tile_accum,
                                    const GsFrameGeom& g, const GsRayPtrs& r, float* image, int* tile_neff,
-                                   float* final_img, const GsCrop& crop, cudaStream_t st);
+                                   float* final_img, const GsCrop& crop, cudaStream_t st,
+                                   const GsAuxOut* aux = nullptr /*non-null: AUX kernel (gather)*/);
 cudaError_t gs_launch_blend_sh_bwd(const float4* pA, const float2* pB, const float* pS, const GsRec* grec,
                                    const float* rgb, const uint32_t* ids, const uint32_t* goff /*offsets_g*/, int d,
                                    const int* tile_accum,
                                    const GsFrameGeom& g, const GsRayPtrs& r, const float* image,
                                    const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
-                                   uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st);
+                                   uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
+                                   const float* aux = nullptr, const float* grad_aux = nullptr /*non-null: AUX*/);
 
 // ---- blend_sh_tc.cu (wgmma) ---------------------------------------------------------------
 cudaError_t gs_launch_blend_sh_fwd_tc(const GsRec* grec, const float* rgb, const uint32_t* ids, int d,
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, float* image,
-                                      int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st);
+                                      int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st,
+                                      const GsAuxOut* aux = nullptr);
 cudaError_t gs_launch_blend_sh_bwd_tc(const GsRec* grec, const float* rgb, const uint32_t* ids, const uint32_t* goff, int d,
                                       const int* tile_accum, const GsFrameGeom& g, const GsRayPtrs& r, const float* image,
                                       const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
-                                      uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st);
+                                      uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
+                                      const float* aux = nullptr, const float* grad_aux = nullptr);
 
 // ---- project.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const float* opa, const float* quat,
@@ -98,7 +145,8 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         float near_plane, float half_w, float half_h, const uint32_t* offsets_g,
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
-                                        float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st);
+                                        float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
+                                        bool depth_grad = false /*rows carry dL/d|p_c| in column 6 + d*/);
 
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
@@ -120,7 +168,8 @@ cudaError_t gs_launch_iota(uint32_t* out, int n, cudaStream_t st);
 // stream pointers are ignored); else the packed streams written by the pack pass / the legacy draw API.
 cudaError_t gs_launch_blend_fwd(const float4* pA, const float2* pB, const float4* pC, const GsRec* grec,
                                 const uint32_t* ids, const int* tile_accum, const GsFrameGeom& g, float* image,
-                                int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st);
+                                int* tile_neff, float* final_img, const GsCrop& crop, cudaStream_t st,
+                                const GsAuxOut* aux = nullptr /*non-null: AUX kernel (gather path, shipped knobs)*/);
 
 cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4* pC, const GsRec* grec,
                                 const uint32_t* ids, const uint32_t* goff /*offsets_g (gather path)*/,
@@ -128,4 +177,9 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
                                 const float* grad_image, float* grad_inst /*[M,GS_GREC] rows addressed by slot*/,
                                 int grad_is_final, const GsCrop& crop, uint32_t* row_epoch /*nullable (packed only)*/,
                                 uint32_t epoch, int* tile_neff_b /*nullable: instances the backward consumed per tile*/,
-                                cudaStream_t st);
+                                cudaStream_t st, const float* aux = nullptr /*forward's [Hp,Wp,2]*/,
+                                const float* grad_aux = nullptr /*non-null: AUX kernel; [Hp,Wp,2] or [h,w,2]*/);
+// The AUX blend kernels exist only for the shipped configurations of the gather path (RGB: the default blend knobs;
+// SH: the scalar and one-pixel-per-thread tensor-core kernels): 0 when the current tuning knobs for colour width d
+// select one, else GS_ERR_UNSUPPORTED with a message.
+int gs_blend_aux_supported(int d, bool forward, bool backward);

@@ -140,7 +140,9 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
   }
 }
 
-template <int D, int GW, int W>
+// DT: the blend backward stored dL/d|p_c| in the row's pad column 6 + D (aux depth gradient); it enters as g_xyd[2]
+// and reaches pos through p_c / |p_c|.  Without it depth is only a sort key.
+template <int D, int GW, int W, bool DT = false>
 __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
@@ -200,7 +202,8 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     gcov[1] = acc[3] * sc + gsc * kk * o.c;                   // d det/db = -c
     gcov[2] = acc[3] * sc + gsc * kk * o.b;                   // d det/dc = -b
     gcov[3] = acc[2] * sc - gsc * kk * o.a;                   // d det/dd =  a
-    float gxyd[3] = {acc[0], acc[1], 0.f};                    // depth is only a sort key
+    static_assert(!DT || 6 + D < GW, "no pad column for the depth gradient");
+    float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + D] : 0.f};   // without DT depth is only a sort key
     float gq[4], gsv[3];
     gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
     // quat normalisation backward: q = r/|r|
@@ -436,24 +439,28 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         float near_plane, float half_w, float half_h, const uint32_t* offsets_g,
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
-                                        float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st) {
+                                        float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
+                                        bool depth_grad) {
   if (n == 0) return cudaSuccess;
-#define GS_LAUNCH_PBWD(D, GW, W)                                                                                    \
-  fused_project_bwd_kernel<D, GW, W><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, \
-                                                                     near_plane, half_w, half_h, offsets_g, count, \
-                                                                     grad_inst, row_epoch, epoch, g_pos, g_rgb,    \
-                                                                     g_opa, g_quat, g_scale, push)
-#define GS_LAUNCH_PBWD_W(D, GW)                  \
-  switch (push.world) {                          \
-    case 0: GS_LAUNCH_PBWD(D, GW, 0); break;     \
-    case 2: GS_LAUNCH_PBWD(D, GW, 2); break;     \
-    case 4: GS_LAUNCH_PBWD(D, GW, 4); break;     \
-    case 8: GS_LAUNCH_PBWD(D, GW, 8); break;     \
-    default: return cudaErrorInvalidValue;       \
+#define GS_LAUNCH_PBWD(D, GW, W, DT)                                                                                 \
+  fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act,   \
+                                                                         cam, near_plane, half_w, half_h, offsets_g, \
+                                                                         count, grad_inst, row_epoch, epoch, g_pos,  \
+                                                                         g_rgb, g_opa, g_quat, g_scale, push)
+#define GS_LAUNCH_PBWD_W(D, GW, DT)                  \
+  switch (push.world) {                              \
+    case 0: GS_LAUNCH_PBWD(D, GW, 0, DT); break;     \
+    case 2: GS_LAUNCH_PBWD(D, GW, 2, DT); break;     \
+    case 4: GS_LAUNCH_PBWD(D, GW, 4, DT); break;     \
+    case 8: GS_LAUNCH_PBWD(D, GW, 8, DT); break;     \
+    default: return cudaErrorInvalidValue;           \
   }
-  if (d == 3) { GS_LAUNCH_PBWD_W(3, GS_GREC) }
-  else if (d == 27) { GS_LAUNCH_PBWD_W(27, 36) }
-  else { GS_LAUNCH_PBWD_W(48, 56) }
+  if (d == 3 && depth_grad) { GS_LAUNCH_PBWD_W(3, GS_GREC, true) }
+  else if (d == 3) { GS_LAUNCH_PBWD_W(3, GS_GREC, false) }
+  else if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_W(27, 36, true) }
+  else if (d == 27) { GS_LAUNCH_PBWD_W(27, 36, false) }
+  else if (depth_grad) { GS_LAUNCH_PBWD_W(48, 56, true) }
+  else { GS_LAUNCH_PBWD_W(48, 56, false) }
 #undef GS_LAUNCH_PBWD_W
 #undef GS_LAUNCH_PBWD
   return cudaGetLastError();

@@ -142,6 +142,7 @@ struct gs_ctx {
   cudaEvent_t ev_m = nullptr;             // marks the completion of the M read-back
   // state of the last forward
   bool have_forward = false, have_backward = false, gather = false;
+  bool have_aux = false;                  // the last forward wrote (depth, alpha) to a caller's aux buffer
   int n = 0, d = 3, scale_act = 0;
   long long m = 0;
   GsCam cam{};
@@ -221,7 +222,8 @@ static int ceil_log2(unsigned v) {
 
 static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
                                const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
-                               float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream) {
+                               float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream,
+                               const gs_render_aux* ax = nullptr) {
   if (!c || !cam || n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad arguments");
   if (d != 3 && gs_sh_basis_count(d) == 0)
     return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
@@ -231,11 +233,29 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: tile_thresh must be in (0, 1)");
   if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: null tensor pointer");
+  GsAuxOut aux_out{};
+  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
+  if (use_aux) {
+    if (ax->aux_final && !final_img)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: aux_final needs image_final");
+    if (ax->background) {
+      for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(ax->background[k]))
+          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: background must be finite");
+        aux_out.bg[k] = ax->background[k];
+      }
+    }
+    aux_out.aux = ax->aux;
+    aux_out.aux_final = ax->aux_final;
+    // a forward that writes aux may be differentiated through it: its backward kernel must exist too
+    if (int rc = gs_blend_aux_supported(d, true, ax->aux != nullptr)) return rc;
+  }
   if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
   c->have_forward = false;
   c->have_backward = false;
+  c->have_aux = false;
 
   GsFrameGeom g{};
   g.width = cam->width;
@@ -427,7 +447,8 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   if (d == 3) {
     GS_CUDA_TRY(gs_launch_blend_fwd(c->pA.as<float4>(), c->pB.as<float2>(), c->pC.as<float4>(),
                                     gather ? c->rec.as<GsRec>() : nullptr, c->vals_out.as<uint32_t>(),
-                                    c->tile_accum.as<int>(), g, image, c->tile_neff.as<int>(), final_img, crop, st));
+                                    c->tile_accum.as<int>(), g, image, c->tile_neff.as<int>(), final_img, crop, st,
+                                    use_aux ? &aux_out : nullptr));
   } else {
     const float* rp = c->rays.as<float>();
     GsRayPtrs rays{rp, rp + 3, rp + 6, rp + 9};
@@ -435,13 +456,14 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
                                        gather ? c->rec.as<GsRec>() : nullptr, rgb, c->vals_out.as<uint32_t>(),
                                        c->offsets_g.as<uint32_t>(), d,
                                        c->tile_accum.as<int>(), g, rays, image, c->tile_neff.as<int>(), final_img,
-                                       crop, st));
+                                       crop, st, use_aux ? &aux_out : nullptr));
   }
   gs_count_launch();   // blend forward
   gs_mark(c, 6, st);
   c->ev_fwd_valid = c->timing && c->ev_ok;
 
   c->have_forward = true;
+  c->have_aux = aux_out.aux != nullptr;
   c->gather = gather;
   c->n = n;
   c->d = d;
@@ -475,12 +497,19 @@ extern "C" int gs_render_forward_final(gs_ctx* c, const float* pos, const float*
 static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
                                 const float* scale, const float* image, const float* grad_image, int grad_is_final,
                                 float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
-                                float* grad_scale, gs_stream_t stream) {
+                                float* grad_scale, gs_stream_t stream, const float* aux = nullptr,
+                                const float* grad_aux = nullptr) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward: no forward on this ctx");
   if (!image || !grad_image || !grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale ||
       (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null tensor pointer");
+  if (grad_aux) {
+    if (!c->have_aux)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux given but the forward wrote no aux");
+    if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux needs the forward's aux");
+    if (int rc = gs_blend_aux_supported(c->d, false, true)) return rc;
+  }
   if (int rc = gs_check_device(c->device, "gs_render_backward")) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
@@ -509,7 +538,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                       c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image, grad_image,
                                       c->grad_inst.as<float>(),
                                       grad_is_final, crop, c->row_epoch.as<uint32_t>(), c->epoch,
-                                      c->tile_neff_b.as<int>(), st));
+                                      c->tile_neff_b.as<int>(), st, aux, grad_aux));
     } else {
       const float* rp = c->rays.as<float>();
       GsRayPtrs rays{rp, rp + 3, rp + 6, rp + 9};
@@ -518,7 +547,8 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                          c->offsets_g.as<uint32_t>(), d,
                                          c->tile_accum.as<int>(), c->geom, rays, image, grad_image,
                                          c->grad_inst.as<float>(), grad_is_final, crop,
-                                         c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), st));
+                                         c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), st, aux,
+                                         grad_aux));
     }
     gs_count_launch();
     c->have_backward = true;
@@ -540,7 +570,8 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
                                           c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                           c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
-                                          grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st));
+                                          grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
+                                          grad_aux != nullptr));
   if (c->n > 0) gs_count_launch();
   gs_mark(c, 9, st);
   c->ev_bwd_valid = c->timing && c->ev_ok;
@@ -561,6 +592,23 @@ extern "C" int gs_render_backward_final(gs_ctx* c, const float* pos, const float
                                         float* grad_quat, float* grad_scale, gs_stream_t stream) {
   return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_final, 1, grad_pos, grad_rgb,
                               grad_opa, grad_quat, grad_scale, stream);
+}
+
+extern "C" int gs_render_forward_aux(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                     const float* quat, const float* scale, int n, int d, int scale_activation,
+                                     const gs_camera* cam, float* image_raw_padded, float* image_final,
+                                     int64_t* culling_mask, const gs_render_aux* aux, gs_stream_t stream) {
+  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image_raw_padded, image_final,
+                             culling_mask, stream, aux);
+}
+
+extern "C" int gs_render_backward_aux(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                      const float* quat, const float* scale, const float* image_raw_padded,
+                                      const float* grad_image, int grad_is_final, const float* aux,
+                                      const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                      float* grad_quat, float* grad_scale, gs_stream_t stream) {
+  return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
+                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux);
 }
 
 extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {

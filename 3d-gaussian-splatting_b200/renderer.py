@@ -246,3 +246,59 @@ class _RenderFrameFinal(torch.autograd.Function):
 
 
 render_frame_final = _RenderFrameFinal.apply
+
+
+class _RenderFrameAux(torch.autograd.Function):
+    """`render_frame_final` (final=True) or `render_frame` (final=False) over a constant background colour, plus
+    the per-pixel depth sum_i w_i |p_c,i| (accumulated, not normalised; Euclidean distance, not camera z) and
+    alpha 1 - T_f.  All three outputs are differentiable; a graph that never uses depth or alpha passes no
+    gradient for them and runs the plain backward kernels."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                near, tile_thresh, scale_activation, background, final):
+        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
+        bg = None if background is None else [float(v) for v in background]
+        fin, raw, aux, aux_fin, mask = rctx.forward_aux(
+            pos, rgb, opa, quat, scale, int(width), int(height), float(focal_x), float(focal_y), rot.detach().cpu(),
+            tran.detach().cpu(), float(near), float(tile_thresh), SCALE_ACTIVATIONS[scale_activation], bg,
+            bool(final))
+        ctx.rctx = rctx
+        ctx.frame = rctx.frame_id()
+        ctx.final = bool(final)
+        ctx.save_for_backward(pos, rgb, opa, quat, scale, raw, aux)
+        ctx.mark_non_differentiable(mask)
+        ctx.set_materialize_grads(False)
+        image, maps = (fin, aux_fin) if final else (raw, aux)
+        ctx.map_shape = tuple(maps.shape[:2])
+        return image, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
+        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
+        rows, cols = ctx.map_shape
+        if grad_image is None:
+            grad_image = raw.new_zeros(rows, cols, 3)
+        grad_aux = None
+        if grad_depth is not None or grad_alpha is not None:
+            grad_aux = raw.new_zeros(rows, cols, 2)
+            if grad_depth is not None:
+                grad_aux[..., 0] = grad_depth
+            if grad_alpha is not None:
+                grad_aux[..., 1] = grad_alpha
+        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
+        _apply_push(ctx.rctx, push)
+        ctx.rctx.backward_aux_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
+                                   *outs, ctx.frame)
+        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 11
+
+
+def render_frame_aux(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
+                     tile_thresh, scale_activation, background=None, final=True):
+    """-> (image, depth, alpha, culling_mask).  final=True: image [H,W,3] clamped + cropped as in
+    `render_frame_final`, depth / alpha [H,W] (not clamped); final=False: the padded un-clamped image
+    [Hp,Wp,3] and [Hp,Wp] maps.  background: 3 floats (None = black, the reference); per pixel
+    image = sum_i w_i c_i + T_f background, depth = sum_i w_i |p_c,i|, alpha = 1 - T_f.  RGB and per-pixel SH
+    colour on the default kernels."""
+    return _RenderFrameAux.apply(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                                 near, tile_thresh, scale_activation, background, final)

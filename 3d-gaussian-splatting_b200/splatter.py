@@ -27,7 +27,7 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import render_frame, render_frame_final
+from renderer import render_frame, render_frame_aux, render_frame_final
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -282,6 +282,21 @@ class Splatter(nn.Module):
         self.n_gaussians = g.pos.shape[0]
         self.n_tile_gaussians = self._rctx.last_instances()         # train.py:198 reads it every step
         return image
+
+    def render_maps(self, camera_id=None, extrinsics=None, intrinsics=None, background=None):
+        """`forward` plus per-pixel maps: dict(image [H,W,3] (clamped, cropped, over `background`, default black),
+        depth [H,W] (accumulated sum w |p_c|: divide by alpha for the expected Euclidean distance), alpha [H,W]).
+        All three are differentiable (`renderer.render_frame_aux`)."""
+        self.set_camera(camera_id, extrinsics, intrinsics)
+        g, v = self.gaussian_3ds, self.current_view
+        image, depth, alpha, mask = render_frame_aux(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
+                                                     v["height"], v["focal_x"], v["focal_y"], v["rot"], v["tran"],
+                                                     self.near, self.tile_culling_prob_thresh, self.scale_activation,
+                                                     background=background, final=True)
+        self.culling_mask = mask
+        self.n_gaussians = g.pos.shape[0]
+        self.n_tile_gaussians = self._rctx.last_instances()
+        return dict(image=image, depth=depth, alpha=alpha)
 
     def forward_unfused_post(self, camera_id=None, extrinsics=None, intrinsics=None):
         """Same image through the padded raw render + torch clamp/crop (kept for cross-checks)."""

@@ -185,6 +185,43 @@ int gs_render_backward_final(gs_ctx* ctx, const float* pos, const float* rgb, co
                              const float* grad_final, float* grad_pos, float* grad_rgb, float* grad_opa,
                              float* grad_quat, float* grad_scale, gs_stream_t stream);
 
+/* Depth and alpha maps and a background colour (additive; the calls above keep the reference's black
+ * background and produce no maps).  Per pixel, with instances in (tile, depth) order, w_i = alpha_i T_i as in the
+ * blend and T_f the transmittance after the last live instance (the 1e-4 early stop applies):
+ *   image_c = sum_i w_i c_i,c + T_f background_c        (background = 0 is the plain image, bit for bit)
+ *   depth   = sum_i w_i |p_c,i|                          accumulated, NOT normalised (expected depth = depth / alpha);
+ *                                                        Euclidean camera distance (the sort key), not camera z
+ *   alpha   = 1 - T_f
+ * The background is a constant: it has no gradient.  gs_render_backward_aux takes the gradient of
+ * (depth, alpha) too; the depth gradient reaches pos through p_c / |p_c|.
+ *   background : HOST float[3]; NULL = black.  Must be finite (GS_ERR_INVALID_ARG otherwise).
+ *   aux        : DEVICE [Hp,Wp,2] = (depth, alpha) per padded pixel; NULL = not written.
+ *   aux_final  : DEVICE [height,width,2] centre crop of aux (not clamped); needs image_final.
+ * Implemented for RGB and SH colour on the default (gather) path with the shipped kernels; the packed path
+ * (gs_tune("gather", 0)), the two-pixel tensor-core SH backward (sh_tc bit 2) and non-default RGB blend knobs
+ * return GS_ERR_UNSUPPORTED when a map or a background is requested.  Same synchronisation and launch count as gs_render_forward_final; no workspace is allocated for
+ * the maps (the buffers are the caller's). */
+typedef struct gs_render_aux {
+  const float* background;
+  float* aux;
+  float* aux_final;
+} gs_render_aux;
+/* image_final may be NULL (then aux_final must be NULL).  aux == NULL behaves like gs_render_forward[_final]. */
+int gs_render_forward_aux(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa,
+                          const float* quat, const float* scale, int n, int d, int scale_activation,
+                          const gs_camera* cam_host, float* image_raw_padded, float* image_final,
+                          int64_t* culling_mask, const gs_render_aux* aux, gs_stream_t stream);
+/* Backward of gs_render_forward_aux.  grad_image is [Hp,Wp,3] (grad_is_final == 0) or [height,width,3] of the
+ * final image (grad_is_final != 0, as gs_render_backward_final).  aux = the forward's [Hp,Wp,2] buffer;
+ * grad_aux = [Hp,Wp,2] or [height,width,2] (per grad_is_final) gradient of (depth, alpha); NULL = zero, which runs
+ * the plain backward kernels.  grad_aux without an aux written by the forward is GS_ERR_INVALID_ARG.  The
+ * data-parallel push (gs_ctx_set_grad_push) applies as in gs_render_backward. */
+int gs_render_backward_aux(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa,
+                           const float* quat, const float* scale, const float* image_raw_padded,
+                           const float* grad_image, int grad_is_final, const float* aux, const float* grad_aux,
+                           float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
+                           gs_stream_t stream);
+
 /* Per-stage device timing with CUDA events recorded on the frame's stream (off by default).
  * gs_frame_stage_ms fills out[GS_N_STAGES] with the milliseconds of the last frame's stages:
  * 0 project, 1 depth sort of Gaussians + scan + M readback, 2 key emit, 3 tile-id radix sort,

@@ -323,6 +323,10 @@ struct RenderContext {
   }
   void clear_grad_push() { check_rc(gs_ctx_set_grad_push(ctx, nullptr), "gs_ctx_set_grad_push"); }
 
+  // where SH colour is evaluated (gs_ctx_set_sh_eval): SH_EVAL_PIXEL (default) or SH_EVAL_GAUSSIAN; applies to the
+  // forwards that follow, a backward uses the mode of its forward
+  void set_sh_eval(int mode) { check_rc(gs_ctx_set_sh_eval(ctx, mode), "gs_ctx_set_sh_eval"); }
+
   void set_timing(bool on) { check_rc(gs_ctx_set_timing(ctx, on ? 1 : 0), "gs_ctx_set_timing"); }
   std::vector<float> stage_ms() {
     std::vector<float> v(GS_N_STAGES, -1.f);
@@ -682,6 +686,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
       .def("stats", &RenderContext::stats)
+      .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_timing", &RenderContext::set_timing)
       .def("set_grad_push", &RenderContext::set_grad_push)
       .def("clear_grad_push", &RenderContext::clear_grad_push)
@@ -704,4 +709,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("kernel_launches", []() { return (int64_t)gs_kernel_launches(); },
         "kernels of libgs_b200 launched by this process so far");
   m.attr("abi_version") = gs_abi_version();
+  m.attr("SH_EVAL_PIXEL") = GS_SH_EVAL_PIXEL;
+  m.attr("SH_EVAL_GAUSSIAN") = GS_SH_EVAL_GAUSSIAN;
 }

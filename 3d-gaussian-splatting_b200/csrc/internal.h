@@ -130,7 +130,8 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
-                                    unsigned int* n_visible, cudaStream_t st);
+                                    unsigned int* n_visible, cudaStream_t st,
+                                    bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/);
 
 // Data-parallel gradient push (device view of gs_grad_push): world == 0 disables it.
 struct GsGradPush {
@@ -146,7 +147,8 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
-                                        bool depth_grad = false /*rows carry dL/d|p_c| in column 6 + d*/);
+                                        bool depth_grad = false /*rows carry dL/d|p_c| in the column after the colour*/,
+                                        bool sh_gaussian = false /*d = 27 / 48 coefficients, RGB gradient rows*/);
 
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,

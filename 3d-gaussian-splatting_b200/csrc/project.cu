@@ -2,6 +2,7 @@
 // helpers (world2camera, jacobian) and the fused frame-path variants that also apply the
 // parameter activations and the tile-rectangle rule.  All HBM-bound streaming kernels.
 #include "internal.h"
+#include "sh_common.cuh"
 
 namespace {
 
@@ -44,10 +45,36 @@ __device__ __forceinline__ void load_activated(const float* __restrict__ quat, c
   }
 }
 
-__global__ void __launch_bounds__(kBlock) fused_project_kernel(
+// Unit direction from the camera centre C = -R^T t to the mean, in the world frame (the frame of the per-pixel rays,
+// so that an SH coefficient means the same in both evaluation modes); inv_len = 1 / |pos - C| = 1 / |p_c|.
+__device__ __forceinline__ void view_dir(const GsCam& cam, const float p[3], float dir[3], float& inv_len) {
+  float u[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) u[j] = p[j] + (cam.r[j] * cam.t[0] + cam.r[3 + j] * cam.t[1] + cam.r[6 + j] * cam.t[2]);
+  inv_len = 1.f / sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);   // visible: |u| >= z > near
+#pragma unroll
+  for (int j = 0; j < 3; ++j) dir[j] = u[j] * inv_len;
+}
+
+// logits l_c = sum_k Y_k coef[c*K + k] of the channel-major coefficient row coef[3K]
+template <int K>
+__device__ __forceinline__ void sh_logits(const float* coef, const float* Y, float l[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < K; ++k) s = fmaf(Y[k], coef[c * K + k], s);
+    l[c] = s;
+  }
+}
+
+// KG = 0: colour from the rgb[n, 3] logits when d == 3 (per-pixel SH leaves it to the blend).  KG = 9 / 16: SH of
+// degree 2 / 3 evaluated once per Gaussian along view_dir (GS_SH_EVAL_GAUSSIAN); the record then carries an RGB colour.
+template <int KG>
+__device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
+    const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
     unsigned int* __restrict__ n_visible) {
   int i = blockIdx.x * kBlock + threadIdx.x;
@@ -68,10 +95,20 @@ __global__ void __launch_bounds__(kBlock) fused_project_kernel(
         float op = gs_sigmoid(opa[i]);
         GsRec* r = rec + i;
         r->a = make_float4(o.x, o.y, k.ca, k.cb);
-        // RGB colour = sigmoid(logit) (splatter.py:539); SH coefficients stay raw and are gathered
+        // RGB colour = sigmoid(logit) (splatter.py:539); per-pixel SH coefficients stay raw and are gathered
         // from the parameter tensor by the pack pass
         float cr = 0.f, cg = 0.f, cb = 0.f;
-        if (d == 3) {
+        if constexpr (KG > 0) {
+          float coef[3 * KG], dir[3], il, Y[KG], l[3];
+#pragma unroll
+          for (int k = 0; k < 3 * KG; ++k) coef[k] = rgb[(size_t)i * (3 * KG) + k];
+          view_dir(cam, p, dir, il);
+          gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
+          sh_logits<KG>(coef, Y, l);
+          cr = gs_sigmoid(l[0]);
+          cg = gs_sigmoid(l[1]);
+          cb = gs_sigmoid(l[2]);
+        } else if (d == 3) {
           cr = gs_sigmoid(rgb[3 * i]);
           cg = gs_sigmoid(rgb[3 * i + 1]);
           cb = gs_sigmoid(rgb[3 * i + 2]);
@@ -102,6 +139,27 @@ __global__ void __launch_bounds__(kBlock) fused_project_kernel(
     if (nv) atomicAdd(n_visible, (unsigned int)nv);
     if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
   }
+}
+
+__global__ void __launch_bounds__(kBlock) fused_project_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible) {
+  fused_project_body<0>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec, count,
+                        dkey, mask, n_visible);
+}
+
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_sh_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible) {
+  fused_project_body<K>(pos, rgb, opa, quat, scale, n, 3 * K, scale_act, cam, grid, near_plane, half_w, half_h, rec,
+                        count, dkey, mask, n_visible);
 }
 
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
@@ -140,10 +198,14 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
   }
 }
 
-// DT: the blend backward stored dL/d|p_c| in the row's pad column 6 + D (aux depth gradient); it enters as g_xyd[2]
+// DT: the blend backward stored dL/d|p_c| in the row's pad column 6 + DC (aux depth gradient); it enters as g_xyd[2]
 // and reaches pos through p_c / |p_c|.  Without it depth is only a sort key.
-template <int D, int GW, int W, bool DT = false>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
+// KG = 9 / 16: SH evaluated once per Gaussian (fused_project_body<KG>): the rows carry dL/d(colour) like RGB rows
+// (GW = GS_GREC); the D = 3 KG coefficient gradients and the view-direction term are formed here.
+// (cam and push are taken by value, as the kernel parameters they are: by reference, the KG = 0 instantiations would
+// no longer compile to the code fused_project_bwd_kernel had before the body was shared.)
+template <int D, int GW, int W, bool DT, int KG>
+__device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
     float near_plane, float half_w, float half_h, const uint32_t* __restrict__ offsets_g,
@@ -151,6 +213,8 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
     float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
     GsGradPush push) {
+  static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
+  constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   int i = blockIdx.x * kBlock + threadIdx.x;
   // SH colour on one GPU: the warp writes its coefficient gradients together (below), so threads past n stay
   constexpr bool kStagedRgb = (D != 3) && (W == 0);
@@ -161,6 +225,9 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
   float acc[GW];
 #pragma unroll
   for (int k = 0; k < GW; ++k) acc[k] = 0.f;
+  float gsh[KG ? D : 1];                    // KG: coefficient gradients
+#pragma unroll
+  for (int k = 0; k < (KG ? D : 1); ++k) gsh[k] = 0.f;
   const uint32_t cnt = valid ? count[i] : 0u;
   if (cnt > 0) {
     const uint32_t o0 = offsets_g[i], o1 = o0 + cnt;   // this Gaussian's contiguous gradient rows
@@ -170,7 +237,11 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
-    if (D == 3) {
+    float coef[KG ? D : 1];
+    if constexpr (KG > 0) {
+#pragma unroll
+      for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
+    } else if (D == 3) {
       rgb_raw[0] = rgb[3 * i];
       rgb_raw[1] = rgb[3 * i + 1];
       rgb_raw[2] = rgb[3 * i + 2];
@@ -202,10 +273,33 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     gcov[1] = acc[3] * sc + gsc * kk * o.c;                   // d det/db = -c
     gcov[2] = acc[3] * sc + gsc * kk * o.b;                   // d det/dc = -b
     gcov[3] = acc[2] * sc - gsc * kk * o.a;                   // d det/dd =  a
-    static_assert(!DT || 6 + D < GW, "no pad column for the depth gradient");
-    float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + D] : 0.f};   // without DT depth is only a sort key
+    static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
+    float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
     float gq[4], gsv[3];
     gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    if constexpr (KG > 0) {
+      // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
+      // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
+      float dir[3], il, Y[KG], l[3], gl[3], w[KG], gd[3];
+      view_dir(cam, p, dir, il);
+      gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
+      sh_logits<KG>(coef, Y, l);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float sg = gs_sigmoid(l[c]);
+        gl[c] = acc[6 + c] * sg * (1.f - sg);
+      }
+#pragma unroll
+      for (int k = 0; k < KG; ++k) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) gsh[c * KG + k] = gl[c] * Y[k];
+        w[k] = gl[0] * coef[k] + gl[1] * coef[KG + k] + gl[2] * coef[2 * KG + k];
+      }
+      gs_sh::sh_basis_grad<KG>(dir[0], dir[1], dir[2], w, gd);
+      const float dd = dir[0] * gd[0] + dir[1] * gd[1] + dir[2] * gd[2];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) gp[j] += (gd[j] - dir[j] * dd) * il;
+    }
     // quat normalisation backward: q = r/|r|
     float dot = q[0] * gq[0] + q[1] * gq[1] + q[2] * gq[2] + q[3] * gq[3];
 #pragma unroll
@@ -228,6 +322,7 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
       }
     }
   }
+  const float* gcol = KG ? gsh : acc + 6;   // the D gradients of this Gaussian's rgb row
   if (W == 0) {
     if constexpr (kStagedRgb) {
       // The 32 Gaussians of a warp own 32 * D contiguous floats of g_rgb.  One strided 4-byte store per coefficient
@@ -243,7 +338,7 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
       for (int pass = 0; pass < D / HW; ++pass) {
         __syncwarp();
 #pragma unroll
-        for (int k = 0; k < HW; ++k) stage[warp][lane][k] = acc[6 + pass * HW + k];
+        for (int k = 0; k < HW; ++k) stage[warp][lane][k] = gcol[pass * HW + k];
         __syncwarp();
         if (HW == D) {
           float* dst = g_rgb + (size_t)i0 * D;
@@ -258,7 +353,7 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
       if (!valid) return;
     } else {
 #pragma unroll
-      for (int k = 0; k < D; ++k) g_rgb[(size_t)i * D + k] = acc[6 + k];
+      for (int k = 0; k < D; ++k) g_rgb[(size_t)i * D + k] = gcol[k];
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -270,7 +365,7 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
   } else {
     push_store<W, 3>(push, g_pos + 3 * (size_t)i, gp);
     push_store<W, 3>(push, g_scale + 3 * (size_t)i, gs_raw);
-    push_store<W, D>(push, g_rgb + (size_t)i * D, acc + 6);
+    push_store<W, D>(push, g_rgb + (size_t)i * D, gcol);
     // a quaternion is 4 floats at a 16-byte aligned bucket offset and `per` is a multiple of 4:
     // it never straddles two slices
     *reinterpret_cast<float4*>(push_dst<W>(push, g_quat + 4 * (size_t)i, 1)) =
@@ -278,6 +373,30 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
     push_store<W, 1>(push, g_opa + i, &go);
   }
 }
+
+#define GS_PBWD_PARAMS                                                                                             \
+  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                      \
+      const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,             \
+      float near_plane, float half_w, float half_h, const uint32_t* __restrict__ offsets_g,                         \
+      const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,                                      \
+      const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,                            \
+      float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat,                             \
+      float* __restrict__ g_scale, GsGradPush push
+#define GS_PBWD_ARGS                                                                                               \
+  pos, rgb, opa, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, offsets_g, count, grad_inst, row_epoch, \
+      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, push
+
+template <int D, int GW, int W, bool DT = false>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(GS_PBWD_PARAMS) {
+  fused_project_bwd_body<D, GW, W, DT, 0>(GS_PBWD_ARGS);
+}
+
+// per-Gaussian SH of K basis functions (fused_project_sh_kernel<K>)
+template <int K, int W, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_kernel(GS_PBWD_PARAMS) {
+  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K>(GS_PBWD_ARGS);
+}
+#undef GS_PBWD_PARAMS
 
 }  // namespace
 
@@ -427,10 +546,21 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
-                                    unsigned int* n_visible, cudaStream_t st) {
+                                    unsigned int* n_visible, cudaStream_t st, bool sh_gaussian) {
   if (n == 0) return cudaSuccess;
-  fused_project_kernel<<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid,
-                                                       near_plane, half_w, half_h, rec, count, dkey, mask, n_visible);
+  if (sh_gaussian && d == 27)
+    fused_project_sh_kernel<9><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
+                                                               near_plane, half_w, half_h, rec, count, dkey, mask,
+                                                               n_visible);
+  else if (sh_gaussian && d == 48)
+    fused_project_sh_kernel<16><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
+                                                                near_plane, half_w, half_h, rec, count, dkey, mask,
+                                                                n_visible);
+  else if (sh_gaussian)
+    return cudaErrorInvalidValue;
+  else
+    fused_project_kernel<<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid,
+                                                         near_plane, half_w, half_h, rec, count, dkey, mask, n_visible);
   return cudaGetLastError();
 }
 
@@ -440,13 +570,10 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
-                                        bool depth_grad) {
+                                        bool depth_grad, bool sh_gaussian) {
   if (n == 0) return cudaSuccess;
-#define GS_LAUNCH_PBWD(D, GW, W, DT)                                                                                 \
-  fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act,   \
-                                                                         cam, near_plane, half_w, half_h, offsets_g, \
-                                                                         count, grad_inst, row_epoch, epoch, g_pos,  \
-                                                                         g_rgb, g_opa, g_quat, g_scale, push)
+#define GS_LAUNCH_PBWD(D, GW, W, DT) \
+  fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
 #define GS_LAUNCH_PBWD_W(D, GW, DT)                  \
   switch (push.world) {                              \
     case 0: GS_LAUNCH_PBWD(D, GW, 0, DT); break;     \
@@ -455,13 +582,31 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
     case 8: GS_LAUNCH_PBWD(D, GW, 8, DT); break;     \
     default: return cudaErrorInvalidValue;           \
   }
-  if (d == 3 && depth_grad) { GS_LAUNCH_PBWD_W(3, GS_GREC, true) }
+#define GS_LAUNCH_PBWD_SH(K, W, DT) \
+  fused_project_bwd_sh_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
+#define GS_LAUNCH_PBWD_SH_W(K, DT)                   \
+  switch (push.world) {                              \
+    case 0: GS_LAUNCH_PBWD_SH(K, 0, DT); break;      \
+    case 2: GS_LAUNCH_PBWD_SH(K, 2, DT); break;      \
+    case 4: GS_LAUNCH_PBWD_SH(K, 4, DT); break;      \
+    case 8: GS_LAUNCH_PBWD_SH(K, 8, DT); break;      \
+    default: return cudaErrorInvalidValue;           \
+  }
+  if (sh_gaussian && d != 27 && d != 48) return cudaErrorInvalidValue;
+  if (sh_gaussian && d == 27 && depth_grad) { GS_LAUNCH_PBWD_SH_W(9, true) }
+  else if (sh_gaussian && d == 27) { GS_LAUNCH_PBWD_SH_W(9, false) }
+  else if (sh_gaussian && depth_grad) { GS_LAUNCH_PBWD_SH_W(16, true) }
+  else if (sh_gaussian) { GS_LAUNCH_PBWD_SH_W(16, false) }
+  else if (d == 3 && depth_grad) { GS_LAUNCH_PBWD_W(3, GS_GREC, true) }
   else if (d == 3) { GS_LAUNCH_PBWD_W(3, GS_GREC, false) }
   else if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_W(27, 36, true) }
   else if (d == 27) { GS_LAUNCH_PBWD_W(27, 36, false) }
   else if (depth_grad) { GS_LAUNCH_PBWD_W(48, 56, true) }
   else { GS_LAUNCH_PBWD_W(48, 56, false) }
+#undef GS_LAUNCH_PBWD_SH_W
+#undef GS_LAUNCH_PBWD_SH
 #undef GS_LAUNCH_PBWD_W
 #undef GS_LAUNCH_PBWD
+#undef GS_PBWD_ARGS
   return cudaGetLastError();
 }

@@ -143,6 +143,7 @@ struct gs_ctx {
   // state of the last forward
   bool have_forward = false, have_backward = false, gather = false;
   bool have_aux = false;                  // the last forward wrote (depth, alpha) to a caller's aux buffer
+  bool sh_gaussian = false;               // the last forward evaluated its SH colour once per Gaussian
   int n = 0, d = 3, scale_act = 0;
   long long m = 0;
   GsCam cam{};
@@ -157,6 +158,7 @@ struct gs_ctx {
   bool ev_fwd_valid = false, ev_bwd_valid = false;
   // data-parallel gradient push (gs_ctx_set_grad_push); world == 0: off
   GsGradPush push{};
+  int sh_eval = GS_SH_EVAL_PIXEL;         // gs_ctx_set_sh_eval: applies to the forwards that follow
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -233,6 +235,10 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: tile_thresh must be in (0, 1)");
   if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: null tensor pointer");
+  // per-Gaussian SH: the projection writes an RGB colour, and everything that serves the blend runs as for d == 3;
+  // only the projection kernels, the push bucket and the caller's tensors keep the parameter width d
+  const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
+  const int blend_d = sh_gaussian ? 3 : d;   // colour width of the blend
   GsAuxOut aux_out{};
   const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
   if (use_aux) {
@@ -248,7 +254,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     aux_out.aux = ax->aux;
     aux_out.aux_final = ax->aux_final;
     // a forward that writes aux may be differentiated through it: its backward kernel must exist too
-    if (int rc = gs_blend_aux_supported(d, true, ax->aux != nullptr)) return rc;
+    if (int rc = gs_blend_aux_supported(blend_d, true, ax->aux != nullptr)) return rc;
   }
   if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
   g_cur_alloc = &c->allocator;
@@ -304,7 +310,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     c->iota_n = N;
   }
 
-  if (d != 3) {
+  if (blend_d != 3) {
     // world-space ray set-up for per-pixel SH, reference splatter.py:305-321 (RayInfo):
     // c2w = inverse(w2c); rays_o = -c2w t; lefttop = c2w (((-Wp/2+.5)/fx, (-Hp/2+.5)/fy, 1) - t)
     GS_CUDA_TRY(c->rays.reserve(64, st));
@@ -338,7 +344,8 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
   GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
                                       half_w, half_h, c->rec.as<GsRec>(), c->count.as<uint32_t>(),
-                                      c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st));
+                                      c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
+                                      sh_gaussian));
   if (n > 0) gs_count_launch();
   // 2. (a) exclusive scan of the tile counts in Gaussian-id order -> gradient-row bases and M;
   //    (b) stable depth sort of the N Gaussians; (c) scan of the counts in depth order (the
@@ -385,7 +392,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   // tile-id sort key width (GS_TILE_KEY_BYTES=4 forces the wide path, for tests)
   static const int forced_key = getenv("GS_TILE_KEY_BYTES") ? atoi(getenv("GS_TILE_KEY_BYTES")) : 0;
   const int key_bytes = (g.n_tiles <= 65536 && forced_key != 4) ? 2 : 4;
-  const size_t crow = d == 3 ? 16 : (size_t)gs_sh_stream_width(d) * 4;   // colour / SH stream row bytes
+  const size_t crow = blend_d == 3 ? 16 : (size_t)gs_sh_stream_width(d) * 4;   // colour / SH stream row bytes
   if (!gather) {
     GS_CUDA_TRY(c->pA.reserve(M * 16 + 16, st));
     GS_CUDA_TRY(c->pC.reserve(M * crow + 16, st));
@@ -430,7 +437,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     // no pack pass: only the tile ranges are derived from the sorted keys; the blend kernels pull the records
     // of their tile straight from rec[N] through the sorted id list
     GS_CUDA_TRY(gs_launch_tile_ranges(c->keys_out.p, key_bytes, m, g.n_tiles, c->tile_accum.as<int>(), st));
-  } else if (d == 3) {
+  } else if (blend_d == 3) {
     GS_CUDA_TRY(gs_launch_pack_sorted(c->keys_out.p, key_bytes, c->vals_out.as<uint32_t>(), m, g.n_tiles, g.ntx,
                                       c->rec.as<GsRec>(), c->offsets_g.as<uint32_t>(), c->pA.as<float4>(),
                                       c->pB.as<float2>(), c->pC.as<float4>(), c->tile_accum.as<int>(), st));
@@ -444,7 +451,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   // 6. blend (+ optional fused clamp & centre crop, splatter.py:652-653 / :267-272)
   GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
   gs_mark(c, 5, st);
-  if (d == 3) {
+  if (blend_d == 3) {
     GS_CUDA_TRY(gs_launch_blend_fwd(c->pA.as<float4>(), c->pB.as<float2>(), c->pC.as<float4>(),
                                     gather ? c->rec.as<GsRec>() : nullptr, c->vals_out.as<uint32_t>(),
                                     c->tile_accum.as<int>(), g, image, c->tile_neff.as<int>(), final_img, crop, st,
@@ -464,6 +471,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
 
   c->have_forward = true;
   c->have_aux = aux_out.aux != nullptr;
+  c->sh_gaussian = sh_gaussian;
   c->gather = gather;
   c->n = n;
   c->d = d;
@@ -508,14 +516,15 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
     if (!c->have_aux)
       return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux given but the forward wrote no aux");
     if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux needs the forward's aux");
-    if (int rc = gs_blend_aux_supported(c->d, false, true)) return rc;
+    if (int rc = gs_blend_aux_supported(c->sh_gaussian ? 3 : c->d, false, true)) return rc;
   }
   if (int rc = gs_check_device(c->device, "gs_render_backward")) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
   size_t M = (size_t)c->m;
   const int d = c->d;
-  const size_t grow = d == 3 ? (size_t)GS_GREC * 4 : (size_t)gs_sh_grad_width(d) * 4;
+  const int blend_d = c->sh_gaussian ? 3 : d;   // colour width of the blend: the forward's SH mode, not the current one
+  const size_t grow = blend_d == 3 ? (size_t)GS_GREC * 4 : (size_t)gs_sh_grad_width(d) * 4;
   GS_CUDA_TRY(c->grad_inst.reserve(M * grow + 16, st));
   {
     // one u32 tag per gradient row: rows written by this backward carry `epoch`; the tails of
@@ -532,7 +541,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
   gs_mark(c, 7, st);
   if (c->m > 0) {
-    if (d == 3) {
+    if (blend_d == 3) {
       GS_CUDA_TRY(gs_launch_blend_bwd(c->pA.as<float4>(), c->pB.as<float2>(), c->pC.as<float4>(),
                                       c->gather ? c->rec.as<GsRec>() : nullptr, c->vals_out.as<uint32_t>(),
                                       c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image, grad_image,
@@ -571,7 +580,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                           c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                           c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                           grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
-                                          grad_aux != nullptr));
+                                          grad_aux != nullptr, c->sh_gaussian));
   if (c->n > 0) gs_count_launch();
   gs_mark(c, 9, st);
   c->ev_bwd_valid = c->timing && c->ev_ok;
@@ -632,6 +641,14 @@ extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {
     g.staging[k] = p->staging[k];
   }
   c->push = g;
+  return 0;
+}
+
+extern "C" int gs_ctx_set_sh_eval(gs_ctx* c, int mode) {
+  if (mode != GS_SH_EVAL_PIXEL && mode != GS_SH_EVAL_GAUSSIAN)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_sh_eval: mode must be GS_SH_EVAL_PIXEL or GS_SH_EVAL_GAUSSIAN");
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_sh_eval: null ctx");
+  c->sh_eval = mode;
   return 0;
 }
 

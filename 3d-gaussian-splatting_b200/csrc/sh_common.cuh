@@ -41,6 +41,24 @@ __device__ __forceinline__ void sh_basis(float x, float y, float z, float* out) 
   }
 }
 
+// g = sum_k w[k] dY_k / d(x, y, z): the derivative of sh_basis<K> contracted with weights w[K] (direction treated as
+// three free coordinates; the caller projects out the radial part)
+template <int K>
+__device__ __forceinline__ void sh_basis_grad(float x, float y, float z, const float* w, float g[3]) {
+  g[0] = -SH_C1 * w[3] + SH_C2_0 * y * w[4] - 2.f * SH_C2_2 * x * w[6] + SH_C2_3 * z * w[7] + 2.f * SH_C2_4 * x * w[8];
+  g[1] = -SH_C1 * w[1] + SH_C2_0 * x * w[4] + SH_C2_1 * z * w[5] - 2.f * SH_C2_2 * y * w[6] - 2.f * SH_C2_4 * y * w[8];
+  g[2] = SH_C1 * w[2] + SH_C2_1 * y * w[5] + 4.f * SH_C2_2 * z * w[6] + SH_C2_3 * x * w[7];
+  if (K > 9) {
+    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+    g[0] += SH_C3_0 * 6.f * xy * w[9] + SH_C3_1 * yz * w[10] - SH_C3_2 * 2.f * xy * w[11] - SH_C3_3 * 6.f * xz * w[12] +
+            SH_C3_4 * (4.f * zz - 3.f * xx - yy) * w[13] + SH_C3_5 * 2.f * xz * w[14] + SH_C3_6 * 3.f * (xx - yy) * w[15];
+    g[1] += SH_C3_0 * 3.f * (xx - yy) * w[9] + SH_C3_1 * xz * w[10] + SH_C3_2 * (4.f * zz - xx - 3.f * yy) * w[11] -
+            SH_C3_3 * 6.f * yz * w[12] - SH_C3_4 * 2.f * xy * w[13] - SH_C3_5 * 2.f * yz * w[14] - SH_C3_6 * 6.f * xy * w[15];
+    g[2] += SH_C3_1 * xy * w[10] + SH_C3_2 * 8.f * yz * w[11] + SH_C3_3 * (6.f * zz - 3.f * xx - 3.f * yy) * w[12] +
+            SH_C3_4 * 8.f * xz * w[13] + SH_C3_5 * (xx - yy) * w[14];
+  }
+}
+
 // ray direction of padded pixel (ix, iy): gaussian.cu:849-860
 template <int K>
 __device__ __forceinline__ void pixel_sh(int ix, int iy, const float* __restrict__ rays_o,

@@ -137,6 +137,10 @@ global_culling = _GlobalCulling.apply
 # additive: the whole frame as one autograd node (fused path)
 # ----------------------------------------------------------------------------------------
 SCALE_ACTIVATIONS = {"abs": 0, "exp": 1}
+# where SH colour is evaluated (RenderContext.set_sh_eval; the mode travels with the context, so the render_frame*
+# functions take no argument for it): "pixel" = per pixel ray (the reference), "gaussian" = once per Gaussian along
+# the camera-centre -> mean direction, then blended as an RGB colour
+SH_EVAL = {"pixel": gaussian.SH_EVAL_PIXEL, "gaussian": gaussian.SH_EVAL_GAUSSIAN}
 
 
 _flat_grad_allocator = None

@@ -27,7 +27,7 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import render_frame, render_frame_aux, render_frame_final
+from renderer import SH_EVAL, render_frame, render_frame_aux, render_frame_final
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -119,7 +119,8 @@ class Splatter(nn.Module):
                  use_sh_coeff=False, render_weight_normalize=False, opa_init_value=0.1, scale_init_value=0.02,
                  tile_culling_method="prob2", tile_culling_dist_thresh=0.5, tile_culling_prob_thresh=0.1,
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
-                 fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None):
+                 fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
+                 sh_eval="pixel"):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -127,7 +128,12 @@ class Splatter(nn.Module):
         Options that selected slower variants of the same maths in the reference are accepted and
         ignored (`jacobian_calc`, `cudaculling`, `fast_drawing`, `debug`, `debug_align`); options
         whose result would differ are refused (`render_weight_normalize`, tile culling methods other
-        than "prob2", which is train.py's default, train.py:311)."""
+        than "prob2", which is train.py's default, train.py:311).
+
+        `sh_eval` (SH colour only): "pixel" evaluates the SH basis per pixel ray, as the reference does;
+        "gaussian" evaluates it once per Gaussian along the direction from the camera centre to its mean and
+        blends the result as an RGB colour (the usual 3D Gaussian Splatting model, and a much cheaper frame).
+        The two modes use the same coefficient tensor but render it differently."""
         super().__init__()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
@@ -135,6 +141,11 @@ class Splatter(nn.Module):
         if tile_culling_method != "prob2":
             raise NotImplementedError("the fused path implements tile_culling_method='prob2' (train.py's default); "
                                       "methods 'dist' / 'prob' are available through gaussian.calc_tile_list")
+        if sh_eval not in SH_EVAL:
+            raise ValueError(f"sh_eval must be one of {sorted(SH_EVAL)}, not {sh_eval!r}")
+        if sh_eval == "gaussian" and not use_sh_coeff:
+            raise ValueError("sh_eval='gaussian' needs SH colour (use_sh_coeff=True)")
+        self.sh_eval = sh_eval
         self.use_sh_coeff = bool(use_sh_coeff)
         self.near = near
         self.render_downsample = render_downsample
@@ -161,6 +172,7 @@ class Splatter(nn.Module):
                                          for k in ("pos", "rgb", "opa", "quat", "scale")))
         with torch.cuda.device(self.device):                      # the context lives on self.device, not on the current one
             self._rctx = gaussian.RenderContext()
+        self._rctx.set_sh_eval(SH_EVAL[sh_eval])                   # every frame of this Splatter, fused or not
         self.ground_truth = None
         self.culling_mask = None
         self.n_tile_gaussians = 0

@@ -1,0 +1,117 @@
+"""Cost of SH colour evaluated once per Gaussian against per-pixel SH and RGB on the C3 frame (2.4 M Gaussians, 1080p).
+
+Times forward + backward of one frame (render_frame_final) for five variants, alternated in one process so that they
+share the card's state: RGB (D = 3, the floor), and for D = 27 and 48 the per-pixel SH frame (default kernels) and the
+per-Gaussian SH frame (RenderContext.set_sh_eval).  All variants use the same geometry.  Afterwards it reads the
+per-stage device times of each variant (CUDA events, a separate pass): projection forward / backward and blend
+forward / backward.  Prints the card name and power limit read in the same run, then one JSON line.
+
+  python examples/bench_sh_eval.py [--steps 20] [--rounds 5]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "3d-gaussian-splatting_b200"))
+
+import renderer  # noqa: E402
+import synthetic as S  # noqa: E402
+import gaussian  # noqa: E402
+
+NAMES = ("pos", "rgb", "opa", "quat", "scale")
+# gs_frame_stage_ms indices
+STAGES = {"project_fwd": 0, "blend_fwd": 5, "blend_bwd": 6, "project_bwd": 7}
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, limit = (s.strip() for s in out.split(","))
+    except Exception:  # noqa: BLE001 - report what torch knows
+        name, limit = torch.cuda.get_device_name(0), "unknown"
+    return name, limit
+
+
+def median(ts):
+    return sorted(ts)[len(ts) // 2]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=5)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("needs a CUDA device")
+    name, limit = card()
+    dev = torch.device("cuda", 0)
+    n, w, h = 2_400_000, 1920, 1080
+    v = S.make_view(w, h, 0)
+    cam = (w, h, v.fx, v.fy, v.rot, v.tran, v.near, 0.05, "abs")
+    go = ((torch.rand(h, w, 3, generator=torch.Generator().manual_seed(1)) * 2 - 1) / (h * w)).to(dev)
+
+    variants = {}
+    for label, d, mode in (("rgb", 3, "pixel"), ("sh27_pixel", 27, "pixel"), ("sh27_gaussian", 27, "gaussian"),
+                           ("sh48_pixel", 48, "pixel"), ("sh48_gaussian", 48, "gaussian")):
+        # the generator draws colours last: every variant has the same geometry
+        params = {k: t.to(dev).requires_grad_(True) for k, t in S.make_gaussians(n, w, h, 0, sh_dim=d).items()}
+        rctx = gaussian.RenderContext()
+        rctx.set_sh_eval(renderer.SH_EVAL[mode])
+        variants[label] = (rctx, params)
+
+    def frame(label):
+        rctx, params = variants[label]
+        for p in params.values():
+            p.grad = None
+        img, _ = renderer.render_frame_final(rctx, *(params[k] for k in NAMES), *cam)
+        img.backward(go)
+
+    for label in variants:                 # warm-up: module loads, workspace growth
+        for _ in range(3):
+            frame(label)
+    torch.cuda.synchronize()
+    times = {k: [] for k in variants}
+    for _ in range(args.rounds):
+        for label in variants:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.steps):
+                frame(label)
+            e1.record()
+            torch.cuda.synchronize()
+            times[label].append(e0.elapsed_time(e1) / args.steps)
+
+    stages = {k: {s: [] for s in STAGES} for k in variants}
+    for label, (rctx, _) in variants.items():
+        rctx.set_timing(True)
+    for _ in range(args.rounds):
+        for label, (rctx, _) in variants.items():
+            frame(label)
+            ms = rctx.stage_ms()
+            for s, i in STAGES.items():
+                stages[label][s].append(ms[i])
+
+    res = {"card": name, "power_limit": limit, "workload": "C3 forward+backward", "steps": args.steps,
+           "rounds": args.rounds}
+    for label in variants:
+        r = {"frame_ms_median": median(times[label]), "frame_ms_all": [round(t, 4) for t in times[label]]}
+        for s in STAGES:
+            r[f"{s}_ms_median"] = round(median(stages[label][s]), 4)
+        st = variants[label][0].stats()
+        r["n_instances"], r["n_instances_eff"] = st["n_instances"], st["n_instances_eff"]
+        res[label] = r
+    for d in (27, 48):
+        res[f"sh{d}_gaussian_over_rgb"] = res[f"sh{d}_gaussian"]["frame_ms_median"] / res["rgb"]["frame_ms_median"]
+        res[f"sh{d}_pixel_over_gaussian"] = res[f"sh{d}_pixel"]["frame_ms_median"] / res[f"sh{d}_gaussian"]["frame_ms_median"]
+    print(f"card: {name}, power limit {limit}")
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()

@@ -154,10 +154,11 @@ int gs_ctx_set_allocator(gs_ctx* ctx, gs_alloc_fn alloc, gs_free_fn free_fn, voi
 void gs_ctx_destroy(gs_ctx* ctx);          /* frees workspaces (synchronises the device)  */
 
 /* Raw parameters (splatter.py:399-406): pos[n,3], rgb[n,d] (logits if d==3, SH coefficients
- * channel-major [c*K+k] if d==27), opa[n] logits, quat[n,4] wxyz un-normalised, scale[n,3]
+ * channel-major [c*K+k] if d==27 (K = 9) or d==48 (K = 16)), opa[n] logits, quat[n,4] wxyz un-normalised, scale[n,3]
  * raw.  Writes image[Hp,Wp,3] (un-clamped, padded; black background) and, if non-NULL,
  * culling_mask[n] int64 (train.py:150).  Performs ONE host synchronisation on `stream`
- * (reads back the instance count M to size the sort). */
+ * (reads back the instance count M to size the sort).
+ * SH colour is evaluated as set by gs_ctx_set_sh_eval (below): per pixel ray by default. */
 int gs_render_forward(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa,
                       const float* quat, const float* scale, int n, int d, int scale_activation,
                       const gs_camera* cam_host, float* image, int64_t* culling_mask,
@@ -199,7 +200,8 @@ int gs_render_backward_final(gs_ctx* ctx, const float* pos, const float* rgb, co
  *   aux_final  : DEVICE [height,width,2] centre crop of aux (not clamped); needs image_final.
  * Implemented for RGB and SH colour on the default (gather) path with the shipped kernels; the packed path
  * (gs_tune("gather", 0)), the two-pixel tensor-core SH backward (sh_tc bit 2) and non-default RGB blend knobs
- * return GS_ERR_UNSUPPORTED when a map or a background is requested.  Same synchronisation and launch count as gs_render_forward_final; no workspace is allocated for
+ * return GS_ERR_UNSUPPORTED when a map or a background is requested.  SH colour evaluated per Gaussian
+ * (gs_ctx_set_sh_eval) blends on the RGB kernels and follows the RGB rules here.  Same synchronisation and launch count as gs_render_forward_final; no workspace is allocated for
  * the maps (the buffers are the caller's). */
 typedef struct gs_render_aux {
   const float* background;
@@ -221,6 +223,23 @@ int gs_render_backward_aux(gs_ctx* ctx, const float* pos, const float* rgb, cons
                            const float* grad_image, int grad_is_final, const float* aux, const float* grad_aux,
                            float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
                            gs_stream_t stream);
+
+/* Where the SH colour (d == 27 / 48) is evaluated.  Two colour MODELS, not two speeds of one: the same coefficients
+ * render differently.
+ *   GS_SH_EVAL_PIXEL    (default; the reference): the basis is evaluated per pixel, along the pixel's world-space ray,
+ *                       inside the blend:  c_c(pixel) = sigmoid( sum_k Y_k(ray dir) rgb[c*K+k] ).
+ *   GS_SH_EVAL_GAUSSIAN (the usual 3D Gaussian Splatting model): once per Gaussian, along the world-space direction
+ *                       from the camera centre C = -R^T t to the mean, dir = (pos - C) / |pos - C|, in the projection;
+ *                       c_c = sigmoid( sum_k Y_k(dir) rgb[c*K+k] ) then blends like an RGB colour.  The backward
+ *                       includes the direction term: dL/dpos gains (I - dir dir^T) / |pos - C| dL/ddir.
+ * The setting belongs to the context and applies to the forwards that follow; a backward always uses the mode of its
+ * forward.  Frames with d == 3 ignore it.  In per-Gaussian mode the frame runs the RGB blend kernels, so the aux
+ * calls (depth / alpha / background) and the packed path (gs_tune("gather", 0)) behave as for RGB, the per-pixel SH
+ * knobs (gs_tune("sh_tc", ...)) do not apply, and the gradients keep the parameter layout grad_rgb[n,d].
+ * Null ctx or an unknown mode: GS_ERR_INVALID_ARG. */
+#define GS_SH_EVAL_PIXEL 0
+#define GS_SH_EVAL_GAUSSIAN 1
+int gs_ctx_set_sh_eval(gs_ctx* ctx, int mode);
 
 /* Per-stage device timing with CUDA events recorded on the frame's stream (off by default).
  * gs_frame_stage_ms fills out[GS_N_STAGES] with the milliseconds of the last frame's stages:

@@ -473,6 +473,57 @@ struct RenderContext {
              "gs_render_backward_aux");
   }
 
+  // backward_aux_into plus the camera gradient grad_cam[12] = (dL/drot row-major, dL/dtran) of the forward's camera
+  // (gs_render_backward_cam); the five parameter gradients all None: camera only.  aux = None: the forward wrote no
+  // maps (forward / forward_final; then grad_aux must be None too)
+  void backward_cam_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                         torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_image, bool grad_is_final,
+                         std::optional<torch::Tensor> aux, std::optional<torch::Tensor> grad_aux,
+                         std::optional<torch::Tensor> g_pos, std::optional<torch::Tensor> g_rgb,
+                         std::optional<torch::Tensor> g_opa, std::optional<torch::Tensor> g_quat,
+                         std::optional<torch::Tensor> g_scale, torch::Tensor grad_cam, int64_t expected_frame) {
+    check_frame(expected_frame, "RenderContext.backward_cam_into");
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    GS_CHECK_F32(raw); GS_CHECK_F32(grad_cam);
+    TORCH_CHECK(grad_cam.numel() == 12 && grad_cam.device() == pos.device(),
+                "RenderContext.backward_cam_into: grad_cam must be 12 floats on the parameters' device");
+    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3, "RenderContext.backward_cam_into: raw must be [Hp,Wp,3]");
+    if (aux) {
+      GS_CHECK_F32(*aux);
+      TORCH_CHECK(aux->dim() == 3 && aux->size(0) == raw.size(0) && aux->size(1) == raw.size(1) && aux->size(2) == 2,
+                  "RenderContext.backward_cam_into: aux must be [Hp,Wp,2]");
+    }
+    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
+                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
+                "RenderContext.backward_cam_into: grad_image must be [H,W,3] (final) or match raw");
+    if (grad_aux) {
+      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
+                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
+                      grad_aux->size(2) == 2,
+                  "RenderContext.backward_cam_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
+    }
+    const int n_given = (int)g_pos.has_value() + g_rgb.has_value() + g_opa.has_value() + g_quat.has_value() +
+                        g_scale.has_value();
+    TORCH_CHECK(n_given == 0 || n_given == 5,
+                "RenderContext.backward_cam_into: give all five parameter gradients or none (camera only)");
+    if (n_given) {
+      GS_CHECK_F32(*g_pos); GS_CHECK_F32(*g_rgb); GS_CHECK_F32(*g_opa); GS_CHECK_F32(*g_quat); GS_CHECK_F32(*g_scale);
+      TORCH_CHECK(g_pos->numel() == pos.numel() && g_rgb->numel() == rgb.numel() && g_opa->numel() == opa.numel() &&
+                      g_quat->numel() == quat.numel() && g_scale->numel() == scale.numel(),
+                  "RenderContext.backward_cam_into: gradient buffers must match their parameters");
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat->data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+    }
+    auto opt = [](std::optional<torch::Tensor>& t) { return t ? fpm(*t) : nullptr; };
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor ga;
+    if (grad_aux) ga = grad_aux->contiguous();
+    check_rc(gs_render_backward_cam(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
+                                    grad_is_final ? 1 : 0, aux ? fp(*aux) : nullptr, grad_aux ? fp(ga) : nullptr, opt(g_pos),
+                                    opt(g_rgb), opt(g_opa), opt(g_quat), opt(g_scale), fpm(grad_cam), cur_stream()),
+             "gs_render_backward_cam");
+  }
+
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
   py::dict stats() {
@@ -683,6 +734,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
            py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
            py::arg("g_quat"), py::arg("g_scale"), py::arg("expected_frame") = -1)
+      .def("backward_cam_into", &RenderContext::backward_cam_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
+           py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
+           py::arg("g_quat"), py::arg("g_scale"), py::arg("grad_cam"), py::arg("expected_frame") = -1)
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
       .def("stats", &RenderContext::stats)

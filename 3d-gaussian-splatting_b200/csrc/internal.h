@@ -149,6 +149,18 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
                                         bool depth_grad = false /*rows carry dL/d|p_c| in the column after the colour*/,
                                         bool sh_gaussian = false /*d = 27 / 48 coefficients, RGB gradient rows*/);
+// The same without a push, for RGB and per-Gaussian SH, plus the camera gradient: the projection backward leaves one
+// 12-float partial sum per CTA in cam_part (gs_cam_grad_workspace_bytes(n)), and a one-CTA kernel sums them in fp64
+// into grad_cam[12] = {dL/drot row-major, dL/dtran} (zeros when n == 0).  The five gradient pointers may all be NULL
+// (camera only).  Two launches (one when n == 0).
+size_t gs_cam_grad_workspace_bytes(int n);
+cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                            const float* scale, int n, int d, int scale_act, const GsCam& cam,
+                                            float near_plane, float half_w, float half_h, const uint32_t* offsets_g,
+                                            const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
+                                            uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                            float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
+                                            bool depth_grad, bool sh_gaussian);
 
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,

@@ -204,7 +204,9 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
 // (GW = GS_GREC); the D = 3 KG coefficient gradients and the view-direction term are formed here.
 // (cam and push are taken by value, as the kernel parameters they are: by reference, the KG = 0 instantiations would
 // no longer compile to the code fused_project_bwd_kernel had before the body was shared.)
-template <int D, int GW, int W, bool DT, int KG>
+// CG (camera gradient, W = 0 only): also adds this Gaussian's share of dL/d(rot, tran) to cg[12] (gs_cam_grad_add plus
+// the view-direction term of per-Gaussian SH); with all five gradient pointers NULL no parameter gradient is stored.
+template <int D, int GW, int W, bool DT, int KG, bool CG = false>
 __device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
@@ -212,8 +214,9 @@ __device__ __forceinline__ void fused_project_bwd_body(
     const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
     const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
     float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
-    GsGradPush push) {
+    GsGradPush push, float* cg = nullptr) {
   static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
+  static_assert(!CG || (W == 0 && GW == GS_GREC), "camera gradient: RGB gradient rows, no push");
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   int i = blockIdx.x * kBlock + threadIdx.x;
   // SH colour on one GPU: the warp writes its coefficient gradients together (below), so threads past n stay
@@ -276,7 +279,13 @@ __device__ __forceinline__ void fused_project_bwd_body(
     static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
     float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
     float gq[4], gsv[3];
-    gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    if constexpr (CG) {
+      float gc[3], gjw[6];
+      gs_project_backward_cam(cam, p, q, s, gxyd, gcov, gp, gq, gsv, gc, gjw);
+      gs_cam_grad_add(cam, p, gc, gjw, cg);
+    } else {
+      gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    }
     if constexpr (KG > 0) {
       // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
       // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
@@ -299,6 +308,20 @@ __device__ __forceinline__ void fused_project_bwd_body(
       const float dd = dir[0] * gd[0] + dir[1] * gd[1] + dir[2] * gd[2];
 #pragma unroll
       for (int j = 0; j < 3; ++j) gp[j] += (gd[j] - dir[j] * dd) * il;
+      if constexpr (CG) {
+        // the direction leaves from u = pos + R^T t: g_u = il v (the term just added to gp) gives dL/dt += R g_u and
+        // dL/dR += t g_u^T.  il is applied last, so that no product v * il other than gp's exists: gp keeps the
+        // contraction it has in the kernels without CG, bit for bit.
+        float v[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) v[j] = gd[j] - dir[j] * dd;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+          for (int j = 0; j < 3; ++j) cg[3 * r + j] += (cam.t[r] * v[j]) * il;
+          cg[9 + r] += (cam.r[3 * r] * v[0] + cam.r[3 * r + 1] * v[1] + cam.r[3 * r + 2] * v[2]) * il;
+        }
+      }
     }
     // quat normalisation backward: q = r/|r|
     float dot = q[0] * gq[0] + q[1] * gq[1] + q[2] * gq[2] + q[3] * gq[3];
@@ -323,6 +346,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     }
   }
   const float* gcol = KG ? gsh : acc + 6;   // the D gradients of this Gaussian's rgb row
+  if (CG && !g_pos) return;                 // camera only (the pointers are all NULL or all set: uniform)
   if (W == 0) {
     if constexpr (kStagedRgb) {
       // The 32 Gaussians of a warp own 32 * D contiguous floats of g_rgb.  One strided 4-byte store per coefficient
@@ -396,7 +420,66 @@ template <int K, int W, bool DT>
 __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_kernel(GS_PBWD_PARAMS) {
   fused_project_bwd_body<3 * K, GS_GREC, W, DT, K>(GS_PBWD_ARGS);
 }
+
+// Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
+// 12-float shares in a fixed order (butterfly shuffles, then the 8 warp sums in warp order) into row blockIdx.x of
+// cam_part[gridDim.x][12]; cam_grad_finish_kernel adds the rows.  No atomics: the result is bit-deterministic.
+constexpr int kCamGrad = 12;
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part) {
+  float cg[kCamGrad];
+#pragma unroll
+  for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
+  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true>(GS_PBWD_ARGS, cg);
+  __shared__ float wsum[kBlock / 32][kCamGrad];
+#pragma unroll
+  for (int k = 0; k < kCamGrad; ++k) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) cg[k] += __shfl_xor_sync(0xffffffffu, cg[k], o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < kCamGrad; ++k) wsum[threadIdx.x >> 5][k] = cg[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < kCamGrad) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < kBlock / 32; ++w) s += wsum[w][threadIdx.x];
+    cam_part[(size_t)blockIdx.x * kCamGrad + threadIdx.x] = s;
+  }
+}
 #undef GS_PBWD_PARAMS
+
+// One CTA: grad_cam[k] = sum over the `rows` rows of cam_part[., k] in fp64, in a fixed order (strided per-thread sums,
+// butterfly shuffles, warp sums in warp order).  rows == 0 (no Gaussian) writes zeros.
+__global__ void __launch_bounds__(kBlock) cam_grad_finish_kernel(const float* __restrict__ cam_part, int rows,
+                                                                  float* __restrict__ grad_cam) {
+  double s[kCamGrad];
+#pragma unroll
+  for (int k = 0; k < kCamGrad; ++k) s[k] = 0.0;
+  for (int r = threadIdx.x; r < rows; r += kBlock) {
+#pragma unroll
+    for (int k = 0; k < kCamGrad; ++k) s[k] += (double)cam_part[(size_t)r * kCamGrad + k];
+  }
+  __shared__ double wsum[kBlock / 32][kCamGrad];
+#pragma unroll
+  for (int k = 0; k < kCamGrad; ++k) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < kCamGrad; ++k) wsum[threadIdx.x >> 5][k] = s[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < kCamGrad) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kBlock / 32; ++w) t += wsum[w][threadIdx.x];
+    grad_cam[threadIdx.x] = (float)t;
+  }
+}
 
 }  // namespace
 
@@ -607,6 +690,32 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
 #undef GS_LAUNCH_PBWD_SH
 #undef GS_LAUNCH_PBWD_W
 #undef GS_LAUNCH_PBWD
-#undef GS_PBWD_ARGS
   return cudaGetLastError();
 }
+
+size_t gs_cam_grad_workspace_bytes(int n) { return (size_t)grid_for(n) * kCamGrad * sizeof(float); }
+
+cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                            const float* scale, int n, int d, int scale_act, const GsCam& cam,
+                                            float near_plane, float half_w, float half_h, const uint32_t* offsets_g,
+                                            const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
+                                            uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                            float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
+                                            bool depth_grad, bool sh_gaussian) {
+  if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+  const GsGradPush push{};
+  if (n > 0) {
+#define GS_LAUNCH_PBWD_CAM(K, DT) \
+  fused_project_bwd_cam_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part)
+    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_CAM(9, true);
+    else if (d == 27) GS_LAUNCH_PBWD_CAM(9, false);
+    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_CAM(16, true);
+    else if (d == 48) GS_LAUNCH_PBWD_CAM(16, false);
+    else if (depth_grad) GS_LAUNCH_PBWD_CAM(0, true);
+    else GS_LAUNCH_PBWD_CAM(0, false);
+#undef GS_LAUNCH_PBWD_CAM
+  }
+  cam_grad_finish_kernel<<<1, kBlock, 0, st>>>(cam_part, n > 0 ? grid_for(n) : 0, grad_cam);
+  return cudaGetLastError();
+}
+#undef GS_PBWD_ARGS

@@ -136,6 +136,63 @@ __device__ __forceinline__ void gs_project_backward(const GsCam& cam, const floa
   gq[3] = 2.f * (-2.f * z * gR[0] - w * gR[1] + x * gR[2] + w * gR[3] - 2.f * z * gR[4] + y * gR[5] + x * gR[6] + y * gR[7]);
 }
 
+// gs_project_backward plus what the camera gradient needs: gc = dL/dp_c and gjw = dL/d(JW) for the two image-plane
+// rows of JW (row-major 2x3), h (RS)^T with h = (G2 + G2^T) M.  The parameter gradients are gs_project_backward's own
+// (the subexpressions repeated below are shared after inlining).
+__device__ __forceinline__ void gs_project_backward_cam(const GsCam& cam, const float p[3], const float q[4],
+                                                        const float s[3], const float g_xyd[3], const float g_cov[4],
+                                                        float gp[3], float gq[4], float gs[3], float gc[3],
+                                                        float gjw[6]) {
+  gs_project_backward(cam, p, q, s, g_xyd, g_cov, gp, gq, gs);
+  float pc[3];
+  gs_world_to_cam(cam, p, pc);
+  float r = sqrtf(pc[0] * pc[0] + pc[1] * pc[1] + pc[2] * pc[2]);
+  float iz = 1.f / pc[2];
+  float ir = 1.f / r;
+  gc[0] = g_xyd[0] * iz + g_xyd[2] * pc[0] * ir;
+  gc[1] = g_xyd[1] * iz + g_xyd[2] * pc[1] * ir;
+  gc[2] = -(g_xyd[0] * pc[0] + g_xyd[1] * pc[1]) * iz * iz + g_xyd[2] * pc[2] * ir;
+  float jw0[3], jw1[3];
+  gs_jw_rows(cam, pc, jw0, jw1);
+  GsRot R = gs_quat_to_rot(q[0], q[1], q[2], q[3]);
+  float m0[3], m1[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    m0[c] = (jw0[0] * R.m[0 * 3 + c] + jw0[1] * R.m[1 * 3 + c] + jw0[2] * R.m[2 * 3 + c]) * s[c];
+    m1[c] = (jw1[0] * R.m[0 * 3 + c] + jw1[1] * R.m[1 * 3 + c] + jw1[2] * R.m[2 * 3 + c]) * s[c];
+  }
+  float s00 = 2.f * g_cov[0], s01 = g_cov[1] + g_cov[2], s11 = 2.f * g_cov[3];
+  float h0[3], h1[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    h0[c] = s00 * m0[c] + s01 * m1[c];
+    h1[c] = s01 * m0[c] + s11 * m1[c];
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    gjw[k] = (h0[0] * R.m[k * 3 + 0] * s[0] + h0[1] * R.m[k * 3 + 1] * s[1]) + h0[2] * R.m[k * 3 + 2] * s[2];
+    gjw[3 + k] = (h1[0] * R.m[k * 3 + 0] * s[0] + h1[1] * R.m[k * 3 + 1] * s[1]) + h1[2] * R.m[k * 3 + 2] * s[2];
+  }
+}
+
+// One Gaussian's share of the camera gradient, added to cg[12] = {dL/dR row-major [9], dL/dt [3]} for p_c = R p + t:
+// dL/dt += gc, dL/dR += gc p^T + J2^T gjw, with J2 = d(x/z, y/z)/dp_c detached (as for pos) and W = R live in JW.
+__device__ __forceinline__ void gs_cam_grad_add(const GsCam& cam, const float p[3], const float gc[3],
+                                                const float gjw[6], float cg[12]) {
+  float pc[3];
+  gs_world_to_cam(cam, p, pc);
+  const float iz = 1.f / pc[2];
+  const float jx = -pc[0] / (pc[2] * pc[2]);
+  const float jy = -pc[1] / (pc[2] * pc[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    cg[k] += gc[0] * p[k] + iz * gjw[k];
+    cg[3 + k] += gc[1] * p[k] + iz * gjw[3 + k];
+    cg[6 + k] += gc[2] * p[k] + (jx * gjw[k] + jy * gjw[3 + k]);
+    cg[9 + k] += gc[k];
+  }
+}
+
 // Tile rectangle covered by a Gaussian, method 2 "prob2" (gaussian.cu:226-242): axis aligned
 // bbox of the `thresh` iso-probability ellipse; float->uint32 casts truncate / saturate.
 struct GsTileGrid {

@@ -137,6 +137,7 @@ struct gs_ctx {
   uint32_t epoch = 0;                      // tag of the current backward in row_epoch[]
   // per tile / misc
   DevBuf tile_accum, tile_neff, tile_neff_b, cub_tmp, counters, img_dev, gimg_dev, rays;
+  DevBuf cam_part;                        // per-CTA partial sums of the camera gradient (gs_render_backward_cam)
   float* host_rays = nullptr;             // pinned: rays_o, lefttop, dx, dy (SH colour only)
   unsigned long long* host_m = nullptr;   // pinned: {M}
   cudaEvent_t ev_m = nullptr;             // marks the completion of the M read-back
@@ -192,7 +193,7 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   cudaDeviceSynchronize();
   DevBuf* bufs[] = {&c->rec, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
-                    &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays};
+                    &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
@@ -506,12 +507,21 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                 const float* scale, const float* image, const float* grad_image, int grad_is_final,
                                 float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
                                 float* grad_scale, gs_stream_t stream, const float* aux = nullptr,
-                                const float* grad_aux = nullptr) {
+                                const float* grad_aux = nullptr, float* grad_cam = nullptr) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward: no forward on this ctx");
-  if (!image || !grad_image || !grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale ||
+  // camera only (grad_cam, the five parameter gradients all NULL: the caller has checked the set is not mixed)
+  const bool cam_only = grad_cam && !grad_pos;
+  if (!image || !grad_image || (!cam_only && (!grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale)) ||
       (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null tensor pointer");
+  if (grad_cam) {
+    if (c->d != 3 && !c->sh_gaussian)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_cam: SH colour evaluated per pixel has no camera "
+                                                  "gradient (use GS_SH_EVAL_GAUSSIAN)");
+    if (c->push.world)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_cam: not available with a gradient push configured");
+  }
   if (grad_aux) {
     if (!c->have_aux)
       return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux given but the forward wrote no aux");
@@ -576,12 +586,23 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
     if ((grad_quat - lo) % 4)
       return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: grad_quat must sit on a 16-byte bucket offset");
   }
-  GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
-                                          c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
-                                          c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
-                                          grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
-                                          grad_aux != nullptr, c->sh_gaussian));
-  if (c->n > 0) gs_count_launch();
+  if (grad_cam) {
+    GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
+    GS_CUDA_TRY(gs_launch_fused_project_bwd_cam(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam,
+                                                c->near_plane, c->half_w, c->half_h, c->offsets_g.as<uint32_t>(),
+                                                c->count.as<uint32_t>(), c->grad_inst.as<float>(),
+                                                c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
+                                                grad_quat, grad_scale, c->cam_part.as<float>(), grad_cam, st,
+                                                grad_aux != nullptr, c->sh_gaussian));
+    gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sum (always: grad_cam is always written)
+  } else {
+    GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
+                                            c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                            c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
+                                            grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
+                                            grad_aux != nullptr, c->sh_gaussian));
+    if (c->n > 0) gs_count_launch();
+  }
   gs_mark(c, 9, st);
   c->ev_bwd_valid = c->timing && c->ev_ok;
   return 0;
@@ -618,6 +639,21 @@ extern "C" int gs_render_backward_aux(gs_ctx* c, const float* pos, const float* 
                                       float* grad_quat, float* grad_scale, gs_stream_t stream) {
   return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
                               grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux);
+}
+
+extern "C" int gs_render_backward_cam(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                      const float* quat, const float* scale, const float* image_raw_padded,
+                                      const float* grad_image, int grad_is_final, const float* aux,
+                                      const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                      float* grad_quat, float* grad_scale, float* grad_cam, gs_stream_t stream) {
+  if (!grad_cam) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_cam: null grad_cam");
+  const int n_null = !grad_pos + !grad_rgb + !grad_opa + !grad_quat + !grad_scale;
+  if (n_null != 0 && n_null != 5)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG,
+                            "gs_render_backward_cam: the five parameter gradients must be all NULL or all non-NULL");
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_cam: null ctx");
+  return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
+                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, grad_cam);
 }
 
 extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {

@@ -306,3 +306,59 @@ def render_frame_aux(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, f
     colour on the default kernels."""
     return _RenderFrameAux.apply(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
                                  near, tile_thresh, scale_activation, background, final)
+
+
+class _RenderFrameCam(_RenderFrameAux):
+    """`_RenderFrameAux` whose backward also returns dL/drot and dL/dtran (gs_render_backward_cam)."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                near, tile_thresh, scale_activation, background, final):
+        cam = torch.cat([rot.detach().reshape(9), tran.detach().reshape(3)]).cpu()   # one 48-byte host read
+        return _RenderFrameAux.forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y,
+                                       cam[:9].view(3, 3), cam[9:], near, tile_thresh, scale_activation, background,
+                                       final)
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
+        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
+        if not (ctx.needs_input_grad[10] or ctx.needs_input_grad[11]):
+            return _RenderFrameAux.backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask)
+        rows, cols = ctx.map_shape
+        if grad_image is None:
+            grad_image = raw.new_zeros(rows, cols, 3)
+        grad_aux = None
+        if grad_depth is not None or grad_alpha is not None:
+            grad_aux = raw.new_zeros(rows, cols, 2)
+            if grad_depth is not None:
+                grad_aux[..., 0] = grad_depth
+            if grad_alpha is not None:
+                grad_aux[..., 1] = grad_alpha
+        grad_cam = raw.new_empty(12)
+        if any(ctx.needs_input_grad[1:6]):
+            outs, push = _flat_grads((pos, rgb, opa, quat, scale))
+        else:                                                  # tracking: the scene is frozen, camera only
+            outs, push = [None] * 5, None
+        _apply_push(ctx.rctx, push)
+        ctx.rctx.backward_cam_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
+                                   *outs, grad_cam, ctx.frame)
+        return ((None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 4 +
+                (grad_cam[:9].view(3, 3), grad_cam[9:]) + (None,) * 5)
+
+
+def render_frame_cam(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
+                     tile_thresh, scale_activation, background=None, final=True):
+    """`render_frame_aux` differentiable with respect to the camera too: -> (image, depth, alpha, culling_mask), and
+    the backward returns dL/drot and dL/dtran for p_c = rot p + tran (rot used as given, not re-orthonormalised;
+    map them to your own pose parameterisation in torch).  rot [3,3] and tran [3] must be float32 CUDA tensors on the
+    parameters' device (ValueError otherwise); reading them for the forward costs one extra host synchronisation
+    (12 floats).  When none of the five parameters needs a gradient the backward is camera only (pose tracking
+    against a frozen scene).  RGB and per-Gaussian SH colour (RenderContext.set_sh_eval(SH_EVAL["gaussian"]));
+    a per-pixel SH frame or a data-parallel gradient push is refused by the backward (RuntimeError)."""
+    for name, t, shape in (("rot", rot, (3, 3)), ("tran", tran, (3,))):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or tuple(t.shape) != shape:
+            raise ValueError(f"render_frame_cam: {name} must be a float32 CUDA tensor of shape {list(shape)}")
+        if t.device != pos.device:
+            raise ValueError(f"render_frame_cam: {name} is on {t.device}, the parameters on {pos.device}")
+    return _RenderFrameCam.apply(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                                 near, tile_thresh, scale_activation, background, final)

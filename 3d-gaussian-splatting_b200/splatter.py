@@ -27,7 +27,7 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import SH_EVAL, render_frame, render_frame_aux, render_frame_final
+from renderer import SH_EVAL, render_frame, render_frame_aux, render_frame_cam, render_frame_final
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -304,6 +304,27 @@ class Splatter(nn.Module):
         image, depth, alpha, mask = render_frame_aux(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], v["rot"], v["tran"],
                                                      self.near, self.tile_culling_prob_thresh, self.scale_activation,
+                                                     background=background, final=True)
+        self.culling_mask = mask
+        self.n_gaussians = g.pos.shape[0]
+        self.n_tile_gaussians = self._rctx.last_instances()
+        return dict(image=image, depth=depth, alpha=alpha)
+
+    def render_at_pose(self, rot, tran, camera_id=None, background=None):
+        """`render_maps` at a caller-supplied pose, differentiable with respect to it: rot [3,3] and tran [3] are
+        float32 CUDA tensors (world -> camera, p_c = rot p + tran), typically a learnable correction composed with a
+        view's pose in torch (pose refinement) or a pose being tracked against the frozen scene.  The intrinsics and
+        `ground_truth` come from view `camera_id` (default: the current view).  Returns dict(image, depth, alpha) like
+        `render_maps`; backward gives rot and tran their gradients (`renderer.render_frame_cam`), and runs camera
+        only when no scene parameter needs a gradient.  Costs one extra host synchronisation (the 12 pose floats)."""
+        if camera_id is not None:
+            self.set_camera(camera_id)
+        if self.current_view is None:
+            raise ValueError("render_at_pose: no current view; pass camera_id")
+        g, v = self.gaussian_3ds, self.current_view
+        image, depth, alpha, mask = render_frame_cam(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
+                                                     v["height"], v["focal_x"], v["focal_y"], rot, tran, self.near,
+                                                     self.tile_culling_prob_thresh, self.scale_activation,
                                                      background=background, final=True)
         self.culling_mask = mask
         self.n_gaussians = g.pos.shape[0]

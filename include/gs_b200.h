@@ -224,6 +224,23 @@ int gs_render_backward_aux(gs_ctx* ctx, const float* pos, const float* rgb, cons
                            float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
                            gs_stream_t stream);
 
+/* gs_render_backward_aux plus the gradient with respect to the camera of the last forward, p_c = rot p + tran (rot
+ * used as given, not re-orthonormalised): grad_cam (DEVICE float[12]) receives dL/drot row-major [9], then dL/dtran [3].
+ * It follows the semantics of pos: the projection Jacobian is constant, rot stays live in the 2-D covariance
+ * (J rot) Sigma (J rot)^T, culling / tile rectangles / sort order have no gradient; depth gradients (grad_aux) and the
+ * view direction of per-Gaussian SH (GS_SH_EVAL_GAUSSIAN) reach the pose too.  The five parameter gradients are all
+ * NULL (camera only: nothing else is written) or all non-NULL (then equal to gs_render_backward_aux's); a mix, a NULL
+ * grad_cam or ctx is GS_ERR_INVALID_ARG.  grad_cam is always written (zeros for an empty or fully culled frame) and
+ * is bit-deterministic (fixed-order sums, fp64 across CTAs; no atomics).  RGB and per-Gaussian SH frames only: a
+ * per-pixel SH frame, or a context with a gradient push configured, is GS_ERR_UNSUPPORTED.  One more launch than
+ * gs_render_backward_aux; no synchronisation; a workspace of 48 bytes per 256 Gaussians is kept by the context. */
+int gs_render_backward_cam(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                           const float* scale, const float* image_raw_padded, const float* grad_image,
+                           int grad_is_final, const float* aux, const float* grad_aux,
+                           float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
+                           float* grad_cam /* DEVICE [12]: dL/drot row-major [9], then dL/dtran [3] */,
+                           gs_stream_t stream);
+
 /* Where the SH colour (d == 27 / 48) is evaluated.  Two colour MODELS, not two speeds of one: the same coefficients
  * render differently.
  *   GS_SH_EVAL_PIXEL    (default; the reference): the basis is evaluated per pixel, along the pixel's world-space ray,
@@ -245,7 +262,8 @@ int gs_ctx_set_sh_eval(gs_ctx* ctx, int mode);
  * gs_frame_stage_ms fills out[GS_N_STAGES] with the milliseconds of the last frame's stages:
  * 0 project, 1 depth sort of Gaussians + scan + M readback, 2 key emit, 3 tile-id radix sort,
  * 4 range + pack, 5 blend forward,
- * 6 blend backward, 7 project backward (-1 where not available).  Synchronises `stream`. */
+ * 6 blend backward, 7 project backward (with gs_render_backward_cam: both camera-gradient kernels)
+ * (-1 where not available).  Synchronises `stream`. */
 #define GS_N_STAGES 8
 int gs_ctx_set_timing(gs_ctx* ctx, int enable);
 int gs_frame_stage_ms(gs_ctx* ctx, float* out_host, gs_stream_t stream);

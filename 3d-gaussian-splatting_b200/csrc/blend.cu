@@ -766,8 +766,9 @@ struct Bwd2SmemAux : Bwd2Smem<PX, STAGES, RQ, GATHER, CH> {
 };
 
 // one instance x this thread's row of PX pixels: recompute alpha, analytic d/d alpha, six partial sums
-// (AUX: gc and R carry the depth / alpha terms, and d_t = sum g_D w goes to *dst_t)
-template <int PX, bool AUX = false>
+// (AUX: gc and R carry the depth / alpha terms, and d_t = sum g_D w goes to *dst_t).  Only the first NP slots are
+// evaluated (after a live-pixel repack the others are empty).
+template <int PX, bool AUX = false, int NP = PX>
 __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const float4 c, const float (&px)[PX],
                                         const float py, float (&T)[PX], float (&Rr)[PX], const float (&gr)[PX],
                                         const float (&gg)[PX], const float (&gb)[PX], float2* __restrict__ dst,
@@ -778,7 +779,7 @@ __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const fl
   const float m1 = a.w * dy;
   const float ev = fmaf(-b.x * dy, dy, b.y);
 #pragma unroll
-  for (int p = 0; p < PX; ++p) {
+  for (int p = 0; p < NP; ++p) {
     const float dx = px[p] - a.x;
     const float eu = fmaf(a.z, dx, -m1);
     float alpha = gs_ex2(fmaf(-dx, eu, ev));                     // l2o - (ca dx^2 - cb dx dy + cc dy^2)
@@ -806,12 +807,130 @@ __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const fl
   if constexpr (AUX) *dst_t = dt;
 }
 
+// ---- live-pixel repack (one consumer warp) --------------------------------------------------------------------
+// The warp stops only when all 256 pixels of the tile are saturated; until then a saturated pixel still costs a full
+// (pixel, instance) evaluation whose result is discarded.  At a reduction-round boundary the warp may therefore move
+// the live pixels into fewer slots per lane: it halves the slot count S (8 -> 4 -> 2 -> 1) while the sum over rows of
+// ceil(live_r / S) stays <= 32, and deals each row's live pixels to ceil(live_r / S) lanes of their own.  (Only
+// halving: the phase-1 loop is compiled once per S, and on the H100 the extra loops for S = 6 and 3 cost more in
+// code size than the pairs they save.)  Every lane still holds pixels of ONE row, so dy and its factors stay per lane and bwd_row is unchanged;
+// only the pixel-to-lane assignment (the order of the cross-pixel sums) changes.  The rule reads T only, so the plain
+// and the AUX kernel repack alike.  Empty slots have T = 0 and zero upstream gradient: they contribute exact zeros.
+// The repack adds no shared memory (the kernel's CTAs per SM are limited by it): everything it stages lives in the
+// partial buffer, which is free between rounds, and the lanes' row y (read by the reducers) sits in the unused tail
+// of each part of instance slot 0: lane l at bwd_lane_y<SQ, QS>(l), never written by phase 1.
+template <int SQ, int QS>
+__device__ __forceinline__ int bwd_lane_y(int l) {
+  static_assert(QS - SQ * 6 >= SQ, "a part has room for its source lanes' row y");
+  return (l / SQ) * QS + SQ * 6 + l % SQ;
+}
+
+// S: current slot count (warp-uniform, only shrinks); prow / py: this lane's pixel row (GS_TILE: none) and its y.
+// Called after phase 2 of a round, when the partial buffer `st` is free.  Layout of st during the call: planes of 256
+// floats per pixel state variable at 0 .. 8 * 256, then the transient tables below.
+constexpr int RP_ROWLIVE = 2048, RP_SRC = RP_ROWLIVE + GS_TILE, RP_CNT = RP_SRC + 32, RP_ROW = RP_CNT + 32,
+              RP_PY = RP_ROW + 32, RP_END = RP_PY + 32;
+template <int PX, bool AUX, int SQ, int QS>
+__device__ __forceinline__ void bwd_repack(float* __restrict__ st, const float* __restrict__ pyt, int lane, int& S,
+                                           int& prow, float& py, float (&px)[PX], float (&T)[PX], float (&Rr)[PX],
+                                           float (&gr)[PX], float (&gg)[PX], float (&gb)[PX], float (&gD)[PX],
+                                           float (&gA)[PX]) {
+  int* const rowlive = reinterpret_cast<int*>(st + RP_ROWLIVE);
+  int* const lsrc = reinterpret_cast<int*>(st + RP_SRC);
+  int* const lcnt = reinterpret_cast<int*>(st + RP_CNT);
+  int* const lrow = reinterpret_cast<int*>(st + RP_ROW);
+  float* const lpy = st + RP_PY;
+  int c = 0;
+#pragma unroll
+  for (int p = 0; p < PX; ++p) c += T[p] > GS_T_STOP ? 1 : 0;
+  if (__reduce_add_sync(0xffffffffu, c) > 16 * S) return;     // cannot fit into S / 2 slots per lane yet   // cannot fit into fewer slots per lane yet
+  if (lane < GS_TILE) rowlive[lane] = 0;
+  __syncwarp();
+  if (c) atomicAdd(&rowlive[prow], c);
+  __syncwarp();
+  const int live = lane < GS_TILE ? rowlive[lane] : 0;          // lane r < 16: live pixels of row r
+  // lanes needed is non-increasing in S: halve while the rows still fit into 32 lanes
+  int ns = S;
+  while (ns > 1 && __reduce_add_sync(0xffffffffu, (live + ns / 2 - 1) / (ns / 2)) <= 32) ns /= 2;
+  if (ns == S) return;
+
+  // lanes hold their rows in row order, so the exclusive prefix of c over lanes is each lane's first position in the
+  // row-major list of live pixels; stage them there, one plane of 256 per state variable
+  int incl = c;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  int pos = incl - c;
+#pragma unroll
+  for (int p = 0; p < PX; ++p)
+    if (T[p] > GS_T_STOP) {
+      st[pos] = px[p];
+      st[256 + pos] = T[p];
+      st[512 + pos] = Rr[p];
+      st[768 + pos] = gr[p];
+      st[1024 + pos] = gg[p];
+      st[1280 + pos] = gb[p];
+      if constexpr (AUX) {
+        st[1536 + pos] = gD[p];
+        st[1792 + pos] = gA[p];
+      }
+      ++pos;
+    }
+  lsrc[lane] = 0;
+  lcnt[lane] = 0;
+  lrow[lane] = GS_TILE;
+  lpy[lane] = 0.f;
+  // lane r < 16: row r gets lanes [lane0, lane0 + nl), its pixels start at list position px0 (one packed scan)
+  const int nl = (live + ns - 1) / ns;
+  int sc = (nl << 16) | live;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, sc, o);
+    if (lane >= o) sc += t;
+  }
+  sc -= (nl << 16) | live;
+  __syncwarp();
+  for (int q = 0; q < nl; ++q) {
+    const int l = (sc >> 16) + q;
+    lsrc[l] = (sc & 0xffff) + q * ns;
+    lcnt[l] = min(ns, live - q * ns);
+    lrow[l] = lane;
+    lpy[l] = pyt[lane];
+  }
+  __syncwarp();
+  const int src = lsrc[lane], n = lcnt[lane];
+  prow = lrow[lane];
+  py = lpy[lane];
+#pragma unroll
+  for (int p = 0; p < PX; ++p) {
+    const bool v = p < n;
+    px[p] = v ? st[src + p] : 0.f;
+    T[p] = v ? st[256 + src + p] : 0.f;
+    Rr[p] = v ? st[512 + src + p] : 0.f;
+    gr[p] = v ? st[768 + src + p] : 0.f;
+    gg[p] = v ? st[1024 + src + p] : 0.f;
+    gb[p] = v ? st[1280 + src + p] : 0.f;
+    if constexpr (AUX) {
+      gD[p] = v ? st[1536 + src + p] : 0.f;
+      gA[p] = v ? st[1792 + src + p] : 0.f;
+    }
+  }
+  __syncwarp();                   // every lane has read the planes: publish the row y over them for the reducers
+  st[bwd_lane_y<SQ, QS>(lane)] = py;   // (phase 2 reads it after the warp barrier that ends phase 1)
+  S = ns;
+}
+
 // WS: dedicated producer warp (full / empty mbarrier ring); !WS: consumer thread 0 issues the copies at the
 // chunk boundaries (no extra warp holding registers).  UNR: instances per unrolled step of the first phase.
 // AUX (gather only): the upstream gradient also has (g_D, g_A) per pixel (grad_aux, padded or cropped like
 // grad_image); gc and R gain g_D t + g_A and g_D depth + g_A alpha (depth / alpha from the forward's aux), and
 // the 7th sum d_t = sum g_D w lands in column 6 + 3 of the gradient row.
-template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false>
+// REPACK (one consumer warp): live-pixel repack at round boundaries (bwd_repack); until the first repack the kernel
+// computes exactly what it computes without it.
+template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false,
+          bool REPACK = false>
 __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     blend_bwd2_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB, const float4* __restrict__ pC,
                       const GsRec* __restrict__ grec, const uint32_t* __restrict__ ids,
@@ -826,6 +945,8 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   static_assert(!(WS && GATHER), "the gather path issues its copies from all consumer threads");
   static_assert(GATHER || CH == WS_CH, "the packed ring is sized for CH instances per stage");
   static_assert(!AUX || GATHER, "the aux terms read |p_c| from the gathered records");
+  static_assert(!REPACK || (NT == 32 && PX == 8), "the repack deals one warp's 256 pixels into slots of at most 8");
+  static_assert(!REPACK || R * IS >= RP_END, "the partial buffer holds the repack's planes and tables");
   using Smem = typename std::conditional<AUX, Bwd2SmemAux<PX, STAGES, RQ, GATHER, CH>,
                                          Bwd2Smem<PX, STAGES, RQ, GATHER, CH>>::type;
   __shared__ __align__(16) Smem sm;
@@ -869,7 +990,8 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   float px[PX];
 #pragma unroll
   for (int p = 0; p < PX; ++p) px[p] = gs_pixel_coord(ix0 + p, wp, fx);
-  const float py = sm.pyt[tid / TPR];
+  float py = sm.pyt[tid / TPR];
+  int S = PX, prow = tid / TPR;   // REPACK: slots per lane in use, and this lane's pixel row
 
   float T[PX], Rr[PX], gr[PX], gg[PX], gb[PX];
   {
@@ -964,38 +1086,57 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
 
     for (int sub = 0; sub < n; sub += R) {
       const int nr = min(R, n - sub);
-      // ---- phase 1: per-thread partial sums of up to R instances
-      int j = 0;
-      bool wdead = false;
-      for (; j + UNR <= nr; j += UNR) {
-        if (UNR >= 4 || (j & 3) == 0) {
-          bool dead = true;
+      // ---- phase 1: per-thread partial sums of up to R instances (NP: slots per lane in use)
+      // (the repacked loops are not unrolled over instances: unrolling them grows the kernel's code and was measured
+      // slower on the H100 - by ~30 % with 4 instances per step, ~15 % with 2)
+      auto phase1 = [&](auto np) -> int {
+        constexpr int NP = decltype(np)::value, U = NP == PX ? UNR : 1;
+        int j = 0;
+        bool wdead = false;
+#pragma unroll 1
+        for (; j + U <= nr; j += U) {
+          if (U >= 4 || (j & 3) == 0) {
+            bool dead = true;
 #pragma unroll
-          for (int p = 0; p < PX; ++p) dead = dead && !(T[p] > GS_T_STOP);
-          if (__all_sync(0xffffffffu, dead)) {
-            wdead = true;
-            break;
+            for (int p = 0; p < PX; ++p) dead = dead && !(T[p] > GS_T_STOP);
+            if (__all_sync(0xffffffffu, dead)) {
+              wdead = true;
+              break;
+            }
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            if constexpr (AUX)
+              bwd_row<PX, true, NP>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg,
+                                    gb, my_part + (j + u) * (IS / 2), sv.depth(sub + j + u), &gD, &gA,
+                                    my_part_t + (j + u) * Smem::TIS);
+            else
+              bwd_row<PX, false, NP>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg,
+                                     gb, my_part + (j + u) * (IS / 2));
           }
         }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          if constexpr (AUX)
-            bwd_row<PX, true>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg, gb,
-                              my_part + (j + u) * (IS / 2), sv.depth(sub + j + u), &gD, &gA,
-                              my_part_t + (j + u) * Smem::TIS);
-          else
-            bwd_row<PX>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg, gb,
-                        my_part + (j + u) * (IS / 2));
+        if (U > 1 && !wdead)
+          for (; j < nr; ++j) {
+            if constexpr (AUX)
+              bwd_row<PX, true, NP>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
+                                    my_part + j * (IS / 2), sv.depth(sub + j), &gD, &gA, my_part_t + j * Smem::TIS);
+            else
+              bwd_row<PX, false, NP>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
+                                     my_part + j * (IS / 2));
+          }
+        return j;
+      };
+      int j;
+      if constexpr (REPACK) {
+        switch (S) {   // warp-uniform
+          case 8: j = phase1(std::integral_constant<int, 8>{}); break;
+          case 4: j = phase1(std::integral_constant<int, 4>{}); break;
+          case 2: j = phase1(std::integral_constant<int, 2>{}); break;
+          default: j = phase1(std::integral_constant<int, 1>{}); break;
         }
+      } else {
+        j = phase1(std::integral_constant<int, PX>{});
       }
-      if (UNR > 1 && !wdead)
-        for (; j < nr; ++j) {
-          if constexpr (AUX)
-            bwd_row<PX, true>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
-                              my_part + j * (IS / 2), sv.depth(sub + j), &gD, &gA, my_part_t + j * Smem::TIS);
-          else
-            bwd_row<PX>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb, my_part + j * (IS / 2));
-        }
       bool dead = true;
 #pragma unroll
       for (int p = 0; p < PX; ++p) dead = dead && !(T[p] > GS_T_STOP);
@@ -1022,7 +1163,24 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
           b = sv.b(sub + ri);
         }
         const int vq = (NT == 64 && rq * SQ >= 32) ? v1 : v0;   // instances the part's source warp really processed
-        if (act && ri < vq) {
+        if (REPACK && act && ri < vq && S < PX) {
+          // repacked: the source lanes' rows are in the lane table, dy is formed per source lane
+#pragma unroll
+          for (int s = 0; s < SQ; ++s) {
+            const float2 w0 = red_src[s * 3], w1 = red_src[s * 3 + 1], w2 = red_src[s * 3 + 2];
+            float dyl = 0.f;
+            if constexpr (REPACK) dyl = sm.part[bwd_lane_y<SQ, QS>(rq * SQ + s)] - a.y;
+            S0 += w0.x;
+            Sx += w0.y;
+            Sxx += w1.x;
+            C0 += w1.y;
+            C1 += w2.x;
+            C2 += w2.y;
+            Sy = fmaf(dyl, w0.x, Sy);
+            Sxy = fmaf(dyl, w0.y, Sxy);
+            Syy = fmaf(dyl * dyl, w0.x, Syy);
+          }
+        } else if (act && ri < vq) {
 #pragma unroll
           for (int r = 0; r < ROWS; ++r) {
             float2 u0 = red_src[(r * TPR) * 3], u1 = red_src[(r * TPR) * 3 + 1], u2 = red_src[(r * TPR) * 3 + 2];
@@ -1081,6 +1239,8 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
         finished = true;
         break;
       }
+      if constexpr (REPACK)
+        if (S > 1) bwd_repack<PX, AUX, SQ, QS>(sm.part, sm.pyt, lane, S, prow, py, px, T, Rr, gr, gg, gb, gD, gA);
     }
     if constexpr (GATHER) {
       if (!finished && k + STAGES < nchunks) {   // every consumer is past the barrier: the stage is free
@@ -1284,9 +1444,13 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
   if (gather && !row_epoch) return cudaErrorInvalidValue;
   if (grad_aux) {   // the caller has checked gs_blend_aux_supported(..., true)
     if (!gather || !aux) return cudaErrorInvalidValue;
-    blend_bwd2_kernel<8, false, 4, 3, 10, 4, true, 32, true><<<g.n_tiles, 32, 0, st>>>(
-        pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,
-        grad_is_final, crop, row_epoch, epoch, tile_neff_b, aux, grad_aux);
+#define GS_BWD2_AUX(RP)                                                                                            \
+  blend_bwd2_kernel<8, false, 4, 3, 10, 4, true, 32, true, RP><<<g.n_tiles, 32, 0, st>>>(                           \
+      pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,         \
+      grad_is_final, crop, row_epoch, epoch, tile_neff_b, aux, grad_aux)
+    if (tn.blend_repack) GS_BWD2_AUX(true);
+    else GS_BWD2_AUX(false);
+#undef GS_BWD2_AUX
     return cudaGetLastError();
   }
   if (tn.bwd_kernel != 0 || gather) {
@@ -1300,13 +1464,25 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
     const int key = ((((tn.bwd_px * 10 + tn.bwd_ws) * 10 + tn.bwd_unroll) * 10 + tn.bwd_stages) * 10 + tn.bwd_rq) * 100 +
                     tn.bwd_minb;
     if (gather && tn.bwd_ch == 32) {
+      // the shipped configuration runs with or without the live-pixel repack; the other variants have none
+#define GS_BWD2_SHIPPED()                                                                                          \
+  if (tn.blend_repack)                                                                                             \
+    blend_bwd2_kernel<8, false, 4, 3, 10, 4, true, 32, false, true><<<g.n_tiles, 32, 0, st>>>(                      \
+        pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,       \
+        grad_is_final, crop, row_epoch, epoch, tile_neff_b, nullptr, nullptr);                                     \
+  else                                                                                                             \
+    GS_BWD2C(8, false, 4, 3, 10, 4, true, 32)
       switch (key) {
         case 8022416: GS_BWD2C(8, false, 2, 2, 16, 4, true, 32); break;
         case 8023416: GS_BWD2C(8, false, 2, 3, 16, 4, true, 32); break;
         case 8042410: GS_BWD2C(8, false, 4, 2, 10, 4, true, 32); break;
-        case 8043410: GS_BWD2C(8, false, 4, 3, 10, 4, true, 32); break;
-        default: return gs_tuning().strict ? cudaErrorInvalidValue : (GS_BWD2C(8, false, 4, 3, 10, 4, true, 32), cudaGetLastError());
+        case 8043410: GS_BWD2_SHIPPED(); break;
+        default:
+          if (gs_tuning().strict) return cudaErrorInvalidValue;
+          GS_BWD2_SHIPPED();
+          break;
       }
+#undef GS_BWD2_SHIPPED
       return cudaGetLastError();
     }
     if (gather) {

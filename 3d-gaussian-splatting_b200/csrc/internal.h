@@ -88,6 +88,8 @@ struct GsTuning {
   int gather;       // fused frame path (RGB and SH): 1 = no pack pass, blend kernels gather records from rec[N]; 0 = packed streams
   int sh_tc;        // SH blend on the tensor cores (blend_sh_tc.cu, gather path only): -1 = by colour width (gs_sh_tc_mode),
                     // else bit 0 = forward, bit 1 = backward, bit 2 = two pixels per thread in the backward
+  int blend_repack; // shipped RGB backward blend (plain and aux): 1 = repack live pixels into fewer slots per lane as
+                    // pixels saturate, 0 = every lane keeps its 8 pixels until the whole tile is saturated
 };
 GsTuning& gs_tuning();
 

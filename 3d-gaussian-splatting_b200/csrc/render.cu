@@ -51,7 +51,7 @@ GsTuning& gs_tuning() {
                        tune_env("GS_TUNE_BWD_PX", 8),      tune_env("GS_TUNE_BWD_WS", 0),     tune_env("GS_TUNE_BWD_UNROLL", 4),
                        tune_env("GS_TUNE_BWD_STAGES", 3),  tune_env("GS_TUNE_BWD_MINB", 10),  tune_env("GS_TUNE_BWD_RQ", 4),
                        tune_env("GS_TUNE_FWD_PX", 4),      tune_env("GS_TUNE_BWD_CH", 32),    tune_env("GS_TUNE_STRICT", 0),
-                       tune_env("GS_TUNE_GATHER", 1),      tune_env("GS_TUNE_SH_TC", -1)};
+                       tune_env("GS_TUNE_GATHER", 1),      tune_env("GS_TUNE_SH_TC", -1),     tune_env("GS_TUNE_BLEND_REPACK", 1)};
   return t;
 }
 extern "C" int gs_tune(const char* name, int value) {
@@ -63,7 +63,8 @@ extern "C" int gs_tune(const char* name, int value) {
                                              {"bwd_stages", &t.bwd_stages}, {"bwd_minb", &t.bwd_minb},
                                              {"bwd_rq", &t.bwd_rq},         {"fwd_px", &t.fwd_px},
                                              {"gather", &t.gather},         {"bwd_ch", &t.bwd_ch},
-                                             {"strict", &t.strict},         {"sh_tc", &t.sh_tc}};
+                                             {"strict", &t.strict},         {"sh_tc", &t.sh_tc},
+                                             {"blend_repack", &t.blend_repack}};
   for (auto& e : tab)
     if (!strcmp(e.k, name)) {
       *e.v = value;

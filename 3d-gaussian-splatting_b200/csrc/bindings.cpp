@@ -327,6 +327,12 @@ struct RenderContext {
   // forwards that follow, a backward uses the mode of its forward
   void set_sh_eval(int mode) { check_rc(gs_ctx_set_sh_eval(ctx, mode), "gs_ctx_set_sh_eval"); }
 
+  // screen-space 2-D filter (gs_ctx_set_filter2d): FILTER2D_NONE (default), _DILATE or _ANTIALIAS with a variance in
+  // px^2; applies to the forwards that follow, a backward uses the filter of its forward
+  void set_filter2d(int mode, double variance) {
+    check_rc(gs_ctx_set_filter2d(ctx, mode, (float)variance), "gs_ctx_set_filter2d");
+  }
+
   void set_timing(bool on) { check_rc(gs_ctx_set_timing(ctx, on ? 1 : 0), "gs_ctx_set_timing"); }
   std::vector<float> stage_ms() {
     std::vector<float> v(GS_N_STAGES, -1.f);
@@ -742,6 +748,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("last_instances", &RenderContext::last_instances)
       .def("stats", &RenderContext::stats)
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
+      .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
       .def("set_timing", &RenderContext::set_timing)
       .def("set_grad_push", &RenderContext::set_grad_push)
       .def("clear_grad_push", &RenderContext::clear_grad_push)
@@ -766,4 +773,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("abi_version") = gs_abi_version();
   m.attr("SH_EVAL_PIXEL") = GS_SH_EVAL_PIXEL;
   m.attr("SH_EVAL_GAUSSIAN") = GS_SH_EVAL_GAUSSIAN;
+  m.attr("FILTER2D_NONE") = GS_FILTER2D_NONE;
+  m.attr("FILTER2D_DILATE") = GS_FILTER2D_DILATE;
+  m.attr("FILTER2D_ANTIALIAS") = GS_FILTER2D_ANTIALIAS;
 }

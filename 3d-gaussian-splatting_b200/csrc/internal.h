@@ -133,7 +133,8 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
                                     unsigned int* n_visible, cudaStream_t st,
-                                    bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/);
+                                    bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/,
+                                    const GsFilter2d* filt = nullptr /*non-null: 2-D screen-space filter*/);
 
 // Data-parallel gradient push (device view of gs_grad_push): world == 0 disables it.
 struct GsGradPush {
@@ -150,7 +151,8 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
                                         bool depth_grad = false /*rows carry dL/d|p_c| in the column after the colour*/,
-                                        bool sh_gaussian = false /*d = 27 / 48 coefficients, RGB gradient rows*/);
+                                        bool sh_gaussian = false /*d = 27 / 48 coefficients, RGB gradient rows*/,
+                                        const GsFilter2d* filt = nullptr /*the forward's 2-D filter*/);
 // The same without a push, for RGB and per-Gaussian SH, plus the camera gradient: the projection backward leaves one
 // 12-float partial sum per CTA in cam_part (gs_cam_grad_workspace_bytes(n)), and a one-CTA kernel sums them in fp64
 // into grad_cam[12] = {dL/drot row-major, dL/dtran} (zeros when n == 0).  The five gradient pointers may all be NULL
@@ -162,7 +164,7 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                             uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
-                                            bool depth_grad, bool sh_gaussian);
+                                            bool depth_grad, bool sh_gaussian, const GsFilter2d* filt = nullptr);
 
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,

@@ -70,13 +70,15 @@ __device__ __forceinline__ void sh_logits(const float* coef, const float* Y, flo
 
 // KG = 0: colour from the rgb[n, 3] logits when d == 3 (per-pixel SH leaves it to the blend).  KG = 9 / 16: SH of
 // degree 2 / 3 evaluated once per Gaussian along view_dir (GS_SH_EVAL_GAUSSIAN); the record then carries an RGB colour.
-template <int KG>
+// F: the 2-D screen-space filter `filt` (gs_filter2d) is applied to the covariance before the tile rectangle and the
+// conic, and its compensation to l2o.
+template <int KG, bool F = false>
 __device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
     const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible) {
+    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}) {
   int i = blockIdx.x * kBlock + threadIdx.x;
   bool vis = false;
   uint32_t cnt = 0;
@@ -87,7 +89,16 @@ __device__ __forceinline__ void fused_project_body(
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
     vis = o.visible;
     if (mask) mask[i] = o.visible ? 1 : 0;
-    if (o.visible) {
+    bool keep = o.visible;
+    float dl2o = 0.f;
+    if constexpr (F) {
+      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
+      o.a = fo.a;
+      o.d = fo.d;
+      dl2o = fo.dl2o;
+      keep = keep && fo.keep;
+    }
+    if (keep) {
       uint32_t tx0, tx1, ty0, ty1;
       if (gs_tile_rect(grid, o.x, o.y, o.a, o.b, o.c, o.d, tx0, tx1, ty0, ty1)) {
         cnt = (tx1 - tx0) * (ty1 - ty0);
@@ -113,7 +124,7 @@ __device__ __forceinline__ void fused_project_body(
           cg = gs_sigmoid(rgb[3 * i + 1]);
           cb = gs_sigmoid(rgb[3 * i + 2]);
         }
-        r->b = make_float4(k.cc, log2f(op), cr, cg);
+        r->b = make_float4(k.cc, F ? log2f(op) + dl2o : log2f(op), cr, cg);
         r->c = make_float4(cb, o.depth, __uint_as_float(tx0 | (ty0 << 16)),
                            __uint_as_float((tx1 - tx0) | ((ty1 - ty0) << 16)));
         r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
@@ -162,6 +173,18 @@ __global__ void __launch_bounds__(kBlock) fused_project_sh_kernel(
                         count, dkey, mask, n_visible);
 }
 
+// with the 2-D filter: K = 0 is fused_project_kernel's colour rule, K = 9 / 16 fused_project_sh_kernel<K>'s
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_filt_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible, GsFilter2d filt) {
+  fused_project_body<K, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec,
+                              count, dkey, mask, n_visible, filt);
+}
+
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
 // contiguous rows offsets_g[i] .. + count[i]) and chains them to the RAW parameters.  No
 // atomics anywhere: the result is deterministic.  Row layout (GW floats): d/d{x, y, ca, cb, cc,
@@ -206,7 +229,9 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
 // no longer compile to the code fused_project_bwd_kernel had before the body was shared.)
 // CG (camera gradient, W = 0 only): also adds this Gaussian's share of dL/d(rot, tran) to cg[12] (gs_cam_grad_add plus
 // the view-direction term of per-Gaussian SH); with all five gradient pointers NULL no parameter gradient is stored.
-template <int D, int GW, int W, bool DT, int KG, bool CG = false>
+// F: the forward applied the 2-D filter `filt` (fused_project_body<KG, true>): the conic is chained with the filtered
+// covariance, and the compensation's gradient is added to dL/dcov.
+template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false>
 __device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
@@ -214,7 +239,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
     const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
     float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
-    GsGradPush push, float* cg = nullptr) {
+    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}) {
   static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
   static_assert(!CG || (W == 0 && GW == GS_GREC), "camera gradient: RGB gradient rows, no push");
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
@@ -265,6 +290,14 @@ __device__ __forceinline__ void fused_project_bwd_body(
       }
     }
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    float fk[4];                                               // F: d l2o / d cov of the compensation
+    if constexpr (F) {
+      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
+      o.a = fo.a;
+      o.d = fo.d;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) fk[j] = fo.k[j];
+    }
     // conic (ca, cb, cc) = (d, b+c, a) * sc,  sc = log2e / (2 det + 1e-14)
     float det = o.a * o.d - o.b * o.c;
     double pn = 2.0 * (double)det + 1e-14;
@@ -276,6 +309,10 @@ __device__ __forceinline__ void fused_project_bwd_body(
     gcov[1] = acc[3] * sc + gsc * kk * o.c;                   // d det/db = -c
     gcov[2] = acc[3] * sc + gsc * kk * o.b;                   // d det/dc = -b
     gcov[3] = acc[2] * sc - gsc * kk * o.a;                   // d det/dd =  a
+    if constexpr (F) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) gcov[j] += acc[5] * fk[j];
+    }
     static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
     float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
     float gq[4], gsv[3];
@@ -421,16 +458,29 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_kernel(GS_PBWD_PA
   fused_project_bwd_body<3 * K, GS_GREC, W, DT, K>(GS_PBWD_ARGS);
 }
 
+// the same two families for a forward that applied the 2-D filter
+template <int D, int GW, int W, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_filt_kernel(GS_PBWD_PARAMS, GsFilter2d filt) {
+  fused_project_bwd_body<D, GW, W, DT, 0, false, true>(GS_PBWD_ARGS, nullptr, filt);
+}
+
+template <int K, int W, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PBWD_PARAMS, GsFilter2d filt) {
+  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true>(GS_PBWD_ARGS, nullptr, filt);
+}
+
 // Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
 // 12-float shares in a fixed order (butterfly shuffles, then the 8 warp sums in warp order) into row blockIdx.x of
 // cam_part[gridDim.x][12]; cam_grad_finish_kernel adds the rows.  No atomics: the result is bit-deterministic.
+// F: with the 2-D filter of the forward (fused_project_bwd_cam_filt_kernel).
 constexpr int kCamGrad = 12;
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part) {
+template <int K, bool DT, bool F>
+__device__ __forceinline__ void fused_project_bwd_cam_body(GS_PBWD_PARAMS, float* __restrict__ cam_part,
+                                                           GsFilter2d filt) {
   float cg[kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
-  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true>(GS_PBWD_ARGS, cg);
+  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F>(GS_PBWD_ARGS, cg, filt);
   __shared__ float wsum[kBlock / 32][kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) {
@@ -448,6 +498,17 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_kernel(GS_PBWD_P
     for (int w = 0; w < kBlock / 32; ++w) s += wsum[w][threadIdx.x];
     cam_part[(size_t)blockIdx.x * kCamGrad + threadIdx.x] = s;
   }
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part) {
+  fused_project_bwd_cam_body<K, DT, false>(GS_PBWD_ARGS, cam_part, GsFilter2d{});
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
+                                                                            GsFilter2d filt) {
+  fused_project_bwd_cam_body<K, DT, true>(GS_PBWD_ARGS, cam_part, filt);
 }
 #undef GS_PBWD_PARAMS
 
@@ -629,8 +690,20 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
-                                    unsigned int* n_visible, cudaStream_t st, bool sh_gaussian) {
+                                    unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt) {
   if (n == 0) return cudaSuccess;
+  if (filt) {
+#define GS_LAUNCH_PFILT(K)                                                                                      \
+  fused_project_filt_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
+                                                               grid, near_plane, half_w, half_h, rec, count, dkey, \
+                                                               mask, n_visible, *filt)
+    if (sh_gaussian && d == 27) GS_LAUNCH_PFILT(9);
+    else if (sh_gaussian && d == 48) GS_LAUNCH_PFILT(16);
+    else if (sh_gaussian) return cudaErrorInvalidValue;
+    else GS_LAUNCH_PFILT(0);
+#undef GS_LAUNCH_PFILT
+    return cudaGetLastError();
+  }
   if (sh_gaussian && d == 27)
     fused_project_sh_kernel<9><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
                                                                near_plane, half_w, half_h, rec, count, dkey, mask,
@@ -653,10 +726,13 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
-                                        bool depth_grad, bool sh_gaussian) {
+                                        bool depth_grad, bool sh_gaussian, const GsFilter2d* filt) {
   if (n == 0) return cudaSuccess;
-#define GS_LAUNCH_PBWD(D, GW, W, DT) \
-  fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
+#define GS_LAUNCH_PBWD(D, GW, W, DT)                                                               \
+  if (filt)                                                                                        \
+    fused_project_bwd_filt_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
+  else                                                                                             \
+    fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
 #define GS_LAUNCH_PBWD_W(D, GW, DT)                  \
   switch (push.world) {                              \
     case 0: GS_LAUNCH_PBWD(D, GW, 0, DT); break;     \
@@ -665,8 +741,11 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
     case 8: GS_LAUNCH_PBWD(D, GW, 8, DT); break;     \
     default: return cudaErrorInvalidValue;           \
   }
-#define GS_LAUNCH_PBWD_SH(K, W, DT) \
-  fused_project_bwd_sh_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
+#define GS_LAUNCH_PBWD_SH(K, W, DT)                                                               \
+  if (filt)                                                                                       \
+    fused_project_bwd_sh_filt_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
+  else                                                                                            \
+    fused_project_bwd_sh_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
 #define GS_LAUNCH_PBWD_SH_W(K, DT)                   \
   switch (push.world) {                              \
     case 0: GS_LAUNCH_PBWD_SH(K, 0, DT); break;      \
@@ -701,12 +780,15 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                             uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
-                                            bool depth_grad, bool sh_gaussian) {
+                                            bool depth_grad, bool sh_gaussian, const GsFilter2d* filt) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
   const GsGradPush push{};
   if (n > 0) {
-#define GS_LAUNCH_PBWD_CAM(K, DT) \
-  fused_project_bwd_cam_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part)
+#define GS_LAUNCH_PBWD_CAM(K, DT)                                                                             \
+  if (filt)                                                                                                   \
+    fused_project_bwd_cam_filt_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, *filt); \
+  else                                                                                                        \
+    fused_project_bwd_cam_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part)
     if (d == 27 && depth_grad) GS_LAUNCH_PBWD_CAM(9, true);
     else if (d == 27) GS_LAUNCH_PBWD_CAM(9, false);
     else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_CAM(16, true);

@@ -193,6 +193,45 @@ __device__ __forceinline__ void gs_cam_grad_add(const GsCam& cam, const float p[
   }
 }
 
+// Screen-space 2-D filter of the fused frame path (gs_ctx_set_filter2d): Sigma' = Sigma + diag(ex, ey), ex = s / fx^2,
+// ey = s / fy^2 for a filter variance of s px^2.  The conic, the det test and the tile rectangle use Sigma'.
+// compensate (antialias): l2o gains 0.5 log2(det / det'), which keeps the screen-space integral of alpha unchanged.
+struct GsFilter2d {
+  float ex, ey;
+  int compensate;
+};
+
+struct GsFilter2dOut {
+  float a, d;       // Sigma' diagonal (b, c unchanged)
+  float dl2o;       // added to l2o (0 without compensation)
+  float k[4];       // d dl2o / d(a, b, c, d): (d, -c, -b, a) / det - (d', -c, -b, a') / det', over 2 ln 2
+  bool keep;        // false: the compensated Gaussian has det <= 0 and gets no instances
+};
+
+// Forward and backward of the filter for one projected covariance (a, b, c, d).  The backward chains the conic with
+// Sigma' (Sigma' - Sigma is constant) and adds g_l2o * k to dL/dSigma; k is dead code in the forward.
+__device__ __forceinline__ GsFilter2dOut gs_filter2d(const GsFilter2d& f, float a, float b, float c, float d) {
+  GsFilter2dOut o;
+  o.a = a + f.ex;
+  o.d = d + f.ey;
+  o.dl2o = 0.f;
+  o.keep = true;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) o.k[j] = 0.f;
+  if (f.compensate) {
+    const float det = a * d - b * c;
+    const float detf = o.a * o.d - b * c;
+    o.keep = det > 0.f;
+    o.dl2o = 0.5f * log2f(det / detf);
+    const float s = 0.5f / GS_LN2, id = 1.f / det, idf = 1.f / detf;
+    o.k[0] = s * (d * id - o.d * idf);
+    o.k[1] = s * (c * idf - c * id);
+    o.k[2] = s * (b * idf - b * id);
+    o.k[3] = s * (a * id - o.a * idf);
+  }
+  return o;
+}
+
 // Tile rectangle covered by a Gaussian, method 2 "prob2" (gaussian.cu:226-242): axis aligned
 // bbox of the `thresh` iso-probability ellipse; float->uint32 casts truncate / saturate.
 struct GsTileGrid {

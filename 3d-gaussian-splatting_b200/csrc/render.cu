@@ -161,6 +161,10 @@ struct gs_ctx {
   // data-parallel gradient push (gs_ctx_set_grad_push); world == 0: off
   GsGradPush push{};
   int sh_eval = GS_SH_EVAL_PIXEL;         // gs_ctx_set_sh_eval: applies to the forwards that follow
+  int filter2d = GS_FILTER2D_NONE;        // gs_ctx_set_filter2d: applies to the forwards that follow
+  float filter2d_var = 0.3f;              //   its variance in px^2
+  bool filt_on = false;                   // the last forward's filter (its backward uses it)
+  GsFilter2d filt{};
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -241,6 +245,14 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   // only the projection kernels, the push bucket and the caller's tensors keep the parameter width d
   const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
   const int blend_d = sh_gaussian ? 3 : d;   // colour width of the blend
+  // 2-D filter in normalised image-plane units: the variance over the squared pixel pitch 1 / f^2, rounded once
+  const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
+  GsFilter2d filt{};
+  if (filt_on) {
+    filt.ex = (float)((double)c->filter2d_var / ((double)cam->focal_x * (double)cam->focal_x));
+    filt.ey = (float)((double)c->filter2d_var / ((double)cam->focal_y * (double)cam->focal_y));
+    filt.compensate = c->filter2d == GS_FILTER2D_ANTIALIAS;
+  }
   GsAuxOut aux_out{};
   const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
   if (use_aux) {
@@ -347,7 +359,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
                                       half_w, half_h, c->rec.as<GsRec>(), c->count.as<uint32_t>(),
                                       c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
-                                      sh_gaussian));
+                                      sh_gaussian, filt_on ? &filt : nullptr));
   if (n > 0) gs_count_launch();
   // 2. (a) exclusive scan of the tile counts in Gaussian-id order -> gradient-row bases and M;
   //    (b) stable depth sort of the N Gaussians; (c) scan of the counts in depth order (the
@@ -474,6 +486,8 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   c->have_forward = true;
   c->have_aux = aux_out.aux != nullptr;
   c->sh_gaussian = sh_gaussian;
+  c->filt_on = filt_on;
+  c->filt = filt;
   c->gather = gather;
   c->n = n;
   c->d = d;
@@ -594,14 +608,14 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                                 c->count.as<uint32_t>(), c->grad_inst.as<float>(),
                                                 c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
                                                 grad_quat, grad_scale, c->cam_part.as<float>(), grad_cam, st,
-                                                grad_aux != nullptr, c->sh_gaussian));
+                                                grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sum (always: grad_cam is always written)
   } else {
     GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
                                             c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                             c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                             grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
-                                            grad_aux != nullptr, c->sh_gaussian));
+                                            grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
     if (c->n > 0) gs_count_launch();
   }
   gs_mark(c, 9, st);
@@ -686,6 +700,18 @@ extern "C" int gs_ctx_set_sh_eval(gs_ctx* c, int mode) {
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_sh_eval: mode must be GS_SH_EVAL_PIXEL or GS_SH_EVAL_GAUSSIAN");
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_sh_eval: null ctx");
   c->sh_eval = mode;
+  return 0;
+}
+
+extern "C" int gs_ctx_set_filter2d(gs_ctx* c, int mode, float variance_px2) {
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter2d: null ctx");
+  if (mode != GS_FILTER2D_NONE && mode != GS_FILTER2D_DILATE && mode != GS_FILTER2D_ANTIALIAS)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG,
+                            "gs_ctx_set_filter2d: mode must be GS_FILTER2D_NONE, GS_FILTER2D_DILATE or GS_FILTER2D_ANTIALIAS");
+  if (!std::isfinite(variance_px2) || !(variance_px2 > 0.f))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter2d: variance must be finite and > 0");
+  c->filter2d = mode;
+  c->filter2d_var = variance_px2;
   return 0;
 }
 

@@ -141,6 +141,11 @@ SCALE_ACTIVATIONS = {"abs": 0, "exp": 1}
 # functions take no argument for it): "pixel" = per pixel ray (the reference), "gaussian" = once per Gaussian along
 # the camera-centre -> mean direction, then blended as an RGB colour
 SH_EVAL = {"pixel": gaussian.SH_EVAL_PIXEL, "gaussian": gaussian.SH_EVAL_GAUSSIAN}
+# screen-space 2-D filter (RenderContext.set_filter2d(mode, variance); a context setting like SH_EVAL): "none" (the
+# reference), "dilate" (3DGS: + variance px^2 on the 2-D covariance), "antialias" (dilate + opacity compensation
+# sqrt(det / det'), Mip-Splatting's 2-D filter)
+FILTER2D = {"none": gaussian.FILTER2D_NONE, "dilate": gaussian.FILTER2D_DILATE,
+            "antialias": gaussian.FILTER2D_ANTIALIAS}
 
 
 _flat_grad_allocator = None

@@ -27,7 +27,7 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import SH_EVAL, render_frame, render_frame_aux, render_frame_cam, render_frame_final
+from renderer import FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_cam, render_frame_final
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -120,7 +120,7 @@ class Splatter(nn.Module):
                  tile_culling_method="prob2", tile_culling_dist_thresh=0.5, tile_culling_prob_thresh=0.1,
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
-                 sh_eval="pixel"):
+                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -133,7 +133,14 @@ class Splatter(nn.Module):
         `sh_eval` (SH colour only): "pixel" evaluates the SH basis per pixel ray, as the reference does;
         "gaussian" evaluates it once per Gaussian along the direction from the camera centre to its mean and
         blends the result as an RGB colour (the usual 3D Gaussian Splatting model, and a much cheaper frame).
-        The two modes use the same coefficient tensor but render it differently."""
+        The two modes use the same coefficient tensor but render it differently.
+
+        `filter2d`: screen-space low-pass filter of the projected Gaussians, for scenes rendered at more than one
+        resolution.  "none" (default, the reference); "dilate" adds `filter2d_variance` px^2 to every 2-D covariance
+        (the original 3D Gaussian Splatting rasterizer, 0.3); "antialias" dilates and scales the opacity by
+        sqrt(det / det'), keeping each Gaussian's screen-space integral (Mip-Splatting's 2-D filter, gsplat's
+        "antialiased").  Every frame of this Splatter follows it, with gradients.  A scene renders differently under
+        another mode: train and render with the same one."""
         super().__init__()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
@@ -145,7 +152,16 @@ class Splatter(nn.Module):
             raise ValueError(f"sh_eval must be one of {sorted(SH_EVAL)}, not {sh_eval!r}")
         if sh_eval == "gaussian" and not use_sh_coeff:
             raise ValueError("sh_eval='gaussian' needs SH colour (use_sh_coeff=True)")
+        if filter2d not in FILTER2D:
+            raise ValueError(f"filter2d must be one of {sorted(FILTER2D)}, not {filter2d!r}")
+        try:
+            filter2d_variance = float(filter2d_variance)
+        except (TypeError, ValueError):
+            raise ValueError(f"filter2d_variance must be a number, not {filter2d_variance!r}") from None
+        if not (math.isfinite(filter2d_variance) and filter2d_variance > 0):
+            raise ValueError(f"filter2d_variance must be finite and > 0, not {filter2d_variance!r}")
         self.sh_eval = sh_eval
+        self.filter2d, self.filter2d_variance = filter2d, filter2d_variance
         self.use_sh_coeff = bool(use_sh_coeff)
         self.near = near
         self.render_downsample = render_downsample
@@ -173,6 +189,7 @@ class Splatter(nn.Module):
         with torch.cuda.device(self.device):                      # the context lives on self.device, not on the current one
             self._rctx = gaussian.RenderContext()
         self._rctx.set_sh_eval(SH_EVAL[sh_eval])                   # every frame of this Splatter, fused or not
+        self._rctx.set_filter2d(FILTER2D[filter2d], filter2d_variance)
         self.ground_truth = None
         self.culling_mask = None
         self.n_tile_gaussians = 0

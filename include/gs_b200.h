@@ -258,6 +258,29 @@ int gs_render_backward_cam(gs_ctx* ctx, const float* pos, const float* rgb, cons
 #define GS_SH_EVAL_GAUSSIAN 1
 int gs_ctx_set_sh_eval(gs_ctx* ctx, int mode);
 
+/* Screen-space 2-D low-pass filter of the projected Gaussians (additive; default NONE, the reference, which has none).
+ * With a filter variance s px^2 and the pixel pitch 1/fx by 1/fy, the 2-D covariance Sigma = (a, b, c, d) of every
+ * Gaussian becomes Sigma' = (a + s/fx^2, b, c, d + s/fy^2):
+ *   GS_FILTER2D_NONE      : no filter (the variance is kept but not used).
+ *   GS_FILTER2D_DILATE    : the original 3D Gaussian Splatting dilation (s = 0.3): the conic, the det <= 0 test and the
+ *                           tile rectangle come from Sigma'.  A Gaussian below a pixel no longer thins to a needle, and
+ *                           its screen-space integral grows by sqrt(det'/det).
+ *   GS_FILTER2D_ANTIALIAS : the Mip-Splatting 2-D filter (gsplat "antialiased"): as DILATE, and the opacity is scaled by
+ *                           sqrt(det/det'), which keeps every Gaussian's screen-space integral unchanged.  A Gaussian
+ *                           with det <= 0 gets no instances (its culling_mask entry still reports the frustum test).
+ * Backward: Sigma' - Sigma is a constant; the compensation's gradient reaches the 2-D covariance and from there the
+ * parameters and (gs_render_backward_cam) the camera; the opacity-logit gradient is unchanged.
+ * The setting belongs to the context and applies to every fused forward that follows (plain, final, aux, the packed
+ * path and gs_render_forward_backward_host); a backward (plain, final, aux, cam, with or without a gradient push) always
+ * uses the filter of its forward.  Depth, sort order, colour and culling are unchanged.  No launch or synchronisation
+ * is added.  The legacy per-stage API is not affected.  A scene trained under one mode renders differently under
+ * another: train and render with the same one.
+ * Null ctx, an unknown mode, or a variance that is not finite and > 0 (whatever the mode): GS_ERR_INVALID_ARG. */
+#define GS_FILTER2D_NONE 0
+#define GS_FILTER2D_DILATE 1
+#define GS_FILTER2D_ANTIALIAS 2
+int gs_ctx_set_filter2d(gs_ctx* ctx, int mode, float variance_px2);
+
 /* Per-stage device timing with CUDA events recorded on the frame's stream (off by default).
  * gs_frame_stage_ms fills out[GS_N_STAGES] with the milliseconds of the last frame's stages:
  * 0 project, 1 depth sort of Gaussians + scan + M readback, 2 key emit, 3 tile-id radix sort,

@@ -333,6 +333,38 @@ struct RenderContext {
     check_rc(gs_ctx_set_filter2d(ctx, mode, (float)variance), "gs_ctx_set_filter2d");
   }
 
+  // screen-space densification statistics (gs_ctx_set_densify_stats): accumulated by every backward that computes
+  // parameter gradients until cleared.  The context keeps the tensors alive while they are set.
+  std::vector<torch::Tensor> densify_stats_refs;
+  void set_densify_stats(torch::Tensor grad2d, torch::Tensor count, torch::Tensor max_radius,
+                         c10::optional<torch::Tensor> absgrad) {
+    const int64_t n = grad2d.numel();
+    auto check = [&](const torch::Tensor& t, at::ScalarType dt, const char* name) {
+      TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt && t.is_contiguous() && t.dim() == 1 && t.numel() == n,
+                  "set_densify_stats: ", name, " must be a contiguous 1-D CUDA ", dt == at::kInt ? "int32" : "float32",
+                  " tensor of n = grad2d.numel() elements");
+      TORCH_CHECK(t.device().index() == device, "set_densify_stats: ", name, " is on another device than the context");
+    };
+    check(grad2d, at::kFloat, "grad2d");
+    check(count, at::kInt, "count");
+    check(max_radius, at::kFloat, "max_radius");
+    if (absgrad) check(*absgrad, at::kFloat, "absgrad");
+    TORCH_CHECK(n < (int64_t(1) << 31), "set_densify_stats: n too large");
+    gs_densify_stats s{};
+    s.n = (int)n;
+    s.grad2d = fpm(grad2d);
+    s.absgrad = absgrad ? fpm(*absgrad) : nullptr;
+    s.count = count.data_ptr<int>();
+    s.max_radius = fpm(max_radius);
+    check_rc(gs_ctx_set_densify_stats(ctx, &s), "gs_ctx_set_densify_stats");
+    densify_stats_refs = {grad2d, count, max_radius};
+    if (absgrad) densify_stats_refs.push_back(*absgrad);
+  }
+  void clear_densify_stats() {
+    check_rc(gs_ctx_set_densify_stats(ctx, nullptr), "gs_ctx_set_densify_stats");
+    densify_stats_refs.clear();
+  }
+
   void set_timing(bool on) { check_rc(gs_ctx_set_timing(ctx, on ? 1 : 0), "gs_ctx_set_timing"); }
   std::vector<float> stage_ms() {
     std::vector<float> v(GS_N_STAGES, -1.f);
@@ -611,6 +643,32 @@ std::tuple<torch::Tensor, torch::Tensor> loss_l1_ssim(torch::Tensor image, torch
   return {out3, grad};
 }
 
+// the apply half of densify / densify_stats: reads the plan's totals (the one host sync), draws the split samples and
+// writes the five new parameter tensors; returns them + (n_deleted, n_clone, n_split)
+static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_apply(
+    const torch::Tensor& pos, const torch::Tensor& rgb, const torch::Tensor& opa, const torch::Tensor& quat,
+    const torch::Tensor& scale, const float* grad, int scale_activation, double clone_dt,
+    c10::optional<at::Generator> gen, const torch::Tensor& code, const torch::Tensor& dst) {
+  const int64_t n = pos.size(0);
+  int64_t nk = n, nc = 0, nsp = 0;
+  if (n > 0) {
+    auto tot = dst.index({torch::indexing::Slice(), n}).cpu();        // the one host sync: sizes of the new arrays
+    nk = tot[0].item<int>(); nc = tot[1].item<int>(); nsp = tot[2].item<int>();
+  }
+  const int64_t m = nk + nc + nsp;
+  const int64_t d = rgb.size(1);
+  auto z = torch::randn({2, nsp, 3}, gen, pos.options());              // torch's generator: identical on every DP rank
+  std::vector<torch::Tensor> out = {torch::empty({m, 3}, pos.options()), torch::empty({m, d}, pos.options()),
+                                    torch::empty({m}, pos.options()), torch::empty({m, 4}, pos.options()),
+                                    torch::empty({m, 3}, pos.options())};
+  check_rc(gs_densify_apply(fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)d, code.data_ptr<uint8_t>(),
+                            dst.data_ptr<int>(), grad, (float)clone_dt, fp(z), (int)nk, (int)nc, (int)nsp,
+                            scale_activation, fpm(out[0]), fpm(out[1]), fpm(out[2]), fpm(out[3]), fpm(out[4]),
+                            cur_stream()),
+           "gs_densify_apply");
+  return {out, {n - nk, nc, nsp}};
+}
+
 // densification (SURVEY.md §8 f-2): returns the five new parameter tensors + (n_deleted, n_clone, n_split)
 std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify(
     torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale, torch::Tensor grad,
@@ -631,23 +689,38 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify(
                            use_split ? 1 : 0, code.data_ptr<uint8_t>(), dst.data_ptr<int>(), ws.data_ptr(),
                            (size_t)ws.numel(), cur_stream()),
            "gs_densify_plan");
-  int64_t nk = n, nc = 0, nsp = 0;
-  if (n > 0) {
-    auto tot = dst.index({torch::indexing::Slice(), n}).cpu();        // the one host sync: sizes of the new arrays
-    nk = tot[0].item<int>(); nc = tot[1].item<int>(); nsp = tot[2].item<int>();
+  return densify_apply(pos, rgb, opa, quat, scale, grad.data_ptr<float>(), scale_activation, clone_dt, gen, code, dst);
+}
+
+// densification from the screen-space statistics (gs_densify_plan_stats; clones are exact copies, as in 3DGS)
+std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_stats(
+    torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale,
+    torch::Tensor accum, torch::Tensor count, c10::optional<torch::Tensor> max_radius, double max_screen_px,
+    int scale_activation, double opa_logit_min, double delete_thresh, double grad_thresh, double tau, bool use_clone,
+    bool use_split, c10::optional<at::Generator> gen) {
+  GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(accum);
+  const int64_t n = pos.size(0);
+  TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && rgb.dim() == 2 && rgb.size(0) == n && opa.numel() == n &&
+                  quat.numel() == 4 * n && scale.numel() == 3 * n && accum.numel() == n && n < (int64_t(1) << 31),
+              "densify_stats: bad shapes");
+  GS_CHECK_I32(count);
+  TORCH_CHECK(count.numel() == n, "densify_stats: count must have n elements");
+  if (max_radius) {
+    GS_CHECK_F32(*max_radius);
+    TORCH_CHECK(max_radius->numel() == n, "densify_stats: max_radius must have n elements");
   }
-  const int64_t m = nk + nc + nsp;
-  const int64_t d = rgb.size(1);
-  auto z = torch::randn({2, nsp, 3}, gen, pos.options());              // torch's generator: identical on every DP rank
-  std::vector<torch::Tensor> out = {torch::empty({m, 3}, pos.options()), torch::empty({m, d}, pos.options()),
-                                    torch::empty({m}, pos.options()), torch::empty({m, 4}, pos.options()),
-                                    torch::empty({m, 3}, pos.options())};
-  check_rc(gs_densify_apply(fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)d, code.data_ptr<uint8_t>(),
-                            dst.data_ptr<int>(), fp(grad), (float)clone_dt, fp(z), (int)nk, (int)nc, (int)nsp,
-                            scale_activation, fpm(out[0]), fpm(out[1]), fpm(out[2]), fpm(out[3]), fpm(out[4]),
-                            cur_stream()),
-           "gs_densify_apply");
-  return {out, {n - nk, nc, nsp}};
+  c10::cuda::CUDAGuard guard(pos.device());
+  auto bopt = pos.options().dtype(at::kByte);
+  auto code = torch::empty({n + 1}, bopt);
+  auto dst = torch::empty({3, n + 1}, pos.options().dtype(at::kInt));
+  auto ws = torch::empty({(int64_t)gs_densify_workspace_bytes((int)n)}, bopt);
+  check_rc(gs_densify_plan_stats(fp(opa), fp(scale), fp(accum), count.data_ptr<int>(),
+                                 max_radius ? fp(*max_radius) : nullptr, (float)max_screen_px, (int)n,
+                                 scale_activation, (float)opa_logit_min, (float)delete_thresh, (float)grad_thresh,
+                                 (float)tau, use_clone ? 1 : 0, use_split ? 1 : 0, code.data_ptr<uint8_t>(),
+                                 dst.data_ptr<int>(), ws.data_ptr(), (size_t)ws.numel(), cur_stream()),
+           "gs_densify_plan_stats");
+  return densify_apply(pos, rgb, opa, quat, scale, nullptr, scale_activation, 0.0, gen, code, dst);
 }
 
 // NVLS in-place all-reduce of a symmetric flat buffer (multicast address as an integer)
@@ -749,6 +822,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("stats", &RenderContext::stats)
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
+      .def("set_densify_stats", &RenderContext::set_densify_stats, py::arg("grad2d"), py::arg("count"),
+           py::arg("max_radius"), py::arg("absgrad") = py::none())
+      .def("clear_densify_stats", &RenderContext::clear_densify_stats)
       .def("set_timing", &RenderContext::set_timing)
       .def("set_grad_push", &RenderContext::set_grad_push)
       .def("clear_grad_push", &RenderContext::clear_grad_push)
@@ -764,6 +840,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("grad"), py::arg("scale_activation"),
         py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("grad_agg_max"), py::arg("tau"),
         py::arg("use_clone"), py::arg("use_split"), py::arg("clone_dt"), py::arg("generator") = py::none());
+  m.def("densify_stats", &densify_stats,
+        "prune / clone / split on the device from screen-space densification statistics (gs_densify_plan_stats)",
+        py::arg("pos"), py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("accum"),
+        py::arg("count"), py::arg("max_radius"), py::arg("max_screen_px"), py::arg("scale_activation"),
+        py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("tau"),
+        py::arg("use_clone"), py::arg("use_split"), py::arg("generator") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
   m.def("tune", [](const std::string& name, int value) { check_rc(gs_tune(name.c_str(), value), "gs_tune"); },

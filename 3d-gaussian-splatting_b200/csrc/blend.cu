@@ -765,19 +765,33 @@ struct Bwd2SmemAux : Bwd2Smem<PX, STAGES, RQ, GATHER, CH> {
   float part_t[Bwd2Cfg<PX, STAGES, RQ>::R * TIS];
 };
 
+// ABS backward (densification statistics): two more per-(thread, instance) sums, sum_p |g_x,p| and sum_p |g_y,p| of
+// the per-pixel contributions to d/dx and d/dy, in two planes laid out like the AUX d_t plane (one consumer warp:
+// conflict-free stores and reducer loads).  Base: the plain or the AUX layout.
+template <class Base, int R, int NT>
+struct Bwd2SmemAbs : Base {
+  static constexpr int AIS = NT + 1;
+  static_assert(NT == 32, "absolute-gradient planes are conflict free for one consumer warp only");
+  float part_ax[R * AIS];
+  float part_ay[R * AIS];
+};
+
 // one instance x this thread's row of PX pixels: recompute alpha, analytic d/d alpha, six partial sums
 // (AUX: gc and R carry the depth / alpha terms, and d_t = sum g_D w goes to *dst_t).  Only the first NP slots are
-// evaluated (after a live-pixel repack the others are empty).
-template <int PX, bool AUX = false, int NP = PX>
+// evaluated (after a live-pixel repack the others are empty).  ABS: also sum_p |e_p (2 ca dx_p - cb dy)| to *dst_ax and
+// sum_p |e_p (2 cc dy - cb dx_p)| to *dst_ay (the per-pixel terms of d/dx and d/dy, before the factor ln 2).
+template <int PX, bool AUX = false, int NP = PX, bool ABS = false>
 __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const float4 c, const float (&px)[PX],
                                         const float py, float (&T)[PX], float (&Rr)[PX], const float (&gr)[PX],
                                         const float (&gg)[PX], const float (&gb)[PX], float2* __restrict__ dst,
                                         const float t = 0.f, const float (*gD)[PX] = nullptr,
-                                        const float (*gA)[PX] = nullptr, float* __restrict__ dst_t = nullptr) {
-  float s0 = 0.f, sx = 0.f, sxx = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, dt = 0.f;
+                                        const float (*gA)[PX] = nullptr, float* __restrict__ dst_t = nullptr,
+                                        float* __restrict__ dst_ax = nullptr, float* __restrict__ dst_ay = nullptr) {
+  float s0 = 0.f, sx = 0.f, sxx = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, dt = 0.f, ax = 0.f, ay = 0.f;
   const float dy = py - a.y;
   const float m1 = a.w * dy;
   const float ev = fmaf(-b.x * dy, dy, b.y);
+  const float ca2 = 2.f * a.z, ccdy2 = 2.f * b.x * dy;   // ABS only
 #pragma unroll
   for (int p = 0; p < NP; ++p) {
     const float dx = px[p] - a.x;
@@ -800,11 +814,19 @@ __device__ __forceinline__ void bwd_row(const float4 a, const float2 b, const fl
     c1 = fmaf(gg[p], w, c1);
     c2 = fmaf(gb[p], w, c2);
     if constexpr (AUX) dt = fmaf((*gD)[p], w, dt);
+    if constexpr (ABS) {
+      ax += fabsf(e * fmaf(ca2, dx, -m1));
+      ay += fabsf(e * fmaf(-a.w, dx, ccdy2));
+    }
   }
   dst[0] = make_float2(s0, sx);
   dst[1] = make_float2(sxx, c0);
   dst[2] = make_float2(c1, c2);
   if constexpr (AUX) *dst_t = dt;
+  if constexpr (ABS) {
+    *dst_ax = ax;
+    *dst_ay = ay;
+  }
 }
 
 // ---- live-pixel repack (one consumer warp) --------------------------------------------------------------------
@@ -929,8 +951,10 @@ __device__ __forceinline__ void bwd_repack(float* __restrict__ st, const float* 
 // the 7th sum d_t = sum g_D w lands in column 6 + 3 of the gradient row.
 // REPACK (one consumer warp): live-pixel repack at round boundaries (bwd_repack); until the first repack the kernel
 // computes exactly what it computes without it.
+// ABS (one consumer warp): also sum_p |g_x,p| and sum_p |g_y,p| per instance (bwd_row), times ln 2, to the free columns
+// 10 and 11 of the gradient row; every other column is computed as without it.
 template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false,
-          bool REPACK = false>
+          bool REPACK = false, bool ABS = false>
 __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     blend_bwd2_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB, const float4* __restrict__ pC,
                       const GsRec* __restrict__ grec, const uint32_t* __restrict__ ids,
@@ -947,8 +971,9 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   static_assert(!AUX || GATHER, "the aux terms read |p_c| from the gathered records");
   static_assert(!REPACK || (NT == 32 && PX == 8), "the repack deals one warp's 256 pixels into slots of at most 8");
   static_assert(!REPACK || R * IS >= RP_END, "the partial buffer holds the repack's planes and tables");
-  using Smem = typename std::conditional<AUX, Bwd2SmemAux<PX, STAGES, RQ, GATHER, CH>,
-                                         Bwd2Smem<PX, STAGES, RQ, GATHER, CH>>::type;
+  using SmemBase = typename std::conditional<AUX, Bwd2SmemAux<PX, STAGES, RQ, GATHER, CH>,
+                                             Bwd2Smem<PX, STAGES, RQ, GATHER, CH>>::type;
+  using Smem = typename std::conditional<ABS, Bwd2SmemAbs<SmemBase, R, NT>, SmemBase>::type;
   __shared__ __align__(16) Smem sm;
   const int tile = blockIdx.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1063,6 +1088,11 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   float2* const my_part = reinterpret_cast<float2*>(sm.part + (tid / SQ) * QS + (tid % SQ) * 6);
   float* my_part_t = nullptr;   // AUX: this thread's slot in the d_t plane
   if constexpr (AUX) my_part_t = sm.part_t + (tid / SQ) * Smem::TQS + (tid % SQ);
+  float *my_part_ax = nullptr, *my_part_ay = nullptr;   // ABS: this thread's slots in the |g| planes
+  if constexpr (ABS) {
+    my_part_ax = sm.part_ax + tid;
+    my_part_ay = sm.part_ay + tid;
+  }
   // second-phase role: instance ri of the round, quarter rq of the source threads
   const int ri = tid / RQ, rq = tid % RQ;
   const float2* const red_src = reinterpret_cast<const float2*>(sm.part + ri * IS + rq * QS);
@@ -1091,6 +1121,15 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
       // slower on the H100 - by ~30 % with 4 instances per step, ~15 % with 2)
       auto phase1 = [&](auto np) -> int {
         constexpr int NP = decltype(np)::value, U = NP == PX ? UNR : 1;
+        // instance q of the round: its sums go to slot q of the partial buffer and of the d_t (AUX) / |g| (ABS)
+        // planes, whose instance stride is NT + 1 (Bwd2SmemAux::TIS, Bwd2SmemAbs::AIS)
+        auto row = [&](int q) {
+          float t = 0.f;
+          if constexpr (AUX) t = sv.depth(sub + q);
+          bwd_row<PX, AUX, NP, ABS>(sv.a(sub + q), sv.b(sub + q), sv.c(sub + q), px, py, T, Rr, gr, gg, gb,
+                                    my_part + q * (IS / 2), t, &gD, &gA, AUX ? my_part_t + q * (NT + 1) : nullptr,
+                                    ABS ? my_part_ax + q * (NT + 1) : nullptr, ABS ? my_part_ay + q * (NT + 1) : nullptr);
+        };
         int j = 0;
         bool wdead = false;
 #pragma unroll 1
@@ -1105,25 +1144,10 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
             }
           }
 #pragma unroll
-          for (int u = 0; u < U; ++u) {
-            if constexpr (AUX)
-              bwd_row<PX, true, NP>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg,
-                                    gb, my_part + (j + u) * (IS / 2), sv.depth(sub + j + u), &gD, &gA,
-                                    my_part_t + (j + u) * Smem::TIS);
-            else
-              bwd_row<PX, false, NP>(sv.a(sub + j + u), sv.b(sub + j + u), sv.c(sub + j + u), px, py, T, Rr, gr, gg,
-                                     gb, my_part + (j + u) * (IS / 2));
-          }
+          for (int u = 0; u < U; ++u) row(j + u);
         }
         if (U > 1 && !wdead)
-          for (; j < nr; ++j) {
-            if constexpr (AUX)
-              bwd_row<PX, true, NP>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
-                                    my_part + j * (IS / 2), sv.depth(sub + j), &gD, &gA, my_part_t + j * Smem::TIS);
-            else
-              bwd_row<PX, false, NP>(sv.a(sub + j), sv.b(sub + j), sv.c(sub + j), px, py, T, Rr, gr, gg, gb,
-                                     my_part + j * (IS / 2));
-          }
+          for (; j < nr; ++j) row(j);
         return j;
       };
       int j;
@@ -1210,12 +1234,25 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
             for (int s = 0; s < SQ; ++s) Dt += src[s];
           }
         }
+        float Ax = 0.f, Ay = 0.f;
+        if constexpr (ABS) {
+          if (act && ri < vq) {
+            const float* srx = sm.part_ax + ri * Smem::AIS + rq * SQ;
+            const float* sry = sm.part_ay + ri * Smem::AIS + rq * SQ;
+#pragma unroll
+            for (int s = 0; s < SQ; ++s) {
+              Ax += srx[s];
+              Ay += sry[s];
+            }
+          }
+        }
 #define GS_RED4(V)                                   \
   V += __shfl_xor_sync(0xffffffffu, V, 1);           \
   V += __shfl_xor_sync(0xffffffffu, V, 2);           \
   if (RQ == 8) V += __shfl_xor_sync(0xffffffffu, V, 4);
         GS_RED4(S0) GS_RED4(Sx) GS_RED4(Sxx) GS_RED4(Sy) GS_RED4(Sxy) GS_RED4(Syy) GS_RED4(C0) GS_RED4(C1) GS_RED4(C2)
         if constexpr (AUX) { GS_RED4(Dt) }
+        if constexpr (ABS) { GS_RED4(Ax) GS_RED4(Ay) }
 #undef GS_RED4
         if (act) {
           const uint32_t slot = sv.slot(sub + ri, tx, ty);
@@ -1227,7 +1264,8 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
           else if (rq == 1)
             out[1] = make_float4(-GS_LN2 * Syy, GS_LN2 * S0, C0, C1);
           else if (rq == 2)
-            out[2] = make_float4(C2, Dt, 0.f, 0.f);   // | d/db, d/dt (AUX; 0 otherwise)
+            out[2] = ABS ? make_float4(C2, Dt, GS_LN2 * Ax, GS_LN2 * Ay)   // | d/db, d/dt (AUX; 0 otherwise),
+                         : make_float4(C2, Dt, 0.f, 0.f);                  //   sum |d/dx|, sum |d/dy| (ABS)
           else if (rq == 3 && row_epoch)
             row_epoch[slot] = epoch;               // marks the row as written in this frame
         }
@@ -1438,10 +1476,23 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
                                 const float* image,
                                 const float* grad_image, float* grad_inst, int grad_is_final, const GsCrop& crop,
                                 uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st,
-                                const float* aux, const float* grad_aux) {
+                                const float* aux, const float* grad_aux, bool absgrad) {
   const GsTuning& tn = gs_tuning();
   const bool gather = grec != nullptr;
   if (gather && !row_epoch) return cudaErrorInvalidValue;
+  if (absgrad) {   // the caller has checked gs_blend_absgrad_supported (and gs_blend_aux_supported with grad_aux)
+    if (!gather || (grad_aux && !aux)) return cudaErrorInvalidValue;
+#define GS_BWD2_ABS(AX, RP)                                                                                        \
+  blend_bwd2_kernel<8, false, 4, 3, 10, 4, true, 32, AX, RP, true><<<g.n_tiles, 32, 0, st>>>(                       \
+      pA, pB, pC, grec, ids, goff, tile_accum, g.wp, g.hp, g.ntx, g.fx, g.fy, image, grad_image, grad_inst,         \
+      grad_is_final, crop, row_epoch, epoch, tile_neff_b, aux, grad_aux)
+    if (grad_aux && tn.blend_repack) GS_BWD2_ABS(true, true);
+    else if (grad_aux) GS_BWD2_ABS(true, false);
+    else if (tn.blend_repack) GS_BWD2_ABS(false, true);
+    else GS_BWD2_ABS(false, false);
+#undef GS_BWD2_ABS
+    return cudaGetLastError();
+  }
   if (grad_aux) {   // the caller has checked gs_blend_aux_supported(..., true)
     if (!gather || !aux) return cudaErrorInvalidValue;
 #define GS_BWD2_AUX(RP)                                                                                            \
@@ -1542,6 +1593,12 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
   return cudaGetLastError();
 }
 
+// the shipped backward knobs of the gather RGB blend, the only configuration with AUX and ABS kernels
+static bool shipped_rgb_bwd_knobs(const GsTuning& tn) {
+  return tn.bwd_kernel != 0 && tn.bwd_px == 8 && tn.bwd_ws == 0 && tn.bwd_unroll == 4 && tn.bwd_stages == 3 &&
+         tn.bwd_rq == 4 && tn.bwd_minb == 10 && tn.bwd_ch == 32;
+}
+
 int gs_blend_aux_supported(int d, bool forward, bool backward) {
   const GsTuning& tn = gs_tuning();
   if (!tn.gather)
@@ -1555,10 +1612,24 @@ int gs_blend_aux_supported(int d, bool forward, bool backward) {
   if (forward && (tn.fwd_kernel != 0 || tn.fwd_ch != 128 || tn.fwd_px != 4))
     return gs_set_error_msg(GS_ERR_UNSUPPORTED,
                             "depth / alpha / background: only the shipped forward blend knobs (fwd_kernel 0, fwd_ch 128, fwd_px 4) have an aux kernel");
-  if (backward && (tn.bwd_kernel == 0 || tn.bwd_px != 8 || tn.bwd_ws != 0 || tn.bwd_unroll != 4 || tn.bwd_stages != 3 ||
-                   tn.bwd_rq != 4 || tn.bwd_minb != 10 || tn.bwd_ch != 32))
+  if (backward && !shipped_rgb_bwd_knobs(tn))
     return gs_set_error_msg(GS_ERR_UNSUPPORTED,
                             "depth / alpha gradients: only the shipped backward blend knobs have an aux kernel");
+  return 0;
+}
+
+int gs_blend_absgrad_supported(int d, bool gather) {
+  const GsTuning& tn = gs_tuning();
+  if (d != 3)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "densify statistics: absgrad needs the RGB blend (RGB or per-Gaussian SH colour); SH colour "
+                            "evaluated per pixel has only grad2d");
+  if (!gather)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "densify statistics: absgrad is not available on the packed path (gs_tune(\"gather\", 0))");
+  if (!shipped_rgb_bwd_knobs(tn))
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "densify statistics: absgrad needs the shipped backward blend knobs");
   return 0;
 }
 

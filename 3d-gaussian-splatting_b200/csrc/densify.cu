@@ -8,6 +8,8 @@
 #include <cub/iterator/counting_input_iterator.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 
+#include <cmath>
+
 #include "internal.h"
 
 namespace {
@@ -30,6 +32,19 @@ __device__ __forceinline__ float act_norm(const float* s, int act) {
   return sqrtf(a * a + b * b + c * c);                       // |scale| (abs) / |exp(scale)| (exp): splatter.py:129-136
 }
 
+// code of a kept Gaussian: bit 0, plus clone (bit 1, norm <= tau) or split (bit 2) when it densifies
+__device__ __forceinline__ unsigned char densify_code(bool hit, float nrm, float tau, int use_clone, int use_split) {
+  unsigned char c = 1;
+  if (hit) {
+    if (nrm > tau) {
+      if (use_split) c |= 4;
+    } else if (use_clone) {
+      c |= 2;
+    }
+  }
+  return c;
+}
+
 __global__ void __launch_bounds__(kBlock) densify_classify_kernel(const float* __restrict__ opa,
                                                                    const float* __restrict__ scale,
                                                                    const float* __restrict__ grad, int n, int act,
@@ -44,17 +59,27 @@ __global__ void __launch_bounds__(kBlock) densify_classify_kernel(const float* _
   const bool keep = opa[i] > opa_logit_min && nrm < delete_thresh;          // splatter.py:137-139
   unsigned char c = 0;
   if (keep) {
-    c = 1;
     const float g0 = fabsf(grad[3 * i]), g1 = fabsf(grad[3 * i + 1]), g2 = fabsf(grad[3 * i + 2]);
     const float agg = agg_max ? fmaxf(g0, fmaxf(g1, g2)) : (g0 + g1 + g2) / 3.f;   // :152-157
-    if (agg > grad_thresh) {
-      if (nrm > tau) {
-        if (use_split) c |= 4;
-      } else if (use_clone) {
-        c |= 2;
-      }
-    }
+    c = densify_code(agg > grad_thresh, nrm, tau, use_clone, use_split);
   }
+  code[i] = c;
+}
+
+// Screen-space statistics (gs_densify_plan_stats): the 3DGS score accum / max(count, 1) >= grad_thresh, and with
+// max_radius a prune of Gaussians that grew larger than max_screen_px on screen.
+__global__ void __launch_bounds__(kBlock) densify_classify_stats_kernel(
+    const float* __restrict__ opa, const float* __restrict__ scale, const float* __restrict__ accum,
+    const int* __restrict__ count, const float* __restrict__ max_radius, float max_screen_px, int n, int act,
+    float opa_logit_min, float delete_thresh, float grad_thresh, float tau, int use_clone, int use_split,
+    unsigned char* __restrict__ code) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= n) return;
+  const float s[3] = {scale[3 * i], scale[3 * i + 1], scale[3 * i + 2]};
+  const float nrm = act_norm(s, act);
+  const bool keep = opa[i] > opa_logit_min && nrm < delete_thresh && !(max_radius && max_radius[i] > max_screen_px);
+  unsigned char c = 0;
+  if (keep) c = densify_code(accum[i] / (float)max(count[i], 1) >= grad_thresh, nrm, tau, use_clone, use_split);
   code[i] = c;
 }
 
@@ -119,9 +144,13 @@ __global__ void __launch_bounds__(kBlock) densify_apply_kernel(
   } else {
     put(kr, p, s);
     if (c & 2) {
-      const float pc[3] = {p[0] - grad[3 * i] * clone_dt, p[1] - grad[3 * i + 1] * clone_dt,
-                           p[2] - grad[3 * i + 2] * clone_dt};                    // splatter.py:170-171
-      put(n_keep + dst_clone[i], pc, s);
+      if (grad) {
+        const float pc[3] = {p[0] - grad[3 * i] * clone_dt, p[1] - grad[3 * i + 1] * clone_dt,
+                             p[2] - grad[3 * i + 2] * clone_dt};                  // splatter.py:170-171
+        put(n_keep + dst_clone[i], pc, s);
+      } else {
+        put(n_keep + dst_clone[i], p, s);                                       // exact copy (3DGS)
+      }
     }
   }
 }
@@ -141,6 +170,20 @@ size_t scan_tmp_bytes(int n) {
 
 extern "C" size_t gs_densify_workspace_bytes(int n) { return n < 0 ? 0 : up256(scan_tmp_bytes(n)) + 256; }
 
+// dst[3][n+1] = exclusive scans of the three flag bits of code[n+1]
+static int plan_scans(unsigned char* code, int* dst, int n, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  // code[n] is read by the (n+1)-item scans: the caller provides n+1 bytes, the last one zero
+  GS_CUDA_TRY(cudaMemsetAsync(code + n, 0, 1, st));
+  size_t tmp = workspace_bytes;
+  for (int b = 0; b < 3; ++b) {
+    FlagOf f{code, b};
+    cub::CountingInputIterator<int> idx(0);
+    cub::TransformInputIterator<int, FlagOf, cub::CountingInputIterator<int>> it(idx, f);
+    GS_CUDA_TRY(cub::DeviceScan::ExclusiveSum(workspace, tmp, it, dst + (size_t)b * (n + 1), n + 1, st));
+  }
+  return 0;
+}
+
 extern "C" int gs_densify_plan(const float* opa, const float* scale, const float* grad, int n, int scale_activation,
                                float opa_logit_min, float delete_thresh, float grad_thresh, int grad_agg_max, float tau,
                                int use_clone, int use_split, unsigned char* code, int* dst, void* workspace,
@@ -156,16 +199,28 @@ extern "C" int gs_densify_plan(const float* opa, const float* scale, const float
                                                                        grad_agg_max, tau, use_clone, use_split, code);
   GS_CUDA_TRY(cudaGetLastError());
   gs_count_launch();
-  // code[n] is read by the (n+1)-item scans: the caller provides n+1 bytes, the last one zero
-  GS_CUDA_TRY(cudaMemsetAsync(code + n, 0, 1, st));
-  size_t tmp = workspace_bytes;
-  for (int b = 0; b < 3; ++b) {
-    FlagOf f{code, b};
-    cub::CountingInputIterator<int> idx(0);
-    cub::TransformInputIterator<int, FlagOf, cub::CountingInputIterator<int>> it(idx, f);
-    GS_CUDA_TRY(cub::DeviceScan::ExclusiveSum(workspace, tmp, it, dst + (size_t)b * (n + 1), n + 1, st));
-  }
-  return 0;
+  return plan_scans(code, dst, n, workspace, workspace_bytes, st);
+}
+
+extern "C" int gs_densify_plan_stats(const float* opa, const float* scale, const float* accum, const int* count,
+                                     const float* max_radius, float max_screen_px, int n, int scale_activation,
+                                     float opa_logit_min, float delete_thresh, float grad_thresh, float tau,
+                                     int use_clone, int use_split, unsigned char* code, int* dst, void* workspace,
+                                     size_t workspace_bytes, gs_stream_t stream) {
+  if (n < 0 || (n > 0 && (!opa || !scale || !accum || !count || !code || !dst || !workspace)))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_densify_plan_stats: bad arguments");
+  if (max_radius && std::isnan(max_screen_px))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_densify_plan_stats: max_screen_px is NaN");
+  if (workspace_bytes < gs_densify_workspace_bytes(n))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_densify_plan_stats: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) return 0;
+  densify_classify_stats_kernel<<<(n + kBlock - 1) / kBlock, kBlock, 0, st>>>(
+      opa, scale, accum, count, max_radius, max_screen_px, n, scale_activation, opa_logit_min, delete_thresh,
+      grad_thresh, tau, use_clone, use_split, code);
+  GS_CUDA_TRY(cudaGetLastError());
+  gs_count_launch();
+  return plan_scans(code, dst, n, workspace, workspace_bytes, st);
 }
 
 extern "C" int gs_densify_apply(const float* pos, const float* rgb, const float* opa, const float* quat,

@@ -1,0 +1,80 @@
+// Screen-space densification statistics of the fused frame path (gs_ctx_set_densify_stats): one thread per Gaussian
+// after the projection backward, accumulating into the caller's buffers.  A kernel of its own, not a flag on the
+// projection backward: that body has more than 100 instantiations (D, GW, W, DT, KG, CG, F), and this one kernel
+// follows every one of them, the data-parallel push included.
+#include "internal.h"
+
+namespace {
+
+constexpr int kBlock = 256;
+
+// Gaussian i with count[i] > 0 (it got at least one tile instance in the forward):
+//   grad2d  += |(gx sx, gy sy)|, (gx, gy) = sum of columns 0, 1 over its rows tagged with this backward's epoch
+//   absgrad += |(Ax sx, Ay sy)|, (Ax, Ay) = the same sums of columns 10, 11 (ABS: sum_p |g_x,p|, sum_p |g_y,p|)
+//   count   += 1
+//   max_radius = max(max_radius, ceil(3 sqrt(lambda_max))) of the 2-D covariance the forward binned, in px^2
+// (sx, sy) = (W / (2 fx), H / (2 fy)) converts dL/d(x/z, y/z) to the NDC convention of 3DGS's viewspace gradient.
+// One thread owns one Gaussian and sums its rows in order: bit-deterministic, no atomics.
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_kernel(
+    const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n,
+    int scale_act, GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt,
+    const uint32_t* __restrict__ offsets_g, const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
+    int gw, const uint32_t* __restrict__ row_epoch, uint32_t epoch, float sx, float sy, float fx, float fy,
+    float* __restrict__ grad2d, float* __restrict__ absgrad, int* __restrict__ n_views,
+    float* __restrict__ max_radius) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t cnt = count[i];
+  if (cnt == 0) return;
+  float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
+  float q[4], s[3], raw_s[3], qn;
+  gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+  float gx = 0.f, gy = 0.f, ax = 0.f, ay = 0.f;
+  const uint32_t o0 = offsets_g[i], o1 = o0 + cnt;
+  for (uint32_t r = o0; r < o1; ++r) {
+    if (row_epoch[r] != epoch) continue;   // not reached by its (saturated) tile: zero gradient
+    const float* row = grad_inst + (size_t)r * gw;
+    const float2 g = *reinterpret_cast<const float2*>(row);
+    gx += g.x;
+    gy += g.y;
+    if constexpr (ABS) {
+      const float2 a = *reinterpret_cast<const float2*>(row + 10);
+      ax += a.x;
+      ay += a.y;
+    }
+  }
+  // the covariance the forward binned: with the filter its dilated one (a zero filter leaves it as it is)
+  GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+  const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
+  const double A = (double)fo.a * fx * fx, B = (double)o.b * fx * fy, D = (double)fo.d * fy * fy;
+  const double h = 0.5 * (A - D);
+  const double lmax = 0.5 * (A + D) + sqrt(h * h + B * B);
+  const float rad = (float)ceil(3.0 * sqrt(fmax(lmax, 0.0)));
+  grad2d[i] += sqrtf((gx * sx) * (gx * sx) + (gy * sy) * (gy * sy));
+  if constexpr (ABS) absgrad[i] += sqrtf((ax * sx) * (ax * sx) + (ay * sy) * (ay * sy));
+  n_views[i] += 1;
+  max_radius[i] = fmaxf(max_radius[i], rad);
+}
+
+}  // namespace
+
+cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const float* scale, int n, int scale_act,
+                                    const GsCam& cam, float near_plane, float half_w, float half_h,
+                                    const GsFilter2d& filt, const uint32_t* offsets_g, const uint32_t* count,
+                                    const float* grad_inst, int gw, const uint32_t* row_epoch, uint32_t epoch,
+                                    const GsFrameGeom& g, const gs_densify_stats& s, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  const float sx = (float)((double)g.width / (2.0 * (double)g.fx));
+  const float sy = (float)((double)g.height / (2.0 * (double)g.fy));
+  const int blocks = (n + kBlock - 1) / kBlock;
+#define GS_LAUNCH_STATS(ABS)                                                                                       \
+  densify_stats_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, scale_act, cam, near_plane, half_w,    \
+                                                       half_h, filt, offsets_g, count, grad_inst, gw, row_epoch,   \
+                                                       epoch, sx, sy, g.fx, g.fy, s.grad2d, s.absgrad, s.count,    \
+                                                       s.max_radius)
+  if (s.absgrad) GS_LAUNCH_STATS(true);
+  else GS_LAUNCH_STATS(false);
+#undef GS_LAUNCH_STATS
+  return cudaGetLastError();
+}

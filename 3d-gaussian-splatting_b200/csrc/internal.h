@@ -166,6 +166,16 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
                                             bool depth_grad, bool sh_gaussian, const GsFilter2d* filt = nullptr);
 
+// ---- densify_stats.cu ------------------------------------------------------------------
+// Accumulates the screen-space densification statistics of the backward that just wrote grad_inst (rows of gw floats;
+// s.absgrad != NULL reads columns 10, 11 written by the ABS blend kernels) into s's buffers.  One launch when n > 0.
+cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const float* scale, int n, int scale_act,
+                                    const GsCam& cam, float near_plane, float half_w, float half_h,
+                                    const GsFilter2d& filt /*the forward's; zero when it had none*/,
+                                    const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst, int gw,
+                                    const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
+                                    const gs_densify_stats& s, cudaStream_t st);
+
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
                                 void* keys, int key_bytes, uint32_t* vals, cudaStream_t st);
@@ -196,7 +206,12 @@ cudaError_t gs_launch_blend_bwd(const float4* pA, const float2* pB, const float4
                                 int grad_is_final, const GsCrop& crop, uint32_t* row_epoch /*nullable (packed only)*/,
                                 uint32_t epoch, int* tile_neff_b /*nullable: instances the backward consumed per tile*/,
                                 cudaStream_t st, const float* aux = nullptr /*forward's [Hp,Wp,2]*/,
-                                const float* grad_aux = nullptr /*non-null: AUX kernel; [Hp,Wp,2] or [h,w,2]*/);
+                                const float* grad_aux = nullptr /*non-null: AUX kernel; [Hp,Wp,2] or [h,w,2]*/,
+                                bool absgrad = false /*ABS kernel: sum |d/dx|, sum |d/dy| to columns 10, 11*/);
+// The ABS blend backward kernels exist only for the shipped RGB backward of the gather path (with and without AUX):
+// 0 when a frame of blend colour width d on that path (`gather`) runs one under the current knobs, else
+// GS_ERR_UNSUPPORTED with a message.
+int gs_blend_absgrad_supported(int d, bool gather);
 // The AUX blend kernels exist only for the shipped configurations of the gather path (RGB: the default blend knobs;
 // SH: the scalar and one-pixel-per-thread tensor-core kernels): 0 when the current tuning knobs for colour width d
 // select one, else GS_ERR_UNSUPPORTED with a message.

@@ -27,23 +27,8 @@ __global__ void __launch_bounds__(kBlock) jacobian_kernel(const float* __restric
 }
 
 // ---------------------------------------------------------------------------------------
-// Fused frame path.  Activations (splatter.py:519-524,:539-540) are applied in-register.
+// Fused frame path.  Activations (splatter.py:519-524,:539-540) are applied in-register (gs_load_activated).
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void load_activated(const float* __restrict__ quat, const float* __restrict__ scale,
-                                               int i, int scale_act, float q[4], float s[3], float raw_s[3],
-                                               float& qnorm) {
-  float4 q4 = reinterpret_cast<const float4*>(quat)[i];
-  qnorm = sqrtf(q4.x * q4.x + q4.y * q4.y + q4.z * q4.z + q4.w * q4.w);
-  q[0] = q4.x / qnorm;
-  q[1] = q4.y / qnorm;
-  q[2] = q4.z / qnorm;
-  q[3] = q4.w / qnorm;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    raw_s[k] = scale[3 * i + k];
-    s[k] = (scale_act == GS_SCALE_ABS) ? (fabsf(raw_s[k]) + 1e-4f) : expf(raw_s[k]);
-  }
-}
 
 // Unit direction from the camera centre C = -R^T t to the mean, in the world frame (the frame of the per-pixel rays,
 // so that an SH coefficient means the same in both evaluation modes); inv_len = 1 / |pos - C| = 1 / |p_c|.
@@ -85,7 +70,7 @@ __device__ __forceinline__ void fused_project_body(
   if (i < n) {
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
-    load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
     vis = o.visible;
     if (mask) mask[i] = o.visible ? 1 : 0;
@@ -262,7 +247,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     // issue the parameter loads BEFORE the row loop so that both round trips to HBM overlap
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
-    load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
     float coef[KG ? D : 1];

@@ -52,6 +52,24 @@ __device__ __forceinline__ void gs_jw_rows(const GsCam& cam, const float pc[3], 
   }
 }
 
+// Gaussian i's normalised quaternion q (and the norm qnorm of the raw one), activated scale s and raw scale raw_s, as
+// the fused frame path applies them (splatter.py:519-524).
+__device__ __forceinline__ void gs_load_activated(const float* __restrict__ quat, const float* __restrict__ scale,
+                                                  int i, int scale_act, float q[4], float s[3], float raw_s[3],
+                                                  float& qnorm) {
+  float4 q4 = reinterpret_cast<const float4*>(quat)[i];
+  qnorm = sqrtf(q4.x * q4.x + q4.y * q4.y + q4.z * q4.z + q4.w * q4.w);
+  q[0] = q4.x / qnorm;
+  q[1] = q4.y / qnorm;
+  q[2] = q4.z / qnorm;
+  q[3] = q4.w / qnorm;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    raw_s[k] = scale[3 * i + k];
+    s[k] = (scale_act == GS_SCALE_ABS) ? (fabsf(raw_s[k]) + 1e-4f) : expf(raw_s[k]);
+  }
+}
+
 // q (w,x,y,z) must be normalised and s activated by the caller.
 __device__ __forceinline__ GsProj gs_project(const GsCam& cam, const float p[3], const float q[4],
                                              const float s[3], float near_plane, float half_w, float half_h) {

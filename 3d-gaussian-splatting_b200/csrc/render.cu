@@ -165,6 +165,8 @@ struct gs_ctx {
   float filter2d_var = 0.3f;              //   its variance in px^2
   bool filt_on = false;                   // the last forward's filter (its backward uses it)
   GsFilter2d filt{};
+  bool stats_on = false;                  // gs_ctx_set_densify_stats: accumulated by the backwards that follow
+  gs_densify_stats stats{};
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -543,12 +545,21 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
     if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux needs the forward's aux");
     if (int rc = gs_blend_aux_supported(c->sh_gaussian ? 3 : c->d, false, true)) return rc;
   }
+  const int d = c->d;
+  const int blend_d = c->sh_gaussian ? 3 : d;   // colour width of the blend: the forward's SH mode, not the current one
+  // densification statistics: every backward that computes parameter gradients, not a camera-only one
+  const bool stats = c->stats_on && !cam_only;
+  const bool absgrad = stats && c->stats.absgrad;
+  if (stats) {
+    if (c->stats.n != c->n)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: the densify statistics are sized for another n");
+    if (absgrad)
+      if (int rc = gs_blend_absgrad_supported(blend_d, c->gather)) return rc;
+  }
   if (int rc = gs_check_device(c->device, "gs_render_backward")) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
   size_t M = (size_t)c->m;
-  const int d = c->d;
-  const int blend_d = c->sh_gaussian ? 3 : d;   // colour width of the blend: the forward's SH mode, not the current one
   const size_t grow = blend_d == 3 ? (size_t)GS_GREC * 4 : (size_t)gs_sh_grad_width(d) * 4;
   GS_CUDA_TRY(c->grad_inst.reserve(M * grow + 16, st));
   {
@@ -572,7 +583,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                       c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image, grad_image,
                                       c->grad_inst.as<float>(),
                                       grad_is_final, crop, c->row_epoch.as<uint32_t>(), c->epoch,
-                                      c->tile_neff_b.as<int>(), st, aux, grad_aux));
+                                      c->tile_neff_b.as<int>(), st, aux, grad_aux, absgrad));
     } else {
       const float* rp = c->rays.as<float>();
       GsRayPtrs rays{rp, rp + 3, rp + 6, rp + 9};
@@ -616,6 +627,13 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                             c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                             grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
                                             grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
+    if (c->n > 0) gs_count_launch();
+  }
+  if (stats) {
+    GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
+                                        c->half_h, c->filt_on ? c->filt : GsFilter2d{}, c->offsets_g.as<uint32_t>(),
+                                        c->count.as<uint32_t>(), c->grad_inst.as<float>(), (int)(grow / 4),
+                                        c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st));
     if (c->n > 0) gs_count_launch();
   }
   gs_mark(c, 9, st);
@@ -712,6 +730,21 @@ extern "C" int gs_ctx_set_filter2d(gs_ctx* c, int mode, float variance_px2) {
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter2d: variance must be finite and > 0");
   c->filter2d = mode;
   c->filter2d_var = variance_px2;
+  return 0;
+}
+
+extern "C" int gs_ctx_set_densify_stats(gs_ctx* c, const gs_densify_stats* s) {
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_densify_stats: null ctx");
+  if (!s) {
+    c->stats_on = false;
+    c->stats = gs_densify_stats{};
+    return 0;
+  }
+  if (s->n < 0 || (s->n > 0 && (!s->grad2d || !s->count || !s->max_radius)))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG,
+                            "gs_ctx_set_densify_stats: n must be >= 0 and grad2d, count, max_radius non-NULL");
+  c->stats = *s;
+  c->stats_on = true;
   return 0;
 }
 

@@ -94,6 +94,58 @@ class Gaussian3ds(nn.Module):
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.pos.shape[0])
 
 
+DENSIFY_STATS = ("none", "grad", "absgrad")
+
+
+class DensifyStats:
+    """Screen-space densification statistics of the Gaussians, accumulated on the device by every backward of the
+    fused frame path while they are registered with a `RenderContext` (`gaussian.RenderContext.set_densify_stats`):
+
+    - `grad2d[n]`: sum over views of |dL/d(mean2d)| in the NDC units of 3DGS's `viewspace_points.grad`;
+    - `absgrad[n]` (or None): the same with the absolute value of every pixel's contribution taken before summing
+      (AbsGS; gsplat's `absgrad=True`);
+    - `count[n]` (int32): the views in which the Gaussian was binned into at least one tile;
+    - `max_radius[n]`: its largest screen radius in pixels, ceil(3 sqrt(lambda_max)).
+
+    The score 3DGS compares with its threshold (0.0002) is `grad2d / count.clamp(min=1)`."""
+
+    def __init__(self, n, absgrad=False, device=None, rctx=None):
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.with_absgrad = bool(absgrad)
+        self._rctx = rctx
+        self.grad2d = self.absgrad = self.count = self.max_radius = None
+        self.reset(n)
+
+    @property
+    def n(self):
+        return self.grad2d.numel()
+
+    def reset(self, n):
+        """Zero the statistics, sized for n Gaussians (re-registered with the context when n changes)."""
+        n = int(n)
+        if self.grad2d is not None and self.n == n:
+            for t in (self.grad2d, self.absgrad, self.count, self.max_radius):
+                if t is not None:
+                    t.zero_()
+            return
+        f = dict(device=self.device, dtype=torch.float32)
+        self.grad2d = torch.zeros(n, **f)
+        self.absgrad = torch.zeros(n, **f) if self.with_absgrad else None
+        self.count = torch.zeros(n, device=self.device, dtype=torch.int32)
+        self.max_radius = torch.zeros(n, **f)
+        if self._rctx is not None:
+            self._rctx.set_densify_stats(self.grad2d, self.count, self.max_radius, self.absgrad)
+
+    def all_reduce(self, group=None):
+        """Combine the statistics of all ranks of `group` (sums, and the max of max_radius).  Under data parallel
+        every rank renders other views: call this on every rank before densifying."""
+        import torch.distributed as dist
+        for t in (self.grad2d, self.absgrad, self.count):
+            if t is not None:
+                dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(self.max_radius, op=dist.ReduceOp.MAX, group=group)
+
+
 class Tiles:
     """Padded render-target geometry (reference splatter.py:255-272)."""
 
@@ -120,7 +172,7 @@ class Splatter(nn.Module):
                  tile_culling_method="prob2", tile_culling_dist_thresh=0.5, tile_culling_prob_thresh=0.1,
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
-                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3):
+                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none"):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -140,7 +192,12 @@ class Splatter(nn.Module):
         (the original 3D Gaussian Splatting rasterizer, 0.3); "antialias" dilates and scales the opacity by
         sqrt(det / det'), keeping each Gaussian's screen-space integral (Mip-Splatting's 2-D filter, gsplat's
         "antialiased").  Every frame of this Splatter follows it, with gradients.  A scene renders differently under
-        another mode: train and render with the same one."""
+        another mode: train and render with the same one.
+
+        `densify_stats`: "none" (default); "grad" accumulates the screen-space densification statistics of 3D
+        Gaussian Splatting in `self.densify_stats` (a `DensifyStats`: view-space gradient norm, view count, largest
+        screen radius) during every backward; "absgrad" also the absolute gradient of AbsGS (not available with
+        per-pixel SH colour).  `adaptive_control_screen` densifies from them."""
         super().__init__()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
@@ -160,6 +217,10 @@ class Splatter(nn.Module):
             raise ValueError(f"filter2d_variance must be a number, not {filter2d_variance!r}") from None
         if not (math.isfinite(filter2d_variance) and filter2d_variance > 0):
             raise ValueError(f"filter2d_variance must be finite and > 0, not {filter2d_variance!r}")
+        if densify_stats not in DENSIFY_STATS:
+            raise ValueError(f"densify_stats must be one of {DENSIFY_STATS}, not {densify_stats!r}")
+        if densify_stats == "absgrad" and use_sh_coeff and sh_eval == "pixel":
+            raise ValueError("densify_stats='absgrad' needs the RGB blend: RGB colour or sh_eval='gaussian'")
         self.sh_eval = sh_eval
         self.filter2d, self.filter2d_variance = filter2d, filter2d_variance
         self.use_sh_coeff = bool(use_sh_coeff)
@@ -190,6 +251,10 @@ class Splatter(nn.Module):
             self._rctx = gaussian.RenderContext()
         self._rctx.set_sh_eval(SH_EVAL[sh_eval])                   # every frame of this Splatter, fused or not
         self._rctx.set_filter2d(FILTER2D[filter2d], filter2d_variance)
+        self.densify_stats = None
+        if densify_stats != "none":
+            self.densify_stats = DensifyStats(self.gaussian_3ds.pos.shape[0], densify_stats == "absgrad", self.device,
+                                              self._rctx)
         self.ground_truth = None
         self.culling_mask = None
         self.n_tile_gaussians = 0
@@ -292,6 +357,7 @@ class Splatter(nn.Module):
     def render_padded(self):
         """Padded, un-clamped image (what reference `render` returns, splatter.py:563-634)."""
         g, v = self.gaussian_3ds, self.current_view
+        self._size_densify_stats()
         image, mask = render_frame(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                    v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                    self.tile_culling_prob_thresh, self.scale_activation)
@@ -304,6 +370,7 @@ class Splatter(nn.Module):
         kernels (`render_frame_final`)."""
         self.set_camera(camera_id, extrinsics, intrinsics)
         g, v = self.gaussian_3ds, self.current_view
+        self._size_densify_stats()
         image, mask = render_frame_final(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                          v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                          self.tile_culling_prob_thresh, self.scale_activation)
@@ -318,6 +385,7 @@ class Splatter(nn.Module):
         All three are differentiable (`renderer.render_frame_aux`)."""
         self.set_camera(camera_id, extrinsics, intrinsics)
         g, v = self.gaussian_3ds, self.current_view
+        self._size_densify_stats()
         image, depth, alpha, mask = render_frame_aux(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], v["rot"], v["tran"],
                                                      self.near, self.tile_culling_prob_thresh, self.scale_activation,
@@ -339,6 +407,7 @@ class Splatter(nn.Module):
         if self.current_view is None:
             raise ValueError("render_at_pose: no current view; pass camera_id")
         g, v = self.gaussian_3ds, self.current_view
+        self._size_densify_stats()
         image, depth, alpha, mask = render_frame_cam(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], rot, tran, self.near,
                                                      self.tile_culling_prob_thresh, self.scale_activation,
@@ -353,6 +422,43 @@ class Splatter(nn.Module):
         self.set_camera(camera_id, extrinsics, intrinsics)
         padded = self.render_padded()
         return self.tile_info.crop(torch.clamp(padded, 0, 1))
+
+    # -- densification from screen-space statistics ----------------------------------------------
+    def _size_densify_stats(self):
+        # the statistics follow the scene: when its Gaussians were replaced by other means (adaptive_control, a
+        # checkpoint), they restart from zero at the new count
+        if self.densify_stats is not None and self.densify_stats.n != self.gaussian_3ds.pos.shape[0]:
+            self.densify_stats.reset(self.gaussian_3ds.pos.shape[0])
+
+    @torch.no_grad()
+    def adaptive_control_screen(self, taus, delete_thresh, grad_thresh=0.0002, use_abs=False, max_screen_size=None,
+                                use_clone=True, use_split=True, generator=None):
+        """Prune / clone / split from the screen-space statistics (`densify_stats`), with 3DGS's rule: a kept Gaussian
+        densifies when grad2d / count (absgrad / count with `use_abs`) >= `grad_thresh`; clones are exact copies.
+        With `max_screen_size` (pixels), Gaussians whose screen radius exceeded it are pruned too.  Opacity and
+        scale-norm pruning and the clone / split choice by `taus` are `Gaussian3ds.adaptive_control`'s.  The
+        parameters are re-created like `adaptive_control` (the caller rebuilds its optimizer), and the statistics
+        restart from zero.  Under data parallel, call `densify_stats.all_reduce()` first.  Returns the same dict
+        as `adaptive_control`."""
+        st = self.densify_stats
+        if st is None:
+            raise RuntimeError("adaptive_control_screen needs Splatter(..., densify_stats='grad' or 'absgrad')")
+        if use_abs and st.absgrad is None:
+            raise ValueError("use_abs=True needs Splatter(..., densify_stats='absgrad')")
+        g = self.gaussian_3ds
+        if st.n != g.pos.shape[0]:
+            raise RuntimeError("densify_stats are sized for another number of Gaussians than the scene has")
+        args = [t.detach().contiguous() for t in (g.pos, g.rgb, g.opa, g.quat, g.scale)]
+        new, (n_deleted, n_clone, n_split) = gaussian.densify_stats(
+            *args, st.absgrad if use_abs else st.grad2d, st.count,
+            st.max_radius if max_screen_size is not None else None,
+            float(max_screen_size) if max_screen_size is not None else 0.0,
+            0 if self.scale_activation == "abs" else 1, inverse_sigmoid(0.02), float(delete_thresh),
+            float(grad_thresh), float(taus), bool(use_clone), bool(use_split), generator)
+        g.pos, g.rgb, g.opa, g.quat, g.scale = (nn.Parameter(t) for t in new)
+        self.n_gaussians = g.pos.shape[0]
+        st.reset(self.n_gaussians)
+        return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.n_gaussians)
 
     def save_checkpoint(self, path, optimizer=None, iteration=None, trainer_state=None):
         """reference Trainer.save_checkpoint (train.py:283-291) + resume state; see checkpoint.py."""

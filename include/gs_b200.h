@@ -281,6 +281,36 @@ int gs_ctx_set_sh_eval(gs_ctx* ctx, int mode);
 #define GS_FILTER2D_ANTIALIAS 2
 int gs_ctx_set_filter2d(gs_ctx* ctx, int mode, float variance_px2);
 
+/* Screen-space densification statistics (additive; default off).  While a context has them set, every backward that
+ * computes parameter gradients (plain, final, aux, cam with parameter gradients, gs_render_forward_backward_host, with
+ * or without a gradient push) accumulates, for every Gaussian i with count[i] > 0 in its forward (i.e. binned into at
+ * least one tile):
+ *   grad2d[i]    += |(gx W / (2 fx), gy H / (2 fy))|: (gx, gy) = dL/d(mean2d) in normalised image-plane units, the sum
+ *                   of Gaussian i's per-instance gradients; W, H the un-padded image size, fx, fy the focal lengths in
+ *                   pixels.  The scale gives the NDC convention of 3DGS's viewspace_points.grad and gsplat, so their
+ *                   threshold 0.0002 means the same here for the same loss normalisation.
+ *   absgrad[i]   += |(Ax W / (2 fx), Ay H / (2 fy))| with Ax = sum_p |g_x,p|, Ay = sum_p |g_y,p| over the pixels' own
+ *                   contributions to (gx, gy) (AbsGS; gsplat absgrad=True), depth / alpha terms included.  NULL: off.
+ *   count[i]     += 1 (the 3DGS denominator: the views in which the Gaussian got an instance).
+ *   max_radius[i] = max(max_radius[i], ceil(3 sqrt(lambda_max))), lambda_max the largest eigenvalue in px^2 of the
+ *                   2-D covariance the forward binned (after the 2-D filter when one is set); 3DGS's radius without its
+ *                   0.1 floor.
+ * A camera-only gs_render_backward_cam leaves them alone.  The caller zeroes the buffers (all device, [n]) and keeps
+ * them alive while they are set; results are bit-deterministic (no atomics).  One launch per backward when n > 0,
+ * timed in stage 7 of gs_frame_stage_ms.  The backward refuses, before any launch: s->n != the forward's n
+ * (GS_ERR_INVALID_ARG); absgrad on a frame the shipped RGB blend backward of the gather path does not run (per-pixel SH
+ * colour, the packed path, other backward blend knobs: GS_ERR_UNSUPPORTED).
+ * gs_ctx_set_densify_stats: NULL turns them off; a null ctx, n < 0, or a NULL grad2d / count / max_radius with n > 0
+ * is GS_ERR_INVALID_ARG.  The pointers are the caller's, as with gs_ctx_set_grad_push. */
+typedef struct gs_densify_stats {
+  int n;               /* must equal the n of the frame whose backward runs */
+  float* grad2d;       /* [n] */
+  float* absgrad;      /* [n] or NULL */
+  int* count;          /* [n] */
+  float* max_radius;   /* [n] */
+} gs_densify_stats;
+int gs_ctx_set_densify_stats(gs_ctx* ctx, const gs_densify_stats* s /* NULL: off */);
+
 /* Per-stage device timing with CUDA events recorded on the frame's stream (off by default).
  * gs_frame_stage_ms fills out[GS_N_STAGES] with the milliseconds of the last frame's stages:
  * 0 project, 1 depth sort of Gaussians + scan + M readback, 2 key emit, 3 tile-id radix sort,
@@ -339,7 +369,8 @@ int gs_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg
  *                     three flags (dst[b][n] = totals: n_keep, n_clone, n_split).  No synchronisation.
  *   gs_densify_apply: writes the n_keep + n_clone + n_split rows of the new parameter arrays, laid out like the
  *                     reference's torch.cat: kept (in order), clones (in order), second split samples (in order).
- *                     normals: [2][n_split][3].  Output arrays are caller-allocated. */
+ *                     normals: [2][n_split][3].  Output arrays are caller-allocated.  grad == NULL: clones are exact
+ *                     copies (3DGS; the plan of gs_densify_plan_stats). */
 size_t gs_densify_workspace_bytes(int n);
 int gs_densify_plan(const float* opa, const float* scale, const float* grad, int n, int scale_activation,
                     float opa_logit_min, float delete_thresh, float grad_thresh, int grad_agg_max, float tau,
@@ -350,6 +381,15 @@ int gs_densify_apply(const float* pos, const float* rgb, const float* opa, const
                      const float* normals, int n_keep, int n_clone, int n_split, int scale_activation,
                      float* out_pos, float* out_rgb, float* out_opa, float* out_quat, float* out_scale,
                      gs_stream_t stream);
+/* gs_densify_plan from screen-space statistics (gs_ctx_set_densify_stats), as 3DGS scores them: a kept Gaussian
+ * densifies when accum[i] / max(count[i], 1) >= grad_thresh (accum: the caller's grad2d or absgrad).  With a non-NULL
+ * max_radius, a Gaussian whose max_radius > max_screen_px is pruned as well.  Opacity / scale-norm pruning and the
+ * clone / split choice by tau are gs_densify_plan's.  Same outputs, workspace and synchronisation. */
+int gs_densify_plan_stats(const float* opa, const float* scale, const float* accum, const int* count,
+                          const float* max_radius /* nullable */, float max_screen_px, int n, int scale_activation,
+                          float opa_logit_min, float delete_thresh, float grad_thresh, float tau, int use_clone,
+                          int use_split, unsigned char* code, int* dst, void* workspace, size_t workspace_bytes,
+                          gs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * Next-row widening (SURVEY.md §8 f-3): the training loss of reference train.py:99-107 on the device,

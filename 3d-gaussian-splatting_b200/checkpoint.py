@@ -5,7 +5,9 @@ tensors `pos, opa, rgb, quat, scale`, so the reference's own `--ckpt` / `Splatte
 splatter.py:417-424, loads our files and we load theirs) and - what the reference lacks - everything a
 true resume needs under the extra key `"resume"`: optimizer moments and step count, iteration, the
 densification statistics of train.py:82-83, and the RNG states (numpy picks the camera, train.py:93;
-torch samples split positions, utils.py:391-402).  Extra keys are ignored by the reference's loader.
+torch samples split positions, utils.py:391-402).  A scene with per-Gaussian features
+(`Splatter(..., n_features=F)`) also stores them under `"feat"` [n, F].  Extra keys are ignored by the reference's
+loader.
 """
 from __future__ import annotations
 
@@ -35,6 +37,8 @@ def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = N
     """`path` is the checkpoint file (train.py writes `<exp>/ckpt.pth`)."""
     g = splatter.gaussian_3ds
     ckpt = {k: getattr(g, k).detach().clone() for k in KEYS}
+    if g.feat is not None:
+        ckpt["feat"] = g.feat.detach().clone()
     ckpt["resume"] = {
         "iteration": iteration,
         "optimizer": _optimizer_state(optimizer),
@@ -54,7 +58,8 @@ def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = N
 
 def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
     """Returns the dict; with `splatter` the parameters are replaced in place (new nn.Parameters, like
-    adaptive_control - rebuild torch optimizers before passing them here); with `optimizer` its state is restored.
+    adaptive_control - rebuild torch optimizers before passing them here), the features too when the file has them
+    (a splatter with features loading a file without them gets zero features); with `optimizer` its state is restored.
     A reference-written file (five keys only) loads the parameters and returns `resume == None`."""
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     missing = [k for k in KEYS if k not in ckpt]
@@ -67,6 +72,16 @@ def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
             for k in KEYS:
                 t = ckpt[k].detach().to(device=splatter.device, dtype=torch.float32).contiguous()
                 setattr(g, k, torch.nn.Parameter(t))
+            n = g.pos.shape[0]
+            if ckpt.get("feat") is not None:
+                f = ckpt["feat"].detach().to(device=splatter.device, dtype=torch.float32).contiguous()
+                if f.shape[0] != n or (splatter.n_features and f.shape[1] != splatter.n_features):
+                    raise ValueError(f"{path}: feat {list(f.shape)} does not fit {n} Gaussians with "
+                                     f"{splatter.n_features} features")
+                g.feat = torch.nn.Parameter(f)
+                splatter.n_features = int(f.shape[1])
+            elif g.feat is not None:
+                g.feat = torch.nn.Parameter(torch.zeros(n, splatter.n_features, device=splatter.device))
         splatter.n_gaussians = g.pos.shape[0]
     if optimizer is not None and res is not None and res.get("optimizer") is not None:
         st = res["optimizer"]

@@ -562,6 +562,96 @@ struct RenderContext {
              "gs_render_backward_cam");
   }
 
+  // feature maps (gs_render_forward_feat): forward_aux's outputs plus (map padded [Hp,Wp,f], map_final [H,W,f] or None):
+  // (final or None, raw, aux, aux_final or None, map, map_final or None, mask)
+  py::tuple forward_feat(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                         torch::Tensor scale, torch::Tensor feat, int width, int height, float fx, float fy,
+                         torch::Tensor rot, torch::Tensor tran, float near, float thresh, int scale_activation,
+                         std::optional<std::vector<double>> background, bool final) {
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(feat);
+    int64_t n = pos.size(0);
+    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
+                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31) &&
+                    feat.dim() == 2 && feat.size(0) == n,
+                "RenderContext.forward_feat: bad shapes");
+    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
+    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_feat: background must have 3 values");
+    c10::cuda::CUDAGuard guard(pos.device());
+    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
+    const int64_t f = feat.size(1);
+    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
+    auto raw = torch::empty({hp, wp, 3}, pos.options());
+    auto aux = torch::empty({hp, wp, 2}, pos.options());
+    auto map = torch::empty({hp, wp, f}, pos.options());
+    torch::Tensor fin, aux_fin, map_fin;
+    if (final) {
+      fin = torch::empty({height, width, 3}, pos.options());
+      aux_fin = torch::empty({height, width, 2}, pos.options());
+      map_fin = torch::empty({height, width, f}, pos.options());
+    }
+    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
+    float bg[3] = {0.f, 0.f, 0.f};
+    if (background)
+      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
+    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
+    gs_render_feat ft{(int)f, fp(feat), fpm(map), final ? fpm(map_fin) : nullptr};
+    check_rc(gs_render_forward_feat(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                    scale_activation, &cam, fpm(raw), final ? fpm(fin) : nullptr,
+                                    mask.data_ptr<int64_t>(), &ax, &ft, cur_stream()),
+             "gs_render_forward_feat");
+    ++frame;
+    py::object none = py::none();
+    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, map,
+                          final ? py::cast(map_fin) : none, mask);
+  }
+
+  // backward of forward_feat; grad_map = None: the plain / aux backward kernels, g_feat zero-filled
+  void backward_feat_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                          torch::Tensor scale, torch::Tensor feat, torch::Tensor raw, torch::Tensor grad_image,
+                          bool grad_is_final, torch::Tensor aux, std::optional<torch::Tensor> grad_aux,
+                          torch::Tensor map, std::optional<torch::Tensor> grad_map, torch::Tensor g_pos,
+                          torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
+                          torch::Tensor g_feat, int64_t expected_frame) {
+    check_frame(expected_frame, "RenderContext.backward_feat_into");
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    GS_CHECK_F32(feat); GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(map); GS_CHECK_F32(g_pos);
+    GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa); GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale); GS_CHECK_F32(g_feat);
+    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3 && aux.dim() == 3 && aux.size(0) == raw.size(0) &&
+                    aux.size(1) == raw.size(1) && aux.size(2) == 2 && map.dim() == 3 && map.size(0) == raw.size(0) &&
+                    map.size(1) == raw.size(1) && feat.dim() == 2 && map.size(2) == feat.size(1),
+                "RenderContext.backward_feat_into: raw must be [Hp,Wp,3], aux [Hp,Wp,2] and map [Hp,Wp,f]");
+    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
+                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
+                "RenderContext.backward_feat_into: grad_image must be [H,W,3] (final) or match raw");
+    if (grad_aux) {
+      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
+                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
+                      grad_aux->size(2) == 2,
+                  "RenderContext.backward_feat_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
+    }
+    if (grad_map) {
+      TORCH_CHECK(grad_map->is_cuda() && grad_map->scalar_type() == at::kFloat && grad_map->dim() == 3 &&
+                      grad_map->size(0) == grad_image.size(0) && grad_map->size(1) == grad_image.size(1) &&
+                      grad_map->size(2) == feat.size(1),
+                  "RenderContext.backward_feat_into: grad_map must be float32 [rows, cols, f] like grad_image");
+    }
+    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
+                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel() &&
+                    g_feat.numel() == feat.numel(),
+                "RenderContext.backward_feat_into: gradient buffers must match their parameters");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor ga, gm;
+    if (grad_aux) ga = grad_aux->contiguous();
+    if (grad_map) gm = grad_map->contiguous();
+    check_rc(gs_render_backward_feat(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
+                                     grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fp(feat), fp(map),
+                                     grad_map ? fp(gm) : nullptr, fpm(g_pos), fpm(g_rgb), fpm(g_opa), fpm(g_quat),
+                                     fpm(g_scale), fpm(g_feat), cur_stream()),
+             "gs_render_backward_feat");
+  }
+
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
   py::dict stats() {
@@ -648,7 +738,8 @@ std::tuple<torch::Tensor, torch::Tensor> loss_l1_ssim(torch::Tensor image, torch
 static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_apply(
     const torch::Tensor& pos, const torch::Tensor& rgb, const torch::Tensor& opa, const torch::Tensor& quat,
     const torch::Tensor& scale, const float* grad, int scale_activation, double clone_dt,
-    c10::optional<at::Generator> gen, const torch::Tensor& code, const torch::Tensor& dst) {
+    c10::optional<at::Generator> gen, const torch::Tensor& code, const torch::Tensor& dst,
+    const c10::optional<torch::Tensor>& feat) {
   const int64_t n = pos.size(0);
   int64_t nk = n, nc = 0, nsp = 0;
   if (n > 0) {
@@ -666,6 +757,12 @@ static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_appl
                             scale_activation, fpm(out[0]), fpm(out[1]), fpm(out[2]), fpm(out[3]), fpm(out[4]),
                             cur_stream()),
            "gs_densify_apply");
+  if (feat) {   // per-Gaussian features follow the same plan (a 6th tensor)
+    out.push_back(torch::empty({m, feat->size(1)}, pos.options()));
+    check_rc(gs_densify_apply_rows(fp(*feat), (int)n, (int)feat->size(1), code.data_ptr<uint8_t>(), dst.data_ptr<int>(),
+                                   (int)nk, (int)nc, (int)nsp, fpm(out[5]), cur_stream()),
+             "gs_densify_apply_rows");
+  }
   return {out, {n - nk, nc, nsp}};
 }
 
@@ -673,12 +770,17 @@ static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_appl
 std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify(
     torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale, torch::Tensor grad,
     int scale_activation, double opa_logit_min, double delete_thresh, double grad_thresh, bool grad_agg_max, double tau,
-    bool use_clone, bool use_split, double clone_dt, c10::optional<at::Generator> gen) {
+    bool use_clone, bool use_split, double clone_dt, c10::optional<at::Generator> gen,
+    c10::optional<torch::Tensor> feat) {
   GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(grad);
   const int64_t n = pos.size(0);
   TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && rgb.dim() == 2 && rgb.size(0) == n && opa.numel() == n &&
                   quat.numel() == 4 * n && scale.numel() == 3 * n && grad.numel() == 3 * n && n < (int64_t(1) << 31),
               "densify: bad shapes");
+  if (feat) {
+    GS_CHECK_F32(*feat);
+    TORCH_CHECK(feat->dim() == 2 && feat->size(0) == n && feat->size(1) > 0, "densify: feat must be [n, f]");
+  }
   c10::cuda::CUDAGuard guard(pos.device());
   auto bopt = pos.options().dtype(at::kByte);
   auto code = torch::empty({n + 1}, bopt);
@@ -689,7 +791,8 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify(
                            use_split ? 1 : 0, code.data_ptr<uint8_t>(), dst.data_ptr<int>(), ws.data_ptr(),
                            (size_t)ws.numel(), cur_stream()),
            "gs_densify_plan");
-  return densify_apply(pos, rgb, opa, quat, scale, grad.data_ptr<float>(), scale_activation, clone_dt, gen, code, dst);
+  return densify_apply(pos, rgb, opa, quat, scale, grad.data_ptr<float>(), scale_activation, clone_dt, gen, code, dst,
+                       feat);
 }
 
 // densification from the screen-space statistics (gs_densify_plan_stats; clones are exact copies, as in 3DGS)
@@ -697,7 +800,7 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_stats(
     torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale,
     torch::Tensor accum, torch::Tensor count, c10::optional<torch::Tensor> max_radius, double max_screen_px,
     int scale_activation, double opa_logit_min, double delete_thresh, double grad_thresh, double tau, bool use_clone,
-    bool use_split, c10::optional<at::Generator> gen) {
+    bool use_split, c10::optional<at::Generator> gen, c10::optional<torch::Tensor> feat) {
   GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(accum);
   const int64_t n = pos.size(0);
   TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && rgb.dim() == 2 && rgb.size(0) == n && opa.numel() == n &&
@@ -708,6 +811,10 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_stats(
   if (max_radius) {
     GS_CHECK_F32(*max_radius);
     TORCH_CHECK(max_radius->numel() == n, "densify_stats: max_radius must have n elements");
+  }
+  if (feat) {
+    GS_CHECK_F32(*feat);
+    TORCH_CHECK(feat->dim() == 2 && feat->size(0) == n && feat->size(1) > 0, "densify_stats: feat must be [n, f]");
   }
   c10::cuda::CUDAGuard guard(pos.device());
   auto bopt = pos.options().dtype(at::kByte);
@@ -720,7 +827,7 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_stats(
                                  (float)tau, use_clone ? 1 : 0, use_split ? 1 : 0, code.data_ptr<uint8_t>(),
                                  dst.data_ptr<int>(), ws.data_ptr(), (size_t)ws.numel(), cur_stream()),
            "gs_densify_plan_stats");
-  return densify_apply(pos, rgb, opa, quat, scale, nullptr, scale_activation, 0.0, gen, code, dst);
+  return densify_apply(pos, rgb, opa, quat, scale, nullptr, scale_activation, 0.0, gen, code, dst, feat);
 }
 
 // NVLS in-place all-reduce of a symmetric flat buffer (multicast address as an integer)
@@ -817,6 +924,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
            py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
            py::arg("g_quat"), py::arg("g_scale"), py::arg("grad_cam"), py::arg("expected_frame") = -1)
+      .def("forward_feat", &RenderContext::forward_feat, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("feat"), py::arg("width"), py::arg("height"), py::arg("fx"),
+           py::arg("fy"), py::arg("rot"), py::arg("tran"), py::arg("near"), py::arg("thresh"),
+           py::arg("scale_activation"), py::arg("background") = py::none(), py::arg("final") = true)
+      .def("backward_feat_into", &RenderContext::backward_feat_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("feat"), py::arg("raw"), py::arg("grad_image"),
+           py::arg("grad_is_final"), py::arg("aux"), py::arg("grad_aux"), py::arg("map"), py::arg("grad_map"),
+           py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"), py::arg("g_quat"), py::arg("g_scale"),
+           py::arg("g_feat"), py::arg("expected_frame") = -1)
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
       .def("stats", &RenderContext::stats)
@@ -839,13 +955,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("densify", &densify, "prune / clone / split on the device (reference splatter.py:122-228)", py::arg("pos"),
         py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("grad"), py::arg("scale_activation"),
         py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("grad_agg_max"), py::arg("tau"),
-        py::arg("use_clone"), py::arg("use_split"), py::arg("clone_dt"), py::arg("generator") = py::none());
+        py::arg("use_clone"), py::arg("use_split"), py::arg("clone_dt"), py::arg("generator") = py::none(),
+        py::arg("feat") = py::none());
   m.def("densify_stats", &densify_stats,
         "prune / clone / split on the device from screen-space densification statistics (gs_densify_plan_stats)",
         py::arg("pos"), py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("accum"),
         py::arg("count"), py::arg("max_radius"), py::arg("max_screen_px"), py::arg("scale_activation"),
         py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("tau"),
-        py::arg("use_clone"), py::arg("use_split"), py::arg("generator") = py::none());
+        py::arg("use_clone"), py::arg("use_split"), py::arg("generator") = py::none(), py::arg("feat") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
   m.def("tune", [](const std::string& name, int value) { check_rc(gs_tune(name.c_str(), value), "gs_tune"); },

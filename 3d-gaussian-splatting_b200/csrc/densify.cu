@@ -155,6 +155,23 @@ __global__ void __launch_bounds__(kBlock) densify_apply_kernel(
   }
 }
 
+// row i of a per-Gaussian [n, w] tensor to the rows densify_apply_kernel gives Gaussian i: kept, clone, second split
+// sample; every one an exact copy
+__global__ void __launch_bounds__(kBlock) densify_apply_rows_kernel(
+    const float* __restrict__ src, int n, int w, const unsigned char* __restrict__ code,
+    const int* __restrict__ dst_keep, const int* __restrict__ dst_clone, const int* __restrict__ dst_split, int n_keep,
+    int n_clone, float* __restrict__ out) {
+  const long long t = (long long)blockIdx.x * kBlock + threadIdx.x;
+  if (t >= (long long)n * w) return;
+  const int i = (int)(t / w), k = (int)(t % w);
+  const unsigned char c = code[i];
+  if (!(c & 1)) return;                                            // pruned
+  const float v = src[t];
+  out[(size_t)dst_keep[i] * w + k] = v;
+  if (c & 4) out[((size_t)n_keep + n_clone + dst_split[i]) * w + k] = v;
+  else if (c & 2) out[((size_t)n_keep + dst_clone[i]) * w + k] = v;
+}
+
 inline size_t up256(size_t x) { return (x + 255) / 256 * 256; }
 
 size_t scan_tmp_bytes(int n) {
@@ -234,6 +251,20 @@ extern "C" int gs_densify_apply(const float* pos, const float* rgb, const float*
   densify_apply_kernel<<<(n + kBlock - 1) / kBlock, kBlock, 0, (cudaStream_t)stream>>>(
       pos, rgb, opa, quat, scale, n, d, code, dst, dst + (n + 1), dst + 2 * (size_t)(n + 1), grad, clone_dt, normals,
       n_split, scale_activation, n_keep, n_clone, out_pos, out_rgb, out_opa, out_quat, out_scale);
+  GS_CUDA_TRY(cudaGetLastError());
+  gs_count_launch();
+  return 0;
+}
+
+extern "C" int gs_densify_apply_rows(const float* src, int n, int w, const unsigned char* code, const int* dst,
+                                     int n_keep, int n_clone, int n_split, float* out, gs_stream_t stream) {
+  if (n < 0 || w <= 0 || n_keep < 0 || n_clone < 0 || n_split < 0 ||
+      (n > 0 && (!src || !code || !dst || (n_keep + n_clone + n_split > 0 && !out))))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_densify_apply_rows: bad arguments");
+  if (n == 0) return 0;
+  const long long threads = (long long)n * w;
+  densify_apply_rows_kernel<<<(int)((threads + kBlock - 1) / kBlock), kBlock, 0, (cudaStream_t)stream>>>(
+      src, n, w, code, dst, dst + (n + 1), dst + 2 * (size_t)(n + 1), n_keep, n_clone, out);
   GS_CUDA_TRY(cudaGetLastError());
   gs_count_launch();
   return 0;

@@ -176,6 +176,27 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                     const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
                                     const gs_densify_stats& s, cudaStream_t st);
 
+// ---- blend_feat.cu ---------------------------------------------------------------------
+// Feature maps (gs_render_forward_feat / gs_render_backward_feat), gather path only.  f: 8, 16 or 32.
+bool gs_feat_width_ok(int f);
+// the RGB forward (+ AUX: background, depth / alpha) that also writes map[Hp,Wp,f] and map_final[h,w,f] (nullable)
+cudaError_t gs_launch_blend_feat_fwd(const GsRec* grec, const float* feat, int f, const uint32_t* ids,
+                                     const int* tile_accum, const GsFrameGeom& g, float* image, int* tile_neff,
+                                     float* final_img, const GsCrop& crop, const GsAuxOut* aux /*nullable*/, float* map,
+                                     float* map_final, cudaStream_t st);
+// the RGB backward (+ AUX when grad_aux) with the feature terms: GS_GREC rows to grad_inst, f-float rows to
+// grad_feat_inst, both at the instance's slot and tagged in row_epoch
+cudaError_t gs_launch_blend_feat_bwd(const GsRec* grec, const float* feat, int f, const uint32_t* ids,
+                                     const uint32_t* goff, const int* tile_accum, const GsFrameGeom& g,
+                                     const float* image, const float* grad_image, const float* map,
+                                     const float* grad_map, float* grad_inst, float* grad_feat_inst, int grad_is_final,
+                                     const GsCrop& crop, uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b,
+                                     const float* aux, const float* grad_aux, cudaStream_t st);
+// grad_feat[n, f] = per-Gaussian sums of the epoch-tagged rows of grad_feat_inst (one launch when n > 0)
+cudaError_t gs_launch_feat_grad(const uint32_t* offsets_g, const uint32_t* count, const float* grad_feat_inst,
+                                const uint32_t* row_epoch, uint32_t epoch, int n, int f, float* grad_feat,
+                                cudaStream_t st);
+
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
                                 void* keys, int key_bytes, uint32_t* vals, cudaStream_t st);

@@ -135,6 +135,7 @@ struct gs_ctx {
   size_t iota_n = 0;
   // per instance
   DevBuf keys_in, keys_out, vals_in, vals_out, pA, pB, pC, grad_inst, row_epoch;
+  DevBuf grad_feat_inst;                  // [M][f] per-instance feature gradients (gs_render_backward_feat)
   uint32_t epoch = 0;                      // tag of the current backward in row_epoch[]
   // per tile / misc
   DevBuf tile_accum, tile_neff, tile_neff_b, cub_tmp, counters, img_dev, gimg_dev, rays;
@@ -146,6 +147,8 @@ struct gs_ctx {
   bool have_forward = false, have_backward = false, gather = false;
   bool have_aux = false;                  // the last forward wrote (depth, alpha) to a caller's aux buffer
   bool sh_gaussian = false;               // the last forward evaluated its SH colour once per Gaussian
+  int feat_f = 0;                         // the last forward blended feat[n, feat_f] (0: no features)
+  const float* feat = nullptr;
   int n = 0, d = 3, scale_act = 0;
   long long m = 0;
   GsCam cam{};
@@ -200,7 +203,8 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   cudaDeviceSynchronize();
   DevBuf* bufs[] = {&c->rec, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
-                    &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part};
+                    &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
+                    &c->grad_feat_inst};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
@@ -233,7 +237,7 @@ static int ceil_log2(unsigned v) {
 static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
                                const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
                                float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream,
-                               const gs_render_aux* ax = nullptr) {
+                               const gs_render_aux* ax = nullptr, const gs_render_feat* ft = nullptr) {
   if (!c || !cam || n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad arguments");
   if (d != 3 && gs_sh_basis_count(d) == 0)
     return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
@@ -271,6 +275,23 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     aux_out.aux_final = ax->aux_final;
     // a forward that writes aux may be differentiated through it: its backward kernel must exist too
     if (int rc = gs_blend_aux_supported(blend_d, true, ax->aux != nullptr)) return rc;
+  }
+  const bool gather = gs_tuning().gather != 0;   // RGB and SH: no pack pass
+  if (ft) {
+    if (!gs_feat_width_ok(ft->f)) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: f must be 8, 16 or 32");
+    if (!ft->map || (n > 0 && !ft->feat))
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat or map");
+    if ((reinterpret_cast<uintptr_t>(ft->feat) | reinterpret_cast<uintptr_t>(ft->map) |
+         reinterpret_cast<uintptr_t>(ft->map_final)) % 16)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: feat, map and map_final must be 16-byte aligned");
+    if (ft->map_final && !final_img)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: map_final needs image_final");
+    if (blend_d != 3)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: SH colour evaluated per pixel has no feature "
+                                                  "kernel (use GS_SH_EVAL_GAUSSIAN)");
+    if (!gather)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: the packed path (gs_tune(\"gather\", 0)) has "
+                                                  "no feature kernel");
   }
   if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
   g_cur_alloc = &c->allocator;
@@ -403,7 +424,6 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   long long m = (long long)*c->host_m;
   size_t M = (size_t)m;
 
-  const bool gather = gs_tuning().gather != 0;   // RGB and SH: no pack pass
   gs_mark(c, 2, st);
   // tile-id sort key width (GS_TILE_KEY_BYTES=4 forces the wide path, for tests)
   static const int forced_key = getenv("GS_TILE_KEY_BYTES") ? atoi(getenv("GS_TILE_KEY_BYTES")) : 0;
@@ -467,7 +487,11 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   // 6. blend (+ optional fused clamp & centre crop, splatter.py:652-653 / :267-272)
   GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
   gs_mark(c, 5, st);
-  if (blend_d == 3) {
+  if (ft) {
+    GS_CUDA_TRY(gs_launch_blend_feat_fwd(c->rec.as<GsRec>(), ft->feat, ft->f, c->vals_out.as<uint32_t>(),
+                                         c->tile_accum.as<int>(), g, image, c->tile_neff.as<int>(), final_img, crop,
+                                         use_aux ? &aux_out : nullptr, ft->map, ft->map_final, st));
+  } else if (blend_d == 3) {
     GS_CUDA_TRY(gs_launch_blend_fwd(c->pA.as<float4>(), c->pB.as<float2>(), c->pC.as<float4>(),
                                     gather ? c->rec.as<GsRec>() : nullptr, c->vals_out.as<uint32_t>(),
                                     c->tile_accum.as<int>(), g, image, c->tile_neff.as<int>(), final_img, crop, st,
@@ -488,6 +512,8 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   c->have_forward = true;
   c->have_aux = aux_out.aux != nullptr;
   c->sh_gaussian = sh_gaussian;
+  c->feat_f = ft ? ft->f : 0;
+  c->feat = ft ? ft->feat : nullptr;
   c->filt_on = filt_on;
   c->filt = filt;
   c->gather = gather;
@@ -524,7 +550,9 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                 const float* scale, const float* image, const float* grad_image, int grad_is_final,
                                 float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
                                 float* grad_scale, gs_stream_t stream, const float* aux = nullptr,
-                                const float* grad_aux = nullptr, float* grad_cam = nullptr) {
+                                const float* grad_aux = nullptr, float* grad_cam = nullptr,
+                                const float* fmap = nullptr, const float* grad_map = nullptr,
+                                float* grad_feat = nullptr) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward: no forward on this ctx");
   // camera only (grad_cam, the five parameter gradients all NULL: the caller has checked the set is not mixed)
@@ -562,6 +590,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   size_t M = (size_t)c->m;
   const size_t grow = blend_d == 3 ? (size_t)GS_GREC * 4 : (size_t)gs_sh_grad_width(d) * 4;
   GS_CUDA_TRY(c->grad_inst.reserve(M * grow + 16, st));
+  if (grad_map) GS_CUDA_TRY(c->grad_feat_inst.reserve(M * (size_t)c->feat_f * 4 + 16, st));
   {
     // one u32 tag per gradient row: rows written by this backward carry `epoch`; the tails of
     // saturated tiles are never written nor read (saves ~0.2 GB of HBM writes + reads at C3)
@@ -577,7 +606,14 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
   gs_mark(c, 7, st);
   if (c->m > 0) {
-    if (blend_d == 3) {
+    if (grad_map) {
+      GS_CUDA_TRY(gs_launch_blend_feat_bwd(c->rec.as<GsRec>(), c->feat, c->feat_f, c->vals_out.as<uint32_t>(),
+                                           c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image,
+                                           grad_image, fmap, grad_map, c->grad_inst.as<float>(),
+                                           c->grad_feat_inst.as<float>(), grad_is_final, crop,
+                                           c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), aux,
+                                           grad_aux, st));
+    } else if (blend_d == 3) {
       GS_CUDA_TRY(gs_launch_blend_bwd(c->pA.as<float4>(), c->pB.as<float2>(), c->pC.as<float4>(),
                                       c->gather ? c->rec.as<GsRec>() : nullptr, c->vals_out.as<uint32_t>(),
                                       c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image, grad_image,
@@ -627,6 +663,11 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                             c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                             grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
                                             grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
+    if (c->n > 0) gs_count_launch();
+  }
+  if (grad_map) {
+    GS_CUDA_TRY(gs_launch_feat_grad(c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(), c->grad_feat_inst.as<float>(),
+                                    c->row_epoch.as<uint32_t>(), c->epoch, c->n, c->feat_f, grad_feat, st));
     if (c->n > 0) gs_count_launch();
   }
   if (stats) {
@@ -687,6 +728,49 @@ extern "C" int gs_render_backward_cam(gs_ctx* c, const float* pos, const float* 
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_cam: null ctx");
   return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
                               grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, grad_cam);
+}
+
+extern "C" int gs_render_forward_feat(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                      const float* quat, const float* scale, int n, int d, int scale_activation,
+                                      const gs_camera* cam, float* image_raw_padded, float* image_final,
+                                      int64_t* culling_mask, const gs_render_aux* aux, const gs_render_feat* feat,
+                                      gs_stream_t stream) {
+  if (!feat) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat");
+  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image_raw_padded, image_final,
+                             culling_mask, stream, aux, feat);
+}
+
+extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                       const float* quat, const float* scale, const float* image_raw_padded,
+                                       const float* grad_image, int grad_is_final, const float* aux,
+                                       const float* grad_aux, const float* feat, const float* map,
+                                       const float* grad_map, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                       float* grad_quat, float* grad_scale, float* grad_feat, gs_stream_t stream) {
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: null ctx");
+  if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward_feat: no forward on this ctx");
+  if (!c->feat_f)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: the forward blended no features");
+  if (feat != c->feat)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: feat is not the forward's feature tensor");
+  if (c->n > 0 && !grad_feat) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: null grad_feat");
+  if (grad_map) {
+    if (!map) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: grad_map needs the forward's map");
+    if ((reinterpret_cast<uintptr_t>(map) | reinterpret_cast<uintptr_t>(grad_map)) % 16)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: map and grad_map must be 16-byte aligned");
+    if (c->stats_on && c->stats.absgrad)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_feat: absgrad statistics are not available with a "
+                                                  "feature gradient");
+    if (c->push.world)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_feat: a feature gradient is not part of the push "
+                                                  "bucket; not available with a gradient push configured");
+  }
+  const int f = c->feat_f, n = c->n;
+  int rc = render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
+                                grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, nullptr,
+                                map, grad_map, grad_feat);
+  if (rc || grad_map || n == 0) return rc;
+  GS_CUDA_TRY(cudaMemsetAsync(grad_feat, 0, (size_t)n * f * sizeof(float), (cudaStream_t)stream));
+  return 0;
 }
 
 extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {

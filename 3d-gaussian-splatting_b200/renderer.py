@@ -367,3 +367,68 @@ def render_frame_cam(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, f
             raise ValueError(f"render_frame_cam: {name} is on {t.device}, the parameters on {pos.device}")
     return _RenderFrameCam.apply(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
                                  near, tile_thresh, scale_activation, background, final)
+
+
+FEATURE_WIDTHS = (8, 16, 32)
+
+
+class _RenderFrameFeat(torch.autograd.Function):
+    """`_RenderFrameAux` that also blends per-Gaussian feature rows feat[n, F] into an [.., .., F] map with the image's
+    weights (gs_render_forward_feat / gs_render_backward_feat)."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, feat, width, height, focal_x, focal_y, rot, tran,
+                near, tile_thresh, scale_activation, background, final):
+        pos, rgb, opa, quat, scale, feat = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale, feat))
+        bg = None if background is None else [float(v) for v in background]
+        fin, raw, aux, aux_fin, fmap, fmap_fin, mask = rctx.forward_feat(
+            pos, rgb, opa, quat, scale, feat, int(width), int(height), float(focal_x), float(focal_y),
+            rot.detach().cpu(), tran.detach().cpu(), float(near), float(tile_thresh),
+            SCALE_ACTIVATIONS[scale_activation], bg, bool(final))
+        ctx.rctx = rctx
+        ctx.frame = rctx.frame_id()
+        ctx.final = bool(final)
+        ctx.save_for_backward(pos, rgb, opa, quat, scale, feat, raw, aux, fmap)
+        ctx.mark_non_differentiable(mask)
+        ctx.set_materialize_grads(False)
+        image, maps, feats = (fin, aux_fin, fmap_fin) if final else (raw, aux, fmap)
+        ctx.map_shape = tuple(maps.shape[:2])
+        return image, feats, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_feat, grad_depth, grad_alpha, _grad_mask):
+        pos, rgb, opa, quat, scale, feat, raw, aux, fmap = ctx.saved_tensors
+        rows, cols = ctx.map_shape
+        if grad_image is None:
+            grad_image = raw.new_zeros(rows, cols, 3)
+        grad_aux = None
+        if grad_depth is not None or grad_alpha is not None:
+            grad_aux = raw.new_zeros(rows, cols, 2)
+            if grad_depth is not None:
+                grad_aux[..., 0] = grad_depth
+            if grad_alpha is not None:
+                grad_aux[..., 1] = grad_alpha
+        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
+        _apply_push(ctx.rctx, push)
+        g_feat = torch.empty_like(feat)
+        if grad_feat is not None:
+            grad_feat = _f32(grad_feat)
+            if grad_feat.data_ptr() % 16:                      # the kernel reads 16-byte pieces of every pixel's row
+                grad_feat = grad_feat.clone()
+        ctx.rctx.backward_feat_into(pos, rgb, opa, quat, scale, feat, raw, _f32(grad_image), ctx.final, aux, grad_aux,
+                                    fmap, grad_feat, *outs, g_feat, ctx.frame)
+        return (None, outs[0], outs[1], outs[2], outs[3], outs[4], g_feat) + (None,) * 11
+
+
+def render_frame_feat(rctx, pos, rgb, opa, quat, scale, feat, width, height, focal_x, focal_y, rot, tran, near,
+                      tile_thresh, scale_activation, background=None, final=True):
+    """`render_frame_aux` plus a feature map: -> (image, features, depth, alpha, culling_mask).  feat [n, F] holds raw
+    float32 per-Gaussian features (F = 8, 16 or 32; pad another width with zero channels), blended per pixel as
+    features_k = sum_i w_i f_i,k with the image's weights, composited over zero (the background applies to the image
+    only; the expected feature is features / alpha) and not clamped: [H,W,F] (final=True, the centre crop) or
+    [Hp,Wp,F].  Image, depth and alpha are bit-identical to `render_frame_aux`'s.  Differentiable in the five
+    parameters and feat; a graph that never uses `features` runs the plain / aux backward kernels and gets a zero
+    feat gradient.  RGB and per-Gaussian SH colour on the default (gather) path, any 2-D filter; per-pixel SH, the
+    packed path, and (with a feature gradient) absgrad statistics or a data-parallel gradient push raise RuntimeError."""
+    return _RenderFrameFeat.apply(rctx, pos, rgb, opa, quat, scale, feat, width, height, focal_x, focal_y, rot, tran,
+                                  near, tile_thresh, scale_activation, background, final)

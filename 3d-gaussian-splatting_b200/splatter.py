@@ -27,7 +27,8 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_cam, render_frame_final
+from renderer import (FEATURE_WIDTHS, FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_cam,
+                      render_frame_feat, render_frame_final)
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -47,15 +48,17 @@ def quat_to_rotmat(q):
 
 
 class Gaussian3ds(nn.Module):
-    """Parameter holder + densification (reference splatter.py:39-228, init_values=True branch)."""
+    """Parameter holder + densification (reference splatter.py:39-228, init_values=True branch).  `feat`: optional
+    per-Gaussian feature rows [n, F] (`Splatter(..., n_features=F)`), None without features."""
 
-    def __init__(self, pos, rgb, opa, quat, scale):
+    def __init__(self, pos, rgb, opa, quat, scale, feat=None):
         super().__init__()
         self.pos = nn.Parameter(pos)
         self.rgb = nn.Parameter(rgb)
         self.opa = nn.Parameter(opa)
         self.quat = nn.Parameter(quat)
         self.scale = nn.Parameter(scale)
+        self.feat = None if feat is None else nn.Parameter(feat)
 
     def reset_opa(self):                                        # reference splatter.py:119-120
         with torch.no_grad():
@@ -89,9 +92,18 @@ class Gaussian3ds(nn.Module):
         new, (n_deleted, n_clone, n_split) = gaussian.densify(
             *args, g, 0 if scale_activation == "abs" else 1, inverse_sigmoid(0.02), float(delete_thresh),
             float(grad_thresh), grad_aggregation == "max", float(taus), bool(use_clone), bool(use_split),
-            float(clone_dt), generator)
-        self.pos, self.rgb, self.opa, self.quat, self.scale = (nn.Parameter(t) for t in new)
+            float(clone_dt), generator, self._feat_arg())
+        self._replace(new)
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.pos.shape[0])
+
+    def _feat_arg(self):
+        return None if self.feat is None else self.feat.detach().contiguous()
+
+    def _replace(self, new):
+        """New parameters from a densification: the five, then the feature rows laid out by the same plan."""
+        self.pos, self.rgb, self.opa, self.quat, self.scale = (nn.Parameter(t) for t in new[:5])
+        if self.feat is not None:
+            self.feat = nn.Parameter(new[5])
 
 
 DENSIFY_STATS = ("none", "grad", "absgrad")
@@ -146,6 +158,15 @@ class DensifyStats:
         dist.all_reduce(self.max_radius, op=dist.ReduceOp.MAX, group=group)
 
 
+def _check_features(n_features, use_sh_coeff, sh_eval, densify_stats):
+    if n_features != 0 and n_features not in FEATURE_WIDTHS:
+        raise ValueError(f"n_features must be 0 or one of {FEATURE_WIDTHS} (pad with zero channels), not {n_features!r}")
+    if n_features and use_sh_coeff and sh_eval == "pixel":
+        raise ValueError("features need the RGB blend: RGB colour or sh_eval='gaussian', not per-pixel SH")
+    if n_features and densify_stats == "absgrad":
+        raise ValueError("features are not available with densify_stats='absgrad' (use 'grad')")
+
+
 class Tiles:
     """Padded render-target geometry (reference splatter.py:255-272)."""
 
@@ -172,7 +193,7 @@ class Splatter(nn.Module):
                  tile_culling_method="prob2", tile_culling_dist_thresh=0.5, tile_culling_prob_thresh=0.1,
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
-                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none"):
+                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none", n_features=0):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -197,7 +218,12 @@ class Splatter(nn.Module):
         `densify_stats`: "none" (default); "grad" accumulates the screen-space densification statistics of 3D
         Gaussian Splatting in `self.densify_stats` (a `DensifyStats`: view-space gradient norm, view count, largest
         screen radius) during every backward; "absgrad" also the absolute gradient of AbsGS (not available with
-        per-pixel SH colour).  `adaptive_control_screen` densifies from them."""
+        per-pixel SH colour).  `adaptive_control_screen` densifies from them.
+
+        `n_features`: 0 (default) or F = 8, 16, 32 raw per-Gaussian features in `gaussian_3ds.feat` (an nn.Parameter
+        [n, F], zero-initialised; `from_tensors` / a checkpoint may provide a "feat" tensor, whose width then sets F),
+        blended with the image's weights by `render_features` and carried through densification and checkpoints.
+        Not available with per-pixel SH colour, nor with densify_stats="absgrad"."""
         super().__init__()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
@@ -221,6 +247,9 @@ class Splatter(nn.Module):
             raise ValueError(f"densify_stats must be one of {DENSIFY_STATS}, not {densify_stats!r}")
         if densify_stats == "absgrad" and use_sh_coeff and sh_eval == "pixel":
             raise ValueError("densify_stats='absgrad' needs the RGB blend: RGB colour or sh_eval='gaussian'")
+        if isinstance(colmap_path, dict) and colmap_path.get("feat") is not None and not n_features:
+            n_features = int(colmap_path["feat"].shape[1])
+        _check_features(n_features, use_sh_coeff, sh_eval, densify_stats)
         self.sh_eval = sh_eval
         self.filter2d, self.filter2d_variance = filter2d, filter2d_variance
         self.use_sh_coeff = bool(use_sh_coeff)
@@ -239,14 +268,29 @@ class Splatter(nn.Module):
             self.imgs = [] if images is None else [im.to(self.device) for im in images]
         else:
             params = self._load_colmap(colmap_path, image_path, opa_init_value, scale_init_value)
+        if isinstance(colmap_path, dict) and colmap_path.get("feat") is not None:
+            params["feat"] = colmap_path["feat"]
         if load_ckpt is not None:                                   # reference splatter.py:417-424
             ckpt = torch.load(load_ckpt, map_location="cpu", weights_only=False)   # nn.Parameters, train.py:284-290
             params = {k: ckpt[k].detach() for k in ("pos", "rgb", "opa", "quat", "scale")}
+            if ckpt.get("feat") is not None:                       # a checkpoint with features (checkpoint.py)
+                params["feat"] = ckpt["feat"].detach()
+                if not n_features:
+                    n_features = int(params["feat"].shape[1])
+                    _check_features(n_features, use_sh_coeff, sh_eval, densify_stats)
         if self.use_sh_coeff != (params["rgb"].shape[1] != 3):
             raise ValueError("use_sh_coeff must match the colour width (3 = RGB logits, 27 / 48 = SH)")
+        n = params["pos"].shape[0]
+        feat = params.get("feat")
+        if feat is not None and tuple(feat.shape) != (n, n_features):
+            raise ValueError(f"feat must be [n, n_features] = [{n}, {n_features}], not {list(feat.shape)}")
+        if feat is None and n_features:
+            feat = torch.zeros(n, n_features)
+        self.n_features = int(n_features)
         to = dict(device=self.device, dtype=torch.float32)
         self.gaussian_3ds = Gaussian3ds(*(params[k].detach().to(**to).contiguous()
-                                         for k in ("pos", "rgb", "opa", "quat", "scale")))
+                                         for k in ("pos", "rgb", "opa", "quat", "scale")),
+                                        feat=None if feat is None else feat.detach().to(**to).contiguous())
         with torch.cuda.device(self.device):                      # the context lives on self.device, not on the current one
             self._rctx = gaussian.RenderContext()
         self._rctx.set_sh_eval(SH_EVAL[sh_eval])                   # every frame of this Splatter, fused or not
@@ -395,6 +439,26 @@ class Splatter(nn.Module):
         self.n_tile_gaussians = self._rctx.last_instances()
         return dict(image=image, depth=depth, alpha=alpha)
 
+    def render_features(self, camera_id=None, extrinsics=None, intrinsics=None, background=None):
+        """`render_maps` plus the feature map: dict(image, features [H,W,F], depth, alpha).  features_k = sum_i w_i
+        f_i,k with the image's weights, composited over zero (the background applies to the image only; divide by
+        alpha for the expected feature), not clamped.  All four are differentiable (`renderer.render_frame_feat`);
+        the feature loss reaches `gaussian_3ds.feat` and, through alpha, the geometry.  Needs n_features > 0."""
+        g = self.gaussian_3ds
+        if g.feat is None:
+            raise RuntimeError("render_features needs Splatter(..., n_features=8, 16 or 32)")
+        self.set_camera(camera_id, extrinsics, intrinsics)
+        v = self.current_view
+        self._size_densify_stats()
+        image, features, depth, alpha, mask = render_frame_feat(
+            self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, g.feat, v["width"], v["height"], v["focal_x"],
+            v["focal_y"], v["rot"], v["tran"], self.near, self.tile_culling_prob_thresh, self.scale_activation,
+            background=background, final=True)
+        self.culling_mask = mask
+        self.n_gaussians = g.pos.shape[0]
+        self.n_tile_gaussians = self._rctx.last_instances()
+        return dict(image=image, features=features, depth=depth, alpha=alpha)
+
     def render_at_pose(self, rot, tran, camera_id=None, background=None):
         """`render_maps` at a caller-supplied pose, differentiable with respect to it: rot [3,3] and tran [3] are
         float32 CUDA tensors (world -> camera, p_c = rot p + tran), typically a learnable correction composed with a
@@ -454,8 +518,8 @@ class Splatter(nn.Module):
             st.max_radius if max_screen_size is not None else None,
             float(max_screen_size) if max_screen_size is not None else 0.0,
             0 if self.scale_activation == "abs" else 1, inverse_sigmoid(0.02), float(delete_thresh),
-            float(grad_thresh), float(taus), bool(use_clone), bool(use_split), generator)
-        g.pos, g.rgb, g.opa, g.quat, g.scale = (nn.Parameter(t) for t in new)
+            float(grad_thresh), float(taus), bool(use_clone), bool(use_split), generator, g._feat_arg())
+        g._replace(new)
         self.n_gaussians = g.pos.shape[0]
         st.reset(self.n_gaussians)
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.n_gaussians)

@@ -241,6 +241,47 @@ int gs_render_backward_cam(gs_ctx* ctx, const float* pos, const float* rgb, cons
                            float* grad_cam /* DEVICE [12]: dL/drot row-major [9], then dL/dtran [3] */,
                            gs_stream_t stream);
 
+/* Feature maps (additive): per-Gaussian raw float32 features feat[n, f] (no activation), f = 8, 16 or 32, blended in
+ * the same pass as the image with the image's weights w_i = alpha_i T_i:
+ *   feature_k = sum_i w_i f_i,k     composited over zero (the background applies to the image only; the expected
+ *                                   feature is feature / alpha).  Features are not clamped.
+ * Another width: pad with zero channels.  Image, depth and alpha are bit-identical to gs_render_forward_aux's with the
+ * same arguments, and the launch count is the same.
+ *   feat      : DEVICE [n, f], 16-byte aligned.
+ *   map       : DEVICE [Hp, Wp, f], 16-byte aligned; required (the feature backward reads it).
+ *   map_final : DEVICE [height, width, f] centre crop of map, or NULL; needs image_final.
+ * Frames that blend on the RGB kernels of the gather path only: RGB colour and SH with GS_SH_EVAL_GAUSSIAN, with or
+ * without maps / background (aux), under any 2-D filter.  Refused before any launch: f not 8 / 16 / 32, a NULL or
+ * misaligned pointer (GS_ERR_INVALID_ARG); a per-pixel SH frame, the packed path (gs_tune("gather", 0))
+ * (GS_ERR_UNSUPPORTED). */
+typedef struct gs_render_feat {
+  int f;
+  const float* feat;
+  float* map;
+  float* map_final;
+} gs_render_feat;
+int gs_render_forward_feat(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                           const float* scale, int n, int d, int scale_activation, const gs_camera* cam_host,
+                           float* image_raw_padded, float* image_final, int64_t* culling_mask,
+                           const gs_render_aux* aux /* nullable */, const gs_render_feat* feat, gs_stream_t stream);
+/* Backward of gs_render_forward_feat: gs_render_backward_aux's arguments plus the feature terms.  grad_map is
+ * [Hp, Wp, f] or [height, width, f] (per grad_is_final; only the crop masks it), 16-byte aligned; NULL = zero, which
+ * runs the plain or aux backward kernels and zero-fills grad_feat.  grad_feat (DEVICE [n, f]) receives
+ * dL/dfeat = sum_p w_p,i g_F(p), bit-deterministic; the other gradients gain the feature loss's terms through alpha.
+ * feat must be the forward's pointer and map the forward's buffer.  After a feature forward the other backward entries
+ * (plain, final, aux, cam) work unchanged and treat the feature gradient as zero.  Densification statistics
+ * (gs_ctx_set_densify_stats, grad2d) include the feature loss.
+ * GS_ERR_INVALID_ARG: the forward blended no features, feat differs from the forward's, NULL grad_feat (n > 0),
+ * grad_map without map, misaligned map / grad_map.  GS_ERR_UNSUPPORTED, before any launch, with a non-NULL grad_map:
+ * absgrad statistics set; a gradient push configured (grad_feat is not part of the bucket).
+ * One more launch than gs_render_backward_aux when grad_map is set; the context keeps M * f * 4 bytes of workspace. */
+int gs_render_backward_feat(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                            const float* scale, const float* image_raw_padded, const float* grad_image,
+                            int grad_is_final, const float* aux, const float* grad_aux, const float* feat,
+                            const float* map, const float* grad_map, float* grad_pos, float* grad_rgb,
+                            float* grad_opa, float* grad_quat, float* grad_scale, float* grad_feat,
+                            gs_stream_t stream);
+
 /* Where the SH colour (d == 27 / 48) is evaluated.  Two colour MODELS, not two speeds of one: the same coefficients
  * render differently.
  *   GS_SH_EVAL_PIXEL    (default; the reference): the basis is evaluated per pixel, along the pixel's world-space ray,
@@ -381,6 +422,11 @@ int gs_densify_apply(const float* pos, const float* rgb, const float* opa, const
                      const float* normals, int n_keep, int n_clone, int n_split, int scale_activation,
                      float* out_pos, float* out_rgb, float* out_opa, float* out_quat, float* out_scale,
                      gs_stream_t stream);
+/* Another per-Gaussian row tensor src[n, w] (e.g. features) laid out like gs_densify_apply's outputs for the same
+ * plan: kept rows, clones, second split samples; both split halves and clones are exact copies.  out: caller-allocated
+ * [n_keep + n_clone + n_split, w].  One launch when n > 0; no synchronisation. */
+int gs_densify_apply_rows(const float* src, int n, int w, const unsigned char* code, const int* dst, int n_keep,
+                          int n_clone, int n_split, float* out, gs_stream_t stream);
 /* gs_densify_plan from screen-space statistics (gs_ctx_set_densify_stats), as 3DGS scores them: a kept Gaussian
  * densifies when accum[i] / max(count[i], 1) >= grad_thresh (accum: the caller's grad2d or absgrad).  With a non-NULL
  * max_radius, a Gaussian whose max_radius > max_screen_px is pruned as well.  Opacity / scale-norm pruning and the

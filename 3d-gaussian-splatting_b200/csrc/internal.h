@@ -131,8 +131,8 @@ cudaError_t gs_launch_blend_sh_bwd_tc(const GsRec* grec, const float* rgb, const
 cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const float* opa, const float* quat,
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
-                                    GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
-                                    unsigned int* n_visible, cudaStream_t st,
+                                    GsRec* rec, uint2* rect /*[n]: tile rectangle, zero without instances*/,
+                                    uint32_t* count, uint32_t* dkey, int64_t* mask, unsigned int* n_visible, cudaStream_t st,
                                     bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/,
                                     const GsFilter2d* filt = nullptr /*non-null: 2-D screen-space filter*/);
 
@@ -198,7 +198,7 @@ cudaError_t gs_launch_feat_grad(const uint32_t* offsets_g, const uint32_t* count
                                 cudaStream_t st);
 
 // ---- binning.cu ------------------------------------------------------------------------
-cudaError_t gs_launch_emit_keys(const GsRec* rec, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
+cudaError_t gs_launch_emit_keys(const uint2* rect, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
                                 void* keys, int key_bytes, uint32_t* vals, cudaStream_t st);
 cudaError_t gs_launch_tile_ranges(const void* keys, int key_bytes, long long m, int n_tiles, int* tile_accum,
                                   cudaStream_t st);

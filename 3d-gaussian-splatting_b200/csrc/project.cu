@@ -62,7 +62,7 @@ __device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
     const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
     unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}) {
   int i = blockIdx.x * kBlock + threadIdx.x;
   bool vis = false;
@@ -71,6 +71,15 @@ __device__ __forceinline__ void fused_project_body(
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    // opacity and RGB logits are issued with the geometry, so that the thread makes one round trip to HBM, not two
+    // (a warp almost always has a binned Gaussian, so their sectors are fetched anyway)
+    const float opa_raw = opa[i];
+    float rgb_raw[3] = {0.f, 0.f, 0.f};
+    if (KG == 0 && d == 3) {
+      rgb_raw[0] = rgb[3 * i];
+      rgb_raw[1] = rgb[3 * i + 1];
+      rgb_raw[2] = rgb[3 * i + 2];
+    }
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
     vis = o.visible;
     if (mask) mask[i] = o.visible ? 1 : 0;
@@ -83,12 +92,14 @@ __device__ __forceinline__ void fused_project_body(
       dl2o = fo.dl2o;
       keep = keep && fo.keep;
     }
+    uint2 rc = make_uint2(0u, 0u);
     if (keep) {
       uint32_t tx0, tx1, ty0, ty1;
       if (gs_tile_rect(grid, o.x, o.y, o.a, o.b, o.c, o.d, tx0, tx1, ty0, ty1)) {
         cnt = (tx1 - tx0) * (ty1 - ty0);
+        rc = make_uint2(tx0 | (ty0 << 16), (tx1 - tx0) | ((ty1 - ty0) << 16));
         GsConic k = gs_make_conic(o.a, o.b, o.c, o.d);
-        float op = gs_sigmoid(opa[i]);
+        float op = gs_sigmoid(opa_raw);
         GsRec* r = rec + i;
         r->a = make_float4(o.x, o.y, k.ca, k.cb);
         // RGB colour = sigmoid(logit) (splatter.py:539); per-pixel SH coefficients stay raw and are gathered
@@ -105,16 +116,18 @@ __device__ __forceinline__ void fused_project_body(
           cg = gs_sigmoid(l[1]);
           cb = gs_sigmoid(l[2]);
         } else if (d == 3) {
-          cr = gs_sigmoid(rgb[3 * i]);
-          cg = gs_sigmoid(rgb[3 * i + 1]);
-          cb = gs_sigmoid(rgb[3 * i + 2]);
+          cr = gs_sigmoid(rgb_raw[0]);
+          cg = gs_sigmoid(rgb_raw[1]);
+          cb = gs_sigmoid(rgb_raw[2]);
         }
         r->b = make_float4(k.cc, F ? log2f(op) + dl2o : log2f(op), cr, cg);
-        r->c = make_float4(cb, o.depth, __uint_as_float(tx0 | (ty0 << 16)),
-                           __uint_as_float((tx1 - tx0) | ((ty1 - ty0) << 16)));
+        r->c = make_float4(cb, o.depth, __uint_as_float(rc.x), __uint_as_float(rc.y));
         r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
       }
     }
+    // the tile rectangle again, densely (zero without instances: whole sectors), for the instance emission: an 8-byte
+    // read from a 19 MB array at C3 instead of a 16-byte gather from the 154 MB records
+    rect[i] = rc;
     count[i] = cnt;
     // depth sort key: positive float bits order like the floats; Gaussians without instances last
     dkey[i] = cnt ? __float_as_uint(o.depth) : 0xffffffffu;
@@ -141,10 +154,10 @@ __global__ void __launch_bounds__(kBlock) fused_project_kernel(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
     GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
     unsigned int* __restrict__ n_visible) {
-  fused_project_body<0>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec, count,
-                        dkey, mask, n_visible);
+  fused_project_body<0>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec, rect,
+                        count, dkey, mask, n_visible);
 }
 
 template <int K>
@@ -152,10 +165,10 @@ __global__ void __launch_bounds__(kBlock) fused_project_sh_kernel(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
     GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
     unsigned int* __restrict__ n_visible) {
   fused_project_body<K>(pos, rgb, opa, quat, scale, n, 3 * K, scale_act, cam, grid, near_plane, half_w, half_h, rec,
-                        count, dkey, mask, n_visible);
+                        rect, count, dkey, mask, n_visible);
 }
 
 // with the 2-D filter: K = 0 is fused_project_kernel's colour rule, K = 9 / 16 fused_project_sh_kernel<K>'s
@@ -164,10 +177,10 @@ __global__ void __launch_bounds__(kBlock) fused_project_filt_kernel(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
     GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
     unsigned int* __restrict__ n_visible, GsFilter2d filt) {
   fused_project_body<K, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec,
-                              count, dkey, mask, n_visible, filt);
+                              rect, count, dkey, mask, n_visible, filt);
 }
 
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
@@ -242,8 +255,9 @@ __device__ __forceinline__ void fused_project_bwd_body(
 #pragma unroll
   for (int k = 0; k < (KG ? D : 1); ++k) gsh[k] = 0.f;
   const uint32_t cnt = valid ? count[i] : 0u;
+  const uint32_t o0 = valid ? offsets_g[i] : 0u;      // loaded with the count: one round trip, not two
   if (cnt > 0) {
-    const uint32_t o0 = offsets_g[i], o1 = o0 + cnt;   // this Gaussian's contiguous gradient rows
+    const uint32_t o1 = o0 + cnt;                      // this Gaussian's contiguous gradient rows
     // issue the parameter loads BEFORE the row loop so that both round trips to HBM overlap
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
@@ -259,19 +273,50 @@ __device__ __forceinline__ void fused_project_bwd_body(
       rgb_raw[1] = rgb[3 * i + 1];
       rgb_raw[2] = rgb[3 * i + 2];
     }
-    // (one row at a time; alternatives tried on an earlier GPU and found slower: loading the tags and rows of
-    //  4 instances at once (80 registers), a warp-cooperative version streaming the 32 Gaussians' contiguous row
-    //  span through shared memory)
-    for (uint32_t r = o0; r < o1; ++r) {
-      if (row_epoch[r] != epoch) continue;     // instance not reached by its (saturated) tile: zero gradient
-      const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)r * GW);
+    // The rows are summed one by one in row order.  For an RGB frame the rows are loaded in groups: the tags of four
+    // rows at once, then the live rows among them (48 registers of payload), so that a Gaussian with a few instances
+    // waits for two round trips to HBM per group instead of two per row (H100, C3: 0.235 -> 0.230 ms).  Grouping only
+    // the tags and loading the rows one at a time was slower (RGB 0.245 ms; per-pixel SH, D = 27: 0.496 -> 0.526 ms),
+    // and so was the grouped loop with per-Gaussian SH of degree 2 (80 -> 99 registers, 0.409 -> 0.464 ms): those
+    // kernels keep the plain loop.  An instance its (saturated) tile did not reach has a stale tag and contributes
+    // nothing.
+    if constexpr (GW > GS_GREC || KG > 0) {
+      for (uint32_t r = o0; r < o1; ++r) {
+        if (row_epoch[r] != epoch) continue;
+        const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)r * GW);
 #pragma unroll
-      for (int qq = 0; qq < GW / 4; ++qq) {
-        const float4 v = row[qq];
-        acc[4 * qq] += v.x;
-        acc[4 * qq + 1] += v.y;
-        acc[4 * qq + 2] += v.z;
-        acc[4 * qq + 3] += v.w;
+        for (int qq = 0; qq < GW / 4; ++qq) {
+          const float4 v = row[qq];
+          acc[4 * qq] += v.x;
+          acc[4 * qq + 1] += v.y;
+          acc[4 * qq + 2] += v.z;
+          acc[4 * qq + 3] += v.w;
+        }
+      }
+    } else {
+      constexpr int kGroup = 4;
+      for (uint32_t r0 = o0; r0 < o1; r0 += kGroup) {
+        bool live[kGroup];
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) live[j] = r0 + j < o1 && row_epoch[r0 + j] == epoch;
+        float4 v[kGroup][GW / 4];
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) {
+          const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)(r0 + j) * GW);
+#pragma unroll
+          for (int qq = 0; qq < GW / 4; ++qq) v[j][qq] = live[j] ? row[qq] : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) {
+          if (!live[j]) continue;
+#pragma unroll
+          for (int qq = 0; qq < GW / 4; ++qq) {
+            acc[4 * qq] += v[j][qq].x;
+            acc[4 * qq + 1] += v[j][qq].y;
+            acc[4 * qq + 2] += v[j][qq].z;
+            acc[4 * qq + 3] += v[j][qq].w;
+          }
+        }
       }
     }
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
@@ -674,14 +719,14 @@ extern "C" int gs_jacobian(const float* pos_cam, int n, float* jac, gs_stream_t 
 cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const float* opa, const float* quat,
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
-                                    GsRec* rec, uint32_t* count, uint32_t* dkey, int64_t* mask,
+                                    GsRec* rec, uint2* rect, uint32_t* count, uint32_t* dkey, int64_t* mask,
                                     unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt) {
   if (n == 0) return cudaSuccess;
   if (filt) {
 #define GS_LAUNCH_PFILT(K)                                                                                      \
   fused_project_filt_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
-                                                               grid, near_plane, half_w, half_h, rec, count, dkey, \
-                                                               mask, n_visible, *filt)
+                                                               grid, near_plane, half_w, half_h, rec, rect, count, \
+                                                               dkey, mask, n_visible, *filt)
     if (sh_gaussian && d == 27) GS_LAUNCH_PFILT(9);
     else if (sh_gaussian && d == 48) GS_LAUNCH_PFILT(16);
     else if (sh_gaussian) return cudaErrorInvalidValue;
@@ -691,17 +736,17 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
   }
   if (sh_gaussian && d == 27)
     fused_project_sh_kernel<9><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
-                                                               near_plane, half_w, half_h, rec, count, dkey, mask,
-                                                               n_visible);
+                                                               near_plane, half_w, half_h, rec, rect, count, dkey,
+                                                               mask, n_visible);
   else if (sh_gaussian && d == 48)
     fused_project_sh_kernel<16><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
-                                                                near_plane, half_w, half_h, rec, count, dkey, mask,
-                                                                n_visible);
+                                                                near_plane, half_w, half_h, rec, rect, count, dkey,
+                                                                mask, n_visible);
   else if (sh_gaussian)
     return cudaErrorInvalidValue;
   else
     fused_project_kernel<<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid,
-                                                         near_plane, half_w, half_h, rec, count, dkey, mask, n_visible);
+                                                         near_plane, half_w, half_h, rec, rect, count, dkey, mask, n_visible);
   return cudaGetLastError();
 }
 

@@ -131,7 +131,7 @@ struct gs_ctx {
   int device = 0;
   GsAllocator allocator{};
   // per Gaussian
-  DevBuf rec, count, offsets, dkey_in, dkey_out, perm, iota, offsets_g;
+  DevBuf rec, rect, count, offsets, dkey_in, dkey_out, perm, iota, offsets_g;
   size_t iota_n = 0;
   // per instance
   DevBuf keys_in, keys_out, vals_in, vals_out, pA, pB, pC, grad_inst, row_epoch;
@@ -201,7 +201,7 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   int cur = -1;
   const bool switched = cudaGetDevice(&cur) == cudaSuccess && cur != c->device && cudaSetDevice(c->device) == cudaSuccess;
   cudaDeviceSynchronize();
-  DevBuf* bufs[] = {&c->rec, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
+  DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
                     &c->grad_feat_inst};
@@ -330,6 +330,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
 
   size_t N = (size_t)n;
   GS_CUDA_TRY(c->rec.reserve(N * sizeof(GsRec), st));
+  GS_CUDA_TRY(c->rect.reserve(N * sizeof(uint2), st));
   GS_CUDA_TRY(c->count.reserve((N + 1) * 4, st));
   GS_CUDA_TRY(c->offsets.reserve((N + 1) * 4, st));
   GS_CUDA_TRY(c->dkey_in.reserve(N * 4 + 4, st));
@@ -380,7 +381,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
   GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
   GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
-                                      half_w, half_h, c->rec.as<GsRec>(), c->count.as<uint32_t>(),
+                                      half_w, half_h, c->rec.as<GsRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
                                       c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
                                       sh_gaussian, filt_on ? &filt : nullptr));
   if (n > 0) gs_count_launch();
@@ -440,7 +441,7 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     GS_CUDA_TRY(c->vals_in.reserve(M * 4, st));
     GS_CUDA_TRY(c->vals_out.reserve(M * 4, st));
     // 3. instances in (depth, id) order: tile-id keys + Gaussian-id values
-    GS_CUDA_TRY(gs_launch_emit_keys(c->rec.as<GsRec>(), c->perm.as<uint32_t>(), c->offsets.as<uint32_t>(), n, g.ntx,
+    GS_CUDA_TRY(gs_launch_emit_keys(c->rect.as<uint2>(), c->perm.as<uint32_t>(), c->offsets.as<uint32_t>(), n, g.ntx,
                                     c->keys_in.p, key_bytes, c->vals_in.as<uint32_t>(), st));
     gs_count_launch();
     // 4. stable radix sort on the tile id only -> (tile, depth, id)

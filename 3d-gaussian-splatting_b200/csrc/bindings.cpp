@@ -11,6 +11,7 @@
 #include <torch/extension.h>
 
 #include <string>
+#include <array>
 #include <vector>
 
 #include "../../include/gs_b200.h"
@@ -511,6 +512,97 @@ struct RenderContext {
              "gs_render_backward_aux");
   }
 
+  // a batch of B views as one frame (gs_render_forward_batch): focal [B,2] = (fx, fy), rot [B,3,3], tran [B,3] are
+  // CPU tensors; returns (final[B,H,W,3] or None, raw padded[B,Hp,Wp,3], aux padded[B,Hp,Wp,2],
+  // aux_final[B,H,W,2] or None, mask[B,n])
+  py::tuple forward_batch(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                          torch::Tensor scale, int width, int height, torch::Tensor focal, torch::Tensor rot,
+                          torch::Tensor tran, float near, float thresh, int scale_activation,
+                          std::optional<std::vector<double>> background, bool final) {
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    int64_t n = pos.size(0);
+    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
+                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
+                "RenderContext.forward_batch: bad shapes");
+    TORCH_CHECK(!focal.is_cuda() && !rot.is_cuda() && !tran.is_cuda(),
+                "RenderContext.forward_batch: focal / rot / tran must be CPU tensors (cameras are host data)");
+    const int64_t b = focal.dim() == 2 ? focal.size(0) : -1;
+    TORCH_CHECK(b >= 1 && b <= GS_MAX_VIEWS && focal.size(1) == 2 && rot.dim() == 3 && rot.size(0) == b &&
+                    rot.size(1) == 3 && rot.size(2) == 3 && tran.dim() == 2 && tran.size(0) == b && tran.size(1) == 3,
+                "RenderContext.forward_batch: focal must be [B,2], rot [B,3,3] and tran [B,3] with 1 <= B <= ",
+                GS_MAX_VIEWS);
+    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
+    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_batch: background must have 3 values");
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto f = focal.to(at::kFloat).contiguous();
+    std::vector<gs_camera> cams;
+    for (int64_t v = 0; v < b; ++v)
+      cams.push_back(make_cam(width, height, f[v][0].item<float>(), f[v][1].item<float>(), rot[v], tran[v], near, thresh));
+    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
+    auto raw = torch::empty({b, hp, wp, 3}, pos.options());
+    auto aux = torch::empty({b, hp, wp, 2}, pos.options());
+    torch::Tensor fin, aux_fin;
+    if (final) {
+      fin = torch::empty({b, height, width, 3}, pos.options());
+      aux_fin = torch::empty({b, height, width, 2}, pos.options());
+    }
+    auto mask = torch::empty({b, n}, pos.options().dtype(at::kLong));
+    float bg[3] = {0.f, 0.f, 0.f};
+    if (background)
+      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
+    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
+    check_rc(gs_render_forward_batch(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                     scale_activation, (int)b, cams.data(), fpm(raw), final ? fpm(fin) : nullptr,
+                                     mask.data_ptr<int64_t>(), &ax, cur_stream()),
+             "gs_render_forward_batch");
+    ++frame;
+    batch = {b, height, width};
+    py::object none = py::none();
+    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, mask);
+  }
+
+  // (views, height, width) of the last forward_batch: its backward's tensors are checked against them
+  std::array<int64_t, 3> batch{0, 0, 0};
+
+  // backward of forward_batch: gradients are the sums over the views; grad_aux = None runs the plain kernels
+  void backward_batch_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                           torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_image, bool grad_is_final,
+                           torch::Tensor aux, std::optional<torch::Tensor> grad_aux, torch::Tensor g_pos,
+                           torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
+                           int64_t expected_frame) {
+    check_frame(expected_frame, "RenderContext.backward_batch_into");
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa);
+    GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale);
+    const int64_t b = batch[0], hp = (batch[1] + 15) / 16 * 16, wp = (batch[2] + 15) / 16 * 16;
+    TORCH_CHECK(raw.dim() == 4 && raw.size(0) == b && raw.size(1) == hp && raw.size(2) == wp && raw.size(3) == 3 &&
+                    aux.sizes() == at::IntArrayRef({b, hp, wp, 2}),
+                "RenderContext.backward_batch_into: raw must be [B,Hp,Wp,3] and aux [B,Hp,Wp,2] of the last forward_batch");
+    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 4 &&
+                    grad_image.size(0) == b && grad_image.size(3) == 3 &&
+                    (grad_is_final ? (grad_image.size(1) == batch[1] && grad_image.size(2) == batch[2])
+                                   : grad_image.sizes() == raw.sizes()),
+                "RenderContext.backward_batch_into: grad_image must be [B,H,W,3] (final) or match raw");
+    if (grad_aux) {
+      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 4 &&
+                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
+                      grad_aux->size(2) == grad_image.size(2) && grad_aux->size(3) == 2,
+                  "RenderContext.backward_batch_into: grad_aux must be float32 [B, rows, cols, 2] like grad_image");
+    }
+    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
+                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
+                "RenderContext.backward_batch_into: gradient buffers must match their parameters");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor ga;
+    if (grad_aux) ga = grad_aux->contiguous();
+    check_rc(gs_render_backward_batch(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
+                                      grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fpm(g_pos),
+                                      fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
+             "gs_render_backward_batch");
+  }
+
   // backward_aux_into plus the camera gradient grad_cam[12] = (dL/drot row-major, dL/dtran) of the forward's camera
   // (gs_render_backward_cam); the five parameter gradients all None: camera only.  aux = None: the forward wrote no
   // maps (forward / forward_final; then grad_aux must be None too)
@@ -917,6 +1009,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("tran"), py::arg("near"), py::arg("thresh"), py::arg("scale_activation"),
            py::arg("background") = py::none(), py::arg("final") = true)
       .def("backward_aux_into", &RenderContext::backward_aux_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
+           py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
+           py::arg("g_quat"), py::arg("g_scale"), py::arg("expected_frame") = -1)
+      .def("forward_batch", &RenderContext::forward_batch, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("width"), py::arg("height"), py::arg("focal"), py::arg("rot"),
+           py::arg("tran"), py::arg("near"), py::arg("thresh"), py::arg("scale_activation"),
+           py::arg("background") = py::none(), py::arg("final") = true)
+      .def("backward_batch_into", &RenderContext::backward_batch_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
            py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
            py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
            py::arg("g_quat"), py::arg("g_scale"), py::arg("expected_frame") = -1)

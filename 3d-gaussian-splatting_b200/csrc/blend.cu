@@ -141,32 +141,41 @@ __device__ __forceinline__ void gather_issue(SM& sm, int stage, const GsRec* __r
 // issue slots per (pixel, instance) instead of 17-18 with one pixel per thread.
 // AUX (gather only): one more FFMA per (pixel, instance) accumulates the depth sum w t; at the end the background
 // T_f bg is added to the colour and (depth, 1 - T_f) is stored to aux / aux_final.
-template <int FWD_CH, int PX, bool GATHER, bool AUX = false>
-__global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __restrict__ pA,
-                                                                 const float2* __restrict__ pB,
-                                                                 const float4* __restrict__ pC,
-                                                                 const GsRec* __restrict__ grec,
-                                                                 const uint32_t* __restrict__ ids,
-                                                                 const int* __restrict__ tile_accum, int wp, int hp,
-                                                                 int ntx, float fx, float fy,
-                                                                 float* __restrict__ image,
-                                                                 int* __restrict__ tile_neff,
-                                                                 float* __restrict__ final_img, GsCrop crop,
-                                                                 GsAuxOut aux) {
+// BATCH (gather, batched frame): the tile's view v = ty / (hp / GS_TILE) gives the pixel coordinates (its own rows, its
+// fx / fy from views[v]) and the final / aux_final crop ([B, height, width, .]); the padded image and aux are the tall
+// [B Hp, Wp, .] ones and are addressed as without it.
+template <int FWD_CH, int PX, bool GATHER, bool AUX = false, bool BATCH = false>
+__device__ __forceinline__ void blend_fwd_body(const float4* __restrict__ pA, const float2* __restrict__ pB,
+                                               const float4* __restrict__ pC, const GsRec* __restrict__ grec,
+                                               const uint32_t* __restrict__ ids, const int* __restrict__ tile_accum,
+                                               int wp, int hp, int ntx, float fx, float fy, float* __restrict__ image,
+                                               int* __restrict__ tile_neff, float* __restrict__ final_img, GsCrop crop,
+                                               GsAuxOut aux, const GsView* __restrict__ views) {
   static_assert(!AUX || GATHER, "the aux outputs read |p_c| from the gathered records");
+  static_assert(!BATCH || GATHER, "batched frames run the gather path");
   using Smem = typename std::conditional<GATHER, GatherRing<FWD_CH, FWD_STAGES, 3>, FwdSmem<FWD_CH>>::type;
   __shared__ __align__(16) Smem sm;
   const int tile = blockIdx.x;
   const int tid = threadIdx.x;
   const int tx = tile % ntx, ty = tile / ntx;
+  int lty = ty;   // the tile's row in its view
+  if constexpr (BATCH) {
+    const int v = ty / (hp / GS_TILE);
+    lty = ty - v * (hp / GS_TILE);
+    fx = views[v].fx;
+    fy = views[v].fy;
+    if (final_img) final_img += (size_t)v * crop.width * crop.height * 3;
+    if (aux.aux_final) aux.aux_final += (size_t)v * crop.width * crop.height * 2;
+  }
   // thread -> a row of PX adjacent pixels (ix0 .. ix0+PX-1, iy); PX = 4: 2 warps per tile, 8: one warp
   constexpr int FWD_PX = PX, TPR = GS_TILE / PX, NTHREADS = 256 / PX;
   const int ix0 = tx * GS_TILE + (tid % TPR) * FWD_PX;
   const int iy = ty * GS_TILE + (tid / TPR);
+  const int iyv = lty * GS_TILE + (tid / TPR);   // its row in the view
   float px[FWD_PX];
 #pragma unroll
   for (int p = 0; p < FWD_PX; ++p) px[p] = gs_pixel_coord(ix0 + p, wp, fx);
-  const float py = gs_pixel_coord(iy, hp, fy);
+  const float py = gs_pixel_coord(iyv, hp, fy);
 
   const int start = tile_accum[tile];
   const int cnt = tile_accum[tile + 1] - start;
@@ -296,7 +305,7 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
     if (aux.aux_final) {
 #pragma unroll
       for (int p = 0; p < FWD_PX; ++p) {
-        const int x = ix0 + p - crop.left, y = iy - crop.top;
+        const int x = ix0 + p - crop.left, y = iyv - crop.top;
         if (x >= 0 && x < crop.width && y >= 0 && y < crop.height)
           *reinterpret_cast<float2*>(aux.aux_final + ((size_t)y * crop.width + x) * 2) = make_float2(ab[2 * p], ab[2 * p + 1]);
       }
@@ -318,9 +327,37 @@ __global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __res
   if (final_img) {
 #pragma unroll
     for (int p = 0; p < FWD_PX; ++p)
-      gs_store_final(final_img, ix0 + p, iy, crop.left, crop.top, crop.width, crop.height, cr[p], cg[p], cb[p]);
+      gs_store_final(final_img, ix0 + p, iyv, crop.left, crop.top, crop.width, crop.height, cr[p], cg[p], cb[p]);
   }
   if (tile_neff && tid == 0) tile_neff[tile] = consumed;
+}
+
+template <int FWD_CH, int PX, bool GATHER, bool AUX = false>
+__global__ void __launch_bounds__(256 / PX) blend_fwd_kernel(const float4* __restrict__ pA,
+                                                                 const float2* __restrict__ pB,
+                                                                 const float4* __restrict__ pC,
+                                                                 const GsRec* __restrict__ grec,
+                                                                 const uint32_t* __restrict__ ids,
+                                                                 const int* __restrict__ tile_accum, int wp, int hp,
+                                                                 int ntx, float fx, float fy,
+                                                                 float* __restrict__ image,
+                                                                 int* __restrict__ tile_neff,
+                                                                 float* __restrict__ final_img, GsCrop crop,
+                                                                 GsAuxOut aux) {
+  blend_fwd_body<FWD_CH, PX, GATHER, AUX>(pA, pB, pC, grec, ids, tile_accum, wp, hp, ntx, fx, fy, image, tile_neff,
+                                          final_img, crop, aux, nullptr);
+}
+
+// the shipped gather forward (FWD_CH 128, 4 pixels per thread) of a batched frame
+template <bool AUX>
+__global__ void __launch_bounds__(64) blend_fwd_batch_kernel(const GsRec* __restrict__ grec,
+                                                             const uint32_t* __restrict__ ids,
+                                                             const int* __restrict__ tile_accum, int wp, int hp,
+                                                             int ntx, const GsView* __restrict__ views,
+                                                             float* __restrict__ image, int* __restrict__ tile_neff,
+                                                             float* __restrict__ final_img, GsCrop crop, GsAuxOut aux) {
+  blend_fwd_body<128, 4, true, AUX, true>(nullptr, nullptr, nullptr, grec, ids, tile_accum, wp, hp, ntx, 0.f, 0.f,
+                                          image, tile_neff, final_img, crop, aux, views);
 }
 
 // =======================================================================================
@@ -953,16 +990,19 @@ __device__ __forceinline__ void bwd_repack(float* __restrict__ st, const float* 
 // computes exactly what it computes without it.
 // ABS (one consumer warp): also sum_p |g_x,p| and sum_p |g_y,p| per instance (bwd_row), times ln 2, to the free columns
 // 10 and 11 of the gradient row; every other column is computed as without it.
+// BATCH (gather, batched frame): as in blend_fwd_body, the tile's view gives the pixel coordinates and the crop of a
+// final upstream gradient ([B, height, width, .]); slots come from the records' rectangles, whose rows the batched
+// projection offset by the view's, so the tile's frame-wide (tx, ty) address them as without it.
 template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false,
-          bool REPACK = false, bool ABS = false>
-__global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
-    blend_bwd2_kernel(const float4* __restrict__ pA, const float2* __restrict__ pB, const float4* __restrict__ pC,
-                      const GsRec* __restrict__ grec, const uint32_t* __restrict__ ids,
-                      const uint32_t* __restrict__ goff, const int* __restrict__ tile_accum, int wp, int hp, int ntx, float fx, float fy,
-                      const float* __restrict__ image, const float* __restrict__ grad_image,
-                      float* __restrict__ grad_inst, int grad_is_final, GsCrop crop, uint32_t* __restrict__ row_epoch,
-                      uint32_t epoch, int* __restrict__ tile_neff_b, const float* __restrict__ aux,
-                      const float* __restrict__ grad_aux) {
+          bool REPACK = false, bool ABS = false, bool BATCH = false>
+__device__ __forceinline__ void blend_bwd2_body(
+    const float4* __restrict__ pA, const float2* __restrict__ pB, const float4* __restrict__ pC,
+    const GsRec* __restrict__ grec, const uint32_t* __restrict__ ids, const uint32_t* __restrict__ goff,
+    const int* __restrict__ tile_accum, int wp, int hp, int ntx, float fx, float fy, const float* __restrict__ image,
+    const float* __restrict__ grad_image, float* __restrict__ grad_inst, int grad_is_final, GsCrop crop,
+    uint32_t* __restrict__ row_epoch, uint32_t epoch, int* __restrict__ tile_neff_b, const float* __restrict__ aux,
+    const float* __restrict__ grad_aux, const GsView* __restrict__ views) {
+  static_assert(!BATCH || GATHER, "batched frames run the gather path");
   using Cfg = Bwd2Cfg<PX, STAGES, RQ>;
   constexpr int NT = Cfg::NT, TPR = Cfg::TPR, R = Cfg::R, SQ = Cfg::SQ, QS = Cfg::QS, IS = Cfg::IS, ROWS = Cfg::ROWS;
   static_assert(IS % 2 == 0 && QS % 2 == 0 && IS % 32 == 2 && QS % 32 == 32 / RQ, "partial buffer strides");
@@ -983,7 +1023,18 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   const int nchunks = (cnt + CH - 1) / CH;
   const int tx = tile % ntx, ty = tile / ntx;
   const int shift = start & 1;
-  if (tid < GS_TILE) sm.pyt[tid] = gs_pixel_coord(ty * GS_TILE + tid, hp, fy);
+  int lty = ty;   // the tile's row in its view
+  if constexpr (BATCH) {
+    const int v = ty / (hp / GS_TILE);
+    lty = ty - v * (hp / GS_TILE);
+    fx = views[v].fx;
+    fy = views[v].fy;
+    if (grad_is_final) {
+      grad_image += (size_t)v * crop.width * crop.height * 3;
+      if (grad_aux) grad_aux += (size_t)v * crop.width * crop.height * 2;
+    }
+  }
+  if (tid < GS_TILE) sm.pyt[tid] = gs_pixel_coord(lty * GS_TILE + tid, hp, fy);
   if constexpr (GATHER) {
     if (tid == 0) {
       for (int s = 0; s < STAGES; ++s) gs_mbar_init(&sm.full[s], NT);
@@ -1012,6 +1063,7 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
   }
   const int ix0 = tx * GS_TILE + (tid % TPR) * PX;
   const int iy = ty * GS_TILE + (tid / TPR);
+  const int iyv = lty * GS_TILE + (tid / TPR);   // its row in the view
   float px[PX];
 #pragma unroll
   for (int p = 0; p < PX; ++p) px[p] = gs_pixel_coord(ix0 + p, wp, fx);
@@ -1038,7 +1090,7 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     } else {
 #pragma unroll
       for (int p = 0; p < PX; ++p)
-        gs_load_final_grad(grad_image, ibuf + 3 * p, ix0 + p, iy, crop.left, crop.top, crop.width, crop.height,
+        gs_load_final_grad(grad_image, ibuf + 3 * p, ix0 + p, iyv, crop.left, crop.top, crop.width, crop.height,
                            gbuf[3 * p], gbuf[3 * p + 1], gbuf[3 * p + 2]);
     }
 #pragma unroll
@@ -1069,7 +1121,7 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     } else {
 #pragma unroll
       for (int p = 0; p < PX; ++p) {   // depth / alpha are not clamped: only the crop masks their gradient
-        const int x = ix0 + p - crop.left, y = iy - crop.top;
+        const int x = ix0 + p - crop.left, y = iyv - crop.top;
         float2 v = make_float2(0.f, 0.f);
         if (x >= 0 && x < crop.width && y >= 0 && y < crop.height)
           v = *reinterpret_cast<const float2*>(grad_aux + ((size_t)y * crop.width + x) * 2);
@@ -1320,6 +1372,31 @@ __global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB)
     out[2] = z;
   }
 }
+
+#define GS_BWD2_PARAMS                                                                                              \
+  const float4 *__restrict__ pA, const float2 *__restrict__ pB, const float4 *__restrict__ pC,                      \
+      const GsRec *__restrict__ grec, const uint32_t *__restrict__ ids, const uint32_t *__restrict__ goff,          \
+      const int *__restrict__ tile_accum, int wp, int hp, int ntx, float fx, float fy,                              \
+      const float *__restrict__ image, const float *__restrict__ grad_image, float *__restrict__ grad_inst,         \
+      int grad_is_final, GsCrop crop, uint32_t *__restrict__ row_epoch, uint32_t epoch,                             \
+      int *__restrict__ tile_neff_b, const float *__restrict__ aux, const float *__restrict__ grad_aux
+#define GS_BWD2_ARGS                                                                                              \
+  pA, pB, pC, grec, ids, goff, tile_accum, wp, hp, ntx, fx, fy, image, grad_image, grad_inst, grad_is_final, crop, \
+      row_epoch, epoch, tile_neff_b, aux, grad_aux
+
+template <int PX, bool WS, int UNR, int STAGES, int MINB, int RQ, bool GATHER, int CH, bool AUX = false,
+          bool REPACK = false, bool ABS = false>
+__global__ void __launch_bounds__(256 / PX + (WS ? 32 : 0), MINB) blend_bwd2_kernel(GS_BWD2_PARAMS) {
+  blend_bwd2_body<PX, WS, UNR, STAGES, MINB, RQ, GATHER, CH, AUX, REPACK, ABS>(GS_BWD2_ARGS, nullptr);
+}
+
+// the shipped gather backward with the live-pixel repack (AUX, ABS as in blend_bwd2_kernel) of a batched frame
+template <bool AUX, bool ABS>
+__global__ void __launch_bounds__(32, 10) blend_bwd2_batch_kernel(GS_BWD2_PARAMS, const GsView* __restrict__ views) {
+  blend_bwd2_body<8, false, 4, 3, 10, 4, true, 32, AUX, true, ABS, true>(GS_BWD2_ARGS, views);
+}
+#undef GS_BWD2_ARGS
+#undef GS_BWD2_PARAMS
 
 // =======================================================================================
 // legacy boundary helpers: per-instance tensors <-> packed record streams
@@ -1631,6 +1708,47 @@ int gs_blend_absgrad_supported(int d, bool gather) {
     return gs_set_error_msg(GS_ERR_UNSUPPORTED,
                             "densify statistics: absgrad needs the shipped backward blend knobs");
   return 0;
+}
+
+int gs_blend_batch_supported() {
+  const GsTuning& tn = gs_tuning();
+  if (!tn.gather)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "batched frame: the packed path (gs_tune(\"gather\", 0)) has no batched kernel");
+  if (tn.fwd_kernel != 0 || tn.fwd_ch != 128 || tn.fwd_px != 4 || !shipped_rgb_bwd_knobs(tn) || !tn.blend_repack)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED,
+                            "batched frame: only the shipped RGB blend knobs (with the live-pixel repack) have batched kernels");
+  return 0;
+}
+
+cudaError_t gs_launch_blend_fwd_batch(const GsRec* grec, const uint32_t* ids, const int* tile_accum,
+                                      const GsFrameGeom& g, const GsView* views, float* image, int* tile_neff,
+                                      float* final_img, const GsCrop& crop, cudaStream_t st, const GsAuxOut* aux) {
+  if (aux)
+    blend_fwd_batch_kernel<true><<<g.n_tiles, 64, 0, st>>>(grec, ids, tile_accum, g.wp, g.hp, g.ntx, views, image,
+                                                           tile_neff, final_img, crop, *aux);
+  else
+    blend_fwd_batch_kernel<false><<<g.n_tiles, 64, 0, st>>>(grec, ids, tile_accum, g.wp, g.hp, g.ntx, views, image,
+                                                            tile_neff, final_img, crop, GsAuxOut{});
+  return cudaGetLastError();
+}
+
+cudaError_t gs_launch_blend_bwd_batch(const GsRec* grec, const uint32_t* ids, const uint32_t* goff,
+                                      const int* tile_accum, const GsFrameGeom& g, const GsView* views,
+                                      const float* image, const float* grad_image, float* grad_inst, int grad_is_final,
+                                      const GsCrop& crop, uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b,
+                                      cudaStream_t st, const float* aux, const float* grad_aux, bool absgrad) {
+  if (!row_epoch || (grad_aux && !aux)) return cudaErrorInvalidValue;
+#define GS_BWD2_BATCH(AX, AB)                                                                                      \
+  blend_bwd2_batch_kernel<AX, AB><<<g.n_tiles, 32, 0, st>>>(nullptr, nullptr, nullptr, grec, ids, goff, tile_accum, \
+                                                            g.wp, g.hp, g.ntx, 0.f, 0.f, image, grad_image,         \
+                                                            grad_inst, grad_is_final, crop, row_epoch, epoch,       \
+                                                            tile_neff_b, aux, grad_aux, views)
+  if (grad_aux && absgrad) GS_BWD2_BATCH(true, true);
+  else if (grad_aux) GS_BWD2_BATCH(true, false);
+  else if (absgrad) GS_BWD2_BATCH(false, true);
+  else GS_BWD2_BATCH(false, false);
+#undef GS_BWD2_BATCH
+  return cudaGetLastError();
 }
 
 extern "C" size_t gs_draw_workspace_bytes(int m, int d) {

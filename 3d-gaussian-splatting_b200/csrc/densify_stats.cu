@@ -57,7 +57,84 @@ __global__ void __launch_bounds__(kBlock) densify_stats_kernel(
   max_radius[i] = fmaxf(max_radius[i], rad);
 }
 
+// Batched frame: Gaussian i's views in view order, each one's statistics formed as densify_stats_kernel forms them
+// (pair v n + i, view v's camera, filter and (sx, sy) = (W / (2 fx), H / (2 fy))) and added to running values that are
+// loaded and stored once: the result of B single-view backwards run in view order.
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_batch_kernel(
+    const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views,
+    int scale_act, const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
+    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, int gw,
+    const uint32_t* __restrict__ row_epoch, uint32_t epoch, int width, int height, float* __restrict__ grad2d,
+    float* __restrict__ absgrad, int* __restrict__ n_views_out, float* __restrict__ max_radius) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  if (i >= n) return;
+  float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
+  float q[4], s[3], raw_s[3], qn;
+  gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+  float g2 = grad2d[i], ga = ABS ? absgrad[i] : 0.f, mr = max_radius[i];
+  int nv = n_views_out[i];
+  bool any = false;
+  for (int v = 0; v < n_views; ++v) {
+    const int j = v * n + i;
+    const uint32_t cnt = count[j];
+    if (cnt == 0) continue;
+    any = true;
+    const GsView vw = views[v];
+    const float sx = (float)((double)width / (2.0 * (double)vw.fx));
+    const float sy = (float)((double)height / (2.0 * (double)vw.fy));
+    float gx = 0.f, gy = 0.f, ax = 0.f, ay = 0.f;
+    const uint32_t o0 = offsets_g[j], o1 = o0 + cnt;
+    for (uint32_t r = o0; r < o1; ++r) {
+      if (row_epoch[r] != epoch) continue;
+      const float* row = grad_inst + (size_t)r * gw;
+      const float2 g = *reinterpret_cast<const float2*>(row);
+      gx += g.x;
+      gy += g.y;
+      if constexpr (ABS) {
+        const float2 a = *reinterpret_cast<const float2*>(row + 10);
+        ax += a.x;
+        ay += a.y;
+      }
+    }
+    GsProj o = gs_project(vw.cam, p, q, s, near_plane, vw.half_w, vw.half_h);
+    const GsFilter2dOut fo = gs_filter2d(vw.filt, o.a, o.b, o.c, o.d);
+    const float fx = vw.fx, fy = vw.fy;
+    const double A = (double)fo.a * fx * fx, B = (double)o.b * fx * fy, D = (double)fo.d * fy * fy;
+    const double h = 0.5 * (A - D);
+    const double lmax = 0.5 * (A + D) + sqrt(h * h + B * B);
+    const float rad = (float)ceil(3.0 * sqrt(fmax(lmax, 0.0)));
+    g2 += sqrtf((gx * sx) * (gx * sx) + (gy * sy) * (gy * sy));
+    if constexpr (ABS) ga += sqrtf((ax * sx) * (ax * sx) + (ay * sy) * (ay * sy));
+    nv += 1;
+    mr = fmaxf(mr, rad);
+  }
+  if (!any) return;
+  grad2d[i] = g2;
+  if constexpr (ABS) absgrad[i] = ga;
+  n_views_out[i] = nv;
+  max_radius[i] = mr;
+}
+
 }  // namespace
+
+cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, const float* scale, int n, int n_views,
+                                          int scale_act, const GsView* views, float near_plane,
+                                          const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
+                                          int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
+                                          const gs_densify_stats& s, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  const int blocks = (n + kBlock - 1) / kBlock;
+#define GS_LAUNCH_STATS_BATCH(ABS)                                                                                 \
+  densify_stats_batch_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, n_views, scale_act, views,       \
+                                                             near_plane, offsets_g, count, grad_inst, gw, row_epoch, \
+                                                             epoch, g.width, g.height, s.grad2d, s.absgrad, s.count, \
+                                                             s.max_radius)
+  if (s.absgrad) GS_LAUNCH_STATS_BATCH(true);
+  else GS_LAUNCH_STATS_BATCH(false);
+#undef GS_LAUNCH_STATS_BATCH
+  return cudaGetLastError();
+}
 
 cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const float* scale, int n, int scale_act,
                                     const GsCam& cam, float near_plane, float half_w, float half_h,

@@ -136,6 +136,24 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/,
                                     const GsFilter2d* filt = nullptr /*non-null: 2-D screen-space filter*/);
 
+// One view of a batched frame (gs_render_forward_batch): the per-view constants of the projection, the blend, the
+// projection backward and the densification statistics, formed on the host exactly as a single-view frame forms them
+// and read by the batched kernels from a device table [n_views].  View v owns tile rows v nty .. (v + 1) nty - 1 of
+// the frame's tile grid and rows v Hp .. (v + 1) Hp - 1 of the tall padded image.
+struct GsView {
+  GsCam cam;
+  GsTileGrid grid;     // the view's own grid (nty rows); the projection offsets the rectangle's rows by v nty
+  GsFilter2d filt;     // zero when the frame has no 2-D filter
+  float half_w, half_h, fx, fy;
+};
+
+cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                          const float* scale, int n, int n_views, int d, int scale_act,
+                                          const GsView* views, float near_plane, GsRec* rec /*[B n]*/,
+                                          uint2* rect /*[B n]*/, uint32_t* count /*[B n]*/, uint32_t* dkey /*[B n]*/,
+                                          int64_t* mask /*[B, n], nullable*/, unsigned int* n_visible,
+                                          cudaStream_t st, bool sh_gaussian, bool filt);
+
 // Data-parallel gradient push (device view of gs_grad_push): world == 0 disables it.
 struct GsGradPush {
   float* bucket;                  // this rank's flat gradient bucket (the five grad pointers lie inside)
@@ -166,6 +184,17 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
                                             bool depth_grad, bool sh_gaussian, const GsFilter2d* filt = nullptr);
 
+// Batched frame: one thread per Gaussian sums, view by view in view order, the rows of pair v n + i exactly as
+// gs_launch_fused_project_bwd does for one view, chains them with view v's camera and filter, and writes the sum over
+// the views of each parameter gradient once.  No push.  One launch when n > 0.
+cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                              const float* scale, int n, int n_views, int d, int scale_act,
+                                              const GsView* views, float near_plane, const uint32_t* offsets_g,
+                                              const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
+                                              uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                              float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
+                                              bool filt);
+
 // ---- densify_stats.cu ------------------------------------------------------------------
 // Accumulates the screen-space densification statistics of the backward that just wrote grad_inst (rows of gw floats;
 // s.absgrad != NULL reads columns 10, 11 written by the ABS blend kernels) into s's buffers.  One launch when n > 0.
@@ -175,6 +204,12 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                     const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst, int gw,
                                     const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
                                     const gs_densify_stats& s, cudaStream_t st);
+// The same for a batched frame: each view's statistics are added in view order (g: the per-view width and height)
+cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, const float* scale, int n, int n_views,
+                                          int scale_act, const GsView* views, float near_plane,
+                                          const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
+                                          int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
+                                          const gs_densify_stats& s, cudaStream_t st);
 
 // ---- blend_feat.cu ---------------------------------------------------------------------
 // Feature maps (gs_render_forward_feat / gs_render_backward_feat), gather path only.  f: 8, 16 or 32.
@@ -237,3 +272,20 @@ int gs_blend_absgrad_supported(int d, bool gather);
 // SH: the scalar and one-pixel-per-thread tensor-core kernels): 0 when the current tuning knobs for colour width d
 // select one, else GS_ERR_UNSUPPORTED with a message.
 int gs_blend_aux_supported(int d, bool forward, bool backward);
+
+// Batched frames (gs_render_forward_batch) run the shipped RGB gather kernels with the batched flag: the view of a tile
+// is its tile row / (hp / GS_TILE), pixel coordinates use the view's rows and views[v].fx / fy, and final / aux_final /
+// a final upstream gradient are addressed per view ([B, height, width, .]).  g: per-view wp, hp, width, height; the
+// frame's ntx and n_tiles = B T.  0 when the current knobs select those kernels (the shipped forward and backward blend
+// knobs with the live-pixel repack, gather path), else GS_ERR_UNSUPPORTED with a message.
+int gs_blend_batch_supported();
+cudaError_t gs_launch_blend_fwd_batch(const GsRec* grec, const uint32_t* ids, const int* tile_accum,
+                                      const GsFrameGeom& g, const GsView* views, float* image, int* tile_neff,
+                                      float* final_img, const GsCrop& crop, cudaStream_t st,
+                                      const GsAuxOut* aux /*nullable*/);
+cudaError_t gs_launch_blend_bwd_batch(const GsRec* grec, const uint32_t* ids, const uint32_t* goff,
+                                      const int* tile_accum, const GsFrameGeom& g, const GsView* views,
+                                      const float* image, const float* grad_image, float* grad_inst, int grad_is_final,
+                                      const GsCrop& crop, uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b,
+                                      cudaStream_t st, const float* aux, const float* grad_aux /*nullable*/,
+                                      bool absgrad);

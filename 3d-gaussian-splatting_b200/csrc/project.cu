@@ -57,6 +57,7 @@ __device__ __forceinline__ void sh_logits(const float* coef, const float* Y, flo
 // degree 2 / 3 evaluated once per Gaussian along view_dir (GS_SH_EVAL_GAUSSIAN); the record then carries an RGB colour.
 // F: the 2-D screen-space filter `filt` (gs_filter2d) is applied to the covariance before the tile rectangle and the
 // conic, and its compensation to l2o.
+// The batched frame's fused_project_one repeats this arithmetic: a change to it must be made to both.
 template <int KG, bool F = false>
 __device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
@@ -183,6 +184,132 @@ __global__ void __launch_bounds__(kBlock) fused_project_filt_kernel(
                               rect, count, dkey, mask, n_visible, filt);
 }
 
+// Batched frames.  Gaussian i (loaded parameters p, q, s, opa_raw, rgb_raw) seen by one view: the arithmetic of
+// fused_project_body, with its record, rectangle, count and depth key going to pair j = v n + i and the rectangle's
+// rows offset by ty_off (the view's first tile row).  Returns the instance count; vis: in the frustum.  (The
+// single-view kernels keep their own copy: routed through this function they compile to different SASS; a change
+// to the arithmetic of either copy must be made to both.)
+template <int KG, bool F>
+__device__ __forceinline__ uint32_t fused_project_one(
+    const float* __restrict__ rgb, int i, int d, const GsCam& cam, const GsTileGrid& grid, float near_plane,
+    float half_w, float half_h, const GsFilter2d& filt, const float p[3], const float q[4], const float s[3],
+    float opa_raw, const float rgb_raw[3], uint32_t ty_off, int j, GsRec* __restrict__ rec, uint2* __restrict__ rect,
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis) {
+  uint32_t cnt = 0;
+  {
+    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    vis = o.visible;
+    if (mask) mask[j] = o.visible ? 1 : 0;
+    bool keep = o.visible;
+    float dl2o = 0.f;
+    if constexpr (F) {
+      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
+      o.a = fo.a;
+      o.d = fo.d;
+      dl2o = fo.dl2o;
+      keep = keep && fo.keep;
+    }
+    uint2 rc = make_uint2(0u, 0u);
+    if (keep) {
+      uint32_t tx0, tx1, ty0, ty1;
+      if (gs_tile_rect(grid, o.x, o.y, o.a, o.b, o.c, o.d, tx0, tx1, ty0, ty1)) {
+        cnt = (tx1 - tx0) * (ty1 - ty0);
+        rc = make_uint2(tx0 | ((ty0 + ty_off) << 16), (tx1 - tx0) | ((ty1 - ty0) << 16));
+        GsConic k = gs_make_conic(o.a, o.b, o.c, o.d);
+        float op = gs_sigmoid(opa_raw);
+        GsRec* r = rec + j;
+        r->a = make_float4(o.x, o.y, k.ca, k.cb);
+        // RGB colour = sigmoid(logit) (splatter.py:539); per-pixel SH coefficients stay raw and are gathered
+        // from the parameter tensor by the pack pass
+        float cr = 0.f, cg = 0.f, cb = 0.f;
+        if constexpr (KG > 0) {
+          float coef[3 * KG], dir[3], il, Y[KG], l[3];
+#pragma unroll
+          for (int k = 0; k < 3 * KG; ++k) coef[k] = rgb[(size_t)i * (3 * KG) + k];
+          view_dir(cam, p, dir, il);
+          gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
+          sh_logits<KG>(coef, Y, l);
+          cr = gs_sigmoid(l[0]);
+          cg = gs_sigmoid(l[1]);
+          cb = gs_sigmoid(l[2]);
+        } else if (d == 3) {
+          cr = gs_sigmoid(rgb_raw[0]);
+          cg = gs_sigmoid(rgb_raw[1]);
+          cb = gs_sigmoid(rgb_raw[2]);
+        }
+        r->b = make_float4(k.cc, F ? log2f(op) + dl2o : log2f(op), cr, cg);
+        r->c = make_float4(cb, o.depth, __uint_as_float(rc.x), __uint_as_float(rc.y));
+        r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
+      }
+    }
+    // the tile rectangle again, densely (zero without instances: whole sectors), for the instance emission: an 8-byte
+    // read from a 19 MB array at C3 instead of a 16-byte gather from the 154 MB records
+    rect[j] = rc;
+    count[j] = cnt;
+    // depth sort key: positive float bits order like the floats; Gaussians without instances last
+    dkey[j] = cnt ? __float_as_uint(o.depth) : 0xffffffffu;
+  }
+  return cnt;
+}
+
+// Batched frame: one thread per Gaussian loads its parameters once and projects it into each view in turn, writing
+// pair j = v n + i with view v's constants (K, F as in fused_project_filt_kernel; F reads views[v].filt).  The
+// counters receive the frame's totals over the pairs.
+template <int K, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,
+    const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible) {
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  unsigned int nv = 0;
+  unsigned long long c64 = 0;
+  if (i < n) {
+    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
+    float q[4], s[3], raw_s[3], qn;
+    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    const float opa_raw = opa[i];
+    float rgb_raw[3] = {0.f, 0.f, 0.f};
+    if (K == 0 && d == 3) {
+      rgb_raw[0] = rgb[3 * i];
+      rgb_raw[1] = rgb[3 * i + 1];
+      rgb_raw[2] = rgb[3 * i + 2];
+    }
+    for (int v = 0; v < n_views; ++v) {
+      const GsView vw = views[v];
+      bool vis = false;
+      c64 += fused_project_one<K, F>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p, q, s,
+                                     opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect, count, dkey,
+                                     mask, vis);
+      nv += vis ? 1u : 0u;
+    }
+  }
+  __shared__ unsigned long long wsum[kBlock / 32];
+  __shared__ unsigned int wvis[kBlock / 32];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    c64 += __shfl_xor_sync(0xffffffffu, c64, o);
+    nv += __shfl_xor_sync(0xffffffffu, nv, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    wsum[threadIdx.x >> 5] = c64;
+    wvis[threadIdx.x >> 5] = nv;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long tot = 0;
+    unsigned int tv = 0;
+#pragma unroll
+    for (int w = 0; w < kBlock / 32; ++w) {
+      tot += wsum[w];
+      tv += wvis[w];
+    }
+    if (tv) atomicAdd(n_visible, tv);
+    if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
+  }
+}
+
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
 // contiguous rows offsets_g[i] .. + count[i]) and chains them to the RAW parameters.  No
 // atomics anywhere: the result is deterministic.  Row layout (GW floats): d/d{x, y, ca, cb, cc,
@@ -229,6 +356,7 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
 // the view-direction term of per-Gaussian SH); with all five gradient pointers NULL no parameter gradient is stored.
 // F: the forward applied the 2-D filter `filt` (fused_project_body<KG, true>): the conic is chained with the filtered
 // covariance, and the compensation's gradient is added to dL/dcov.
+// The batched frame's fused_project_bwd_one repeats this arithmetic: a change to it must be made to both.
 template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false>
 __device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
@@ -497,6 +625,255 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_filt_kernel(GS_PBWD_
 template <int K, int W, bool DT>
 __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PBWD_PARAMS, GsFilter2d filt) {
   fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true>(GS_PBWD_ARGS, nullptr, filt);
+}
+
+// Batched frames.  One view's share of Gaussian i's parameter gradients, the arithmetic of fused_project_bwd_body for
+// RGB gradient rows without a push or a camera gradient (rows o0 .. o1 - 1 of grad_inst, the loaded parameters p, q,
+// s, raw_s, qn, opa_raw, rgb_raw / coef): acc receives the row sums, then gp, gq_raw, gs_raw, go and the colour
+// gradients (acc + 6 for D == 3, gsh for KG > 0) are formed.  The single-view kernels keep their own copy (routed
+// through this function they compile to different SASS): a change to the arithmetic of either copy must be made to
+// both.
+template <int D, bool DT, int KG, bool F>
+__device__ __forceinline__ void fused_project_bwd_one(
+    GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
+    const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
+    const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, float opa_raw,
+    const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GS_GREC], float (&gsh)[KG ? D : 1],
+    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go) {
+  constexpr int GW = GS_GREC;
+  constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
+  {
+    // The rows are summed one by one in row order.  For an RGB frame the rows are loaded in groups: the tags of four
+    // rows at once, then the live rows among them (48 registers of payload), so that a Gaussian with a few instances
+    // waits for two round trips to HBM per group instead of two per row (H100, C3: 0.235 -> 0.230 ms).  Grouping only
+    // the tags and loading the rows one at a time was slower (RGB 0.245 ms; per-pixel SH, D = 27: 0.496 -> 0.526 ms),
+    // and so was the grouped loop with per-Gaussian SH of degree 2 (80 -> 99 registers, 0.409 -> 0.464 ms): those
+    // kernels keep the plain loop.  An instance its (saturated) tile did not reach has a stale tag and contributes
+    // nothing.
+    if constexpr (KG > 0) {
+      for (uint32_t r = o0; r < o1; ++r) {
+        if (row_epoch[r] != epoch) continue;
+        const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)r * GW);
+#pragma unroll
+        for (int qq = 0; qq < GW / 4; ++qq) {
+          const float4 v = row[qq];
+          acc[4 * qq] += v.x;
+          acc[4 * qq + 1] += v.y;
+          acc[4 * qq + 2] += v.z;
+          acc[4 * qq + 3] += v.w;
+        }
+      }
+    } else {
+      constexpr int kGroup = 4;
+      for (uint32_t r0 = o0; r0 < o1; r0 += kGroup) {
+        bool live[kGroup];
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) live[j] = r0 + j < o1 && row_epoch[r0 + j] == epoch;
+        float4 v[kGroup][GW / 4];
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) {
+          const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)(r0 + j) * GW);
+#pragma unroll
+          for (int qq = 0; qq < GW / 4; ++qq) v[j][qq] = live[j] ? row[qq] : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int j = 0; j < kGroup; ++j) {
+          if (!live[j]) continue;
+#pragma unroll
+          for (int qq = 0; qq < GW / 4; ++qq) {
+            acc[4 * qq] += v[j][qq].x;
+            acc[4 * qq + 1] += v[j][qq].y;
+            acc[4 * qq + 2] += v[j][qq].z;
+            acc[4 * qq + 3] += v[j][qq].w;
+          }
+        }
+      }
+    }
+    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    float fk[4];                                               // F: d l2o / d cov of the compensation
+    if constexpr (F) {
+      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
+      o.a = fo.a;
+      o.d = fo.d;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) fk[j] = fo.k[j];
+    }
+    // conic (ca, cb, cc) = (d, b+c, a) * sc,  sc = log2e / (2 det + 1e-14)
+    float det = o.a * o.d - o.b * o.c;
+    double pn = 2.0 * (double)det + 1e-14;
+    float sc = (float)((double)GS_LOG2E / pn);
+    float kk = 2.f * sc * sc / GS_LOG2E;                      // d sc / d det = -kk
+    float gsc = acc[2] * o.d + acc[3] * (o.b + o.c) + acc[4] * o.a;
+    float gcov[4];
+    gcov[0] = acc[4] * sc - gsc * kk * o.d;                   // d det/da =  d
+    gcov[1] = acc[3] * sc + gsc * kk * o.c;                   // d det/db = -c
+    gcov[2] = acc[3] * sc + gsc * kk * o.b;                   // d det/dc = -b
+    gcov[3] = acc[2] * sc - gsc * kk * o.a;                   // d det/dd =  a
+    if constexpr (F) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) gcov[j] += acc[5] * fk[j];
+    }
+    static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
+    float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
+    float gq[4], gsv[3];
+    gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    if constexpr (KG > 0) {
+      // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
+      // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
+      float dir[3], il, Y[KG], l[3], gl[3], w[KG], gd[3];
+      view_dir(cam, p, dir, il);
+      gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
+      sh_logits<KG>(coef, Y, l);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float sg = gs_sigmoid(l[c]);
+        gl[c] = acc[6 + c] * sg * (1.f - sg);
+      }
+#pragma unroll
+      for (int k = 0; k < KG; ++k) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) gsh[c * KG + k] = gl[c] * Y[k];
+        w[k] = gl[0] * coef[k] + gl[1] * coef[KG + k] + gl[2] * coef[2 * KG + k];
+      }
+      gs_sh::sh_basis_grad<KG>(dir[0], dir[1], dir[2], w, gd);
+      const float dd = dir[0] * gd[0] + dir[1] * gd[1] + dir[2] * gd[2];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) gp[j] += (gd[j] - dir[j] * dd) * il;
+    }
+    // quat normalisation backward: q = r/|r|
+    float dot = q[0] * gq[0] + q[1] * gq[1] + q[2] * gq[2] + q[3] * gq[3];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) gq_raw[k] = (gq[k] - q[k] * dot) / qn;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      if (scale_act == GS_SCALE_ABS)
+        gs_raw[k] = gsv[k] * (raw_s[k] > 0.f ? 1.f : (raw_s[k] < 0.f ? -1.f : 0.f));
+      else
+        gs_raw[k] = gsv[k] * expf(fminf(fmaxf(raw_s[k], -1.f), 1.f));   // renderer.py:98-100
+    }
+    float op = gs_sigmoid(opa_raw);
+    // l2o = log2(op):  d/d logit = d_l2o / (op ln2) * op (1-op) = d_l2o (1-op) / ln2
+    go = acc[5] * (1.f - op) / GS_LN2;
+    if (D == 3) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        float c = gs_sigmoid(rgb_raw[k]);
+        acc[6 + k] *= c * (1.f - c);
+      }
+    }
+  }
+}
+
+// The parameter gradients of Gaussian i to the caller's tensors (no push).  Per-Gaussian and per-pixel SH colour (D != 3)
+// stage the warp's coefficient rows: every thread of the warp takes part, `valid` or not.
+template <int D>
+__device__ __forceinline__ void fused_project_bwd_store(int i, int n, bool valid, const float* gcol, const float (&gp)[3],
+                                                        const float (&gs_raw)[3], const float (&gq_raw)[4], float go,
+                                                        float* __restrict__ g_pos, float* __restrict__ g_rgb,
+                                                        float* __restrict__ g_opa, float* __restrict__ g_quat,
+                                                        float* __restrict__ g_scale) {
+  constexpr bool kStagedRgb = D != 3;
+  if constexpr (kStagedRgb) {
+    // The 32 Gaussians of a warp own 32 * D contiguous floats of g_rgb.  One strided 4-byte store per coefficient
+    // makes every store a partial-sector write (read-modify-write under ECC: 8x the bytes): the rows go through
+    // shared memory and leave as whole sectors.
+    // D = 48: two passes of 24 floats (96-byte, sector-aligned pieces); D = 27: the whole 32 x 108-byte span.
+    constexpr int HW = (D % 8 == 0) ? D / 2 : D;
+    __shared__ float stage[kBlock / 32][32][HW + 1];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i0 = blockIdx.x * kBlock + warp * 32;
+    const int nrow = min(32, n - i0);
+#pragma unroll
+    for (int pass = 0; pass < D / HW; ++pass) {
+      __syncwarp();
+#pragma unroll
+      for (int k = 0; k < HW; ++k) stage[warp][lane][k] = gcol[pass * HW + k];
+      __syncwarp();
+      if (HW == D) {
+        float* dst = g_rgb + (size_t)i0 * D;
+        for (int t = lane; t < nrow * D; t += 32) dst[t] = stage[warp][t / D][t % D];
+      } else {
+        for (int t = lane; t < nrow * HW; t += 32) {
+          const int g = t / HW, c = t % HW;
+          g_rgb[(size_t)(i0 + g) * D + pass * HW + c] = stage[warp][g][c];
+        }
+      }
+    }
+    if (!valid) return;
+  } else {
+#pragma unroll
+    for (int k = 0; k < D; ++k) g_rgb[(size_t)i * D + k] = gcol[k];
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    g_pos[3 * i + k] = gp[k];
+    g_scale[3 * i + k] = gs_raw[k];
+  }
+  reinterpret_cast<float4*>(g_quat)[i] = make_float4(gq_raw[0], gq_raw[1], gq_raw[2], gq_raw[3]);
+  g_opa[i] = go;
+}
+
+// Batched frame: K = 0 RGB, 9 / 16 per-Gaussian SH; DT, F as above (F reads views[v].filt).  Thread i loads Gaussian
+// i's parameters once and takes its views in order: view v's share is fused_project_bwd_one over the rows of pair
+// v n + i with view v's camera, and the shares are added in view order with no contraction into their last products:
+// the sum of B single-view backwards accumulated in view order, to within the FMA contractions the compiler chooses
+// differently inside the view loop (measured: 1e-6 relative at most).
+template <int K, bool DT, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,
+    const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
+    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
+    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
+    float* __restrict__ g_quat, float* __restrict__ g_scale) {
+  constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  const bool valid = i < n;
+  if (!valid && D == 3) return;   // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
+  float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f}, go = 0.f;
+  float gcol[D];
+#pragma unroll
+  for (int k = 0; k < D; ++k) gcol[k] = 0.f;
+  if (valid) {
+    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
+    float q[4], s[3], raw_s[3], qn;
+    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    const float opa_raw = opa[i];
+    float rgb_raw[3] = {0.f, 0.f, 0.f};
+    float coef[K ? D : 1];
+    if constexpr (K > 0) {
+#pragma unroll
+      for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
+    } else {
+      rgb_raw[0] = rgb[3 * i];
+      rgb_raw[1] = rgb[3 * i + 1];
+      rgb_raw[2] = rgb[3 * i + 2];
+    }
+    for (int v = 0; v < n_views; ++v) {
+      const int j = v * n + i;
+      const uint32_t cnt = count[j], o0 = offsets_g[j];
+      if (cnt == 0) continue;
+      const GsView vw = views[v];
+      float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
+#pragma unroll
+      for (int k = 0; k < GW; ++k) acc[k] = 0.f;
+      fused_project_bwd_one<D, DT, K, F>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0, o0 + cnt,
+                                         grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw, rgb_raw, coef, acc,
+                                         gsh, vp, vq, vs, vo);
+      const float* vc = K ? gsh : acc + 6;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        gp[k] = __fadd_rn(gp[k], vp[k]);
+        gs_raw[k] = __fadd_rn(gs_raw[k], vs[k]);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) gq_raw[k] = __fadd_rn(gq_raw[k], vq[k]);
+      go = __fadd_rn(go, vo);
+#pragma unroll
+      for (int k = 0; k < D; ++k) gcol[k] = __fadd_rn(gcol[k], vc[k]);
+    }
+  }
+  fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
 }
 
 // Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
@@ -831,3 +1208,52 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
   return cudaGetLastError();
 }
 #undef GS_PBWD_ARGS
+
+cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                          const float* scale, int n, int n_views, int d, int scale_act,
+                                          const GsView* views, float near_plane, GsRec* rec, uint2* rect,
+                                          uint32_t* count, uint32_t* dkey, int64_t* mask, unsigned int* n_visible,
+                                          cudaStream_t st, bool sh_gaussian, bool filt) {
+  if (n == 0) return cudaSuccess;
+  if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+#define GS_LAUNCH_PBATCH(K, F)                                                                                    \
+  fused_project_batch_kernel<K, F><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,     \
+                                                                   scale_act, views, near_plane, rec, rect, count, \
+                                                                   dkey, mask, n_visible)
+  const int k = d == 27 ? 9 : (d == 48 ? 16 : 0);
+  if (k == 9 && filt) GS_LAUNCH_PBATCH(9, true);
+  else if (k == 9) GS_LAUNCH_PBATCH(9, false);
+  else if (k == 16 && filt) GS_LAUNCH_PBATCH(16, true);
+  else if (k == 16) GS_LAUNCH_PBATCH(16, false);
+  else if (filt) GS_LAUNCH_PBATCH(0, true);
+  else GS_LAUNCH_PBATCH(0, false);
+#undef GS_LAUNCH_PBATCH
+  return cudaGetLastError();
+}
+
+cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                              const float* scale, int n, int n_views, int d, int scale_act,
+                                              const GsView* views, float near_plane, const uint32_t* offsets_g,
+                                              const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
+                                              uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                              float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
+                                              bool filt) {
+  if (n == 0) return cudaSuccess;
+  if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+#define GS_LAUNCH_PBWD_BATCH(K, DT, F)                                                                              \
+  fused_project_bwd_batch_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                         \
+      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
+      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale)
+#define GS_LAUNCH_PBWD_BATCH_F(K, DT)       \
+  if (filt) GS_LAUNCH_PBWD_BATCH(K, DT, true); \
+  else GS_LAUNCH_PBWD_BATCH(K, DT, false)
+  if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_F(9, true); }
+  else if (d == 27) { GS_LAUNCH_PBWD_BATCH_F(9, false); }
+  else if (d == 48 && depth_grad) { GS_LAUNCH_PBWD_BATCH_F(16, true); }
+  else if (d == 48) { GS_LAUNCH_PBWD_BATCH_F(16, false); }
+  else if (depth_grad) { GS_LAUNCH_PBWD_BATCH_F(0, true); }
+  else { GS_LAUNCH_PBWD_BATCH_F(0, false); }
+#undef GS_LAUNCH_PBWD_BATCH_F
+#undef GS_LAUNCH_PBWD_BATCH
+  return cudaGetLastError();
+}

@@ -140,14 +140,18 @@ struct gs_ctx {
   // per tile / misc
   DevBuf tile_accum, tile_neff, tile_neff_b, cub_tmp, counters, img_dev, gimg_dev, rays;
   DevBuf cam_part;                        // per-CTA partial sums of the camera gradient (gs_render_backward_cam)
+  DevBuf views;                           // GsView[n_views] of the last batched forward (gs_render_forward_batch)
   float* host_rays = nullptr;             // pinned: rays_o, lefttop, dx, dy (SH colour only)
+  GsView* host_views = nullptr;           // pinned: staging of the view table (GS_MAX_VIEWS entries)
   unsigned long long* host_m = nullptr;   // pinned: {M}
   cudaEvent_t ev_m = nullptr;             // marks the completion of the M read-back
+  cudaEvent_t ev_views = nullptr;         // marks the completion of the view table's upload from host_views
   // state of the last forward
   bool have_forward = false, have_backward = false, gather = false;
   bool have_aux = false;                  // the last forward wrote (depth, alpha) to a caller's aux buffer
   bool sh_gaussian = false;               // the last forward evaluated its SH colour once per Gaussian
   int feat_f = 0;                         // the last forward blended feat[n, feat_f] (0: no features)
+  int n_views = 0;                        // the last forward was batched over n_views views (0: a single-view forward)
   const float* feat = nullptr;
   int n = 0, d = 3, scale_act = 0;
   long long m = 0;
@@ -186,7 +190,9 @@ extern "C" int gs_ctx_create(gs_ctx** out) {
   GS_CUDA_TRY(cudaGetDevice(&c->device));
   cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&c->host_m), 64);
   if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->host_rays), 64);
+  if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->host_views), GS_MAX_VIEWS * sizeof(GsView));
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_m, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_views, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     delete c;
     return gs_set_error(e, "cudaMallocHost");
@@ -204,11 +210,13 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
-                    &c->grad_feat_inst};
+                    &c->grad_feat_inst, &c->views};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
+  if (c->host_views) cudaFreeHost(c->host_views);
   if (c->ev_m) cudaEventDestroy(c->ev_m);
+  if (c->ev_views) cudaEventDestroy(c->ev_views);
   if (c->ev_ok)
     for (cudaEvent_t e : c->ev) cudaEventDestroy(e);
   if (switched) cudaSetDevice(cur);
@@ -234,101 +242,34 @@ static int ceil_log2(unsigned v) {
   return b;
 }
 
-static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
-                               const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
-                               float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream,
-                               const gs_render_aux* ax = nullptr, const gs_render_feat* ft = nullptr) {
-  if (!c || !cam || n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad arguments");
-  if (d != 3 && gs_sh_basis_count(d) == 0)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
-  if (cam->width <= 0 || cam->height <= 0 || !(cam->focal_x > 0.f) || !(cam->focal_y > 0.f))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad camera");
-  if (!(cam->tile_thresh > 0.f && cam->tile_thresh < 1.f))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: tile_thresh must be in (0, 1)");
-  if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: null tensor pointer");
-  // per-Gaussian SH: the projection writes an RGB colour, and everything that serves the blend runs as for d == 3;
-  // only the projection kernels, the push bucket and the caller's tensors keep the parameter width d
-  const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
-  const int blend_d = sh_gaussian ? 3 : d;   // colour width of the blend
-  // 2-D filter in normalised image-plane units: the variance over the squared pixel pitch 1 / f^2, rounded once
-  const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
-  GsFilter2d filt{};
-  if (filt_on) {
-    filt.ex = (float)((double)c->filter2d_var / ((double)cam->focal_x * (double)cam->focal_x));
-    filt.ey = (float)((double)c->filter2d_var / ((double)cam->focal_y * (double)cam->focal_y));
-    filt.compensate = c->filter2d == GS_FILTER2D_ANTIALIAS;
+// The per-camera constants of a frame of padded size g.wp x g.hp, formed from host scalars in double then narrowed, like
+// the Python floats that the reference passes through pybind (splatter.py:279-282, :532-533).  The 2-D filter is in
+// normalised image-plane units: the variance over the squared pixel pitch 1 / f^2, rounded once (zero without one).
+static GsView view_constants(const gs_ctx* c, const gs_camera* cam, const GsFrameGeom& g) {
+  GsView v{};
+  if (c->filter2d != GS_FILTER2D_NONE) {
+    v.filt.ex = (float)((double)c->filter2d_var / ((double)cam->focal_x * (double)cam->focal_x));
+    v.filt.ey = (float)((double)c->filter2d_var / ((double)cam->focal_y * (double)cam->focal_y));
+    v.filt.compensate = c->filter2d == GS_FILTER2D_ANTIALIAS;
   }
-  GsAuxOut aux_out{};
-  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
-  if (use_aux) {
-    if (ax->aux_final && !final_img)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: aux_final needs image_final");
-    if (ax->background) {
-      for (int k = 0; k < 3; ++k) {
-        if (!std::isfinite(ax->background[k]))
-          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: background must be finite");
-        aux_out.bg[k] = ax->background[k];
-      }
-    }
-    aux_out.aux = ax->aux;
-    aux_out.aux_final = ax->aux_final;
-    // a forward that writes aux may be differentiated through it: its backward kernel must exist too
-    if (int rc = gs_blend_aux_supported(blend_d, true, ax->aux != nullptr)) return rc;
-  }
-  const bool gather = gs_tuning().gather != 0;   // RGB and SH: no pack pass
-  if (ft) {
-    if (!gs_feat_width_ok(ft->f)) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: f must be 8, 16 or 32");
-    if (!ft->map || (n > 0 && !ft->feat))
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat or map");
-    if ((reinterpret_cast<uintptr_t>(ft->feat) | reinterpret_cast<uintptr_t>(ft->map) |
-         reinterpret_cast<uintptr_t>(ft->map_final)) % 16)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: feat, map and map_final must be 16-byte aligned");
-    if (ft->map_final && !final_img)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: map_final needs image_final");
-    if (blend_d != 3)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: SH colour evaluated per pixel has no feature "
-                                                  "kernel (use GS_SH_EVAL_GAUSSIAN)");
-    if (!gather)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: the packed path (gs_tune(\"gather\", 0)) has "
-                                                  "no feature kernel");
-  }
-  if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
-  g_cur_alloc = &c->allocator;
-  cudaStream_t st = (cudaStream_t)stream;
-  c->have_forward = false;
-  c->have_backward = false;
-  c->have_aux = false;
+  v.grid.lx = (float)(16.0 / (double)cam->focal_x);
+  v.grid.ly = (float)(16.0 / (double)cam->focal_y);
+  v.grid.leftmost = (float)(-(double)g.wp / 2.0 / (double)cam->focal_x);
+  v.grid.topmost = (float)(-(double)g.hp / 2.0 / (double)cam->focal_y);
+  v.grid.t2 = -2.f * logf(cam->tile_thresh);
+  v.grid.ntx = g.wp / GS_TILE;
+  v.grid.nty = g.hp / GS_TILE;
+  memcpy(v.cam.r, cam->rot, sizeof(v.cam.r));
+  memcpy(v.cam.t, cam->tran, sizeof(v.cam.t));
+  v.half_w = (float)((double)cam->width * 1.2 / 2.0 / (double)cam->focal_x);
+  v.half_h = (float)((double)cam->height * 1.2 / 2.0 / (double)cam->focal_y);
+  v.fx = cam->focal_x;
+  v.fy = cam->focal_y;
+  return v;
+}
 
-  GsFrameGeom g{};
-  g.width = cam->width;
-  g.height = cam->height;
-  g.wp = (cam->width + GS_TILE - 1) / GS_TILE * GS_TILE;     // splatter.py:259-260
-  g.hp = (cam->height + GS_TILE - 1) / GS_TILE * GS_TILE;
-  g.ntx = g.wp / GS_TILE;
-  g.nty = g.hp / GS_TILE;
-  g.n_tiles = g.ntx * g.nty;
-  g.fx = cam->focal_x;
-  g.fy = cam->focal_y;
-  if (g.ntx > 65535 || g.nty > 65535) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: image too large");
-
-  // Host scalars are formed in double then narrowed, like the Python floats that the reference
-  // passes through pybind (splatter.py:279-282, :532-533).
-  GsTileGrid grid{};
-  grid.lx = (float)(16.0 / (double)cam->focal_x);
-  grid.ly = (float)(16.0 / (double)cam->focal_y);
-  grid.leftmost = (float)(-(double)g.wp / 2.0 / (double)cam->focal_x);
-  grid.topmost = (float)(-(double)g.hp / 2.0 / (double)cam->focal_y);
-  grid.t2 = -2.f * logf(cam->tile_thresh);
-  grid.ntx = g.ntx;
-  grid.nty = g.nty;
-  GsCam dc{};
-  memcpy(dc.r, cam->rot, sizeof(dc.r));
-  memcpy(dc.t, cam->tran, sizeof(dc.t));
-  float half_w = (float)((double)cam->width * 1.2 / 2.0 / (double)cam->focal_x);
-  float half_h = (float)((double)cam->height * 1.2 / 2.0 / (double)cam->focal_y);
-
-  size_t N = (size_t)n;
+// per-Gaussian (per-pair in a batched frame) and per-tile workspaces of a frame of N items
+static int reserve_frame(gs_ctx* c, size_t N, int n_tiles, cudaStream_t st) {
   GS_CUDA_TRY(c->rec.reserve(N * sizeof(GsRec), st));
   GS_CUDA_TRY(c->rect.reserve(N * sizeof(uint2), st));
   GS_CUDA_TRY(c->count.reserve((N + 1) * 4, st));
@@ -337,54 +278,23 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   GS_CUDA_TRY(c->dkey_out.reserve(N * 4 + 4, st));
   GS_CUDA_TRY(c->perm.reserve(N * 4 + 4, st));
   GS_CUDA_TRY(c->offsets_g.reserve((N + 1) * 4, st));
-  GS_CUDA_TRY(c->tile_accum.reserve((size_t)(g.n_tiles + 1) * 4, st));
-  GS_CUDA_TRY(c->tile_neff.reserve((size_t)g.n_tiles * 4, st));
-  GS_CUDA_TRY(c->tile_neff_b.reserve((size_t)g.n_tiles * 4, st));
+  GS_CUDA_TRY(c->tile_accum.reserve((size_t)(n_tiles + 1) * 4, st));
+  GS_CUDA_TRY(c->tile_neff.reserve((size_t)n_tiles * 4, st));
+  GS_CUDA_TRY(c->tile_neff_b.reserve((size_t)n_tiles * 4, st));
   GS_CUDA_TRY(c->counters.reserve(64, st));
   if (c->iota_n < N) {   // 0..N-1 values for the depth sort (kept across frames)
     GS_CUDA_TRY(c->iota.reserve(N * 4 + 4, st));
-    GS_CUDA_TRY(gs_launch_iota(c->iota.as<uint32_t>(), n, st));
+    GS_CUDA_TRY(gs_launch_iota(c->iota.as<uint32_t>(), (int)N, st));
     gs_count_launch();
     c->iota_n = N;
   }
+  return 0;
+}
 
-  if (blend_d != 3) {
-    // world-space ray set-up for per-pixel SH, reference splatter.py:305-321 (RayInfo):
-    // c2w = inverse(w2c); rays_o = -c2w t; lefttop = c2w (((-Wp/2+.5)/fx, (-Hp/2+.5)/fy, 1) - t)
-    GS_CUDA_TRY(c->rays.reserve(64, st));
-    double m3[9], inv[9];
-    for (int k = 0; k < 9; ++k) m3[k] = cam->rot[k];
-    double det3 = m3[0] * (m3[4] * m3[8] - m3[5] * m3[7]) - m3[1] * (m3[3] * m3[8] - m3[5] * m3[6]) +
-                  m3[2] * (m3[3] * m3[7] - m3[4] * m3[6]);
-    inv[0] = (m3[4] * m3[8] - m3[5] * m3[7]) / det3;
-    inv[1] = (m3[2] * m3[7] - m3[1] * m3[8]) / det3;
-    inv[2] = (m3[1] * m3[5] - m3[2] * m3[4]) / det3;
-    inv[3] = (m3[5] * m3[6] - m3[3] * m3[8]) / det3;
-    inv[4] = (m3[0] * m3[8] - m3[2] * m3[6]) / det3;
-    inv[5] = (m3[2] * m3[3] - m3[0] * m3[5]) / det3;
-    inv[6] = (m3[3] * m3[7] - m3[4] * m3[6]) / det3;
-    inv[7] = (m3[1] * m3[6] - m3[0] * m3[7]) / det3;
-    inv[8] = (m3[0] * m3[4] - m3[1] * m3[3]) / det3;
-    double lt[3] = {(-(double)g.wp / 2 + 0.5) / cam->focal_x - cam->tran[0],
-                    (-(double)g.hp / 2 + 0.5) / cam->focal_y - cam->tran[1], 1.0 - cam->tran[2]};
-    for (int k = 0; k < 3; ++k) {
-      c->host_rays[k] = (float)(-(inv[3 * k] * cam->tran[0] + inv[3 * k + 1] * cam->tran[1] + inv[3 * k + 2] * cam->tran[2]));
-      c->host_rays[3 + k] = (float)(inv[3 * k] * lt[0] + inv[3 * k + 1] * lt[1] + inv[3 * k + 2] * lt[2]);
-      c->host_rays[6 + k] = (float)(inv[3 * k] / cam->focal_x);
-      c->host_rays[9 + k] = (float)(inv[3 * k + 1] / cam->focal_y);
-    }
-    GS_CUDA_TRY(cudaMemcpyAsync(c->rays.p, c->host_rays, 48, cudaMemcpyHostToDevice, st));
-  }
-  // 1. projection + activations + tile rectangle
-  c->ev_fwd_valid = false;
-  gs_mark(c, 0, st);
-  GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
-  GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
-  GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
-                                      half_w, half_h, c->rec.as<GsRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
-                                      c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
-                                      sh_gaussian, filt_on ? &filt : nullptr));
-  if (n > 0) gs_count_launch();
+// stages 2-5 of a frame of n items (Gaussians, or (view, Gaussian) pairs): scans and the host read-back of M, the
+// depth sort, instance emission, the tile sort and the tile ranges (gather) or the pack pass
+static int bin_frame(gs_ctx* c, int n, const GsFrameGeom& g, bool gather, int blend_d, int d, const float* rgb,
+                     cudaStream_t st, long long& m_out) {
   // 2. (a) exclusive scan of the tile counts in Gaussian-id order -> gradient-row bases and M;
   //    (b) stable depth sort of the N Gaussians; (c) scan of the counts in depth order (the
   //    count gather is fused into the scan's input iterator) -> instance emission offsets
@@ -422,8 +332,9 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   // not wrap); instance indices are 32-bit from here on
   if (*c->host_m >= (1ull << 31))
     return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: more than 2^31 tile instances");
-  long long m = (long long)*c->host_m;
-  size_t M = (size_t)m;
+  const long long m = (long long)*c->host_m;
+  const size_t M = (size_t)m;
+  m_out = m;
 
   gs_mark(c, 2, st);
   // tile-id sort key width (GS_TILE_KEY_BYTES=4 forces the wide path, for tests)
@@ -485,6 +396,129 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
                                          c->pC.as<float>(), c->tile_accum.as<int>(), st));
   }
   if (m > 0) gs_count_launch();   // pack, or the tile-range pass of the gather path
+  return 0;
+}
+
+static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
+                               const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
+                               float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream,
+                               const gs_render_aux* ax = nullptr, const gs_render_feat* ft = nullptr) {
+  if (!c || !cam || n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad arguments");
+  if (d != 3 && gs_sh_basis_count(d) == 0)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
+  if (cam->width <= 0 || cam->height <= 0 || !(cam->focal_x > 0.f) || !(cam->focal_y > 0.f))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad camera");
+  if (!(cam->tile_thresh > 0.f && cam->tile_thresh < 1.f))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: tile_thresh must be in (0, 1)");
+  if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: null tensor pointer");
+  // per-Gaussian SH: the projection writes an RGB colour, and everything that serves the blend runs as for d == 3;
+  // only the projection kernels, the push bucket and the caller's tensors keep the parameter width d
+  const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
+  const int blend_d = sh_gaussian ? 3 : d;   // colour width of the blend
+  const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
+  GsAuxOut aux_out{};
+  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
+  if (use_aux) {
+    if (ax->aux_final && !final_img)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: aux_final needs image_final");
+    if (ax->background) {
+      for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(ax->background[k]))
+          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: background must be finite");
+        aux_out.bg[k] = ax->background[k];
+      }
+    }
+    aux_out.aux = ax->aux;
+    aux_out.aux_final = ax->aux_final;
+    // a forward that writes aux may be differentiated through it: its backward kernel must exist too
+    if (int rc = gs_blend_aux_supported(blend_d, true, ax->aux != nullptr)) return rc;
+  }
+  const bool gather = gs_tuning().gather != 0;   // RGB and SH: no pack pass
+  if (ft) {
+    if (!gs_feat_width_ok(ft->f)) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: f must be 8, 16 or 32");
+    if (!ft->map || (n > 0 && !ft->feat))
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat or map");
+    if ((reinterpret_cast<uintptr_t>(ft->feat) | reinterpret_cast<uintptr_t>(ft->map) |
+         reinterpret_cast<uintptr_t>(ft->map_final)) % 16)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: feat, map and map_final must be 16-byte aligned");
+    if (ft->map_final && !final_img)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: map_final needs image_final");
+    if (blend_d != 3)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: SH colour evaluated per pixel has no feature "
+                                                  "kernel (use GS_SH_EVAL_GAUSSIAN)");
+    if (!gather)
+      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: the packed path (gs_tune(\"gather\", 0)) has "
+                                                  "no feature kernel");
+  }
+  if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  c->have_forward = false;
+  c->have_backward = false;
+  c->have_aux = false;
+  c->n_views = 0;
+
+  GsFrameGeom g{};
+  g.width = cam->width;
+  g.height = cam->height;
+  g.wp = (cam->width + GS_TILE - 1) / GS_TILE * GS_TILE;     // splatter.py:259-260
+  g.hp = (cam->height + GS_TILE - 1) / GS_TILE * GS_TILE;
+  g.ntx = g.wp / GS_TILE;
+  g.nty = g.hp / GS_TILE;
+  g.n_tiles = g.ntx * g.nty;
+  g.fx = cam->focal_x;
+  g.fy = cam->focal_y;
+  if (g.ntx > 65535 || g.nty > 65535) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: image too large");
+
+  const GsView vw = view_constants(c, cam, g);
+  const GsTileGrid& grid = vw.grid;
+  const GsCam& dc = vw.cam;
+  const GsFilter2d& filt = vw.filt;
+  const float half_w = vw.half_w, half_h = vw.half_h;
+
+  size_t N = (size_t)n;
+  if (int rc = reserve_frame(c, N, g.n_tiles, st)) return rc;
+
+  if (blend_d != 3) {
+    // world-space ray set-up for per-pixel SH, reference splatter.py:305-321 (RayInfo):
+    // c2w = inverse(w2c); rays_o = -c2w t; lefttop = c2w (((-Wp/2+.5)/fx, (-Hp/2+.5)/fy, 1) - t)
+    GS_CUDA_TRY(c->rays.reserve(64, st));
+    double m3[9], inv[9];
+    for (int k = 0; k < 9; ++k) m3[k] = cam->rot[k];
+    double det3 = m3[0] * (m3[4] * m3[8] - m3[5] * m3[7]) - m3[1] * (m3[3] * m3[8] - m3[5] * m3[6]) +
+                  m3[2] * (m3[3] * m3[7] - m3[4] * m3[6]);
+    inv[0] = (m3[4] * m3[8] - m3[5] * m3[7]) / det3;
+    inv[1] = (m3[2] * m3[7] - m3[1] * m3[8]) / det3;
+    inv[2] = (m3[1] * m3[5] - m3[2] * m3[4]) / det3;
+    inv[3] = (m3[5] * m3[6] - m3[3] * m3[8]) / det3;
+    inv[4] = (m3[0] * m3[8] - m3[2] * m3[6]) / det3;
+    inv[5] = (m3[2] * m3[3] - m3[0] * m3[5]) / det3;
+    inv[6] = (m3[3] * m3[7] - m3[4] * m3[6]) / det3;
+    inv[7] = (m3[1] * m3[6] - m3[0] * m3[7]) / det3;
+    inv[8] = (m3[0] * m3[4] - m3[1] * m3[3]) / det3;
+    double lt[3] = {(-(double)g.wp / 2 + 0.5) / cam->focal_x - cam->tran[0],
+                    (-(double)g.hp / 2 + 0.5) / cam->focal_y - cam->tran[1], 1.0 - cam->tran[2]};
+    for (int k = 0; k < 3; ++k) {
+      c->host_rays[k] = (float)(-(inv[3 * k] * cam->tran[0] + inv[3 * k + 1] * cam->tran[1] + inv[3 * k + 2] * cam->tran[2]));
+      c->host_rays[3 + k] = (float)(inv[3 * k] * lt[0] + inv[3 * k + 1] * lt[1] + inv[3 * k + 2] * lt[2]);
+      c->host_rays[6 + k] = (float)(inv[3 * k] / cam->focal_x);
+      c->host_rays[9 + k] = (float)(inv[3 * k + 1] / cam->focal_y);
+    }
+    GS_CUDA_TRY(cudaMemcpyAsync(c->rays.p, c->host_rays, 48, cudaMemcpyHostToDevice, st));
+  }
+  // 1. projection + activations + tile rectangle
+  c->ev_fwd_valid = false;
+  gs_mark(c, 0, st);
+  GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
+  GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
+  GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
+                                      half_w, half_h, c->rec.as<GsRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
+                                      c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
+                                      sh_gaussian, filt_on ? &filt : nullptr));
+  if (n > 0) gs_count_launch();
+  long long m = 0;
+  if (int rc = bin_frame(c, n, g, gather, blend_d, d, rgb, st, m)) return rc;
   // 6. blend (+ optional fused clamp & centre crop, splatter.py:652-653 / :267-272)
   GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
   gs_mark(c, 5, st);
@@ -547,6 +581,19 @@ extern "C" int gs_render_forward_final(gs_ctx* c, const float* pos, const float*
                              culling_mask, stream);
 }
 
+// one u32 tag per gradient row: rows written by this backward carry `epoch`; the tails of
+// saturated tiles are never written nor read (saves ~0.2 GB of HBM writes + reads at C3)
+static int next_row_epoch(gs_ctx* c, size_t M, cudaStream_t st) {
+  const size_t before = c->row_epoch.cap;            // (a caching allocator may hand the same address back)
+  GS_CUDA_TRY(c->row_epoch.reserve(M * 4 + 16, st));
+  if (c->row_epoch.cap != before || c->epoch == 0xffffffffu) {
+    GS_CUDA_TRY(cudaMemsetAsync(c->row_epoch.p, 0, c->row_epoch.cap, st));
+    c->epoch = 0;
+  }
+  ++c->epoch;
+  return 0;
+}
+
 static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
                                 const float* scale, const float* image, const float* grad_image, int grad_is_final,
                                 float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
@@ -556,6 +603,8 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                 float* grad_feat = nullptr) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward: no forward on this ctx");
+  if (c->n_views)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: the last forward was batched (use gs_render_backward_batch)");
   // camera only (grad_cam, the five parameter gradients all NULL: the caller has checked the set is not mixed)
   const bool cam_only = grad_cam && !grad_pos;
   if (!image || !grad_image || (!cam_only && (!grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale)) ||
@@ -592,17 +641,7 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   const size_t grow = blend_d == 3 ? (size_t)GS_GREC * 4 : (size_t)gs_sh_grad_width(d) * 4;
   GS_CUDA_TRY(c->grad_inst.reserve(M * grow + 16, st));
   if (grad_map) GS_CUDA_TRY(c->grad_feat_inst.reserve(M * (size_t)c->feat_f * 4 + 16, st));
-  {
-    // one u32 tag per gradient row: rows written by this backward carry `epoch`; the tails of
-    // saturated tiles are never written nor read (saves ~0.2 GB of HBM writes + reads at C3)
-    const size_t before = c->row_epoch.cap;            // (a caching allocator may hand the same address back)
-    GS_CUDA_TRY(c->row_epoch.reserve(M * 4 + 16, st));
-    if (c->row_epoch.cap != before || c->epoch == 0xffffffffu) {
-      GS_CUDA_TRY(cudaMemsetAsync(c->row_epoch.p, 0, c->row_epoch.cap, st));
-      c->epoch = 0;
-    }
-    ++c->epoch;
-  }
+  if (int rc = next_row_epoch(c, M, st)) return rc;
   c->ev_bwd_valid = false;
   GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
   gs_mark(c, 7, st);
@@ -749,6 +788,9 @@ extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float*
                                        float* grad_quat, float* grad_scale, float* grad_feat, gs_stream_t stream) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward_feat: no forward on this ctx");
+  if (c->n_views)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG,
+                            "gs_render_backward_feat: the last forward was batched (use gs_render_backward_batch)");
   if (!c->feat_f)
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: the forward blended no features");
   if (feat != c->feat)
@@ -771,6 +813,210 @@ extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float*
                                 map, grad_map, grad_feat);
   if (rc || grad_map || n == 0) return rc;
   GS_CUDA_TRY(cudaMemsetAsync(grad_feat, 0, (size_t)n * f * sizeof(float), (cudaStream_t)stream));
+  return 0;
+}
+
+// ---- batched frames ---------------------------------------------------------------------
+extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                       const float* quat, const float* scale, int n, int d, int scale_activation,
+                                       int n_views, const gs_camera* cams, float* image, float* final_img,
+                                       int64_t* culling_mask, const gs_render_aux* ax, gs_stream_t stream) {
+  if (!c || !cams) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: null ctx or cams");
+  if (n_views < 1 || n_views > GS_MAX_VIEWS)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: n_views must be in 1 .. GS_MAX_VIEWS");
+  if (n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: n < 0");
+  if (d != 3 && gs_sh_basis_count(d) == 0)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
+  const gs_camera& c0 = cams[0];
+  for (int v = 0; v < n_views; ++v) {
+    const gs_camera& cv = cams[v];
+    if (cv.width <= 0 || cv.height <= 0 || !(cv.focal_x > 0.f) || !(cv.focal_y > 0.f))
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: bad camera");
+    if (!(cv.tile_thresh > 0.f && cv.tile_thresh < 1.f))
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: tile_thresh must be in (0, 1)");
+    if (cv.width != c0.width || cv.height != c0.height || !(cv.near_plane == c0.near_plane) ||
+        !(cv.tile_thresh == c0.tile_thresh))
+      return gs_set_error_msg(GS_ERR_INVALID_ARG,
+                              "gs_render_forward_batch: the views must share width, height, near_plane and tile_thresh");
+  }
+  // one view's padded size; the frame's tile grid stacks the views' grids vertically
+  GsFrameGeom g{};
+  g.width = c0.width;
+  g.height = c0.height;
+  g.wp = (c0.width + GS_TILE - 1) / GS_TILE * GS_TILE;
+  g.hp = (c0.height + GS_TILE - 1) / GS_TILE * GS_TILE;
+  g.ntx = g.wp / GS_TILE;
+  const int nty = g.hp / GS_TILE;
+  if (g.ntx > 65535 || (long long)nty * n_views > 65535)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: image too large for the batch (B Hp / 16 > 65535)");
+  if ((long long)n * n_views >= (1ll << 31))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: B n must be < 2^31");
+  g.nty = nty * n_views;
+  g.n_tiles = g.ntx * g.nty;
+  g.fx = c0.focal_x;
+  g.fy = c0.focal_y;
+  if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: null tensor pointer");
+  const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
+  if (d != 3 && !sh_gaussian)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: SH colour evaluated per pixel has no batched "
+                                                "kernel (use GS_SH_EVAL_GAUSSIAN)");
+  if (int rc = gs_blend_batch_supported()) return rc;
+  if (c->push.world)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: not available with a gradient push configured");
+  GsAuxOut aux_out{};
+  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
+  if (use_aux) {
+    if (ax->aux_final && !final_img)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: aux_final needs image_final");
+    if (ax->background) {
+      for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(ax->background[k]))
+          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: background must be finite");
+        aux_out.bg[k] = ax->background[k];
+      }
+    }
+    aux_out.aux = ax->aux;
+    aux_out.aux_final = ax->aux_final;
+  }
+  if (int rc = gs_check_device(c->device, "gs_render_forward_batch")) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  c->have_forward = false;
+  c->have_backward = false;
+  c->have_aux = false;
+  c->n_views = 0;
+
+  const int nb = n * n_views;   // (view, Gaussian) pairs
+  if (int rc = reserve_frame(c, (size_t)nb, g.n_tiles, st)) return rc;
+  GS_CUDA_TRY(c->views.reserve(sizeof(GsView) * GS_MAX_VIEWS, st));
+  // the previous upload from the pinned staging may still be pending when its forward returned early on an error
+  GS_CUDA_TRY(cudaEventSynchronize(c->ev_views));
+  for (int v = 0; v < n_views; ++v) c->host_views[v] = view_constants(c, &cams[v], g);
+  GS_CUDA_TRY(cudaMemcpyAsync(c->views.p, c->host_views, sizeof(GsView) * n_views, cudaMemcpyHostToDevice, st));
+  GS_CUDA_TRY(cudaEventRecord(c->ev_views, st));
+  const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
+
+  c->ev_fwd_valid = false;
+  gs_mark(c, 0, st);
+  GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
+  GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + nb, 0, 4, st));
+  GS_CUDA_TRY(gs_launch_fused_project_batch(pos, rgb, opa, quat, scale, n, n_views, d, scale_activation,
+                                            c->views.as<GsView>(), c0.near_plane, c->rec.as<GsRec>(),
+                                            c->rect.as<uint2>(), c->count.as<uint32_t>(), c->dkey_in.as<uint32_t>(),
+                                            culling_mask, c->counters.as<unsigned int>(), st, sh_gaussian, filt_on));
+  if (n > 0) gs_count_launch();
+  long long m = 0;
+  if (int rc = bin_frame(c, nb, g, true, 3, d, rgb, st, m)) return rc;
+  GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
+  gs_mark(c, 5, st);
+  GS_CUDA_TRY(gs_launch_blend_fwd_batch(c->rec.as<GsRec>(), c->vals_out.as<uint32_t>(), c->tile_accum.as<int>(), g,
+                                        c->views.as<GsView>(), image, c->tile_neff.as<int>(), final_img, crop, st,
+                                        use_aux ? &aux_out : nullptr));
+  gs_count_launch();   // blend forward
+  gs_mark(c, 6, st);
+  c->ev_fwd_valid = c->timing && c->ev_ok;
+
+  c->have_forward = true;
+  c->have_aux = aux_out.aux != nullptr;
+  c->sh_gaussian = sh_gaussian;
+  c->feat_f = 0;
+  c->feat = nullptr;
+  c->filt_on = filt_on;
+  c->gather = true;
+  // view 0's constants: a one-view batch is differentiated by the single-view projection backward
+  c->cam = c->host_views[0].cam;
+  c->grid = c->host_views[0].grid;
+  c->filt = c->host_views[0].filt;
+  c->half_w = c->host_views[0].half_w;
+  c->half_h = c->host_views[0].half_h;
+  c->n = n;
+  c->d = d;
+  c->scale_act = scale_activation;
+  c->m = m;
+  c->geom = g;
+  c->near_plane = c0.near_plane;
+  c->n_views = n_views;
+  return 0;
+}
+
+extern "C" int gs_render_backward_batch(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                        const float* quat, const float* scale, const float* image,
+                                        const float* grad_image, int grad_is_final, const float* aux,
+                                        const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                        float* grad_quat, float* grad_scale, gs_stream_t stream) {
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: null ctx");
+  if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward_batch: no forward on this ctx");
+  if (!c->n_views)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: the last forward was not batched");
+  if (!image || !grad_image || !grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale ||
+      (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: null tensor pointer");
+  if (grad_aux) {
+    if (!c->have_aux)
+      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: grad_aux given but the forward wrote no aux");
+    if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: grad_aux needs the forward's aux");
+  }
+  if (c->push.world)
+    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_batch: not available with a gradient push configured");
+  if (int rc = gs_blend_batch_supported()) return rc;
+  const bool stats = c->stats_on;
+  if (stats && c->stats.n != c->n)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: the densify statistics are sized for another n");
+  if (int rc = gs_check_device(c->device, "gs_render_backward_batch")) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t M = (size_t)c->m;
+  GS_CUDA_TRY(c->grad_inst.reserve(M * GS_GREC * 4 + 16, st));
+  if (int rc = next_row_epoch(c, M, st)) return rc;
+  c->ev_bwd_valid = false;
+  const GsFrameGeom& g = c->geom;
+  const GsView* views = c->views.as<GsView>();
+  GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
+  gs_mark(c, 7, st);
+  if (c->m > 0) {
+    GS_CUDA_TRY(gs_launch_blend_bwd_batch(c->rec.as<GsRec>(), c->vals_out.as<uint32_t>(), c->offsets_g.as<uint32_t>(),
+                                          c->tile_accum.as<int>(), g, views, image, grad_image,
+                                          c->grad_inst.as<float>(), grad_is_final ? 1 : 0, crop,
+                                          c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), st, aux,
+                                          grad_aux, stats && c->stats.absgrad));
+    gs_count_launch();
+    c->have_backward = true;
+  }
+  gs_mark(c, 8, st);
+  // One view: the pairs are the Gaussians and the frame is a single-view frame from here on, so the single-view
+  // projection backward and statistics kernels run (the gradients are theirs bit for bit, and they are the faster
+  // kernels for one view); B views: the batched kernels, which take each Gaussian's views in order.
+  const bool one = c->n_views == 1;
+  if (one)
+    GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, c->d, c->scale_act, c->cam, c->near_plane,
+                                            c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                            c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch, grad_pos,
+                                            grad_rgb, grad_opa, grad_quat, grad_scale, GsGradPush{}, st,
+                                            grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
+  else
+    GS_CUDA_TRY(gs_launch_fused_project_bwd_batch(pos, rgb, opa, quat, scale, c->n, c->n_views, c->d, c->scale_act,
+                                                  views, c->near_plane, c->offsets_g.as<uint32_t>(),
+                                                  c->count.as<uint32_t>(), c->grad_inst.as<float>(),
+                                                  c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
+                                                  grad_quat, grad_scale, st, grad_aux != nullptr, c->sh_gaussian,
+                                                  c->filt_on));
+  if (c->n > 0) gs_count_launch();
+  if (stats) {
+    if (one)
+      GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
+                                          c->half_h, c->filt, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                          c->grad_inst.as<float>(), GS_GREC, c->row_epoch.as<uint32_t>(), c->epoch, g,
+                                          c->stats, st));
+    else
+      GS_CUDA_TRY(gs_launch_densify_stats_batch(pos, quat, scale, c->n, c->n_views, c->scale_act, views,
+                                                c->near_plane, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                                c->grad_inst.as<float>(), GS_GREC, c->row_epoch.as<uint32_t>(),
+                                                c->epoch, g, c->stats, st));
+    if (c->n > 0) gs_count_launch();
+  }
+  gs_mark(c, 9, st);
+  c->ev_bwd_valid = c->timing && c->ev_ok;
   return 0;
 }
 

@@ -313,6 +313,77 @@ def render_frame_aux(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, f
                                  near, tile_thresh, scale_activation, background, final)
 
 
+MAX_VIEWS = 64
+
+
+class _RenderFrameBatch(torch.autograd.Function):
+    """`_RenderFrameAux` over a batch of B views rendered as one frame (gs_render_forward_batch); the backward returns
+    the sums over the views of the five parameter gradients."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal, rot, tran, near, tile_thresh,
+                scale_activation, background, final):
+        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
+        bg = None if background is None else [float(v) for v in background]
+        fin, raw, aux, aux_fin, mask = rctx.forward_batch(
+            pos, rgb, opa, quat, scale, int(width), int(height), focal, rot, tran, float(near), float(tile_thresh),
+            SCALE_ACTIVATIONS[scale_activation], bg, bool(final))
+        ctx.rctx = rctx
+        ctx.frame = rctx.frame_id()
+        ctx.final = bool(final)
+        ctx.save_for_backward(pos, rgb, opa, quat, scale, raw, aux)
+        ctx.mark_non_differentiable(mask)
+        ctx.set_materialize_grads(False)
+        image, maps = (fin, aux_fin) if final else (raw, aux)
+        ctx.map_shape = tuple(maps.shape[:3])
+        return image, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
+        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
+        shape = ctx.map_shape
+        if grad_image is None:
+            grad_image = raw.new_zeros(*shape, 3)
+        grad_aux = None
+        if grad_depth is not None or grad_alpha is not None:
+            grad_aux = raw.new_zeros(*shape, 2)
+            if grad_depth is not None:
+                grad_aux[..., 0] = grad_depth
+            if grad_alpha is not None:
+                grad_aux[..., 1] = grad_alpha
+        outs, _ = _flat_grads((pos, rgb, opa, quat, scale))
+        ctx.rctx.backward_batch_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
+                                     *outs, ctx.frame)
+        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 10
+
+
+def render_frame_batch(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
+                       tile_thresh, scale_activation, background=None, final=True):
+    """B camera views of one scene rendered as one frame: -> (image, depth, alpha, culling_mask) with image
+    [B,H,W,3] (final=True, each view clamped and cropped as in `render_frame_aux`) or [B,Hp,Wp,3], depth / alpha
+    [B,H,W] or [B,Hp,Wp], culling_mask [B,n].  Per view the outputs are those of `render_frame_aux` with that view's
+    camera; the views share width, height, near, tile_thresh and the background.  focal_x / focal_y: B numbers;
+    rot [B,3,3], tran [B,3] (any device: they are read on the host).  Differentiable in the five parameters: their
+    gradients are the SUMS over the views (divide the loss by B for a mean).  RGB and per-Gaussian SH colour, any 2-D
+    filter, densification statistics; per-pixel SH, the packed path, non-default blend knobs and a data-parallel
+    gradient push raise RuntimeError.  A graph that never uses depth or alpha runs the plain backward kernels."""
+    rot = torch.as_tensor(rot).detach()
+    tran = torch.as_tensor(tran).detach()
+    if rot.dim() != 3 or tuple(rot.shape[1:]) != (3, 3):
+        raise ValueError(f"render_frame_batch: rot must be [B,3,3], got {list(rot.shape)}")
+    b = rot.shape[0]
+    if not 1 <= b <= MAX_VIEWS:
+        raise ValueError(f"render_frame_batch: the batch must have 1 .. {MAX_VIEWS} views, got {b}")
+    if tuple(tran.shape) != (b, 3):
+        raise ValueError(f"render_frame_batch: tran must be [{b},3], got {list(tran.shape)}")
+    fx, fy = (torch.as_tensor(f, dtype=torch.float64).detach().reshape(-1).cpu() for f in (focal_x, focal_y))
+    if fx.numel() != b or fy.numel() != b:
+        raise ValueError(f"render_frame_batch: focal_x and focal_y must have {b} values each")
+    return _RenderFrameBatch.apply(rctx, pos, rgb, opa, quat, scale, width, height, torch.stack([fx, fy], 1),
+                                   rot.float().cpu(),
+                                   tran.float().cpu(), near, tile_thresh, scale_activation, background, final)
+
+
 class _RenderFrameCam(_RenderFrameAux):
     """`_RenderFrameAux` whose backward also returns dL/drot and dL/dtran (gs_render_backward_cam)."""
 

@@ -27,8 +27,8 @@ import torch
 import torch.nn as nn
 
 import gaussian
-from renderer import (FEATURE_WIDTHS, FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_cam,
-                      render_frame_feat, render_frame_final)
+from renderer import (FEATURE_WIDTHS, FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_batch,
+                      render_frame_cam, render_frame_feat, render_frame_final)
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -438,6 +438,34 @@ class Splatter(nn.Module):
         self.n_gaussians = g.pos.shape[0]
         self.n_tile_gaussians = self._rctx.last_instances()
         return dict(image=image, depth=depth, alpha=alpha)
+
+    def render_batch(self, camera_ids, background=None):
+        """The views `camera_ids` rendered as one frame (`renderer.render_frame_batch`): dict(image [B,H,W,3],
+        depth [B,H,W], alpha [B,H,W], culling_mask [B,n]), plus `ground_truth` [B,H,W,3] (float16) when the Splatter
+        holds images.  Each view is what `render_maps` returns for it; the gradients are SUMS over the views (divide
+        the loss by B for a mean).  Sets `culling_mask` to the [n] sum over the views and `n_tile_gaussians` to the
+        batch's instance count.  The views must share their size (ValueError otherwise)."""
+        ids = list(camera_ids)
+        if not ids:
+            raise ValueError("render_batch: no camera ids")
+        vs = [self.views[i] for i in ids]
+        if any(v["width"] != vs[0]["width"] or v["height"] != vs[0]["height"] for v in vs):
+            raise ValueError("render_batch: the views of a batch must have the same width and height")
+        g = self.gaussian_3ds
+        self._size_densify_stats()
+        image, depth, alpha, mask = render_frame_batch(
+            self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, vs[0]["width"], vs[0]["height"],
+            [v["focal_x"] for v in vs], [v["focal_y"] for v in vs], torch.stack([v["rot"] for v in vs]),
+            torch.stack([v["tran"] for v in vs]), self.near, self.tile_culling_prob_thresh, self.scale_activation,
+            background=background, final=True)
+        self.culling_mask = mask.sum(0)
+        self.n_gaussians = g.pos.shape[0]
+        self.n_tile_gaussians = self._rctx.last_instances()
+        out = dict(image=image, depth=depth, alpha=alpha, culling_mask=mask)
+        imgs = getattr(self, "imgs", [])
+        if all(i < len(imgs) for i in ids):
+            out["ground_truth"] = torch.stack([imgs[i] for i in ids]).to(torch.float16) / 255.
+        return out
 
     def render_features(self, camera_id=None, extrinsics=None, intrinsics=None, background=None):
         """`render_maps` plus the feature map: dict(image, features [H,W,F], depth, alpha).  features_k = sum_i w_i

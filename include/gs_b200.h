@@ -282,6 +282,34 @@ int gs_render_backward_feat(gs_ctx* ctx, const float* pos, const float* rgb, con
                             float* grad_opa, float* grad_quat, float* grad_scale, float* grad_feat,
                             gs_stream_t stream);
 
+/* A batch of B camera views rendered as one frame.  Per view, the semantics are exactly gs_render_forward_aux /
+ * gs_render_backward_aux with cams_host[v]; the background is shared by all views, and the parameter gradients are the
+ * SUM over the views (divide the loss by B for a mean).  The frame works on the B n (view, Gaussian) pairs j = v n + i
+ * and draws the views stacked vertically: image_raw_padded [B,Hp,Wp,3] (and aux [B,Hp,Wp,2]) is byte for byte the
+ * [B Hp, Wp, .] tall image; image_final [B,height,width,3] and aux_final [B,height,width,2] crop each view on its own;
+ * culling_mask is [B,n].  One host synchronisation and the launch count of one gs_render_forward_aux +
+ * gs_render_backward_aux frame, whatever B.  The context settings sh_eval, filter2d, densification statistics (added
+ * view by view in view order) and timing apply; gs_frame_stats / gs_frame_instances / gs_frame_sorted /
+ * gs_frame_tile_consumed / gs_frame_stage_ms report the batch (totals, B T tiles, pair indices j; width_padded /
+ * height_padded are one view's).  With n_views == 1 the gradients are gs_render_backward_aux's bit for bit.
+ * Refused before any launch:
+ *   GS_ERR_INVALID_ARG: a null ctx or cams; n_views outside 1 .. GS_MAX_VIEWS; views that differ in width, height,
+ *     near_plane or tile_thresh; B n >= 2^31 or B Hp / 16 > 65535; a bad camera or pointer as in gs_render_forward_aux;
+ *     more than 2^31 instances (as in gs_render_forward); gs_render_backward_batch after a single-view forward, and
+ *     every single-view backward entry after gs_render_forward_batch.
+ *   GS_ERR_UNSUPPORTED: SH colour evaluated per pixel; the packed path (gs_tune("gather", 0)); RGB blend knobs other
+ *     than the shipped ones (live-pixel repack on); a gradient push configured (gs_ctx_set_grad_push). */
+#define GS_MAX_VIEWS 64
+int gs_render_forward_batch(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                            const float* scale, int n, int d, int scale_activation, int n_views,
+                            const gs_camera* cams_host /* [n_views] */, float* image_raw_padded /* [B,Hp,Wp,3] */,
+                            float* image_final /* [B,H,W,3] | NULL */, int64_t* culling_mask /* [B,n] | NULL */,
+                            const gs_render_aux* aux /* nullable */, gs_stream_t stream);
+int gs_render_backward_batch(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                             const float* scale, const float* image_raw_padded, const float* grad_image,
+                             int grad_is_final, const float* aux, const float* grad_aux, float* grad_pos,
+                             float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale, gs_stream_t stream);
+
 /* Where the SH colour (d == 27 / 48) is evaluated.  Two colour MODELS, not two speeds of one: the same coefficients
  * render differently.
  *   GS_SH_EVAL_PIXEL    (default; the reference): the basis is evaluated per pixel, along the pixel's world-space ray,

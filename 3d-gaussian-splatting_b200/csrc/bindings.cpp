@@ -746,6 +746,17 @@ struct RenderContext {
 
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
+  // mask[n] (uint8) = the Gaussians the last forward binned (gs_frame_visible); accumulate: OR into mask
+  void visible_into(torch::Tensor mask, bool accumulate) {
+    TORCH_CHECK(mask.is_cuda() && mask.is_contiguous() && mask.scalar_type() == at::kByte && mask.dim() == 1,
+                "RenderContext.visible_into: mask must be a contiguous 1-D CUDA uint8 tensor");
+    TORCH_CHECK(mask.device().index() == device, "RenderContext.visible_into: mask is on another device than the context");
+    TORCH_CHECK(mask.numel() < (int64_t(1) << 31), "RenderContext.visible_into: mask too large");
+    c10::cuda::CUDAGuard guard(mask.device());
+    check_rc(gs_frame_visible(ctx, mask.data_ptr<uint8_t>(), (int)mask.numel(), accumulate ? 1 : 0, cur_stream()),
+             "gs_frame_visible");
+  }
+
   py::dict stats() {
     gs_frame_info fi{};
     check_rc(gs_frame_stats(ctx, &fi, cur_stream()), "gs_frame_stats");
@@ -801,6 +812,35 @@ void adam_step(torch::Tensor param, torch::Tensor grad, torch::Tensor exp_avg, t
   check_rc(gs_adam_step(fpm(param), fp(grad), fpm(exp_avg), fpm(exp_avg_sq), n, ends.data(), lr.data(), (int)ends.size(),
                         (float)beta1, (float)beta2, (float)eps, (int)step, cur_stream()),
            "gs_adam_step");
+}
+
+// Adam on the rows of the visible Gaussians only (gs_adam_step_visible); segment s is [visible.numel(), seg_widths[s]]
+// at float seg_starts[s] of the flat buffers
+void adam_step_visible(torch::Tensor param, torch::Tensor grad, torch::Tensor exp_avg, torch::Tensor exp_avg_sq,
+                       std::vector<int64_t> seg_starts, std::vector<int64_t> seg_widths, std::vector<double> lrs,
+                       torch::Tensor visible, double beta1, double beta2, double eps, int64_t step) {
+  GS_CHECK_F32(param); GS_CHECK_F32(grad); GS_CHECK_F32(exp_avg); GS_CHECK_F32(exp_avg_sq);
+  int64_t n = param.numel();
+  TORCH_CHECK(grad.numel() == n && exp_avg.numel() == n && exp_avg_sq.numel() == n, "adam_step_visible: size mismatch");
+  TORCH_CHECK(seg_starts.size() == lrs.size() && seg_widths.size() == lrs.size() && !lrs.empty(),
+              "adam_step_visible: one start, width and learning rate per segment");
+  TORCH_CHECK(visible.is_cuda() && visible.is_contiguous() && visible.scalar_type() == at::kByte &&
+                  visible.device() == param.device() && visible.numel() < (int64_t(1) << 31),
+              "adam_step_visible: visible must be a contiguous CUDA uint8 tensor on the parameters' device");
+  for (auto* t : {&param, &grad, &exp_avg, &exp_avg_sq})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "adam_step_visible: buffers must be 16-byte aligned");
+  std::vector<long long> starts(seg_starts.begin(), seg_starts.end());
+  std::vector<int> widths;
+  for (int64_t w : seg_widths) {
+    TORCH_CHECK(w >= 1 && w < (int64_t(1) << 31), "adam_step_visible: bad segment width");
+    widths.push_back((int)w);
+  }
+  std::vector<float> lr(lrs.begin(), lrs.end());
+  c10::cuda::CUDAGuard guard(param.device());
+  check_rc(gs_adam_step_visible(fpm(param), fp(grad), fpm(exp_avg), fpm(exp_avg_sq), n, starts.data(), widths.data(),
+                                lr.data(), (int)lr.size(), (int)visible.numel(), visible.data_ptr<uint8_t>(),
+                                (float)beta1, (float)beta2, (float)eps, (int)step, cur_stream()),
+           "gs_adam_step_visible");
 }
 
 // fused L1 + SSIM loss (SURVEY.md §8 f-3, reference train.py:99-107): returns (out3 = {total, l1, ssim}, grad_image)
@@ -1035,6 +1075,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("g_feat"), py::arg("expected_frame") = -1)
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
+      .def("visible_into", &RenderContext::visible_into, py::arg("mask"), py::arg("accumulate") = false)
       .def("stats", &RenderContext::stats)
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
@@ -1065,6 +1106,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("use_clone"), py::arg("use_split"), py::arg("generator") = py::none(), py::arg("feat") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
+  m.def("adam_step_visible", &adam_step_visible,
+        "Adam over the rows of the visible Gaussians of flat parameter / gradient buffers (CUDA)");
   m.def("tune", [](const std::string& name, int value) { check_rc(gs_tune(name.c_str(), value), "gs_tune"); },
         "set an A/B tuning knob of the blend kernels (see include/gs_b200.h gs_tune)");
   m.def("kernel_launches", []() { return (int64_t)gs_kernel_launches(); },

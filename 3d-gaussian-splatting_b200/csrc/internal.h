@@ -211,6 +211,12 @@ cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, c
                                           int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
                                           const gs_densify_stats& s, cudaStream_t st);
 
+// ---- optim.cu --------------------------------------------------------------------------
+// visible[n] (uint8) = count[v n + i] > 0 in any of the n_views views, OR-ed into visible when accumulate is set
+// (gs_frame_visible).  One launch when n > 0.
+cudaError_t gs_launch_frame_visible(const uint32_t* count, int n, int n_views, int accumulate, unsigned char* visible,
+                                    cudaStream_t st);
+
 // ---- blend_feat.cu ---------------------------------------------------------------------
 // Feature maps (gs_render_forward_feat / gs_render_backward_feat), gather path only.  f: 8, 16 or 32.
 bool gs_feat_width_ok(int f);

@@ -1153,6 +1153,17 @@ extern "C" int gs_frame_tile_consumed(gs_ctx* c, int* tile_consumed, gs_stream_t
   return 0;
 }
 
+extern "C" int gs_frame_visible(gs_ctx* c, unsigned char* visible, int n, int accumulate, gs_stream_t stream) {
+  if (!c || !visible) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_frame_visible: null argument");
+  if (!c->have_forward) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_frame_visible: no forward on this ctx");
+  if (n != c->n) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_frame_visible: n differs from the last forward's");
+  if (int rc = gs_check_device(c->device, "gs_frame_visible")) return rc;
+  GS_CUDA_TRY(gs_launch_frame_visible(c->count.as<uint32_t>(), n, c->n_views ? c->n_views : 1, accumulate, visible,
+                                      (cudaStream_t)stream));
+  if (n > 0) gs_count_launch();
+  return 0;
+}
+
 extern "C" int gs_render_forward_backward_host(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
                                                const float* quat, const float* scale, int n, int d,
                                                int scale_activation, const gs_camera* cam,

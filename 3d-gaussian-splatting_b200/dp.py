@@ -275,3 +275,13 @@ def allreduce_stats(tensors: Iterable[torch.Tensor], group=None):
         return
     for t in tensors:
         dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+
+
+def all_reduce_visible(mask: torch.Tensor, group=None) -> torch.Tensor:
+    """Union over the ranks of the visibility masks (`Splatter.visible_mask()`, uint8 [n]) for a visible-only
+    optimizer step (`FlatAdam.step(visible=...)`), in place.  The gradients are summed over the ranks, so the rows to
+    update are those any rank saw, and the replicas stay bit-identical only if every rank steps the same rows.
+    n bytes per step."""
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(mask, op=dist.ReduceOp.MAX, group=group)
+    return mask

@@ -8,6 +8,11 @@ Drop-in for the way the reference steps its optimizer (train.py:56-64 / :173-181
 (`gaussian.adam_step` -> `gs_adam_step`) over flat parameter / moment buffers instead of
 5 x (foreach) kernel groups.  No CPU / torch fallback: gradients that are not one flat bucket are
 an error.
+
+`step(visible=mask)` is a second optimizer, opt-in: Adam on the rows of the Gaussians the last frames binned
+(`Splatter.visible_mask()`), the "sparse Adam" of 3DGS / gsplat's `SelectiveAdam`
+(`gaussian.adam_step_visible` -> `gs_adam_step_visible`).  A Gaussian that was not seen is frozen, moments included,
+where dense Adam lets it drift on its momentum; the bias corrections use the global step count either way.
 """
 from __future__ import annotations
 
@@ -72,7 +77,10 @@ class FlatAdam:
         self._flat = (flat, m, v, ordered, ends, base)
 
     @torch.no_grad()
-    def step(self):
+    def step(self, visible=None):
+        """One Adam step.  `visible` None: every float of the bucket (dense).  A CUDA uint8 tensor [n]: only the rows
+        i with visible[i] != 0 of every parameter (each must have shape[0] == n); the others keep their value and
+        their moments, bit for bit.  `step_count` advances by one either way."""
         params = [p for g in self.param_groups for p in g["params"] if p.grad is not None]
         if not params:
             return
@@ -95,6 +103,19 @@ class FlatAdam:
         gflat = torch.empty(0, dtype=torch.float32, device=g0.device).set_(g0.untyped_storage(), base, (flat.numel(),))
         if (base * 4 + g0.untyped_storage().data_ptr()) % 16:
             raise RuntimeError("FlatAdam: gradient bucket must be 16-byte aligned")
+        lrs = [self._lr_of(p) for p in ordered]
+        if visible is None:
+            self.step_count += 1
+            gaussian.adam_step(flat, gflat, m, v, ends, lrs, self.betas[0], self.betas[1], self.eps, self.step_count)
+            return
+        if not (torch.is_tensor(visible) and visible.is_cuda and visible.dtype == torch.uint8 and visible.dim() == 1):
+            raise TypeError("FlatAdam.step: visible must be a 1-D CUDA uint8 tensor (Splatter.visible_mask())")
+        n = visible.numel()
+        if any(p.dim() == 0 or p.shape[0] != n for p in ordered):
+            raise ValueError(f"FlatAdam.step: visible has {n} entries but the parameters have "
+                             f"{[tuple(p.shape) for p in ordered]}: every parameter needs shape[0] == visible.numel()")
+        starts = [p.grad.storage_offset() - base for p in ordered]
+        widths = [p.numel() // n if n else 1 for p in ordered]
         self.step_count += 1
-        gaussian.adam_step(flat, gflat, m, v, ends, [self._lr_of(p) for p in ordered], self.betas[0], self.betas[1],
-                           self.eps, self.step_count)
+        gaussian.adam_step_visible(flat, gflat, m, v, starts, widths, lrs, visible.contiguous(), self.betas[0],
+                                   self.betas[1], self.eps, self.step_count)

@@ -299,6 +299,7 @@ class Splatter(nn.Module):
         if densify_stats != "none":
             self.densify_stats = DensifyStats(self.gaussian_3ds.pos.shape[0], densify_stats == "absgrad", self.device,
                                               self._rctx)
+        self._visible = None                                        # visible_mask()'s buffer
         self.ground_truth = None
         self.culling_mask = None
         self.n_tile_gaussians = 0
@@ -551,6 +552,21 @@ class Splatter(nn.Module):
         self.n_gaussians = g.pos.shape[0]
         st.reset(self.n_gaussians)
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.n_gaussians)
+
+    @torch.no_grad()
+    def visible_mask(self, accumulate=False):
+        """uint8 [n]: 1 where the last frame rendered through this Splatter (`forward`, `render_maps`, `render_batch`:
+        any of its views, `render_features`, `render_at_pose`) binned the Gaussian into at least one tile, the set
+        with a gradient and the one `densify_stats.count` counts; every other Gaussian's gradient row is exactly
+        zero.  `accumulate=True` ORs into the previous mask (several frames before one optimizer step).  For
+        `optim.FlatAdam.step(visible=...)`; under data parallel reduce it with `dp.all_reduce_visible` first.  The
+        buffer belongs to the Splatter, is rewritten by the next call and re-sized (from zero) when the number of
+        Gaussians changes."""
+        n = self.gaussian_3ds.pos.shape[0]
+        if self._visible is None or self._visible.numel() != n:
+            self._visible = torch.zeros(n, device=self.device, dtype=torch.uint8)
+        self._rctx.visible_into(self._visible, bool(accumulate))
+        return self._visible
 
     def save_checkpoint(self, path, optimizer=None, iteration=None, trainer_state=None):
         """reference Trainer.save_checkpoint (train.py:283-291) + resume state; see checkpoint.py."""

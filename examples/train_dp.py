@@ -51,7 +51,7 @@ def make_optimizer(sp, lr=0.003, fused=True):
         {"params": g.scale, "lr": lr}, {"params": g.quat, "lr": lr}], betas=(0.9, 0.99))
 
 
-def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True):
+def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False):
     opt = make_optimizer(sp, lr, fused_adam)
     params = list(sp.gaussian_3ds.parameters())
     bucket = dp.make_grad_bucket(params, average=True)   # peer-memory exchange when available, else NCCL
@@ -65,7 +65,10 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True):
         loss = (img - gts[view]).abs().mean()                        # train.py:99
         loss.backward()
         bucket.allreduce()
-        opt.step()
+        if visible_adam:                                              # step only the Gaussians some rank binned
+            opt.step(visible=dp.all_reduce_visible(sp.visible_mask()))
+        else:
+            opt.step()
         if it % log_every == 0 or it == iters - 1:
             with torch.no_grad():
                 mse = ((img - gts[view]) ** 2).mean()
@@ -84,7 +87,11 @@ def main():
     ap.add_argument("--iters", type=int, default=300)
     ap.add_argument("--views", type=int, default=8)
     ap.add_argument("--torch-adam", action="store_true", help="use torch.optim.Adam instead of the fused flat Adam")
+    ap.add_argument("--visible-adam", action="store_true",
+                    help="update only the Gaussians binned this step (3DGS sparse Adam); unseen ones stay frozen")
     args = ap.parse_args()
+    if args.visible_adam and args.torch_adam:
+        ap.error("--visible-adam is a mode of the fused flat Adam")
     w, h = (int(x) for x in args.res.split("x"))
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
@@ -93,7 +100,8 @@ def main():
         torch.distributed.init_process_group("nccl", device_id=dev)
     torch.manual_seed(2023)                                           # identical torch RNG on all ranks
     sp, gts = build(args.gaussians, w, h, args.views, dev)
-    hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam)
+    hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam,
+                      visible_adam=args.visible_adam)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
               f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB")

@@ -407,6 +407,16 @@ int gs_frame_sorted(gs_ctx* ctx, int* gauss_idx, long long capacity, int* tile_a
  * saturated (M_eff = their sum).  For parity tests / roofline accounting. */
 int gs_frame_tile_consumed(gs_ctx* ctx, int* tile_consumed, gs_stream_t stream);
 
+/* Which Gaussians the last forward on ctx binned: visible[i] (DEVICE uint8 [n]) = 1 if Gaussian i got at least one
+ * tile instance (for a batched forward: in any of its views), else 0.  accumulate != 0 ORs into what visible holds
+ * (several frames before one optimizer step); 0 overwrites.  This is "binned", the rule the projection backward, the
+ * feature gradient and the densification statistics (count += 1) use for "took part", not the frustum test that
+ * culling_mask reports: a Gaussian can pass the cull and get no tile (a non-positive determinant, an ANTIALIAS
+ * det <= 0).  A Gaussian that is not visible has an exactly zero gradient row.  Valid after every forward entry, on
+ * the gather and the packed path, for every colour model.  One launch when n > 0, no synchronisation, no atomics.
+ * GS_ERR_INVALID_ARG: a null ctx or pointer, no forward on ctx yet, n different from the last forward's. */
+int gs_frame_visible(gs_ctx* ctx, unsigned char* visible, int n, int accumulate, gs_stream_t stream);
+
 /* End-to-end convenience with HOST buffers (bench `e2e` leg and plain-C callers): copies
  * the camera + grad_image from host, runs forward + backward on device-resident parameters,
  * copies the padded image back.  Host buffers should be pinned.  Synchronises. */
@@ -427,6 +437,24 @@ int gs_render_forward_backward_host(gs_ctx* ctx, const float* pos, const float* 
 int gs_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
                  const long long* seg_end_host, const float* lr_host, int n_seg, float beta1, float beta2,
                  float eps, int step, gs_stream_t stream);
+
+/* Adam on the rows of the visible Gaussians only (the "sparse Adam" of 3DGS, gsplat's SelectiveAdam): a different
+ * optimizer from gs_adam_step, not a faster route to its numbers.  A Gaussian that is not visible is frozen: its
+ * parameters and both moments keep their bits (dense Adam would let it drift on its momentum and decay the moments).
+ * The flat buffers are those of gs_adam_step; segment s is the row-major [n_rows, seg_width_host[s]] array that starts
+ * at float seg_start_host[s] (a multiple of 4) and has learning rate lr_host[s].  For every i with visible[i] != 0
+ * (DEVICE uint8 [n_rows], e.g. from gs_frame_visible), every float of row i of every segment gets exactly
+ * gs_adam_step's update: the same rounded operations, the same bias corrections from the global `step` (not from a
+ * per-row count).  Nothing else in param / exp_avg / exp_avg_sq is read or written, the pad floats between segments
+ * included; DRAM traffic follows the number of visible rows.  Bit-deterministic (no atomics).  One launch, no
+ * synchronisation; n_rows == 0 returns 0 without a launch.
+ * GS_ERR_INVALID_ARG, before any launch: step < 1; n_seg outside 1 .. 8; n_flat negative or not a multiple of 4;
+ * n_rows < 0; a width outside 1 .. 2^24; starts that are not ascending multiples of 4; segments that overlap or end
+ * beyond n_flat; a NULL host array; a NULL device buffer or mask with n_rows > 0. */
+int gs_adam_step_visible(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n_flat,
+                         const long long* seg_start_host, const int* seg_width_host, const float* lr_host, int n_seg,
+                         int n_rows, const unsigned char* visible, float beta1, float beta2, float eps, int step,
+                         gs_stream_t stream);
 
 /* Densification on the device (SURVEY.md §8 f-2; reference splatter.py:122-228 `adaptive_control`, called
  * from train.py:156-172): prune Gaussians with opacity logit <= opa_logit_min or activated-scale norm >=

@@ -36,7 +36,7 @@ static inline void check_rc(int rc, const char* fn) {
 }
 static inline gs_stream_t cur_stream() { return (gs_stream_t)at::cuda::getCurrentCUDAStream().stream(); }
 static inline const float* fp(const torch::Tensor& t) { return t.data_ptr<float>(); }
-static inline float* fpm(torch::Tensor& t) { return t.data_ptr<float>(); }
+static inline float* fpm(const torch::Tensor& t) { return t.data_ptr<float>(); }
 
 // Same attribute names as reference common.hpp:36-74; distinct C++ types so both modules can
 // live in one interpreter during parity tests.
@@ -272,45 +272,6 @@ struct RenderContext {
     return cam;
   }
 
-  // returns (image[Hp,Wp,3], culling_mask[n] int64)
-  std::tuple<torch::Tensor, torch::Tensor> forward(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa,
-                                                   torch::Tensor quat, torch::Tensor scale, int width, int height,
-                                                   float fx, float fy, torch::Tensor rot, torch::Tensor tran,
-                                                   float near, float thresh, int scale_activation) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    int64_t n = pos.size(0);
-    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
-                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
-                "RenderContext.forward: bad shapes");
-    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
-    c10::cuda::CUDAGuard guard(pos.device());
-    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
-    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
-    auto image = torch::empty({hp, wp, 3}, pos.options());
-    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
-    check_rc(gs_render_forward(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
-                               scale_activation, &cam, fpm(image), mask.data_ptr<int64_t>(), cur_stream()),
-             "gs_render_forward");
-    ++frame;
-    return {image, mask};
-  }
-
-  std::vector<torch::Tensor> backward(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
-                                      torch::Tensor scale, torch::Tensor image, torch::Tensor grad_image) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(image);
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.sizes() == image.sizes(),
-                "RenderContext.backward: grad_image must match image");
-    c10::cuda::CUDAGuard guard(pos.device());
-    auto gi = grad_image.contiguous();
-    auto g_pos = torch::empty_like(pos), g_rgb = torch::empty_like(rgb), g_opa = torch::empty_like(opa),
-         g_quat = torch::empty_like(quat), g_scale = torch::empty_like(scale);
-    check_rc(gs_render_backward(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(image), fp(gi), fpm(g_pos),
-                                fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
-             "gs_render_backward");
-    return {g_pos, g_rgb, g_opa, g_quat, g_scale};
-  }
-
   // data-parallel gradient push (gs_grad_push): pointers as integers (symmetric-memory mappings)
   void set_grad_push(int64_t bucket_ptr, std::vector<int64_t> staging_ptrs, int64_t per, int rank) {
     gs_grad_push p{};
@@ -373,70 +334,207 @@ struct RenderContext {
     return v;
   }
 
+  static int64_t padded(int64_t size) { return (size + 15) / 16 * 16; }
+  static float* fpm_or_null(const torch::Tensor& t) { return t.defined() ? fpm(t) : nullptr; }
+  static py::object or_none(const torch::Tensor& t) { return t.defined() ? py::cast(t) : py::none(); }
+
+  // the five parameters (and feat [n, f]) of a frame: contiguous float32 on this context's device; returns n
+  int64_t check_params(const char* fn, const torch::Tensor& pos, const torch::Tensor& rgb, const torch::Tensor& opa,
+                       const torch::Tensor& quat, const torch::Tensor& scale,
+                       const torch::Tensor* feat_or_null = nullptr) const {
+    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+    if (feat_or_null) {
+      const torch::Tensor& feat = *feat_or_null;
+      GS_CHECK_F32(feat);
+    }
+    const int64_t n = pos.size(0);
+    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
+                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31) &&
+                    (!feat_or_null || (feat_or_null->dim() == 2 && feat_or_null->size(0) == n)),
+                fn, ": bad shapes");
+    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
+    return n;
+  }
+
+  // gradient buffers for the parameters, in the same order (pos, rgb, opa, quat, scale[, feat]); the kernels store
+  // quaternion gradients as float4
+  static void check_grads(const char* fn, const std::vector<torch::Tensor>& params,
+                          const std::vector<torch::Tensor>& grads) {
+    static const char* names[] = {"g_pos", "g_rgb", "g_opa", "g_quat", "g_scale", "g_feat"};
+    bool match = true;
+    for (size_t k = 0; k < grads.size(); ++k) {
+      const torch::Tensor& g = grads[k];
+      TORCH_CHECK(g.is_cuda() && g.is_contiguous() && g.scalar_type() == at::kFloat, fn, ": ", names[k],
+                  " must be a contiguous float32 CUDA tensor");
+      match = match && g.numel() == params[k].numel();
+    }
+    TORCH_CHECK(match, fn, ": gradient buffers must match their parameters");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(grads[3].data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+  }
+
+  // a float32 CUDA image of shape pixels + [channels], pixels = [(B,) rows, cols]
+  static void check_image(const char* fn, const char* name, const torch::Tensor& t, std::vector<int64_t> pixels,
+                          int64_t channels, bool contiguous) {
+    pixels.push_back(channels);
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.sizes() == at::IntArrayRef(pixels) &&
+                    (!contiguous || t.is_contiguous()),
+                fn, ": ", name, " must be a float32", contiguous ? " contiguous" : "", " CUDA tensor of shape ",
+                at::IntArrayRef(pixels));
+  }
+
+  // The tensors of a backward of the last forward: raw [(B,) Hp, Wp, 3] with aux (2 channels) and map (feat's f
+  // channels) like it; the upstream gradients grad_image (3 channels), grad_aux and grad_map over raw's pixels, or
+  // (final) over the centre crop's [(B,) H, W].  Batched: B, H, W are those of the last forward_batch.
+  void check_backward(const char* fn, int64_t expected_frame, bool batched, bool final, const torch::Tensor& pos,
+                      const torch::Tensor& rgb, const torch::Tensor& opa, const torch::Tensor& quat,
+                      const torch::Tensor& scale, const torch::Tensor& raw, const torch::Tensor& grad_image,
+                      const torch::Tensor* aux, const torch::Tensor* grad_aux, const torch::Tensor* feat = nullptr,
+                      const torch::Tensor* map = nullptr, const torch::Tensor* grad_map = nullptr) const {
+    check_frame(expected_frame, fn);
+    check_params(fn, pos, rgb, opa, quat, scale, feat);
+    TORCH_CHECK(raw.dim() == (batched ? 4 : 3), fn, ": raw must be ", batched ? "[B,Hp,Wp,3]" : "[Hp,Wp,3]");
+    std::vector<int64_t> pixels = batched ? std::vector<int64_t>{batch[0], padded(batch[1]), padded(batch[2])}
+                                          : std::vector<int64_t>{raw.size(0), raw.size(1)};
+    check_image(fn, "raw", raw, pixels, 3, true);
+    if (aux) check_image(fn, "aux", *aux, pixels, 2, true);
+    if (map) check_image(fn, "map", *map, pixels, feat->size(1), true);
+    if (final) {
+      TORCH_CHECK(grad_image.dim() == raw.dim(), fn, ": grad_image must be ", batched ? "[B,H,W,3]" : "[H,W,3]",
+                  " (final) or match raw");
+      pixels = batched ? std::vector<int64_t>{batch[0], batch[1], batch[2]}
+                       : std::vector<int64_t>{grad_image.size(0), grad_image.size(1)};
+    }
+    check_image(fn, "grad_image", grad_image, pixels, 3, false);
+    if (grad_aux) check_image(fn, "grad_aux", *grad_aux, pixels, 2, false);
+    if (grad_map) check_image(fn, "grad_map", *grad_map, pixels, feat->size(1), false);
+  }
+
+  // backward of the last single-view (gs_render_backward_aux) or batched (gs_render_backward_batch) forward into the
+  // caller's gradient buffers; aux / grad_aux NULL: the plain backward kernels
+  void backward_checked(const char* fn, bool batched, const torch::Tensor& pos, const torch::Tensor& rgb,
+                        const torch::Tensor& opa, const torch::Tensor& quat, const torch::Tensor& scale,
+                        const torch::Tensor& raw, const torch::Tensor& grad_image, bool final,
+                        const torch::Tensor* aux, const std::optional<torch::Tensor>& grad_aux,
+                        const std::vector<torch::Tensor>& grads, int64_t expected_frame) {
+    check_backward(fn, expected_frame, batched, final, pos, rgb, opa, quat, scale, raw, grad_image, aux,
+                   grad_aux ? &*grad_aux : nullptr);
+    check_grads(fn, {pos, rgb, opa, quat, scale}, grads);
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor ga;
+    if (grad_aux) ga = grad_aux->contiguous();
+    auto entry = batched ? &gs_render_backward_batch : &gs_render_backward_aux;
+    check_rc(entry(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi), final ? 1 : 0,
+                   aux ? fp(*aux) : nullptr, fpm_or_null(ga), fpm(grads[0]), fpm(grads[1]), fpm(grads[2]),
+                   fpm(grads[3]), fpm(grads[4]), cur_stream()),
+             fn);
+  }
+
+  // what a forward renders: raw / aux / map padded [(B,) Hp, Wp, .], fin / aux_fin / map_fin the centre crops
+  // [(B,) H, W, .] (final), mask [(B,) n]; tensors a forward does not write stay undefined
+  struct Outputs {
+    torch::Tensor raw, aux, map, fin, aux_fin, map_fin, mask;
+  };
+  static Outputs alloc_outputs(const torch::Tensor& pos, int64_t b, int64_t n, int64_t height, int64_t width,
+                               bool maps, int64_t f, bool final) {
+    auto shape = [b](int64_t rows, int64_t cols, int64_t ch) {
+      return b ? std::vector<int64_t>{b, rows, cols, ch} : std::vector<int64_t>{rows, cols, ch};
+    };
+    const int64_t hp = padded(height), wp = padded(width);
+    Outputs o;
+    o.raw = torch::empty(shape(hp, wp, 3), pos.options());
+    if (maps) o.aux = torch::empty(shape(hp, wp, 2), pos.options());
+    if (f) o.map = torch::empty(shape(hp, wp, f), pos.options());
+    if (final) {
+      o.fin = torch::empty(shape(height, width, 3), pos.options());
+      if (maps) o.aux_fin = torch::empty(shape(height, width, 2), pos.options());
+      if (f) o.map_fin = torch::empty(shape(height, width, f), pos.options());
+    }
+    o.mask = torch::empty(b ? std::vector<int64_t>{b, n} : std::vector<int64_t>{n}, pos.options().dtype(at::kLong));
+    return o;
+  }
+
+  struct Background {
+    float rgb[3] = {0.f, 0.f, 0.f};
+    bool given = false;
+    const float* ptr() const { return given ? rgb : nullptr; }
+  };
+  static Background background_of(const char* fn, const std::optional<std::vector<double>>& background) {
+    TORCH_CHECK(!background || background->size() == 3, fn, ": background must have 3 values");
+    Background bg;
+    if (background) {
+      bg.given = true;
+      for (int k = 0; k < 3; ++k) bg.rgb[k] = (float)(*background)[k];
+    }
+    return bg;
+  }
+
+  // the C call of a forward; on success the context holds a new frame
+  void rendered(int rc, const char* fn) {
+    check_rc(rc, fn);
+    ++frame;
+  }
+
+  // one view through gs_render_forward_aux: maps = the depth / alpha maps, final = the clamped centre crops
+  Outputs render(const char* fn, const torch::Tensor& pos, const torch::Tensor& rgb, const torch::Tensor& opa,
+                 const torch::Tensor& quat, const torch::Tensor& scale, int width, int height, float fx, float fy,
+                 const torch::Tensor& rot, const torch::Tensor& tran, float near, float thresh, int scale_activation,
+                 const std::optional<std::vector<double>>& background, bool maps, bool final) {
+    const int64_t n = check_params(fn, pos, rgb, opa, quat, scale);
+    const Background bg = background_of(fn, background);
+    c10::cuda::CUDAGuard guard(pos.device());
+    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
+    Outputs o = alloc_outputs(pos, 0, n, height, width, maps, 0, final);
+    gs_render_aux ax{bg.ptr(), fpm_or_null(o.aux), fpm_or_null(o.aux_fin)};
+    rendered(gs_render_forward_aux(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                   scale_activation, &cam, fpm(o.raw), fpm_or_null(o.fin),
+                                   o.mask.data_ptr<int64_t>(), &ax, cur_stream()),
+             fn);
+    return o;
+  }
+
+  // returns (image[Hp,Wp,3], culling_mask[n] int64)
+  std::tuple<torch::Tensor, torch::Tensor> forward(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa,
+                                                   torch::Tensor quat, torch::Tensor scale, int width, int height,
+                                                   float fx, float fy, torch::Tensor rot, torch::Tensor tran,
+                                                   float near, float thresh, int scale_activation) {
+    Outputs o = render("RenderContext.forward", pos, rgb, opa, quat, scale, width, height, fx, fy, rot, tran, near,
+                       thresh, scale_activation, std::nullopt, false, false);
+    return {o.raw, o.mask};
+  }
+
+  std::vector<torch::Tensor> backward(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                                      torch::Tensor scale, torch::Tensor image, torch::Tensor grad_image) {
+    std::vector<torch::Tensor> grads = {torch::empty_like(pos), torch::empty_like(rgb), torch::empty_like(opa),
+                                        torch::empty_like(quat), torch::empty_like(scale)};
+    backward_checked("RenderContext.backward", false, pos, rgb, opa, quat, scale, image, grad_image, false, nullptr,
+                     std::nullopt, grads, -1);
+    return grads;
+  }
+
+  void backward_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale,
+                     torch::Tensor image, torch::Tensor grad_image, torch::Tensor g_pos, torch::Tensor g_rgb,
+                     torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale, int64_t expected_frame) {
+    backward_checked("RenderContext.backward_into", false, pos, rgb, opa, quat, scale, image, grad_image, false,
+                     nullptr, std::nullopt, {g_pos, g_rgb, g_opa, g_quat, g_scale}, expected_frame);
+  }
+
   // fused clamp + centre crop: returns (final[H,W,3], raw padded[Hp,Wp,3], mask)
   std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> forward_final(
       torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale, int width,
       int height, float fx, float fy, torch::Tensor rot, torch::Tensor tran, float near, float thresh,
       int scale_activation) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    int64_t n = pos.size(0);
-    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
-                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
-                "RenderContext.forward: bad shapes");
-    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
-    c10::cuda::CUDAGuard guard(pos.device());
-    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
-    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
-    auto raw = torch::empty({hp, wp, 3}, pos.options());
-    auto fin = torch::empty({height, width, 3}, pos.options());
-    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
-    check_rc(gs_render_forward_final(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
-                                     scale_activation, &cam, fpm(raw), fpm(fin), mask.data_ptr<int64_t>(),
-                                     cur_stream()),
-             "gs_render_forward_final");
-    ++frame;
-    return {fin, raw, mask};
+    Outputs o = render("RenderContext.forward_final", pos, rgb, opa, quat, scale, width, height, fx, fy, rot, tran,
+                       near, thresh, scale_activation, std::nullopt, false, true);
+    return {o.fin, o.raw, o.mask};
   }
 
   void backward_final_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
                            torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_final, torch::Tensor g_pos,
                            torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
                            int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_final_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(raw); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa); GS_CHECK_F32(g_quat);
-    GS_CHECK_F32(g_scale);
-    TORCH_CHECK(grad_final.is_cuda() && grad_final.scalar_type() == at::kFloat && grad_final.dim() == 3 &&
-                    grad_final.size(2) == 3, "RenderContext.backward_final_into: grad_final must be [H,W,3] float32");
-    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
-                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
-                "RenderContext.backward_final_into: gradient buffers must match their parameters");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
-    c10::cuda::CUDAGuard guard(pos.device());
-    auto gf = grad_final.contiguous();
-    check_rc(gs_render_backward_final(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gf), fpm(g_pos),
-                                      fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
-             "gs_render_backward_final");
-  }
-
-  void backward_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat, torch::Tensor scale,
-                     torch::Tensor image, torch::Tensor grad_image, torch::Tensor g_pos, torch::Tensor g_rgb,
-                     torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale, int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(image); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa); GS_CHECK_F32(g_quat);
-    GS_CHECK_F32(g_scale);
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.sizes() == image.sizes(),
-                "RenderContext.backward_into: grad_image must match image");
-    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
-                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
-                "RenderContext.backward_into: gradient buffers must match their parameters");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
-    c10::cuda::CUDAGuard guard(pos.device());
-    auto gi = grad_image.contiguous();
-    check_rc(gs_render_backward(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(image), fp(gi), fpm(g_pos),
-                                fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
-             "gs_render_backward");
+    backward_checked("RenderContext.backward_final_into", false, pos, rgb, opa, quat, scale, raw, grad_final, true,
+                     nullptr, std::nullopt, {g_pos, g_rgb, g_opa, g_quat, g_scale}, expected_frame);
   }
 
   // depth / alpha maps and a background colour (gs_render_forward_aux): returns
@@ -445,35 +543,9 @@ struct RenderContext {
                         torch::Tensor scale, int width, int height, float fx, float fy, torch::Tensor rot,
                         torch::Tensor tran, float near, float thresh, int scale_activation,
                         std::optional<std::vector<double>> background, bool final) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    int64_t n = pos.size(0);
-    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
-                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
-                "RenderContext.forward_aux: bad shapes");
-    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
-    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_aux: background must have 3 values");
-    c10::cuda::CUDAGuard guard(pos.device());
-    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
-    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
-    auto raw = torch::empty({hp, wp, 3}, pos.options());
-    auto aux = torch::empty({hp, wp, 2}, pos.options());
-    torch::Tensor fin, aux_fin;
-    if (final) {
-      fin = torch::empty({height, width, 3}, pos.options());
-      aux_fin = torch::empty({height, width, 2}, pos.options());
-    }
-    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
-    float bg[3] = {0.f, 0.f, 0.f};
-    if (background)
-      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
-    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
-    check_rc(gs_render_forward_aux(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
-                                   scale_activation, &cam, fpm(raw), final ? fpm(fin) : nullptr,
-                                   mask.data_ptr<int64_t>(), &ax, cur_stream()),
-             "gs_render_forward_aux");
-    ++frame;
-    py::object none = py::none();
-    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, mask);
+    Outputs o = render("RenderContext.forward_aux", pos, rgb, opa, quat, scale, width, height, fx, fy, rot, tran, near,
+                       thresh, scale_activation, background, true, final);
+    return py::make_tuple(or_none(o.fin), o.raw, o.aux, or_none(o.aux_fin), o.mask);
   }
 
   // backward of forward_aux; grad_aux = None: the plain backward kernels (zero depth / alpha gradient)
@@ -482,34 +554,8 @@ struct RenderContext {
                          torch::Tensor aux, std::optional<torch::Tensor> grad_aux, torch::Tensor g_pos,
                          torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
                          int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_aux_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa);
-    GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale);
-    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3 && aux.dim() == 3 && aux.size(0) == raw.size(0) &&
-                    aux.size(1) == raw.size(1) && aux.size(2) == 2,
-                "RenderContext.backward_aux_into: raw must be [Hp,Wp,3] and aux [Hp,Wp,2]");
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
-                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
-                "RenderContext.backward_aux_into: grad_image must be [H,W,3] (final) or match raw");
-    if (grad_aux) {
-      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
-                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
-                      grad_aux->size(2) == 2,
-                  "RenderContext.backward_aux_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
-    }
-    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
-                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
-                "RenderContext.backward_aux_into: gradient buffers must match their parameters");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
-    c10::cuda::CUDAGuard guard(pos.device());
-    auto gi = grad_image.contiguous();
-    torch::Tensor ga;
-    if (grad_aux) ga = grad_aux->contiguous();
-    check_rc(gs_render_backward_aux(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
-                                    grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fpm(g_pos),
-                                    fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
-             "gs_render_backward_aux");
+    backward_checked("RenderContext.backward_aux_into", false, pos, rgb, opa, quat, scale, raw, grad_image,
+                     grad_is_final, &aux, grad_aux, {g_pos, g_rgb, g_opa, g_quat, g_scale}, expected_frame);
   }
 
   // a batch of B views as one frame (gs_render_forward_batch): focal [B,2] = (fx, fy), rot [B,3,3], tran [B,3] are
@@ -519,11 +565,8 @@ struct RenderContext {
                           torch::Tensor scale, int width, int height, torch::Tensor focal, torch::Tensor rot,
                           torch::Tensor tran, float near, float thresh, int scale_activation,
                           std::optional<std::vector<double>> background, bool final) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    int64_t n = pos.size(0);
-    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
-                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31),
-                "RenderContext.forward_batch: bad shapes");
+    const char* fn = "RenderContext.forward_batch";
+    const int64_t n = check_params(fn, pos, rgb, opa, quat, scale);
     TORCH_CHECK(!focal.is_cuda() && !rot.is_cuda() && !tran.is_cuda(),
                 "RenderContext.forward_batch: focal / rot / tran must be CPU tensors (cameras are host data)");
     const int64_t b = focal.dim() == 2 ? focal.size(0) : -1;
@@ -531,34 +574,20 @@ struct RenderContext {
                     rot.size(1) == 3 && rot.size(2) == 3 && tran.dim() == 2 && tran.size(0) == b && tran.size(1) == 3,
                 "RenderContext.forward_batch: focal must be [B,2], rot [B,3,3] and tran [B,3] with 1 <= B <= ",
                 GS_MAX_VIEWS);
-    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
-    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_batch: background must have 3 values");
+    const Background bg = background_of(fn, background);
     c10::cuda::CUDAGuard guard(pos.device());
     auto f = focal.to(at::kFloat).contiguous();
     std::vector<gs_camera> cams;
     for (int64_t v = 0; v < b; ++v)
       cams.push_back(make_cam(width, height, f[v][0].item<float>(), f[v][1].item<float>(), rot[v], tran[v], near, thresh));
-    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
-    auto raw = torch::empty({b, hp, wp, 3}, pos.options());
-    auto aux = torch::empty({b, hp, wp, 2}, pos.options());
-    torch::Tensor fin, aux_fin;
-    if (final) {
-      fin = torch::empty({b, height, width, 3}, pos.options());
-      aux_fin = torch::empty({b, height, width, 2}, pos.options());
-    }
-    auto mask = torch::empty({b, n}, pos.options().dtype(at::kLong));
-    float bg[3] = {0.f, 0.f, 0.f};
-    if (background)
-      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
-    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
-    check_rc(gs_render_forward_batch(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
-                                     scale_activation, (int)b, cams.data(), fpm(raw), final ? fpm(fin) : nullptr,
-                                     mask.data_ptr<int64_t>(), &ax, cur_stream()),
-             "gs_render_forward_batch");
-    ++frame;
+    Outputs o = alloc_outputs(pos, b, n, height, width, true, 0, final);
+    gs_render_aux ax{bg.ptr(), fpm(o.aux), fpm_or_null(o.aux_fin)};
+    rendered(gs_render_forward_batch(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                     scale_activation, (int)b, cams.data(), fpm(o.raw), fpm_or_null(o.fin),
+                                     o.mask.data_ptr<int64_t>(), &ax, cur_stream()),
+             fn);
     batch = {b, height, width};
-    py::object none = py::none();
-    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, mask);
+    return py::make_tuple(or_none(o.fin), o.raw, o.aux, or_none(o.aux_fin), o.mask);
   }
 
   // (views, height, width) of the last forward_batch: its backward's tensors are checked against them
@@ -570,37 +599,8 @@ struct RenderContext {
                            torch::Tensor aux, std::optional<torch::Tensor> grad_aux, torch::Tensor g_pos,
                            torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
                            int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_batch_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(g_pos); GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa);
-    GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale);
-    const int64_t b = batch[0], hp = (batch[1] + 15) / 16 * 16, wp = (batch[2] + 15) / 16 * 16;
-    TORCH_CHECK(raw.dim() == 4 && raw.size(0) == b && raw.size(1) == hp && raw.size(2) == wp && raw.size(3) == 3 &&
-                    aux.sizes() == at::IntArrayRef({b, hp, wp, 2}),
-                "RenderContext.backward_batch_into: raw must be [B,Hp,Wp,3] and aux [B,Hp,Wp,2] of the last forward_batch");
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 4 &&
-                    grad_image.size(0) == b && grad_image.size(3) == 3 &&
-                    (grad_is_final ? (grad_image.size(1) == batch[1] && grad_image.size(2) == batch[2])
-                                   : grad_image.sizes() == raw.sizes()),
-                "RenderContext.backward_batch_into: grad_image must be [B,H,W,3] (final) or match raw");
-    if (grad_aux) {
-      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 4 &&
-                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
-                      grad_aux->size(2) == grad_image.size(2) && grad_aux->size(3) == 2,
-                  "RenderContext.backward_batch_into: grad_aux must be float32 [B, rows, cols, 2] like grad_image");
-    }
-    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
-                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel(),
-                "RenderContext.backward_batch_into: gradient buffers must match their parameters");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
-    c10::cuda::CUDAGuard guard(pos.device());
-    auto gi = grad_image.contiguous();
-    torch::Tensor ga;
-    if (grad_aux) ga = grad_aux->contiguous();
-    check_rc(gs_render_backward_batch(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
-                                      grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fpm(g_pos),
-                                      fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale), cur_stream()),
-             "gs_render_backward_batch");
+    backward_checked("RenderContext.backward_batch_into", true, pos, rgb, opa, quat, scale, raw, grad_image,
+                     grad_is_final, &aux, grad_aux, {g_pos, g_rgb, g_opa, g_quat, g_scale}, expected_frame);
   }
 
   // backward_aux_into plus the camera gradient grad_cam[12] = (dL/drot row-major, dL/dtran) of the forward's camera
@@ -612,46 +612,26 @@ struct RenderContext {
                          std::optional<torch::Tensor> g_pos, std::optional<torch::Tensor> g_rgb,
                          std::optional<torch::Tensor> g_opa, std::optional<torch::Tensor> g_quat,
                          std::optional<torch::Tensor> g_scale, torch::Tensor grad_cam, int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_cam_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(raw); GS_CHECK_F32(grad_cam);
+    const char* fn = "RenderContext.backward_cam_into";
+    check_backward(fn, expected_frame, false, grad_is_final, pos, rgb, opa, quat, scale, raw, grad_image,
+                   aux ? &*aux : nullptr, grad_aux ? &*grad_aux : nullptr);
+    GS_CHECK_F32(grad_cam);
     TORCH_CHECK(grad_cam.numel() == 12 && grad_cam.device() == pos.device(),
                 "RenderContext.backward_cam_into: grad_cam must be 12 floats on the parameters' device");
-    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3, "RenderContext.backward_cam_into: raw must be [Hp,Wp,3]");
-    if (aux) {
-      GS_CHECK_F32(*aux);
-      TORCH_CHECK(aux->dim() == 3 && aux->size(0) == raw.size(0) && aux->size(1) == raw.size(1) && aux->size(2) == 2,
-                  "RenderContext.backward_cam_into: aux must be [Hp,Wp,2]");
-    }
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
-                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
-                "RenderContext.backward_cam_into: grad_image must be [H,W,3] (final) or match raw");
-    if (grad_aux) {
-      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
-                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
-                      grad_aux->size(2) == 2,
-                  "RenderContext.backward_cam_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
-    }
     const int n_given = (int)g_pos.has_value() + g_rgb.has_value() + g_opa.has_value() + g_quat.has_value() +
                         g_scale.has_value();
     TORCH_CHECK(n_given == 0 || n_given == 5,
                 "RenderContext.backward_cam_into: give all five parameter gradients or none (camera only)");
-    if (n_given) {
-      GS_CHECK_F32(*g_pos); GS_CHECK_F32(*g_rgb); GS_CHECK_F32(*g_opa); GS_CHECK_F32(*g_quat); GS_CHECK_F32(*g_scale);
-      TORCH_CHECK(g_pos->numel() == pos.numel() && g_rgb->numel() == rgb.numel() && g_opa->numel() == opa.numel() &&
-                      g_quat->numel() == quat.numel() && g_scale->numel() == scale.numel(),
-                  "RenderContext.backward_cam_into: gradient buffers must match their parameters");
-      TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat->data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
-    }
-    auto opt = [](std::optional<torch::Tensor>& t) { return t ? fpm(*t) : nullptr; };
+    if (n_given) check_grads(fn, {pos, rgb, opa, quat, scale}, {*g_pos, *g_rgb, *g_opa, *g_quat, *g_scale});
+    auto opt = [](const std::optional<torch::Tensor>& t) { return t ? fpm(*t) : nullptr; };
     c10::cuda::CUDAGuard guard(pos.device());
     auto gi = grad_image.contiguous();
     torch::Tensor ga;
     if (grad_aux) ga = grad_aux->contiguous();
     check_rc(gs_render_backward_cam(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
-                                    grad_is_final ? 1 : 0, aux ? fp(*aux) : nullptr, grad_aux ? fp(ga) : nullptr, opt(g_pos),
+                                    grad_is_final ? 1 : 0, aux ? fp(*aux) : nullptr, fpm_or_null(ga), opt(g_pos),
                                     opt(g_rgb), opt(g_opa), opt(g_quat), opt(g_scale), fpm(grad_cam), cur_stream()),
-             "gs_render_backward_cam");
+             fn);
   }
 
   // feature maps (gs_render_forward_feat): forward_aux's outputs plus (map padded [Hp,Wp,f], map_final [H,W,f] or None):
@@ -660,41 +640,20 @@ struct RenderContext {
                          torch::Tensor scale, torch::Tensor feat, int width, int height, float fx, float fy,
                          torch::Tensor rot, torch::Tensor tran, float near, float thresh, int scale_activation,
                          std::optional<std::vector<double>> background, bool final) {
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(feat);
-    int64_t n = pos.size(0);
-    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && opa.numel() == n && quat.numel() == n * 4 &&
-                    scale.numel() == n * 3 && rgb.dim() == 2 && rgb.size(0) == n && n < (int64_t(1) << 31) &&
-                    feat.dim() == 2 && feat.size(0) == n,
-                "RenderContext.forward_feat: bad shapes");
-    TORCH_CHECK(pos.device().index() == device, "RenderContext was created on another device");
-    TORCH_CHECK(!background || background->size() == 3, "RenderContext.forward_feat: background must have 3 values");
+    const char* fn = "RenderContext.forward_feat";
+    const int64_t n = check_params(fn, pos, rgb, opa, quat, scale, &feat);
+    const Background bg = background_of(fn, background);
     c10::cuda::CUDAGuard guard(pos.device());
     gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
     const int64_t f = feat.size(1);
-    int wp = (width + 15) / 16 * 16, hp = (height + 15) / 16 * 16;
-    auto raw = torch::empty({hp, wp, 3}, pos.options());
-    auto aux = torch::empty({hp, wp, 2}, pos.options());
-    auto map = torch::empty({hp, wp, f}, pos.options());
-    torch::Tensor fin, aux_fin, map_fin;
-    if (final) {
-      fin = torch::empty({height, width, 3}, pos.options());
-      aux_fin = torch::empty({height, width, 2}, pos.options());
-      map_fin = torch::empty({height, width, f}, pos.options());
-    }
-    auto mask = torch::empty({n}, pos.options().dtype(at::kLong));
-    float bg[3] = {0.f, 0.f, 0.f};
-    if (background)
-      for (int k = 0; k < 3; ++k) bg[k] = (float)(*background)[k];
-    gs_render_aux ax{background ? bg : nullptr, fpm(aux), final ? fpm(aux_fin) : nullptr};
-    gs_render_feat ft{(int)f, fp(feat), fpm(map), final ? fpm(map_fin) : nullptr};
-    check_rc(gs_render_forward_feat(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
-                                    scale_activation, &cam, fpm(raw), final ? fpm(fin) : nullptr,
-                                    mask.data_ptr<int64_t>(), &ax, &ft, cur_stream()),
-             "gs_render_forward_feat");
-    ++frame;
-    py::object none = py::none();
-    return py::make_tuple(final ? py::cast(fin) : none, raw, aux, final ? py::cast(aux_fin) : none, map,
-                          final ? py::cast(map_fin) : none, mask);
+    Outputs o = alloc_outputs(pos, 0, n, height, width, true, f, final);
+    gs_render_aux ax{bg.ptr(), fpm(o.aux), fpm_or_null(o.aux_fin)};
+    gs_render_feat ft{(int)f, fp(feat), fpm(o.map), fpm_or_null(o.map_fin)};
+    rendered(gs_render_forward_feat(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                    scale_activation, &cam, fpm(o.raw), fpm_or_null(o.fin),
+                                    o.mask.data_ptr<int64_t>(), &ax, &ft, cur_stream()),
+             fn);
+    return py::make_tuple(or_none(o.fin), o.raw, o.aux, or_none(o.aux_fin), o.map, or_none(o.map_fin), o.mask);
   }
 
   // backward of forward_feat; grad_map = None: the plain / aux backward kernels, g_feat zero-filled
@@ -704,44 +663,20 @@ struct RenderContext {
                           torch::Tensor map, std::optional<torch::Tensor> grad_map, torch::Tensor g_pos,
                           torch::Tensor g_rgb, torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale,
                           torch::Tensor g_feat, int64_t expected_frame) {
-    check_frame(expected_frame, "RenderContext.backward_feat_into");
-    GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
-    GS_CHECK_F32(feat); GS_CHECK_F32(raw); GS_CHECK_F32(aux); GS_CHECK_F32(map); GS_CHECK_F32(g_pos);
-    GS_CHECK_F32(g_rgb); GS_CHECK_F32(g_opa); GS_CHECK_F32(g_quat); GS_CHECK_F32(g_scale); GS_CHECK_F32(g_feat);
-    TORCH_CHECK(raw.dim() == 3 && raw.size(2) == 3 && aux.dim() == 3 && aux.size(0) == raw.size(0) &&
-                    aux.size(1) == raw.size(1) && aux.size(2) == 2 && map.dim() == 3 && map.size(0) == raw.size(0) &&
-                    map.size(1) == raw.size(1) && feat.dim() == 2 && map.size(2) == feat.size(1),
-                "RenderContext.backward_feat_into: raw must be [Hp,Wp,3], aux [Hp,Wp,2] and map [Hp,Wp,f]");
-    TORCH_CHECK(grad_image.is_cuda() && grad_image.scalar_type() == at::kFloat && grad_image.dim() == 3 &&
-                    grad_image.size(2) == 3 && (grad_is_final || grad_image.sizes() == raw.sizes()),
-                "RenderContext.backward_feat_into: grad_image must be [H,W,3] (final) or match raw");
-    if (grad_aux) {
-      TORCH_CHECK(grad_aux->is_cuda() && grad_aux->scalar_type() == at::kFloat && grad_aux->dim() == 3 &&
-                      grad_aux->size(0) == grad_image.size(0) && grad_aux->size(1) == grad_image.size(1) &&
-                      grad_aux->size(2) == 2,
-                  "RenderContext.backward_feat_into: grad_aux must be float32 [rows, cols, 2] like grad_image");
-    }
-    if (grad_map) {
-      TORCH_CHECK(grad_map->is_cuda() && grad_map->scalar_type() == at::kFloat && grad_map->dim() == 3 &&
-                      grad_map->size(0) == grad_image.size(0) && grad_map->size(1) == grad_image.size(1) &&
-                      grad_map->size(2) == feat.size(1),
-                  "RenderContext.backward_feat_into: grad_map must be float32 [rows, cols, f] like grad_image");
-    }
-    TORCH_CHECK(g_pos.numel() == pos.numel() && g_rgb.numel() == rgb.numel() && g_opa.numel() == opa.numel() &&
-                    g_quat.numel() == quat.numel() && g_scale.numel() == scale.numel() &&
-                    g_feat.numel() == feat.numel(),
-                "RenderContext.backward_feat_into: gradient buffers must match their parameters");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(g_quat.data_ptr()) % 16 == 0, "grad_quat must be 16-byte aligned");
+    const char* fn = "RenderContext.backward_feat_into";
+    check_backward(fn, expected_frame, false, grad_is_final, pos, rgb, opa, quat, scale, raw, grad_image, &aux,
+                   grad_aux ? &*grad_aux : nullptr, &feat, &map, grad_map ? &*grad_map : nullptr);
+    check_grads(fn, {pos, rgb, opa, quat, scale, feat}, {g_pos, g_rgb, g_opa, g_quat, g_scale, g_feat});
     c10::cuda::CUDAGuard guard(pos.device());
     auto gi = grad_image.contiguous();
     torch::Tensor ga, gm;
     if (grad_aux) ga = grad_aux->contiguous();
     if (grad_map) gm = grad_map->contiguous();
     check_rc(gs_render_backward_feat(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
-                                     grad_is_final ? 1 : 0, fp(aux), grad_aux ? fp(ga) : nullptr, fp(feat), fp(map),
-                                     grad_map ? fp(gm) : nullptr, fpm(g_pos), fpm(g_rgb), fpm(g_opa), fpm(g_quat),
-                                     fpm(g_scale), fpm(g_feat), cur_stream()),
-             "gs_render_backward_feat");
+                                     grad_is_final ? 1 : 0, fp(aux), fpm_or_null(ga), fp(feat), fp(map),
+                                     fpm_or_null(gm), fpm(g_pos), fpm(g_rgb), fpm(g_opa), fpm(g_quat), fpm(g_scale),
+                                     fpm(g_feat), cur_stream()),
+             fn);
   }
 
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }

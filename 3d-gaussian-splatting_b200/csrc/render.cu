@@ -242,6 +242,94 @@ static int ceil_log2(unsigned v) {
   return b;
 }
 
+// "who: what" as the last error
+static int gs_fail(int code, const char* who, const char* what) {
+  char msg[512];
+  snprintf(msg, sizeof(msg), "%s: %s", who, what);
+  return gs_set_error_msg(code, msg);
+}
+
+static int check_camera(const gs_camera& cam, const char* who) {
+  if (cam.width <= 0 || cam.height <= 0 || !(cam.focal_x > 0.f) || !(cam.focal_y > 0.f))
+    return gs_fail(GS_ERR_INVALID_ARG, who, "bad camera");
+  if (!(cam.tile_thresh > 0.f && cam.tile_thresh < 1.f))
+    return gs_fail(GS_ERR_INVALID_ARG, who, "tile_thresh must be in (0, 1)");
+  return 0;
+}
+
+// one view's padded size (splatter.py:259-260); the frame's tile grid stacks the n_views views' grids vertically
+static int frame_geom(const gs_camera& cam, int n_views, GsFrameGeom& g, const char* who) {
+  g = GsFrameGeom{};
+  g.width = cam.width;
+  g.height = cam.height;
+  g.wp = (cam.width + GS_TILE - 1) / GS_TILE * GS_TILE;
+  g.hp = (cam.height + GS_TILE - 1) / GS_TILE * GS_TILE;
+  g.ntx = g.wp / GS_TILE;
+  const int nty = g.hp / GS_TILE;
+  if (g.ntx > 65535 || (long long)nty * n_views > 65535)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "image too large (Wp / 16 and B Hp / 16 must not exceed 65535)");
+  g.nty = nty * n_views;
+  g.n_tiles = g.ntx * g.nty;
+  g.fx = cam.focal_x;
+  g.fy = cam.focal_y;
+  return 0;
+}
+
+// the caller's background and depth / alpha outputs; use_aux: the blend runs its aux variant
+static int parse_aux(const gs_render_aux* ax, const float* final_img, GsAuxOut& out, bool& use_aux, const char* who) {
+  out = GsAuxOut{};
+  use_aux = ax && (ax->background || ax->aux || ax->aux_final);
+  if (!use_aux) return 0;
+  if (ax->aux_final && !final_img) return gs_fail(GS_ERR_INVALID_ARG, who, "aux_final needs image_final");
+  if (ax->background) {
+    for (int k = 0; k < 3; ++k) {
+      if (!std::isfinite(ax->background[k])) return gs_fail(GS_ERR_INVALID_ARG, who, "background must be finite");
+      out.bg[k] = ax->background[k];
+    }
+  }
+  out.aux = ax->aux;
+  out.aux_final = ax->aux_final;
+  return 0;
+}
+
+// a forward is about to touch the context: until it completes, the context holds no frame to differentiate
+static int begin_forward(gs_ctx* c, const char* who) {
+  if (int rc = gs_check_device(c->device, who)) return rc;
+  g_cur_alloc = &c->allocator;
+  c->have_forward = false;
+  c->have_backward = false;
+  c->have_aux = false;
+  c->n_views = 0;
+  c->ev_fwd_valid = false;
+  return 0;
+}
+
+// what the backward of a completed forward needs; v: the constants of its (first) view
+static void commit_forward(gs_ctx* c, int n, int d, int scale_activation, long long m, const GsFrameGeom& g,
+                           const GsView& v, float near_plane, int n_views, bool sh_gaussian, bool gather, bool filt_on,
+                           const GsAuxOut& aux_out, const gs_render_feat* ft) {
+  c->ev_fwd_valid = c->timing && c->ev_ok;
+  c->have_forward = true;
+  c->have_aux = aux_out.aux != nullptr;
+  c->sh_gaussian = sh_gaussian;
+  c->feat_f = ft ? ft->f : 0;
+  c->feat = ft ? ft->feat : nullptr;
+  c->filt_on = filt_on;
+  c->filt = v.filt;
+  c->gather = gather;
+  c->n = n;
+  c->d = d;
+  c->scale_act = scale_activation;
+  c->m = m;
+  c->cam = v.cam;
+  c->grid = v.grid;
+  c->geom = g;
+  c->near_plane = near_plane;
+  c->half_w = v.half_w;
+  c->half_h = v.half_h;
+  c->n_views = n_views;
+}
+
 // The per-camera constants of a frame of padded size g.wp x g.hp, formed from host scalars in double then narrowed, like
 // the Python floats that the reference passes through pybind (splatter.py:279-282, :532-533).  The 2-D filter is in
 // normalised image-plane units: the variance over the squared pixel pitch 1 / f^2, rounded once (zero without one).
@@ -399,77 +487,45 @@ static int bin_frame(gs_ctx* c, int n, const GsFrameGeom& g, bool gather, int bl
   return 0;
 }
 
-static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
-                               const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
-                               float* image, float* final_img, int64_t* culling_mask, gs_stream_t stream,
-                               const gs_render_aux* ax = nullptr, const gs_render_feat* ft = nullptr) {
-  if (!c || !cam || n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad arguments");
+static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, const float* rgb, const float* opa,
+                               const float* quat, const float* scale, int n, int d, int scale_activation,
+                               const gs_camera* cam, float* image, float* final_img, int64_t* culling_mask,
+                               gs_stream_t stream, const gs_render_aux* ax = nullptr,
+                               const gs_render_feat* ft = nullptr) {
+  if (!c || !cam || n < 0) return gs_fail(GS_ERR_INVALID_ARG, who, "bad arguments");
   if (d != 3 && gs_sh_basis_count(d) == 0)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
-  if (cam->width <= 0 || cam->height <= 0 || !(cam->focal_x > 0.f) || !(cam->focal_y > 0.f))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: bad camera");
-  if (!(cam->tile_thresh > 0.f && cam->tile_thresh < 1.f))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: tile_thresh must be in (0, 1)");
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
+  if (int rc = check_camera(*cam, who)) return rc;
   if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: null tensor pointer");
+    return gs_fail(GS_ERR_INVALID_ARG, who, "null tensor pointer");
   // per-Gaussian SH: the projection writes an RGB colour, and everything that serves the blend runs as for d == 3;
   // only the projection kernels, the push bucket and the caller's tensors keep the parameter width d
   const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
   const int blend_d = sh_gaussian ? 3 : d;   // colour width of the blend
   const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
-  GsAuxOut aux_out{};
-  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
-  if (use_aux) {
-    if (ax->aux_final && !final_img)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: aux_final needs image_final");
-    if (ax->background) {
-      for (int k = 0; k < 3; ++k) {
-        if (!std::isfinite(ax->background[k]))
-          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_aux: background must be finite");
-        aux_out.bg[k] = ax->background[k];
-      }
-    }
-    aux_out.aux = ax->aux;
-    aux_out.aux_final = ax->aux_final;
-    // a forward that writes aux may be differentiated through it: its backward kernel must exist too
+  GsAuxOut aux_out;
+  bool use_aux;
+  if (int rc = parse_aux(ax, final_img, aux_out, use_aux, who)) return rc;
+  // a forward that writes aux may be differentiated through it: its backward kernel must exist too
+  if (use_aux)
     if (int rc = gs_blend_aux_supported(blend_d, true, ax->aux != nullptr)) return rc;
-  }
   const bool gather = gs_tuning().gather != 0;   // RGB and SH: no pack pass
   if (ft) {
-    if (!gs_feat_width_ok(ft->f)) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: f must be 8, 16 or 32");
-    if (!ft->map || (n > 0 && !ft->feat))
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat or map");
+    if (!gs_feat_width_ok(ft->f)) return gs_fail(GS_ERR_INVALID_ARG, who, "f must be 8, 16 or 32");
+    if (!ft->map || (n > 0 && !ft->feat)) return gs_fail(GS_ERR_INVALID_ARG, who, "null feat or map");
     if ((reinterpret_cast<uintptr_t>(ft->feat) | reinterpret_cast<uintptr_t>(ft->map) |
          reinterpret_cast<uintptr_t>(ft->map_final)) % 16)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: feat, map and map_final must be 16-byte aligned");
-    if (ft->map_final && !final_img)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: map_final needs image_final");
+      return gs_fail(GS_ERR_INVALID_ARG, who, "feat, map and map_final must be 16-byte aligned");
+    if (ft->map_final && !final_img) return gs_fail(GS_ERR_INVALID_ARG, who, "map_final needs image_final");
     if (blend_d != 3)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: SH colour evaluated per pixel has no feature "
-                                                  "kernel (use GS_SH_EVAL_GAUSSIAN)");
+      return gs_fail(GS_ERR_UNSUPPORTED, who, "SH colour evaluated per pixel has no feature kernel (use GS_SH_EVAL_GAUSSIAN)");
     if (!gather)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_feat: the packed path (gs_tune(\"gather\", 0)) has "
-                                                  "no feature kernel");
+      return gs_fail(GS_ERR_UNSUPPORTED, who, "the packed path (gs_tune(\"gather\", 0)) has no feature kernel");
   }
-  if (int rc = gs_check_device(c->device, "gs_render_forward")) return rc;
-  g_cur_alloc = &c->allocator;
+  if (int rc = begin_forward(c, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  c->have_forward = false;
-  c->have_backward = false;
-  c->have_aux = false;
-  c->n_views = 0;
-
-  GsFrameGeom g{};
-  g.width = cam->width;
-  g.height = cam->height;
-  g.wp = (cam->width + GS_TILE - 1) / GS_TILE * GS_TILE;     // splatter.py:259-260
-  g.hp = (cam->height + GS_TILE - 1) / GS_TILE * GS_TILE;
-  g.ntx = g.wp / GS_TILE;
-  g.nty = g.hp / GS_TILE;
-  g.n_tiles = g.ntx * g.nty;
-  g.fx = cam->focal_x;
-  g.fy = cam->focal_y;
-  if (g.ntx > 65535 || g.nty > 65535) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward: image too large");
+  GsFrameGeom g;
+  if (int rc = frame_geom(*cam, 1, g, who)) return rc;
 
   const GsView vw = view_constants(c, cam, g);
   const GsTileGrid& grid = vw.grid;
@@ -508,7 +564,6 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
     GS_CUDA_TRY(cudaMemcpyAsync(c->rays.p, c->host_rays, 48, cudaMemcpyHostToDevice, st));
   }
   // 1. projection + activations + tile rectangle
-  c->ev_fwd_valid = false;
   gs_mark(c, 0, st);
   GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
   GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
@@ -542,34 +597,15 @@ static int render_forward_impl(gs_ctx* c, const float* pos, const float* rgb, co
   }
   gs_count_launch();   // blend forward
   gs_mark(c, 6, st);
-  c->ev_fwd_valid = c->timing && c->ev_ok;
-
-  c->have_forward = true;
-  c->have_aux = aux_out.aux != nullptr;
-  c->sh_gaussian = sh_gaussian;
-  c->feat_f = ft ? ft->f : 0;
-  c->feat = ft ? ft->feat : nullptr;
-  c->filt_on = filt_on;
-  c->filt = filt;
-  c->gather = gather;
-  c->n = n;
-  c->d = d;
-  c->scale_act = scale_activation;
-  c->m = m;
-  c->cam = dc;
-  c->grid = grid;
-  c->geom = g;
-  c->near_plane = cam->near_plane;
-  c->half_w = half_w;
-  c->half_h = half_h;
+  commit_forward(c, n, d, scale_activation, m, g, vw, cam->near_plane, 0, sh_gaussian, gather, filt_on, aux_out, ft);
   return 0;
 }
 
 extern "C" int gs_render_forward(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
                                  const float* scale, int n, int d, int scale_activation, const gs_camera* cam,
                                  float* image, int64_t* culling_mask, gs_stream_t stream) {
-  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image, nullptr, culling_mask,
-                             stream);
+  return render_forward_impl(c, "gs_render_forward", pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image,
+                             nullptr, culling_mask, stream);
 }
 
 extern "C" int gs_render_forward_final(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
@@ -577,8 +613,8 @@ extern "C" int gs_render_forward_final(gs_ctx* c, const float* pos, const float*
                                        const gs_camera* cam, float* image_raw_padded, float* image_final,
                                        int64_t* culling_mask, gs_stream_t stream) {
   if (!image_final) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_final: null image_final");
-  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image_raw_padded, image_final,
-                             culling_mask, stream);
+  return render_forward_impl(c, "gs_render_forward_final", pos, rgb, opa, quat, scale, n, d, scale_activation, cam,
+                             image_raw_padded, image_final, culling_mask, stream);
 }
 
 // one u32 tag per gradient row: rows written by this backward carry `epoch`; the tails of
@@ -594,33 +630,32 @@ static int next_row_epoch(gs_ctx* c, size_t M, cudaStream_t st) {
   return 0;
 }
 
-static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, const float* opa, const float* quat,
-                                const float* scale, const float* image, const float* grad_image, int grad_is_final,
-                                float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
-                                float* grad_scale, gs_stream_t stream, const float* aux = nullptr,
-                                const float* grad_aux = nullptr, float* grad_cam = nullptr,
-                                const float* fmap = nullptr, const float* grad_map = nullptr,
-                                float* grad_feat = nullptr) {
-  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null ctx");
-  if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward: no forward on this ctx");
-  if (c->n_views)
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: the last forward was batched (use gs_render_backward_batch)");
+// The backward of the last forward, single-view or batched (batch: the caller is gs_render_backward_batch, which has
+// checked what only a batched frame needs).
+static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const float* pos, const float* rgb,
+                                const float* opa, const float* quat, const float* scale, const float* image,
+                                const float* grad_image, int grad_is_final, float* grad_pos, float* grad_rgb,
+                                float* grad_opa, float* grad_quat, float* grad_scale, gs_stream_t stream,
+                                const float* aux = nullptr, const float* grad_aux = nullptr,
+                                float* grad_cam = nullptr, const float* fmap = nullptr,
+                                const float* grad_map = nullptr, float* grad_feat = nullptr) {
+  if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
+  if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (c->n_views && !batch)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was batched (use gs_render_backward_batch)");
   // camera only (grad_cam, the five parameter gradients all NULL: the caller has checked the set is not mixed)
   const bool cam_only = grad_cam && !grad_pos;
   if (!image || !grad_image || (!cam_only && (!grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale)) ||
       (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: null tensor pointer");
+    return gs_fail(GS_ERR_INVALID_ARG, who, "null tensor pointer");
   if (grad_cam) {
     if (c->d != 3 && !c->sh_gaussian)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_cam: SH colour evaluated per pixel has no camera "
-                                                  "gradient (use GS_SH_EVAL_GAUSSIAN)");
-    if (c->push.world)
-      return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_cam: not available with a gradient push configured");
+      return gs_fail(GS_ERR_UNSUPPORTED, who, "SH colour evaluated per pixel has no camera gradient (use GS_SH_EVAL_GAUSSIAN)");
+    if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
   }
   if (grad_aux) {
-    if (!c->have_aux)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux given but the forward wrote no aux");
-    if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_aux: grad_aux needs the forward's aux");
+    if (!c->have_aux) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_aux given but the forward wrote no aux");
+    if (!aux) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_aux needs the forward's aux");
     if (int rc = gs_blend_aux_supported(c->sh_gaussian ? 3 : c->d, false, true)) return rc;
   }
   const int d = c->d;
@@ -629,12 +664,11 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   const bool stats = c->stats_on && !cam_only;
   const bool absgrad = stats && c->stats.absgrad;
   if (stats) {
-    if (c->stats.n != c->n)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: the densify statistics are sized for another n");
+    if (c->stats.n != c->n) return gs_fail(GS_ERR_INVALID_ARG, who, "the densify statistics are sized for another n");
     if (absgrad)
       if (int rc = gs_blend_absgrad_supported(blend_d, c->gather)) return rc;
   }
-  if (int rc = gs_check_device(c->device, "gs_render_backward")) return rc;
+  if (int rc = gs_check_device(c->device, who)) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
   size_t M = (size_t)c->m;
@@ -646,7 +680,12 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
   GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
   gs_mark(c, 7, st);
   if (c->m > 0) {
-    if (grad_map) {
+    if (c->n_views) {
+      GS_CUDA_TRY(gs_launch_blend_bwd_batch(c->rec.as<GsRec>(), c->vals_out.as<uint32_t>(), c->offsets_g.as<uint32_t>(),
+                                            c->tile_accum.as<int>(), c->geom, c->views.as<GsView>(), image, grad_image,
+                                            c->grad_inst.as<float>(), grad_is_final, crop, c->row_epoch.as<uint32_t>(),
+                                            c->epoch, c->tile_neff_b.as<int>(), st, aux, grad_aux, absgrad));
+    } else if (grad_map) {
       GS_CUDA_TRY(gs_launch_blend_feat_bwd(c->rec.as<GsRec>(), c->feat, c->feat_f, c->vals_out.as<uint32_t>(),
                                            c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, image,
                                            grad_image, fmap, grad_map, c->grad_inst.as<float>(),
@@ -684,9 +723,8 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
     const size_t len[5] = {3 * nn, (size_t)d * nn, nn, 4 * nn, 3 * nn};
     for (int k = 0; k < 5; ++k)
       if (seg[k] < lo || seg[k] + len[k] > hi)
-        return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: gradient buffers are not inside the push bucket");
-    if ((grad_quat - lo) % 4)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward: grad_quat must sit on a 16-byte bucket offset");
+        return gs_fail(GS_ERR_INVALID_ARG, who, "gradient buffers are not inside the push bucket");
+    if ((grad_quat - lo) % 4) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_quat must sit on a 16-byte bucket offset");
   }
   if (grad_cam) {
     GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
@@ -697,6 +735,16 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
                                                 grad_quat, grad_scale, c->cam_part.as<float>(), grad_cam, st,
                                                 grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sum (always: grad_cam is always written)
+  } else if (c->n_views > 1) {
+    // B views: the batched kernels, which take each Gaussian's views in order.  One view: the pairs are the Gaussians,
+    // so the single-view kernels run (the gradients are theirs bit for bit, and they are the faster kernels for one view)
+    GS_CUDA_TRY(gs_launch_fused_project_bwd_batch(pos, rgb, opa, quat, scale, c->n, c->n_views, d, c->scale_act,
+                                                  c->views.as<GsView>(), c->near_plane, c->offsets_g.as<uint32_t>(),
+                                                  c->count.as<uint32_t>(), c->grad_inst.as<float>(),
+                                                  c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
+                                                  grad_quat, grad_scale, st, grad_aux != nullptr, c->sh_gaussian,
+                                                  c->filt_on));
+    if (c->n > 0) gs_count_launch();
   } else {
     GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
                                             c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
@@ -711,10 +759,16 @@ static int render_backward_impl(gs_ctx* c, const float* pos, const float* rgb, c
     if (c->n > 0) gs_count_launch();
   }
   if (stats) {
-    GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
-                                        c->half_h, c->filt_on ? c->filt : GsFilter2d{}, c->offsets_g.as<uint32_t>(),
-                                        c->count.as<uint32_t>(), c->grad_inst.as<float>(), (int)(grow / 4),
-                                        c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st));
+    if (c->n_views > 1)
+      GS_CUDA_TRY(gs_launch_densify_stats_batch(pos, quat, scale, c->n, c->n_views, c->scale_act, c->views.as<GsView>(),
+                                                c->near_plane, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                                c->grad_inst.as<float>(), (int)(grow / 4), c->row_epoch.as<uint32_t>(),
+                                                c->epoch, c->geom, c->stats, st));
+    else
+      GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
+                                          c->half_h, c->filt_on ? c->filt : GsFilter2d{}, c->offsets_g.as<uint32_t>(),
+                                          c->count.as<uint32_t>(), c->grad_inst.as<float>(), (int)(grow / 4),
+                                          c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st));
     if (c->n > 0) gs_count_launch();
   }
   gs_mark(c, 9, st);
@@ -726,24 +780,24 @@ extern "C" int gs_render_backward(gs_ctx* c, const float* pos, const float* rgb,
                                   const float* scale, const float* image, const float* grad_image, float* grad_pos,
                                   float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
                                   gs_stream_t stream) {
-  return render_backward_impl(c, pos, rgb, opa, quat, scale, image, grad_image, 0, grad_pos, grad_rgb, grad_opa,
-                              grad_quat, grad_scale, stream);
+  return render_backward_impl(c, "gs_render_backward", false, pos, rgb, opa, quat, scale, image, grad_image, 0,
+                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream);
 }
 
 extern "C" int gs_render_backward_final(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
                                         const float* quat, const float* scale, const float* image_raw_padded,
                                         const float* grad_final, float* grad_pos, float* grad_rgb, float* grad_opa,
                                         float* grad_quat, float* grad_scale, gs_stream_t stream) {
-  return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_final, 1, grad_pos, grad_rgb,
-                              grad_opa, grad_quat, grad_scale, stream);
+  return render_backward_impl(c, "gs_render_backward_final", false, pos, rgb, opa, quat, scale, image_raw_padded,
+                              grad_final, 1, grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream);
 }
 
 extern "C" int gs_render_forward_aux(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
                                      const float* quat, const float* scale, int n, int d, int scale_activation,
                                      const gs_camera* cam, float* image_raw_padded, float* image_final,
                                      int64_t* culling_mask, const gs_render_aux* aux, gs_stream_t stream) {
-  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image_raw_padded, image_final,
-                             culling_mask, stream, aux);
+  return render_forward_impl(c, "gs_render_forward_aux", pos, rgb, opa, quat, scale, n, d, scale_activation, cam,
+                             image_raw_padded, image_final, culling_mask, stream, aux);
 }
 
 extern "C" int gs_render_backward_aux(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
@@ -751,8 +805,9 @@ extern "C" int gs_render_backward_aux(gs_ctx* c, const float* pos, const float* 
                                       const float* grad_image, int grad_is_final, const float* aux,
                                       const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
                                       float* grad_quat, float* grad_scale, gs_stream_t stream) {
-  return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
-                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux);
+  return render_backward_impl(c, "gs_render_backward_aux", false, pos, rgb, opa, quat, scale, image_raw_padded,
+                              grad_image, grad_is_final ? 1 : 0, grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
+                              stream, aux, grad_aux);
 }
 
 extern "C" int gs_render_backward_cam(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
@@ -766,8 +821,9 @@ extern "C" int gs_render_backward_cam(gs_ctx* c, const float* pos, const float* 
     return gs_set_error_msg(GS_ERR_INVALID_ARG,
                             "gs_render_backward_cam: the five parameter gradients must be all NULL or all non-NULL");
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_cam: null ctx");
-  return render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
-                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, grad_cam);
+  return render_backward_impl(c, "gs_render_backward_cam", false, pos, rgb, opa, quat, scale, image_raw_padded,
+                              grad_image, grad_is_final ? 1 : 0, grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
+                              stream, aux, grad_aux, grad_cam);
 }
 
 extern "C" int gs_render_forward_feat(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
@@ -776,8 +832,8 @@ extern "C" int gs_render_forward_feat(gs_ctx* c, const float* pos, const float* 
                                       int64_t* culling_mask, const gs_render_aux* aux, const gs_render_feat* feat,
                                       gs_stream_t stream) {
   if (!feat) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_feat: null feat");
-  return render_forward_impl(c, pos, rgb, opa, quat, scale, n, d, scale_activation, cam, image_raw_padded, image_final,
-                             culling_mask, stream, aux, feat);
+  return render_forward_impl(c, "gs_render_forward_feat", pos, rgb, opa, quat, scale, n, d, scale_activation, cam,
+                             image_raw_padded, image_final, culling_mask, stream, aux, feat);
 }
 
 extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
@@ -808,9 +864,9 @@ extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float*
                                                   "bucket; not available with a gradient push configured");
   }
   const int f = c->feat_f, n = c->n;
-  int rc = render_backward_impl(c, pos, rgb, opa, quat, scale, image_raw_padded, grad_image, grad_is_final ? 1 : 0,
-                                grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, nullptr,
-                                map, grad_map, grad_feat);
+  int rc = render_backward_impl(c, "gs_render_backward_feat", false, pos, rgb, opa, quat, scale, image_raw_padded,
+                                grad_image, grad_is_final ? 1 : 0, grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
+                                stream, aux, grad_aux, nullptr, map, grad_map, grad_feat);
   if (rc || grad_map || n == 0) return rc;
   GS_CUDA_TRY(cudaMemsetAsync(grad_feat, 0, (size_t)n * f * sizeof(float), (cudaStream_t)stream));
   return 0;
@@ -821,71 +877,35 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
                                        const float* quat, const float* scale, int n, int d, int scale_activation,
                                        int n_views, const gs_camera* cams, float* image, float* final_img,
                                        int64_t* culling_mask, const gs_render_aux* ax, gs_stream_t stream) {
-  if (!c || !cams) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: null ctx or cams");
-  if (n_views < 1 || n_views > GS_MAX_VIEWS)
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: n_views must be in 1 .. GS_MAX_VIEWS");
-  if (n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: n < 0");
+  const char* who = "gs_render_forward_batch";
+  if (!c || !cams) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx or cams");
+  if (n_views < 1 || n_views > GS_MAX_VIEWS) return gs_fail(GS_ERR_INVALID_ARG, who, "n_views must be in 1 .. GS_MAX_VIEWS");
+  if (n < 0) return gs_fail(GS_ERR_INVALID_ARG, who, "n < 0");
   if (d != 3 && gs_sh_basis_count(d) == 0)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
   const gs_camera& c0 = cams[0];
   for (int v = 0; v < n_views; ++v) {
     const gs_camera& cv = cams[v];
-    if (cv.width <= 0 || cv.height <= 0 || !(cv.focal_x > 0.f) || !(cv.focal_y > 0.f))
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: bad camera");
-    if (!(cv.tile_thresh > 0.f && cv.tile_thresh < 1.f))
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: tile_thresh must be in (0, 1)");
+    if (int rc = check_camera(cv, who)) return rc;
     if (cv.width != c0.width || cv.height != c0.height || !(cv.near_plane == c0.near_plane) ||
         !(cv.tile_thresh == c0.tile_thresh))
-      return gs_set_error_msg(GS_ERR_INVALID_ARG,
-                              "gs_render_forward_batch: the views must share width, height, near_plane and tile_thresh");
+      return gs_fail(GS_ERR_INVALID_ARG, who, "the views must share width, height, near_plane and tile_thresh");
   }
-  // one view's padded size; the frame's tile grid stacks the views' grids vertically
-  GsFrameGeom g{};
-  g.width = c0.width;
-  g.height = c0.height;
-  g.wp = (c0.width + GS_TILE - 1) / GS_TILE * GS_TILE;
-  g.hp = (c0.height + GS_TILE - 1) / GS_TILE * GS_TILE;
-  g.ntx = g.wp / GS_TILE;
-  const int nty = g.hp / GS_TILE;
-  if (g.ntx > 65535 || (long long)nty * n_views > 65535)
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: image too large for the batch (B Hp / 16 > 65535)");
-  if ((long long)n * n_views >= (1ll << 31))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: B n must be < 2^31");
-  g.nty = nty * n_views;
-  g.n_tiles = g.ntx * g.nty;
-  g.fx = c0.focal_x;
-  g.fy = c0.focal_y;
+  GsFrameGeom g;
+  if (int rc = frame_geom(c0, n_views, g, who)) return rc;
+  if ((long long)n * n_views >= (1ll << 31)) return gs_fail(GS_ERR_INVALID_ARG, who, "B n must be < 2^31");
   if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: null tensor pointer");
+    return gs_fail(GS_ERR_INVALID_ARG, who, "null tensor pointer");
   const bool sh_gaussian = d != 3 && c->sh_eval == GS_SH_EVAL_GAUSSIAN;
   if (d != 3 && !sh_gaussian)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: SH colour evaluated per pixel has no batched "
-                                                "kernel (use GS_SH_EVAL_GAUSSIAN)");
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "SH colour evaluated per pixel has no batched kernel (use GS_SH_EVAL_GAUSSIAN)");
   if (int rc = gs_blend_batch_supported()) return rc;
-  if (c->push.world)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_forward_batch: not available with a gradient push configured");
-  GsAuxOut aux_out{};
-  const bool use_aux = ax && (ax->background || ax->aux || ax->aux_final);
-  if (use_aux) {
-    if (ax->aux_final && !final_img)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: aux_final needs image_final");
-    if (ax->background) {
-      for (int k = 0; k < 3; ++k) {
-        if (!std::isfinite(ax->background[k]))
-          return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_batch: background must be finite");
-        aux_out.bg[k] = ax->background[k];
-      }
-    }
-    aux_out.aux = ax->aux;
-    aux_out.aux_final = ax->aux_final;
-  }
-  if (int rc = gs_check_device(c->device, "gs_render_forward_batch")) return rc;
-  g_cur_alloc = &c->allocator;
+  if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
+  GsAuxOut aux_out;
+  bool use_aux;
+  if (int rc = parse_aux(ax, final_img, aux_out, use_aux, who)) return rc;
+  if (int rc = begin_forward(c, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  c->have_forward = false;
-  c->have_backward = false;
-  c->have_aux = false;
-  c->n_views = 0;
 
   const int nb = n * n_views;   // (view, Gaussian) pairs
   if (int rc = reserve_frame(c, (size_t)nb, g.n_tiles, st)) return rc;
@@ -897,7 +917,6 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   GS_CUDA_TRY(cudaEventRecord(c->ev_views, st));
   const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
 
-  c->ev_fwd_valid = false;
   gs_mark(c, 0, st);
   GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
   GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + nb, 0, 4, st));
@@ -915,28 +934,9 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
                                         use_aux ? &aux_out : nullptr));
   gs_count_launch();   // blend forward
   gs_mark(c, 6, st);
-  c->ev_fwd_valid = c->timing && c->ev_ok;
-
-  c->have_forward = true;
-  c->have_aux = aux_out.aux != nullptr;
-  c->sh_gaussian = sh_gaussian;
-  c->feat_f = 0;
-  c->feat = nullptr;
-  c->filt_on = filt_on;
-  c->gather = true;
   // view 0's constants: a one-view batch is differentiated by the single-view projection backward
-  c->cam = c->host_views[0].cam;
-  c->grid = c->host_views[0].grid;
-  c->filt = c->host_views[0].filt;
-  c->half_w = c->host_views[0].half_w;
-  c->half_h = c->host_views[0].half_h;
-  c->n = n;
-  c->d = d;
-  c->scale_act = scale_activation;
-  c->m = m;
-  c->geom = g;
-  c->near_plane = c0.near_plane;
-  c->n_views = n_views;
+  commit_forward(c, n, d, scale_activation, m, g, c->host_views[0], c0.near_plane, n_views, sh_gaussian, true, filt_on,
+                 aux_out, nullptr);
   return 0;
 }
 
@@ -945,79 +945,14 @@ extern "C" int gs_render_backward_batch(gs_ctx* c, const float* pos, const float
                                         const float* grad_image, int grad_is_final, const float* aux,
                                         const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
                                         float* grad_quat, float* grad_scale, gs_stream_t stream) {
-  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: null ctx");
-  if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward_batch: no forward on this ctx");
-  if (!c->n_views)
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: the last forward was not batched");
-  if (!image || !grad_image || !grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale ||
-      (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: null tensor pointer");
-  if (grad_aux) {
-    if (!c->have_aux)
-      return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: grad_aux given but the forward wrote no aux");
-    if (!aux) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: grad_aux needs the forward's aux");
-  }
-  if (c->push.world)
-    return gs_set_error_msg(GS_ERR_UNSUPPORTED, "gs_render_backward_batch: not available with a gradient push configured");
+  const char* who = "gs_render_backward_batch";
+  if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
+  if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (!c->n_views) return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was not batched");
+  if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
   if (int rc = gs_blend_batch_supported()) return rc;
-  const bool stats = c->stats_on;
-  if (stats && c->stats.n != c->n)
-    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_batch: the densify statistics are sized for another n");
-  if (int rc = gs_check_device(c->device, "gs_render_backward_batch")) return rc;
-  g_cur_alloc = &c->allocator;
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t M = (size_t)c->m;
-  GS_CUDA_TRY(c->grad_inst.reserve(M * GS_GREC * 4 + 16, st));
-  if (int rc = next_row_epoch(c, M, st)) return rc;
-  c->ev_bwd_valid = false;
-  const GsFrameGeom& g = c->geom;
-  const GsView* views = c->views.as<GsView>();
-  GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
-  gs_mark(c, 7, st);
-  if (c->m > 0) {
-    GS_CUDA_TRY(gs_launch_blend_bwd_batch(c->rec.as<GsRec>(), c->vals_out.as<uint32_t>(), c->offsets_g.as<uint32_t>(),
-                                          c->tile_accum.as<int>(), g, views, image, grad_image,
-                                          c->grad_inst.as<float>(), grad_is_final ? 1 : 0, crop,
-                                          c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), st, aux,
-                                          grad_aux, stats && c->stats.absgrad));
-    gs_count_launch();
-    c->have_backward = true;
-  }
-  gs_mark(c, 8, st);
-  // One view: the pairs are the Gaussians and the frame is a single-view frame from here on, so the single-view
-  // projection backward and statistics kernels run (the gradients are theirs bit for bit, and they are the faster
-  // kernels for one view); B views: the batched kernels, which take each Gaussian's views in order.
-  const bool one = c->n_views == 1;
-  if (one)
-    GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, c->d, c->scale_act, c->cam, c->near_plane,
-                                            c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
-                                            c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch, grad_pos,
-                                            grad_rgb, grad_opa, grad_quat, grad_scale, GsGradPush{}, st,
-                                            grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
-  else
-    GS_CUDA_TRY(gs_launch_fused_project_bwd_batch(pos, rgb, opa, quat, scale, c->n, c->n_views, c->d, c->scale_act,
-                                                  views, c->near_plane, c->offsets_g.as<uint32_t>(),
-                                                  c->count.as<uint32_t>(), c->grad_inst.as<float>(),
-                                                  c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
-                                                  grad_quat, grad_scale, st, grad_aux != nullptr, c->sh_gaussian,
-                                                  c->filt_on));
-  if (c->n > 0) gs_count_launch();
-  if (stats) {
-    if (one)
-      GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
-                                          c->half_h, c->filt, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
-                                          c->grad_inst.as<float>(), GS_GREC, c->row_epoch.as<uint32_t>(), c->epoch, g,
-                                          c->stats, st));
-    else
-      GS_CUDA_TRY(gs_launch_densify_stats_batch(pos, quat, scale, c->n, c->n_views, c->scale_act, views,
-                                                c->near_plane, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
-                                                c->grad_inst.as<float>(), GS_GREC, c->row_epoch.as<uint32_t>(),
-                                                c->epoch, g, c->stats, st));
-    if (c->n > 0) gs_count_launch();
-  }
-  gs_mark(c, 9, st);
-  c->ev_bwd_valid = c->timing && c->ev_ok;
-  return 0;
+  return render_backward_impl(c, who, true, pos, rgb, opa, quat, scale, image, grad_image, grad_is_final ? 1 : 0,
+                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux);
 }
 
 extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {
@@ -1174,10 +1109,11 @@ extern "C" int gs_render_forward_backward_host(gs_ctx* c, const float* pos, cons
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_backward_host: null argument");
   if (cam->width <= 0 || cam->height <= 0)
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_forward_backward_host: bad camera");
+  GsFrameGeom g;
+  if (int rc = frame_geom(*cam, 1, g, "gs_render_forward_backward_host")) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_cur_alloc = &c->allocator;
-  int wp = (cam->width + GS_TILE - 1) / GS_TILE * GS_TILE, hp = (cam->height + GS_TILE - 1) / GS_TILE * GS_TILE;
-  size_t img_bytes = (size_t)wp * hp * 3 * sizeof(float);
+  size_t img_bytes = (size_t)g.wp * g.hp * 3 * sizeof(float);
   DevBuf& img_dev = c->img_dev;
   DevBuf& gimg_dev = c->gimg_dev;
   GS_CUDA_TRY(img_dev.reserve(img_bytes, st));

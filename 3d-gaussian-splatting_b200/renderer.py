@@ -195,6 +195,47 @@ def _apply_push(rctx, push):
         rctx.set_grad_push(*push)
 
 
+def _params(*tensors):
+    """The frame's inputs as the contiguous float32 tensors the kernels read."""
+    return tuple(_f32(t.detach()) for t in tensors)
+
+
+def _save_frame(ctx, rctx, mask, saved, final=None, map_shape=None):
+    """Keep what the backward of the frame `rctx` has just rendered needs: the context, the frame's id and `saved`.
+    Frames with depth / alpha maps also keep `final` and the [(B,) rows, cols] of the maps they return, and let
+    autograd pass None for outputs that got no gradient."""
+    ctx.rctx = rctx
+    ctx.frame = rctx.frame_id()
+    ctx.save_for_backward(*saved)
+    ctx.mark_non_differentiable(mask)
+    if final is not None:
+        ctx.final = bool(final)
+        ctx.map_shape = tuple(map_shape)
+        ctx.set_materialize_grads(False)
+
+
+def _param_grads(rctx, params):
+    """The five parameter gradient buffers of a backward, with its gradient push (or none) set on `rctx`."""
+    outs, push = _flat_grads(params)
+    _apply_push(rctx, push)
+    return outs
+
+
+def _upstream(raw, shape, grad_image, grad_depth, grad_alpha):
+    """(grad_image [*shape, 3], grad_aux [*shape, 2]) from the gradients autograd passed (None: no gradient).  grad_aux
+    is None when neither map got one, so the backward runs the plain kernels."""
+    if grad_image is None:
+        grad_image = raw.new_zeros(*shape, 3)
+    grad_aux = None
+    if grad_depth is not None or grad_alpha is not None:
+        grad_aux = raw.new_zeros(*shape, 2)
+        if grad_depth is not None:
+            grad_aux[..., 0] = grad_depth
+        if grad_alpha is not None:
+            grad_aux[..., 1] = grad_alpha
+    return _f32(grad_image), grad_aux
+
+
 class _RenderFrame(torch.autograd.Function):
     """raw parameters -> padded un-clamped image, replacing splatter.py:513-634's glue.
 
@@ -205,23 +246,19 @@ class _RenderFrame(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
                 near, tile_thresh, scale_activation):
-        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
-        image, mask = rctx.forward(pos, rgb, opa, quat, scale, int(width), int(height), float(focal_x),
-                                   float(focal_y), rot.detach().cpu(), tran.detach().cpu(), float(near),
-                                   float(tile_thresh), SCALE_ACTIVATIONS[scale_activation])
-        ctx.rctx = rctx
-        ctx.frame = rctx.frame_id()
-        ctx.save_for_backward(pos, rgb, opa, quat, scale, image)
-        ctx.mark_non_differentiable(mask)
+        params = _params(pos, rgb, opa, quat, scale)
+        image, mask = rctx.forward(*params, int(width), int(height), float(focal_x), float(focal_y),
+                                   rot.detach().cpu(), tran.detach().cpu(), float(near), float(tile_thresh),
+                                   SCALE_ACTIVATIONS[scale_activation])
+        _save_frame(ctx, rctx, mask, params + (image,))
         return image, mask
 
     @staticmethod
     def backward(ctx, grad_image, _grad_mask):
-        pos, rgb, opa, quat, scale, image = ctx.saved_tensors
-        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
-        _apply_push(ctx.rctx, push)
-        ctx.rctx.backward_into(pos, rgb, opa, quat, scale, image, _f32(grad_image), *outs, ctx.frame)
-        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 9
+        *params, image = ctx.saved_tensors
+        outs = _param_grads(ctx.rctx, params)
+        ctx.rctx.backward_into(*params, image, _f32(grad_image), *outs, ctx.frame)
+        return (None, *outs) + (None,) * 9
 
 
 render_frame = _RenderFrame.apply
@@ -235,23 +272,19 @@ class _RenderFrameFinal(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
                 near, tile_thresh, scale_activation):
-        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
-        final, raw, mask = rctx.forward_final(pos, rgb, opa, quat, scale, int(width), int(height), float(focal_x),
-                                              float(focal_y), rot.detach().cpu(), tran.detach().cpu(), float(near),
+        params = _params(pos, rgb, opa, quat, scale)
+        final, raw, mask = rctx.forward_final(*params, int(width), int(height), float(focal_x), float(focal_y),
+                                              rot.detach().cpu(), tran.detach().cpu(), float(near),
                                               float(tile_thresh), SCALE_ACTIVATIONS[scale_activation])
-        ctx.rctx = rctx
-        ctx.frame = rctx.frame_id()
-        ctx.save_for_backward(pos, rgb, opa, quat, scale, raw)
-        ctx.mark_non_differentiable(mask)
+        _save_frame(ctx, rctx, mask, params + (raw,))
         return final, mask
 
     @staticmethod
     def backward(ctx, grad_final, _grad_mask):
-        pos, rgb, opa, quat, scale, raw = ctx.saved_tensors
-        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
-        _apply_push(ctx.rctx, push)
-        ctx.rctx.backward_final_into(pos, rgb, opa, quat, scale, raw, _f32(grad_final), *outs, ctx.frame)
-        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 9
+        *params, raw = ctx.saved_tensors
+        outs = _param_grads(ctx.rctx, params)
+        ctx.rctx.backward_final_into(*params, raw, _f32(grad_final), *outs, ctx.frame)
+        return (None, *outs) + (None,) * 9
 
 
 render_frame_final = _RenderFrameFinal.apply
@@ -266,40 +299,39 @@ class _RenderFrameAux(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
                 near, tile_thresh, scale_activation, background, final):
-        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
+        params = _params(pos, rgb, opa, quat, scale)
         bg = None if background is None else [float(v) for v in background]
         fin, raw, aux, aux_fin, mask = rctx.forward_aux(
-            pos, rgb, opa, quat, scale, int(width), int(height), float(focal_x), float(focal_y), rot.detach().cpu(),
+            *params, int(width), int(height), float(focal_x), float(focal_y), rot.detach().cpu(),
             tran.detach().cpu(), float(near), float(tile_thresh), SCALE_ACTIVATIONS[scale_activation], bg,
             bool(final))
-        ctx.rctx = rctx
-        ctx.frame = rctx.frame_id()
-        ctx.final = bool(final)
-        ctx.save_for_backward(pos, rgb, opa, quat, scale, raw, aux)
-        ctx.mark_non_differentiable(mask)
-        ctx.set_materialize_grads(False)
         image, maps = (fin, aux_fin) if final else (raw, aux)
-        ctx.map_shape = tuple(maps.shape[:2])
+        _save_frame(ctx, rctx, mask, params + (raw, aux), final, maps.shape[:2])
         return image, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
 
     @staticmethod
     def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
-        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
-        rows, cols = ctx.map_shape
-        if grad_image is None:
-            grad_image = raw.new_zeros(rows, cols, 3)
-        grad_aux = None
-        if grad_depth is not None or grad_alpha is not None:
-            grad_aux = raw.new_zeros(rows, cols, 2)
-            if grad_depth is not None:
-                grad_aux[..., 0] = grad_depth
-            if grad_alpha is not None:
-                grad_aux[..., 1] = grad_alpha
-        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
-        _apply_push(ctx.rctx, push)
-        ctx.rctx.backward_aux_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
-                                   *outs, ctx.frame)
-        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 11
+        outs, _ = _RenderFrameAux.backward_with(ctx, grad_image, grad_depth, grad_alpha, cam=False)
+        return (None, *outs) + (None,) * 11
+
+    @staticmethod
+    def backward_with(ctx, grad_image, grad_depth, grad_alpha, cam):
+        """-> (the five parameter gradients, grad_cam[12] or None).  cam: through backward_cam_into, camera only
+        (parameter gradients None) when none of the five parameters needs a gradient."""
+        *params, raw, aux = ctx.saved_tensors
+        grad_image, grad_aux = _upstream(raw, ctx.map_shape, grad_image, grad_depth, grad_alpha)
+        if cam and not any(ctx.needs_input_grad[1:6]):          # tracking: the scene is frozen, camera only
+            outs = [None] * 5
+            _apply_push(ctx.rctx, None)
+        else:
+            outs = _param_grads(ctx.rctx, params)
+        args = (*params, raw, grad_image, ctx.final, aux, grad_aux, *outs)
+        if not cam:
+            ctx.rctx.backward_aux_into(*args, ctx.frame)
+            return outs, None
+        grad_cam = raw.new_empty(12)
+        ctx.rctx.backward_cam_into(*args, grad_cam, ctx.frame)
+        return outs, grad_cam
 
 
 def render_frame_aux(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
@@ -323,38 +355,22 @@ class _RenderFrameBatch(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal, rot, tran, near, tile_thresh,
                 scale_activation, background, final):
-        pos, rgb, opa, quat, scale = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale))
+        params = _params(pos, rgb, opa, quat, scale)
         bg = None if background is None else [float(v) for v in background]
         fin, raw, aux, aux_fin, mask = rctx.forward_batch(
-            pos, rgb, opa, quat, scale, int(width), int(height), focal, rot, tran, float(near), float(tile_thresh),
+            *params, int(width), int(height), focal, rot, tran, float(near), float(tile_thresh),
             SCALE_ACTIVATIONS[scale_activation], bg, bool(final))
-        ctx.rctx = rctx
-        ctx.frame = rctx.frame_id()
-        ctx.final = bool(final)
-        ctx.save_for_backward(pos, rgb, opa, quat, scale, raw, aux)
-        ctx.mark_non_differentiable(mask)
-        ctx.set_materialize_grads(False)
         image, maps = (fin, aux_fin) if final else (raw, aux)
-        ctx.map_shape = tuple(maps.shape[:3])
+        _save_frame(ctx, rctx, mask, params + (raw, aux), final, maps.shape[:3])
         return image, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
 
     @staticmethod
     def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
-        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
-        shape = ctx.map_shape
-        if grad_image is None:
-            grad_image = raw.new_zeros(*shape, 3)
-        grad_aux = None
-        if grad_depth is not None or grad_alpha is not None:
-            grad_aux = raw.new_zeros(*shape, 2)
-            if grad_depth is not None:
-                grad_aux[..., 0] = grad_depth
-            if grad_alpha is not None:
-                grad_aux[..., 1] = grad_alpha
-        outs, _ = _flat_grads((pos, rgb, opa, quat, scale))
-        ctx.rctx.backward_batch_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
-                                     *outs, ctx.frame)
-        return (None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 10
+        *params, raw, aux = ctx.saved_tensors
+        grad_image, grad_aux = _upstream(raw, ctx.map_shape, grad_image, grad_depth, grad_alpha)
+        outs, _ = _flat_grads(params)
+        ctx.rctx.backward_batch_into(*params, raw, grad_image, ctx.final, aux, grad_aux, *outs, ctx.frame)
+        return (None, *outs) + (None,) * 10
 
 
 def render_frame_batch(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
@@ -397,29 +413,10 @@ class _RenderFrameCam(_RenderFrameAux):
 
     @staticmethod
     def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
-        pos, rgb, opa, quat, scale, raw, aux = ctx.saved_tensors
         if not (ctx.needs_input_grad[10] or ctx.needs_input_grad[11]):
             return _RenderFrameAux.backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask)
-        rows, cols = ctx.map_shape
-        if grad_image is None:
-            grad_image = raw.new_zeros(rows, cols, 3)
-        grad_aux = None
-        if grad_depth is not None or grad_alpha is not None:
-            grad_aux = raw.new_zeros(rows, cols, 2)
-            if grad_depth is not None:
-                grad_aux[..., 0] = grad_depth
-            if grad_alpha is not None:
-                grad_aux[..., 1] = grad_alpha
-        grad_cam = raw.new_empty(12)
-        if any(ctx.needs_input_grad[1:6]):
-            outs, push = _flat_grads((pos, rgb, opa, quat, scale))
-        else:                                                  # tracking: the scene is frozen, camera only
-            outs, push = [None] * 5, None
-        _apply_push(ctx.rctx, push)
-        ctx.rctx.backward_cam_into(pos, rgb, opa, quat, scale, raw, _f32(grad_image), ctx.final, aux, grad_aux,
-                                   *outs, grad_cam, ctx.frame)
-        return ((None, outs[0], outs[1], outs[2], outs[3], outs[4]) + (None,) * 4 +
-                (grad_cam[:9].view(3, 3), grad_cam[9:]) + (None,) * 5)
+        outs, grad_cam = _RenderFrameAux.backward_with(ctx, grad_image, grad_depth, grad_alpha, cam=True)
+        return (None, *outs) + (None,) * 4 + (grad_cam[:9].view(3, 3), grad_cam[9:]) + (None,) * 5
 
 
 def render_frame_cam(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
@@ -450,45 +447,28 @@ class _RenderFrameFeat(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rctx, pos, rgb, opa, quat, scale, feat, width, height, focal_x, focal_y, rot, tran,
                 near, tile_thresh, scale_activation, background, final):
-        pos, rgb, opa, quat, scale, feat = (_f32(t.detach()) for t in (pos, rgb, opa, quat, scale, feat))
+        *params, feat = _params(pos, rgb, opa, quat, scale, feat)
         bg = None if background is None else [float(v) for v in background]
         fin, raw, aux, aux_fin, fmap, fmap_fin, mask = rctx.forward_feat(
-            pos, rgb, opa, quat, scale, feat, int(width), int(height), float(focal_x), float(focal_y),
-            rot.detach().cpu(), tran.detach().cpu(), float(near), float(tile_thresh),
-            SCALE_ACTIVATIONS[scale_activation], bg, bool(final))
-        ctx.rctx = rctx
-        ctx.frame = rctx.frame_id()
-        ctx.final = bool(final)
-        ctx.save_for_backward(pos, rgb, opa, quat, scale, feat, raw, aux, fmap)
-        ctx.mark_non_differentiable(mask)
-        ctx.set_materialize_grads(False)
+            *params, feat, int(width), int(height), float(focal_x), float(focal_y), rot.detach().cpu(),
+            tran.detach().cpu(), float(near), float(tile_thresh), SCALE_ACTIVATIONS[scale_activation], bg, bool(final))
         image, maps, feats = (fin, aux_fin, fmap_fin) if final else (raw, aux, fmap)
-        ctx.map_shape = tuple(maps.shape[:2])
+        _save_frame(ctx, rctx, mask, (*params, feat, raw, aux, fmap), final, maps.shape[:2])
         return image, feats, maps[..., 0].contiguous(), maps[..., 1].contiguous(), mask
 
     @staticmethod
     def backward(ctx, grad_image, grad_feat, grad_depth, grad_alpha, _grad_mask):
-        pos, rgb, opa, quat, scale, feat, raw, aux, fmap = ctx.saved_tensors
-        rows, cols = ctx.map_shape
-        if grad_image is None:
-            grad_image = raw.new_zeros(rows, cols, 3)
-        grad_aux = None
-        if grad_depth is not None or grad_alpha is not None:
-            grad_aux = raw.new_zeros(rows, cols, 2)
-            if grad_depth is not None:
-                grad_aux[..., 0] = grad_depth
-            if grad_alpha is not None:
-                grad_aux[..., 1] = grad_alpha
-        outs, push = _flat_grads((pos, rgb, opa, quat, scale))
-        _apply_push(ctx.rctx, push)
+        *params, feat, raw, aux, fmap = ctx.saved_tensors
+        grad_image, grad_aux = _upstream(raw, ctx.map_shape, grad_image, grad_depth, grad_alpha)
+        outs = _param_grads(ctx.rctx, params)
         g_feat = torch.empty_like(feat)
         if grad_feat is not None:
             grad_feat = _f32(grad_feat)
             if grad_feat.data_ptr() % 16:                      # the kernel reads 16-byte pieces of every pixel's row
                 grad_feat = grad_feat.clone()
-        ctx.rctx.backward_feat_into(pos, rgb, opa, quat, scale, feat, raw, _f32(grad_image), ctx.final, aux, grad_aux,
-                                    fmap, grad_feat, *outs, g_feat, ctx.frame)
-        return (None, outs[0], outs[1], outs[2], outs[3], outs[4], g_feat) + (None,) * 11
+        ctx.rctx.backward_feat_into(*params, feat, raw, grad_image, ctx.final, aux, grad_aux, fmap, grad_feat, *outs,
+                                    g_feat, ctx.frame)
+        return (None, *outs, g_feat) + (None,) * 11
 
 
 def render_frame_feat(rctx, pos, rgb, opa, quat, scale, feat, width, height, focal_x, focal_y, rot, tran, near,

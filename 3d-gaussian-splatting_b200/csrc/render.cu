@@ -668,6 +668,18 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
     if (absgrad)
       if (int rc = gs_blend_absgrad_supported(blend_d, c->gather)) return rc;
   }
+  if (c->push.world) {
+    // every gradient segment must lie inside the sliced bucket, quaternions on 16-byte offsets
+    const float* lo = c->push.bucket;
+    const float* hi = lo + (size_t)c->push.world * c->push.per;
+    const size_t nn = (size_t)c->n;
+    const float* seg[5] = {grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale};
+    const size_t len[5] = {3 * nn, (size_t)d * nn, nn, 4 * nn, 3 * nn};
+    for (int k = 0; k < 5; ++k)
+      if (seg[k] < lo || seg[k] + len[k] > hi)
+        return gs_fail(GS_ERR_INVALID_ARG, who, "gradient buffers are not inside the push bucket");
+    if ((grad_quat - lo) % 4) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_quat must sit on a 16-byte bucket offset");
+  }
   if (int rc = gs_check_device(c->device, who)) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
@@ -714,18 +726,6 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
     c->have_backward = true;
   }
   gs_mark(c, 8, st);
-  if (c->push.world) {
-    // every gradient segment must lie inside the sliced bucket, quaternions on 16-byte offsets
-    const float* lo = c->push.bucket;
-    const float* hi = lo + (size_t)c->push.world * c->push.per;
-    const size_t nn = (size_t)c->n;
-    const float* seg[5] = {grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale};
-    const size_t len[5] = {3 * nn, (size_t)d * nn, nn, 4 * nn, 3 * nn};
-    for (int k = 0; k < 5; ++k)
-      if (seg[k] < lo || seg[k] + len[k] > hi)
-        return gs_fail(GS_ERR_INVALID_ARG, who, "gradient buffers are not inside the push bucket");
-    if ((grad_quat - lo) % 4) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_quat must sit on a 16-byte bucket offset");
-  }
   if (grad_cam) {
     GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
     GS_CUDA_TRY(gs_launch_fused_project_bwd_cam(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam,

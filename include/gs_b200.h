@@ -531,12 +531,15 @@ int gs_allreduce_p2p_f32(void* const* peer_ptrs, long long n_floats, int rank, i
 
 /* Exchange fused into the backward ("push"): the flat bucket is cut into `world` slices of `per`
  * floats (multiple of 4; world * per >= bucket length, < 2^32); rank r owns slice r.  While a
- * context has a push configuration, gs_render_backward[_final] stores every gradient float that
- * belongs to ANOTHER rank's slice straight into slot `rank` of that owner's staging buffer
- * (staging[p] = rank p's [world][per] float buffer as mapped into this process) from inside the
- * projection-backward kernel, and only its own slice into `bucket` - the reduce half of the
- * exchange overlaps the kernel.  The five gradient pointers of the backward call must lie inside
- * [bucket, bucket + world * per).  gs_allreduce_push_finish_f32 (after a cross-rank barrier)
+ * context has a push configuration, gs_render_backward, gs_render_backward_final,
+ * gs_render_backward_aux and gs_render_backward_feat (without a feature-map gradient) store every
+ * gradient float that belongs to ANOTHER rank's slice straight into slot `rank` of that owner's
+ * staging buffer (staging[p] = rank p's [world][per] float buffer as mapped into this process)
+ * from inside the projection-backward kernel, and only its own slice into `bucket` - the reduce
+ * half of the exchange overlaps the kernel; the camera-gradient, feature-map-gradient and batched
+ * backwards refuse a push configuration.  The five gradient pointers of the backward call must lie
+ * inside [bucket, bucket + world * per) with grad_quat on a 16-byte bucket offset; a call that
+ * breaks this is refused before any launch.  gs_allreduce_push_finish_f32 (after a cross-rank barrier)
  * completes it: rank r sums its own slice with the world-1 pushed contributions and stores the sum
  * into every rank's bucket (`peer_buckets`: host array of `world` device pointers); a second
  * barrier makes all slices visible.  world must be 2, 4 or 8.  NULL clears the configuration. */

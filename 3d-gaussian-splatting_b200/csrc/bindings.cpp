@@ -612,25 +612,56 @@ struct RenderContext {
                          std::optional<torch::Tensor> g_pos, std::optional<torch::Tensor> g_rgb,
                          std::optional<torch::Tensor> g_opa, std::optional<torch::Tensor> g_quat,
                          std::optional<torch::Tensor> g_scale, torch::Tensor grad_cam, int64_t expected_frame) {
-    const char* fn = "RenderContext.backward_cam_into";
-    check_backward(fn, expected_frame, false, grad_is_final, pos, rgb, opa, quat, scale, raw, grad_image,
-                   aux ? &*aux : nullptr, grad_aux ? &*grad_aux : nullptr);
+    backward_cam_checked("RenderContext.backward_cam_into", false, pos, rgb, opa, quat, scale, raw, grad_image,
+                         grad_is_final, aux ? &*aux : nullptr, grad_aux, {g_pos, g_rgb, g_opa, g_quat, g_scale},
+                         grad_cam, expected_frame);
+  }
+
+  // backward_batch_into plus each view's camera gradient grad_cams[B,12] (gs_render_backward_batch_cam); the five
+  // parameter gradients all None: camera only
+  void backward_batch_cam_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                               torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_image, bool grad_is_final,
+                               torch::Tensor aux, std::optional<torch::Tensor> grad_aux,
+                               std::optional<torch::Tensor> g_pos, std::optional<torch::Tensor> g_rgb,
+                               std::optional<torch::Tensor> g_opa, std::optional<torch::Tensor> g_quat,
+                               std::optional<torch::Tensor> g_scale, torch::Tensor grad_cams, int64_t expected_frame) {
+    backward_cam_checked("RenderContext.backward_batch_cam_into", true, pos, rgb, opa, quat, scale, raw, grad_image,
+                         grad_is_final, &aux, grad_aux, {g_pos, g_rgb, g_opa, g_quat, g_scale}, grad_cams,
+                         expected_frame);
+  }
+
+  // the camera-gradient backward of the last single-view (gs_render_backward_cam: grad_cam [12]) or batched
+  // (gs_render_backward_batch_cam: grad_cam [B,12]) forward; the five parameter gradients all given or all None
+  void backward_cam_checked(const char* fn, bool batched, const torch::Tensor& pos, const torch::Tensor& rgb,
+                            const torch::Tensor& opa, const torch::Tensor& quat, const torch::Tensor& scale,
+                            const torch::Tensor& raw, const torch::Tensor& grad_image, bool grad_is_final,
+                            const torch::Tensor* aux, const std::optional<torch::Tensor>& grad_aux,
+                            const std::array<std::optional<torch::Tensor>, 5>& g, const torch::Tensor& grad_cam,
+                            int64_t expected_frame) {
+    check_backward(fn, expected_frame, batched, grad_is_final, pos, rgb, opa, quat, scale, raw, grad_image, aux,
+                   grad_aux ? &*grad_aux : nullptr);
     GS_CHECK_F32(grad_cam);
-    TORCH_CHECK(grad_cam.numel() == 12 && grad_cam.device() == pos.device(),
-                "RenderContext.backward_cam_into: grad_cam must be 12 floats on the parameters' device");
-    const int n_given = (int)g_pos.has_value() + g_rgb.has_value() + g_opa.has_value() + g_quat.has_value() +
-                        g_scale.has_value();
-    TORCH_CHECK(n_given == 0 || n_given == 5,
-                "RenderContext.backward_cam_into: give all five parameter gradients or none (camera only)");
-    if (n_given) check_grads(fn, {pos, rgb, opa, quat, scale}, {*g_pos, *g_rgb, *g_opa, *g_quat, *g_scale});
+    if (batched) {
+      TORCH_CHECK(grad_cam.dim() == 2 && grad_cam.size(0) == batch[0] && grad_cam.size(1) == 12 &&
+                      grad_cam.device() == pos.device(),
+                  fn, ": grad_cams must be [", batch[0], ",12] on the parameters' device");
+    } else {
+      TORCH_CHECK(grad_cam.numel() == 12 && grad_cam.device() == pos.device(), fn,
+                  ": grad_cam must be 12 floats on the parameters' device");
+    }
+    int n_given = 0;
+    for (const auto& t : g) n_given += t.has_value();
+    TORCH_CHECK(n_given == 0 || n_given == 5, fn, ": give all five parameter gradients or none (camera only)");
+    if (n_given) check_grads(fn, {pos, rgb, opa, quat, scale}, {*g[0], *g[1], *g[2], *g[3], *g[4]});
     auto opt = [](const std::optional<torch::Tensor>& t) { return t ? fpm(*t) : nullptr; };
     c10::cuda::CUDAGuard guard(pos.device());
     auto gi = grad_image.contiguous();
     torch::Tensor ga;
     if (grad_aux) ga = grad_aux->contiguous();
-    check_rc(gs_render_backward_cam(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
-                                    grad_is_final ? 1 : 0, aux ? fp(*aux) : nullptr, fpm_or_null(ga), opt(g_pos),
-                                    opt(g_rgb), opt(g_opa), opt(g_quat), opt(g_scale), fpm(grad_cam), cur_stream()),
+    auto entry = batched ? &gs_render_backward_batch_cam : &gs_render_backward_cam;
+    check_rc(entry(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi), grad_is_final ? 1 : 0,
+                   aux ? fp(*aux) : nullptr, fpm_or_null(ga), opt(g[0]), opt(g[1]), opt(g[2]), opt(g[3]), opt(g[4]),
+                   fpm(grad_cam), cur_stream()),
              fn);
   }
 
@@ -999,6 +1030,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"), py::arg("grad_is_final"),
            py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
            py::arg("g_quat"), py::arg("g_scale"), py::arg("grad_cam"), py::arg("expected_frame") = -1)
+      .def("backward_batch_cam_into", &RenderContext::backward_batch_cam_into, py::arg("pos"), py::arg("rgb"),
+           py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"),
+           py::arg("grad_is_final"), py::arg("aux"), py::arg("grad_aux"), py::arg("g_pos"), py::arg("g_rgb"),
+           py::arg("g_opa"), py::arg("g_quat"), py::arg("g_scale"), py::arg("grad_cams"),
+           py::arg("expected_frame") = -1)
       .def("forward_feat", &RenderContext::forward_feat, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
            py::arg("quat"), py::arg("scale"), py::arg("feat"), py::arg("width"), py::arg("height"), py::arg("fx"),
            py::arg("fy"), py::arg("rot"), py::arg("tran"), py::arg("near"), py::arg("thresh"),

@@ -194,6 +194,18 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
                                               uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                               float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
                                               bool filt);
+// The same plus each view's camera gradient (RGB and per-Gaussian SH): the projection backward leaves view v's per-CTA
+// partial sums in cam_part[v][grid][12] (n_views * gs_cam_grad_workspace_bytes(n)), and one CTA per view sums them in
+// fp64 into grad_cams[v][12] (zeros when n == 0).  The five gradient pointers may all be NULL (camera only).  Two
+// launches (one when n == 0), whatever n_views.
+cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float* rgb, const float* opa,
+                                                  const float* quat, const float* scale, int n, int n_views, int d,
+                                                  int scale_act, const GsView* views, float near_plane,
+                                                  const uint32_t* offsets_g, const uint32_t* count,
+                                                  const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
+                                                  float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                                  float* g_scale, float* cam_part, float* grad_cams, cudaStream_t st,
+                                                  bool depth_grad, bool sh_gaussian, bool filt);
 
 // ---- densify_stats.cu ------------------------------------------------------------------
 // Accumulates the screen-space densification statistics of the backward that just wrote grad_inst (rows of gw floats;

@@ -632,14 +632,15 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PB
 // s, raw_s, qn, opa_raw, rgb_raw / coef): acc receives the row sums, then gp, gq_raw, gs_raw, go and the colour
 // gradients (acc + 6 for D == 3, gsh for KG > 0) are formed.  The single-view kernels keep their own copy (routed
 // through this function they compile to different SASS): a change to the arithmetic of either copy must be made to
-// both.
-template <int D, bool DT, int KG, bool F>
+// both.  CG: also adds the view's camera terms to cg[12], as fused_project_bwd_body<..., CG = true> does (the parameter
+// gradients are the same bits either way).
+template <int D, bool DT, int KG, bool F, bool CG = false>
 __device__ __forceinline__ void fused_project_bwd_one(
     GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
     const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
     const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, float opa_raw,
     const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GS_GREC], float (&gsh)[KG ? D : 1],
-    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go) {
+    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr) {
   constexpr int GW = GS_GREC;
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   {
@@ -716,7 +717,13 @@ __device__ __forceinline__ void fused_project_bwd_one(
     static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
     float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
     float gq[4], gsv[3];
-    gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    if constexpr (CG) {
+      float gc[3], gjw[6];
+      gs_project_backward_cam(cam, p, q, s, gxyd, gcov, gp, gq, gsv, gc, gjw);
+      gs_cam_grad_add(cam, p, gc, gjw, cg);
+    } else {
+      gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
+    }
     if constexpr (KG > 0) {
       // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
       // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
@@ -739,6 +746,18 @@ __device__ __forceinline__ void fused_project_bwd_one(
       const float dd = dir[0] * gd[0] + dir[1] * gd[1] + dir[2] * gd[2];
 #pragma unroll
       for (int j = 0; j < 3; ++j) gp[j] += (gd[j] - dir[j] * dd) * il;
+      if constexpr (CG) {
+        // the direction term of fused_project_bwd_body, with il applied last for the same reason (gp keeps its bits)
+        float v[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) v[j] = gd[j] - dir[j] * dd;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+          for (int j = 0; j < 3; ++j) cg[3 * r + j] += (cam.t[r] * v[j]) * il;
+          cg[9 + r] += (cam.r[3 * r] * v[0] + cam.r[3 * r + 1] * v[1] + cam.r[3 * r + 2] * v[2]) * il;
+        }
+      }
     }
     // quat normalisation backward: q = r/|r|
     float dot = q[0] * gq[0] + q[1] * gq[1] + q[2] * gq[2] + q[3] * gq[3];
@@ -881,6 +900,29 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
 // cam_part[gridDim.x][12]; cam_grad_finish_kernel adds the rows.  No atomics: the result is bit-deterministic.
 // F: with the 2-D filter of the forward (fused_project_bwd_cam_filt_kernel).
 constexpr int kCamGrad = 12;
+
+// The CTA's sum of its threads' cg[12] into row[12], in fused_project_bwd_cam_body's order (that kernel keeps its own
+// copy: routed through this function it compiles to different SASS).  Every thread of the CTA calls it.
+__device__ __forceinline__ void cam_grad_cta_sum(float (&cg)[kCamGrad], float (&wsum)[kBlock / 32][kCamGrad],
+                                                 float* __restrict__ row) {
+#pragma unroll
+  for (int k = 0; k < kCamGrad; ++k) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) cg[k] += __shfl_xor_sync(0xffffffffu, cg[k], o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < kCamGrad; ++k) wsum[threadIdx.x >> 5][k] = cg[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < kCamGrad) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < kBlock / 32; ++w) s += wsum[w][threadIdx.x];
+    row[threadIdx.x] = s;
+  }
+}
+
 template <int K, bool DT, bool F>
 __device__ __forceinline__ void fused_project_bwd_cam_body(GS_PBWD_PARAMS, float* __restrict__ cam_part,
                                                            GsFilter2d filt) {
@@ -917,12 +959,94 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt_kernel(GS_P
                                                                             GsFilter2d filt) {
   fused_project_bwd_cam_body<K, DT, true>(GS_PBWD_ARGS, cam_part, filt);
 }
+
+// Camera gradients of a batched frame (gs_render_backward_batch_cam): fused_project_bwd_batch_kernel's parameter
+// gradients, the same bits, plus the camera terms of each view with that view's camera, filter and SH direction.  Per
+// view v the CTA sums its threads' terms in fused_project_bwd_cam_body's order into row blockIdx.x of
+// cam_part[v][gridDim.x][12].  The view loop and the sums are uniform across the CTA: threads past n and Gaussians
+// without a row in view v take part with zeros, and a CTA without a row in view v stores a zero row (the bits the
+// shuffles would give) without reducing.  With the five gradient pointers NULL only cam_part is written.
+template <int K, bool DT, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,
+    const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
+    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
+    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
+    float* __restrict__ g_quat, float* __restrict__ g_scale, float* __restrict__ cam_part) {
+  constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  const bool valid = i < n;
+  float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f}, go = 0.f;
+  float gcol[D];
+#pragma unroll
+  for (int k = 0; k < D; ++k) gcol[k] = 0.f;
+  float p[3] = {0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, s[3] = {0.f, 0.f, 0.f}, raw_s[3] = {0.f, 0.f, 0.f};
+  float qn = 1.f, opa_raw = 0.f, rgb_raw[3] = {0.f, 0.f, 0.f};
+  float coef[K ? D : 1];
+#pragma unroll
+  for (int k = 0; k < (K ? D : 1); ++k) coef[k] = 0.f;
+  if (valid) {
+    p[0] = pos[3 * i];
+    p[1] = pos[3 * i + 1];
+    p[2] = pos[3 * i + 2];
+    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    opa_raw = opa[i];
+    if constexpr (K > 0) {
+#pragma unroll
+      for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
+    } else {
+      rgb_raw[0] = rgb[3 * i];
+      rgb_raw[1] = rgb[3 * i + 1];
+      rgb_raw[2] = rgb[3 * i + 2];
+    }
+  }
+  __shared__ float wsum[kBlock / 32][kCamGrad];
+  for (int v = 0; v < n_views; ++v) {
+    const int j = v * n + i;
+    const uint32_t cnt = valid ? count[j] : 0u;
+    float cg[kCamGrad];
+#pragma unroll
+    for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
+    if (cnt > 0) {
+      const uint32_t o0 = offsets_g[j];
+      const GsView vw = views[v];
+      float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
+#pragma unroll
+      for (int k = 0; k < GW; ++k) acc[k] = 0.f;
+      fused_project_bwd_one<D, DT, K, F, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                               o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
+                                               rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg);
+      const float* vc = K ? gsh : acc + 6;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        gp[k] = __fadd_rn(gp[k], vp[k]);
+        gs_raw[k] = __fadd_rn(gs_raw[k], vs[k]);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) gq_raw[k] = __fadd_rn(gq_raw[k], vq[k]);
+      go = __fadd_rn(go, vo);
+#pragma unroll
+      for (int k = 0; k < D; ++k) gcol[k] = __fadd_rn(gcol[k], vc[k]);
+    }
+    float* row = cam_part + ((size_t)v * gridDim.x + blockIdx.x) * kCamGrad;
+    // the barrier also keeps the previous view's readers of wsum ahead of this view's writers
+    if (__syncthreads_or(cnt > 0)) {
+      cam_grad_cta_sum(cg, wsum, row);
+    } else if (threadIdx.x < kCamGrad) {
+      row[threadIdx.x] = 0.f;
+    }
+  }
+  if (!g_pos) return;                    // camera only (the pointers are all NULL or all set: uniform)
+  if (!valid && D == 3) return;          // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
+  fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
+}
 #undef GS_PBWD_PARAMS
 
 // One CTA: grad_cam[k] = sum over the `rows` rows of cam_part[., k] in fp64, in a fixed order (strided per-thread sums,
 // butterfly shuffles, warp sums in warp order).  rows == 0 (no Gaussian) writes zeros.
-__global__ void __launch_bounds__(kBlock) cam_grad_finish_kernel(const float* __restrict__ cam_part, int rows,
-                                                                  float* __restrict__ grad_cam) {
+__device__ __forceinline__ void cam_grad_finish_rows(const float* __restrict__ cam_part, int rows,
+                                                     float* __restrict__ grad_cam) {
   double s[kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) s[k] = 0.0;
@@ -947,6 +1071,17 @@ __global__ void __launch_bounds__(kBlock) cam_grad_finish_kernel(const float* __
     for (int w = 0; w < kBlock / 32; ++w) t += wsum[w][threadIdx.x];
     grad_cam[threadIdx.x] = (float)t;
   }
+}
+
+__global__ void __launch_bounds__(kBlock) cam_grad_finish_kernel(const float* __restrict__ cam_part, int rows,
+                                                                  float* __restrict__ grad_cam) {
+  cam_grad_finish_rows(cam_part, rows, grad_cam);
+}
+
+// A batched frame: CTA v sums view v's `rows` rows, cam_part[v][rows][12], into grad_cams[v][12]
+__global__ void __launch_bounds__(kBlock) cam_grad_finish_batch_kernel(const float* __restrict__ cam_part, int rows,
+                                                                        float* __restrict__ grad_cams) {
+  cam_grad_finish_rows(cam_part + (size_t)blockIdx.x * rows * kCamGrad, rows, grad_cams + blockIdx.x * kCamGrad);
 }
 
 }  // namespace
@@ -1255,5 +1390,35 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
   else { GS_LAUNCH_PBWD_BATCH_F(0, false); }
 #undef GS_LAUNCH_PBWD_BATCH_F
 #undef GS_LAUNCH_PBWD_BATCH
+  return cudaGetLastError();
+}
+
+cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float* rgb, const float* opa,
+                                                  const float* quat, const float* scale, int n, int n_views, int d,
+                                                  int scale_act, const GsView* views, float near_plane,
+                                                  const uint32_t* offsets_g, const uint32_t* count,
+                                                  const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
+                                                  float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
+                                                  float* g_scale, float* cam_part, float* grad_cams, cudaStream_t st,
+                                                  bool depth_grad, bool sh_gaussian, bool filt) {
+  if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+  if (n > 0) {
+#define GS_LAUNCH_PBWD_BATCH_CAM(K, DT, F)                                                                          \
+  fused_project_bwd_batch_cam_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                     \
+      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
+      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part)
+#define GS_LAUNCH_PBWD_BATCH_CAM_F(K, DT)          \
+  if (filt) GS_LAUNCH_PBWD_BATCH_CAM(K, DT, true); \
+  else GS_LAUNCH_PBWD_BATCH_CAM(K, DT, false)
+    if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, true); }
+    else if (d == 27) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, false); }
+    else if (d == 48 && depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(16, true); }
+    else if (d == 48) { GS_LAUNCH_PBWD_BATCH_CAM_F(16, false); }
+    else if (depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(0, true); }
+    else { GS_LAUNCH_PBWD_BATCH_CAM_F(0, false); }
+#undef GS_LAUNCH_PBWD_BATCH_CAM_F
+#undef GS_LAUNCH_PBWD_BATCH_CAM
+  }
+  cam_grad_finish_batch_kernel<<<n_views, kBlock, 0, st>>>(cam_part, n > 0 ? grid_for(n) : 0, grad_cams);
   return cudaGetLastError();
 }

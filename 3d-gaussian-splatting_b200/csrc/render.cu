@@ -630,8 +630,8 @@ static int next_row_epoch(gs_ctx* c, size_t M, cudaStream_t st) {
   return 0;
 }
 
-// The backward of the last forward, single-view or batched (batch: the caller is gs_render_backward_batch, which has
-// checked what only a batched frame needs).
+// The backward of the last forward, single-view or batched (batch: the caller is gs_render_backward_batch[_cam], which
+// has checked what only a batched frame needs; grad_cam is then [n_views][12]).
 static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const float* pos, const float* rgb,
                                 const float* opa, const float* quat, const float* scale, const float* image,
                                 const float* grad_image, int grad_is_final, float* grad_pos, float* grad_rgb,
@@ -726,7 +726,19 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
     c->have_backward = true;
   }
   gs_mark(c, 8, st);
-  if (grad_cam) {
+  if (grad_cam && c->n_views > 1) {
+    // B views: one row of 12 partial sums per CTA and view, one finishing CTA per view (grad_cam is [B][12]).  One
+    // view: the single-view kernels below, as for the parameter gradients of a one-view batch
+    GS_CUDA_TRY(c->cam_part.reserve((size_t)c->n_views * gs_cam_grad_workspace_bytes(c->n) + 16, st));
+    GS_CUDA_TRY(gs_launch_fused_project_bwd_batch_cam(pos, rgb, opa, quat, scale, c->n, c->n_views, d, c->scale_act,
+                                                      c->views.as<GsView>(), c->near_plane,
+                                                      c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                                      c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
+                                                      grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
+                                                      c->cam_part.as<float>(), grad_cam, st, grad_aux != nullptr,
+                                                      c->sh_gaussian, c->filt_on));
+    gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sums
+  } else if (grad_cam) {
     GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
     GS_CUDA_TRY(gs_launch_fused_project_bwd_cam(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam,
                                                 c->near_plane, c->half_w, c->half_h, c->offsets_g.as<uint32_t>(),
@@ -953,6 +965,26 @@ extern "C" int gs_render_backward_batch(gs_ctx* c, const float* pos, const float
   if (int rc = gs_blend_batch_supported()) return rc;
   return render_backward_impl(c, who, true, pos, rgb, opa, quat, scale, image, grad_image, grad_is_final ? 1 : 0,
                               grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux);
+}
+
+extern "C" int gs_render_backward_batch_cam(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                            const float* quat, const float* scale, const float* image,
+                                            const float* grad_image, int grad_is_final, const float* aux,
+                                            const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                            float* grad_quat, float* grad_scale, float* grad_cams,
+                                            gs_stream_t stream) {
+  const char* who = "gs_render_backward_batch_cam";
+  if (!grad_cams) return gs_fail(GS_ERR_INVALID_ARG, who, "null grad_cams");
+  const int n_null = !grad_pos + !grad_rgb + !grad_opa + !grad_quat + !grad_scale;
+  if (n_null != 0 && n_null != 5)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the five parameter gradients must be all NULL or all non-NULL");
+  if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
+  if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (!c->n_views) return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was not batched");
+  if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
+  if (int rc = gs_blend_batch_supported()) return rc;
+  return render_backward_impl(c, who, true, pos, rgb, opa, quat, scale, image, grad_image, grad_is_final ? 1 : 0,
+                              grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, stream, aux, grad_aux, grad_cams);
 }
 
 extern "C" int gs_ctx_set_grad_push(gs_ctx* c, const gs_grad_push* p) {

@@ -437,6 +437,66 @@ def render_frame_cam(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, f
                                  near, tile_thresh, scale_activation, background, final)
 
 
+class _RenderFrameBatchCam(_RenderFrameBatch):
+    """`_RenderFrameBatch` whose backward also returns each view's dL/drot and dL/dtran
+    (gs_render_backward_batch_cam)."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal, rot, tran, near, tile_thresh,
+                scale_activation, background, final):
+        b = rot.shape[0]
+        cams = torch.cat([rot.detach().reshape(b, 9), tran.detach().reshape(b, 3)], 1).cpu()   # one 48 B-byte read
+        return _RenderFrameBatch.forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal,
+                                         cams[:, :9].reshape(b, 3, 3), cams[:, 9:].contiguous(), near, tile_thresh,
+                                         scale_activation, background, final)
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask):
+        if not (ctx.needs_input_grad[9] or ctx.needs_input_grad[10]):
+            return _RenderFrameBatch.backward(ctx, grad_image, grad_depth, grad_alpha, _grad_mask)
+        *params, raw, aux = ctx.saved_tensors
+        grad_image, grad_aux = _upstream(raw, ctx.map_shape, grad_image, grad_depth, grad_alpha)
+        if not any(ctx.needs_input_grad[1:6]):                  # tracking: the scene is frozen, camera only
+            outs = [None] * 5
+            _apply_push(ctx.rctx, None)
+        else:
+            outs = _param_grads(ctx.rctx, params)
+        grad_cams = raw.new_empty(ctx.map_shape[0], 12)
+        ctx.rctx.backward_batch_cam_into(*params, raw, grad_image, ctx.final, aux, grad_aux, *outs, grad_cams,
+                                         ctx.frame)
+        return ((None, *outs) + (None,) * 3 + (grad_cams[:, :9].reshape(-1, 3, 3), grad_cams[:, 9:]) +
+                (None,) * 5)
+
+
+def render_frame_batch_cam(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
+                           tile_thresh, scale_activation, background=None, final=True):
+    """`render_frame_batch` differentiable with respect to each view's camera too: -> (image, depth, alpha,
+    culling_mask) as `render_frame_batch` returns them, and the backward returns dL/drot [B,3,3] and dL/dtran [B,3],
+    per view what `render_frame_cam` returns for that view (p_c = rot[v] p + tran[v], rot used as given).  rot
+    [B,3,3] and tran [B,3] (1 <= B <= 64) must be float32 CUDA tensors on the parameters' device (ValueError
+    otherwise); reading them for the forward costs one host synchronisation (48 B bytes).  The parameter gradients are
+    the sums over the views, as in `render_frame_batch`.  When none of the five parameters needs a gradient the
+    backward is camera only (the densification statistics are then left alone); when neither rot nor tran needs one it
+    is `render_frame_batch`'s.  RGB and per-Gaussian SH colour; per-pixel SH, the packed path, non-default blend knobs
+    and a data-parallel gradient push raise RuntimeError."""
+    for name, t, dims in (("rot", rot, 3), ("tran", tran, 2)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != dims:
+            raise ValueError(f"render_frame_batch_cam: {name} must be a float32 CUDA tensor of {dims} dimensions")
+        if t.device != pos.device:
+            raise ValueError(f"render_frame_batch_cam: {name} is on {t.device}, the parameters on {pos.device}")
+    b = rot.shape[0]
+    if tuple(rot.shape[1:]) != (3, 3) or tuple(tran.shape) != (b, 3):
+        raise ValueError(f"render_frame_batch_cam: rot must be [B,3,3] and tran [B,3], got {list(rot.shape)} and "
+                         f"{list(tran.shape)}")
+    if not 1 <= b <= MAX_VIEWS:
+        raise ValueError(f"render_frame_batch_cam: the batch must have 1 .. {MAX_VIEWS} views, got {b}")
+    fx, fy = (torch.as_tensor(f, dtype=torch.float64).detach().reshape(-1).cpu() for f in (focal_x, focal_y))
+    if fx.numel() != b or fy.numel() != b:
+        raise ValueError(f"render_frame_batch_cam: focal_x and focal_y must have {b} values each")
+    return _RenderFrameBatchCam.apply(rctx, pos, rgb, opa, quat, scale, width, height, torch.stack([fx, fy], 1), rot,
+                                      tran, near, tile_thresh, scale_activation, background, final)
+
+
 FEATURE_WIDTHS = (8, 16, 32)
 
 

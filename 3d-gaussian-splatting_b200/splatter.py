@@ -28,7 +28,7 @@ import torch.nn as nn
 
 import gaussian
 from renderer import (FEATURE_WIDTHS, FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_batch,
-                      render_frame_cam, render_frame_feat, render_frame_final)
+                      render_frame_batch_cam, render_frame_cam, render_frame_feat, render_frame_final)
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -446,19 +446,32 @@ class Splatter(nn.Module):
         holds images.  Each view is what `render_maps` returns for it; the gradients are SUMS over the views (divide
         the loss by B for a mean).  Sets `culling_mask` to the [n] sum over the views and `n_tile_gaussians` to the
         batch's instance count.  The views must share their size (ValueError otherwise)."""
+        return self._render_batch("render_batch", render_frame_batch, camera_ids, None, None, background)
+
+    def render_batch_at_poses(self, rots, trans, camera_ids, background=None):
+        """`render_batch` at caller-supplied poses, differentiable with respect to them: rots [B,3,3] and trans [B,3]
+        are float32 CUDA tensors (world -> camera per view), typically a learnable correction per view composed with
+        the views' poses in torch (mini-batch pose refinement) or B candidate poses of a frozen scene (localisation).
+        The intrinsics and `ground_truth` come from `camera_ids` (B ids).  Returns `render_batch`'s dict and sets the
+        same attributes; backward gives rots and trans their gradients (`renderer.render_frame_batch_cam`), and runs
+        camera only when no scene parameter needs a gradient.  Costs one host synchronisation (the 12 B pose floats)."""
+        return self._render_batch("render_batch_at_poses", render_frame_batch_cam, camera_ids, rots, trans, background)
+
+    def _render_batch(self, who, render, camera_ids, rots, trans, background):
         ids = list(camera_ids)
         if not ids:
-            raise ValueError("render_batch: no camera ids")
+            raise ValueError(f"{who}: no camera ids")
         vs = [self.views[i] for i in ids]
         if any(v["width"] != vs[0]["width"] or v["height"] != vs[0]["height"] for v in vs):
-            raise ValueError("render_batch: the views of a batch must have the same width and height")
+            raise ValueError(f"{who}: the views of a batch must have the same width and height")
+        if rots is None:
+            rots, trans = torch.stack([v["rot"] for v in vs]), torch.stack([v["tran"] for v in vs])
         g = self.gaussian_3ds
         self._size_densify_stats()
-        image, depth, alpha, mask = render_frame_batch(
+        image, depth, alpha, mask = render(
             self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, vs[0]["width"], vs[0]["height"],
-            [v["focal_x"] for v in vs], [v["focal_y"] for v in vs], torch.stack([v["rot"] for v in vs]),
-            torch.stack([v["tran"] for v in vs]), self.near, self.tile_culling_prob_thresh, self.scale_activation,
-            background=background, final=True)
+            [v["focal_x"] for v in vs], [v["focal_y"] for v in vs], rots, trans, self.near,
+            self.tile_culling_prob_thresh, self.scale_activation, background=background, final=True)
         self.culling_mask = mask.sum(0)
         self.n_gaussians = g.pos.shape[0]
         self.n_tile_gaussians = self._rctx.last_instances()

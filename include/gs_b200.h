@@ -309,6 +309,26 @@ int gs_render_backward_batch(gs_ctx* ctx, const float* pos, const float* rgb, co
                              const float* scale, const float* image_raw_padded, const float* grad_image,
                              int grad_is_final, const float* aux, const float* grad_aux, float* grad_pos,
                              float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale, gs_stream_t stream);
+/* gs_render_backward_batch plus each view's camera gradient: per view v, gs_render_backward_cam's semantics with view
+ * v's camera cams_host[v] of the last gs_render_forward_batch (projection Jacobian detached, rot used as given, depth
+ * gradients and the per-Gaussian SH view direction reach the pose, view v's 2-D filter).  grad_cams (DEVICE
+ * float[B][12]) receives per view dL/drot row-major [9], then dL/dtran [3]; it is always written (zeros for a view
+ * that bins nothing) and bit-deterministic (fixed-order sums per CTA and view, fp64 across CTAs; no atomics).  The five
+ * parameter gradients are all NULL (camera only: nothing else is written, the densification statistics are left
+ * alone) or all non-NULL (then equal to gs_render_backward_batch's, statistics included).  With n_views == 1 the
+ * single-view kernels run, so grad_cams[0] and the parameter gradients are gs_render_backward_cam's bit for bit.
+ * Refused before any launch: a NULL grad_cams or ctx, or a mixed set of parameter gradients (GS_ERR_INVALID_ARG,
+ * checked before the context is read); no forward (GS_ERR_NO_FORWARD); a single-view last forward
+ * (GS_ERR_INVALID_ARG); a gradient push configured, or a batch the batched blend cannot run (GS_ERR_UNSUPPORTED).
+ * gs_render_backward_cam after gs_render_forward_batch stays refused.  One launch more than gs_render_backward_batch,
+ * whatever B; no synchronisation; the context keeps B * 48 bytes of workspace per 256 Gaussians. */
+int gs_render_backward_batch_cam(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa,
+                                 const float* quat, const float* scale, const float* image_raw_padded,
+                                 const float* grad_image, int grad_is_final, const float* aux,
+                                 const float* grad_aux, float* grad_pos, float* grad_rgb, float* grad_opa,
+                                 float* grad_quat, float* grad_scale,
+                                 float* grad_cams /* DEVICE [B][12]: per view dL/drot row-major [9], dL/dtran [3] */,
+                                 gs_stream_t stream);
 
 /* Where the SH colour (d == 27 / 48) is evaluated.  Two colour MODELS, not two speeds of one: the same coefficients
  * render differently.

@@ -27,10 +27,13 @@ def _optimizer_state(opt):
         return {"kind": "torch", "state": opt.state_dict()}
     # optim.FlatAdam: flat moments + per-group learning rates
     flat = getattr(opt, "_flat", None)
+    staged = getattr(opt, "_staged", None)     # moments carried over a growth (FlatAdam.replace_params), not yet placed
     return {"kind": "flat_adam", "step": opt.step_count, "betas": opt.betas, "eps": opt.eps,
             "lrs": [g["lr"] for g in opt.param_groups],
             "exp_avg": None if flat is None else flat[1].detach().cpu(),
-            "exp_avg_sq": None if flat is None else flat[2].detach().cpu()}
+            "exp_avg_sq": None if flat is None else flat[2].detach().cpu(),
+            "staged": None if staged is None else [None if s is None else (s[0].detach().cpu(), s[1].detach().cpu())
+                                                   for s in staged]}
 
 
 def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = None, trainer_state: Optional[dict] = None):
@@ -92,6 +95,8 @@ def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
             for grp, lr in zip(optimizer.param_groups, st["lrs"]):
                 grp["lr"] = lr
             optimizer._resume = (st["exp_avg"], st["exp_avg_sq"])      # consumed by FlatAdam._build
+            if st.get("staged") is not None:
+                optimizer._staged = st["staged"]
     if restore_rng and res is not None:
         torch.set_rng_state(res["torch_rng"])
         if res.get("cuda_rng") is not None and splatter is not None:

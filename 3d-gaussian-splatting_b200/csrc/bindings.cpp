@@ -928,6 +928,120 @@ std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_stats(
   return densify_apply(pos, rgb, opa, quat, scale, nullptr, scale_activation, 0.0, gen, code, dst, feat);
 }
 
+// shapes shared by the MCMC entries: pos [n,3], rgb [n,d], opa [n], quat [n,4], scale [n,3], feat [n,f] or None
+static void mcmc_check_params(const char* who, const torch::Tensor& pos, const torch::Tensor& rgb,
+                              const torch::Tensor& opa, const torch::Tensor& quat, const torch::Tensor& scale,
+                              const c10::optional<torch::Tensor>& feat) {
+  GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+  const int64_t n = pos.size(0);
+  TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && rgb.dim() == 2 && rgb.size(0) == n && opa.numel() == n &&
+                  quat.dim() == 2 && quat.size(0) == n && quat.size(1) == 4 && scale.dim() == 2 && scale.size(0) == n &&
+                  scale.size(1) == 3 && n < (int64_t(1) << 31),
+              who, ": bad shapes");
+  for (const torch::Tensor* t : {&rgb, &opa, &quat, &scale})
+    TORCH_CHECK(t->device() == pos.device(), who, ": the parameters must be on one device");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(quat.data_ptr()) % 16 == 0, who,
+              ": quat must be 16-byte aligned (its rows are read as float4)");
+  if (feat) {
+    GS_CHECK_F32(*feat);
+    TORCH_CHECK(feat->dim() == 2 && feat->size(0) == n && feat->device() == pos.device(), who, ": feat must be [n, f]");
+  }
+}
+
+// MCMC relocation in place (gs_mcmc_relocate).  u: float32 [n] uniforms; moments: flat Adam buffers + segment table
+// (or None); touched: uint8 [n] or None.  Returns the relocated count as a device int32 [1] (no host sync).
+torch::Tensor mcmc_relocate(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                            torch::Tensor scale, c10::optional<torch::Tensor> feat, int scale_activation,
+                            double min_opacity, torch::Tensor u, c10::optional<torch::Tensor> exp_avg,
+                            c10::optional<torch::Tensor> exp_avg_sq, std::vector<int64_t> seg_starts,
+                            std::vector<int64_t> seg_widths, c10::optional<torch::Tensor> touched) {
+  mcmc_check_params("mcmc_relocate", pos, rgb, opa, quat, scale, feat);
+  const int64_t n = pos.size(0);
+  GS_CHECK_F32(u);
+  TORCH_CHECK(u.numel() == n && u.device() == pos.device(), "mcmc_relocate: u must have n elements");
+  TORCH_CHECK(exp_avg.has_value() == exp_avg_sq.has_value(), "mcmc_relocate: give both moment buffers or neither");
+  long long n_flat = 0;
+  if (exp_avg) {
+    GS_CHECK_F32(*exp_avg); GS_CHECK_F32(*exp_avg_sq);
+    TORCH_CHECK(exp_avg->numel() == exp_avg_sq->numel() && exp_avg->device() == pos.device() &&
+                    exp_avg_sq->device() == pos.device(),
+                "mcmc_relocate: the moment buffers must match and be on the parameters' device");
+    TORCH_CHECK(seg_starts.size() == seg_widths.size() && !seg_starts.empty(),
+                "mcmc_relocate: one start and width per segment");
+    n_flat = exp_avg->numel();
+  }
+  if (touched)
+    TORCH_CHECK(touched->is_cuda() && touched->is_contiguous() && touched->scalar_type() == at::kByte &&
+                    touched->numel() == n && touched->device() == pos.device(),
+                "mcmc_relocate: touched must be a contiguous CUDA uint8 tensor [n]");
+  std::vector<long long> starts(seg_starts.begin(), seg_starts.end());
+  std::vector<int> widths;
+  for (int64_t w : seg_widths) {
+    TORCH_CHECK(w >= 1 && w < (int64_t(1) << 31), "mcmc_relocate: bad segment width");
+    widths.push_back((int)w);
+  }
+  c10::cuda::CUDAGuard guard(pos.device());
+  auto ws = torch::empty({(int64_t)gs_mcmc_workspace_bytes((int)n)}, pos.options().dtype(at::kByte));
+  auto n_rel = torch::zeros({1}, pos.options().dtype(at::kInt));
+  check_rc(gs_mcmc_relocate(fpm(pos), fpm(rgb), fpm(opa), fpm(quat), fpm(scale), feat ? fpm(*feat) : nullptr,
+                            feat ? (int)feat->size(1) : 0, (int)n, (int)rgb.size(1), scale_activation,
+                            (float)min_opacity, fp(u), exp_avg ? fpm(*exp_avg) : nullptr,
+                            exp_avg_sq ? fpm(*exp_avg_sq) : nullptr, n_flat, exp_avg ? starts.data() : nullptr,
+                            exp_avg ? widths.data() : nullptr, exp_avg ? (int)starts.size() : 0,
+                            touched ? touched->data_ptr<uint8_t>() : nullptr, n_rel.data_ptr<int>(), ws.data_ptr(),
+                            (size_t)ws.numel(), cur_stream()),
+           "gs_mcmc_relocate");
+  return n_rel;
+}
+
+// MCMC growth (gs_mcmc_add): u.numel() new Gaussians; returns the new [n + n_new] tensors (pos, rgb, opa, quat, scale
+// and feat when given)
+std::vector<torch::Tensor> mcmc_add(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                                    torch::Tensor scale, c10::optional<torch::Tensor> feat, int scale_activation,
+                                    double min_opacity, torch::Tensor u) {
+  mcmc_check_params("mcmc_add", pos, rgb, opa, quat, scale, feat);
+  GS_CHECK_F32(u);
+  TORCH_CHECK(u.dim() == 1 && u.device() == pos.device(), "mcmc_add: u must be a 1-D tensor on the parameters' device");
+  const int64_t n = pos.size(0), n_new = u.numel(), m = n + n_new, d = rgb.size(1);
+  TORCH_CHECK(m < (int64_t(1) << 31), "mcmc_add: n + n_new too large");
+  c10::cuda::CUDAGuard guard(pos.device());
+  auto ws = torch::empty({(int64_t)gs_mcmc_workspace_bytes((int)std::max(n, n_new))}, pos.options().dtype(at::kByte));
+  std::vector<torch::Tensor> out = {torch::empty({m, 3}, pos.options()), torch::empty({m, d}, pos.options()),
+                                    torch::empty(opa.dim() == 2 ? std::vector<int64_t>{m, 1} : std::vector<int64_t>{m},
+                                                 pos.options()),
+                                    torch::empty({m, 4}, pos.options()), torch::empty({m, 3}, pos.options())};
+  if (feat) out.push_back(torch::empty({m, feat->size(1)}, pos.options()));
+  check_rc(gs_mcmc_add(fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), feat ? fp(*feat) : nullptr,
+                       feat ? (int)feat->size(1) : 0, (int)n, (int)d, scale_activation, (float)min_opacity, (int)n_new,
+                       fp(u), fpm(out[0]), fpm(out[1]), fpm(out[2]), fpm(out[3]), fpm(out[4]),
+                       feat ? fpm(out[5]) : nullptr, ws.data_ptr(), (size_t)ws.numel(), cur_stream()),
+           "gs_mcmc_add");
+  return out;
+}
+
+// MCMC position noise in place (gs_mcmc_noise); z: float32 [n, 3] or None (Philox stream keyed by seed)
+void mcmc_noise(torch::Tensor pos, torch::Tensor quat, torch::Tensor scale, torch::Tensor opa, int scale_activation,
+                double scaler, int64_t seed, c10::optional<torch::Tensor> z) {
+  GS_CHECK_F32(pos); GS_CHECK_F32(quat); GS_CHECK_F32(scale); GS_CHECK_F32(opa);
+  const int64_t n = pos.size(0);
+  TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && quat.dim() == 2 && quat.size(0) == n && quat.size(1) == 4 &&
+                  scale.dim() == 2 && scale.size(0) == n && scale.size(1) == 3 && opa.numel() == n &&
+                  n < (int64_t(1) << 31),
+              "mcmc_noise: bad shapes");
+  for (const torch::Tensor* t : {&quat, &scale, &opa})
+    TORCH_CHECK(t->device() == pos.device(), "mcmc_noise: the parameters must be on one device");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(quat.data_ptr()) % 16 == 0,
+              "mcmc_noise: quat must be 16-byte aligned (its rows are read as float4)");
+  if (z) {
+    GS_CHECK_F32(*z);
+    TORCH_CHECK(z->numel() == 3 * n && z->device() == pos.device(), "mcmc_noise: z must be [n, 3]");
+  }
+  c10::cuda::CUDAGuard guard(pos.device());
+  check_rc(gs_mcmc_noise(fpm(pos), fp(quat), fp(scale), fp(opa), (int)n, scale_activation, (float)scaler,
+                         (unsigned long long)seed, z ? fp(*z) : nullptr, cur_stream()),
+           "gs_mcmc_noise");
+}
+
 // NVLS in-place all-reduce of a symmetric flat buffer (multicast address as an integer)
 void allreduce_multimem(int64_t multicast_ptr, int64_t n_floats, int rank, int world, int device) {
   c10::cuda::CUDAGuard guard(c10::Device(c10::kCUDA, (c10::DeviceIndex)device));
@@ -1075,6 +1189,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("count"), py::arg("max_radius"), py::arg("max_screen_px"), py::arg("scale_activation"),
         py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("tau"),
         py::arg("use_clone"), py::arg("use_split"), py::arg("generator") = py::none(), py::arg("feat") = py::none());
+  m.def("mcmc_relocate", &mcmc_relocate, "MCMC relocation of dead Gaussians, in place (gs_mcmc_relocate)",
+        py::arg("pos"), py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("feat"),
+        py::arg("scale_activation"), py::arg("min_opacity"), py::arg("u"), py::arg("exp_avg") = py::none(),
+        py::arg("exp_avg_sq") = py::none(), py::arg("seg_starts") = std::vector<int64_t>{},
+        py::arg("seg_widths") = std::vector<int64_t>{}, py::arg("touched") = py::none());
+  m.def("mcmc_add", &mcmc_add, "MCMC growth: u.numel() Gaussians appended (gs_mcmc_add)", py::arg("pos"),
+        py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("feat"),
+        py::arg("scale_activation"), py::arg("min_opacity"), py::arg("u"));
+  m.def("mcmc_noise", &mcmc_noise, "MCMC position noise, in place (gs_mcmc_noise)", py::arg("pos"), py::arg("quat"),
+        py::arg("scale"), py::arg("opa"), py::arg("scale_activation"), py::arg("scaler"), py::arg("seed"),
+        py::arg("z") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
   m.def("adam_step_visible", &adam_step_visible,

@@ -36,6 +36,8 @@ class FlatAdam:
         self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
         self.step_count = 0
         self._flat = None          # (flat_param, exp_avg, exp_avg_sq, ordered params, segment ends)
+        self._staged = None        # moments carried over a change of n: see replace_params
+        self._zero_rows = None     # rows whose restored moments the next _build zeroes: see zero_moment_rows
 
     def zero_grad(self, set_to_none: bool = True):
         for g in self.param_groups:
@@ -74,7 +76,75 @@ class FlatAdam:
             v.copy_(resume[1])
             self._keep_step = True
         self._resume = None
+        if self._staged is not None:                     # the old rows lead each segment; the new rows stay zero
+            everyone = self._all_params()
+            for p in ordered:
+                k = next(i for i, q in enumerate(everyone) if q is p)
+                if self._staged[k] is not None:
+                    o, sm, sv = p.data.storage_offset(), self._staged[k][0], self._staged[k][1]
+                    m[o:o + sm.numel()].copy_(sm.reshape(-1))
+                    v[o:o + sv.numel()].copy_(sv.reshape(-1))
+            self._staged = None
+            self._keep_step = True
+        if self._zero_rows is not None:                  # rows relocated between a checkpoint load and this build
+            rows = self._zero_rows.to(flat.device)
+            for p in ordered:
+                if p.dim() and p.shape[0] == rows.numel():
+                    o = p.data.storage_offset()
+                    for t in (m, v):
+                        t[o:o + p.numel()].view(rows.numel(), -1).masked_fill_(rows.view(-1, 1), 0.0)
+            self._zero_rows = None
         self._flat = (flat, m, v, ordered, ends, base)
+
+    def _all_params(self):
+        return [p for g in self.param_groups for p in g["params"]]
+
+    def live_moments(self, params):
+        """(exp_avg, exp_avg_sq, starts, widths) of the flat moment buffers when every parameter they hold is one of
+        `params` and still aliases the flat buffer (all with the same row count), else None (before the first step,
+        or after `replace_params` until the next one)."""
+        if self._flat is None or self._staged is not None:
+            return None
+        flat, m, v, ordered, _, _ = self._flat
+        store = flat.untyped_storage().data_ptr()
+        if any(not any(p is q for q in params) for p in ordered) \
+                or any(p.data.untyped_storage().data_ptr() != store for p in ordered):
+            return None
+        n = ordered[0].shape[0]
+        return m, v, [p.data.storage_offset() for p in ordered], [p.numel() // max(n, 1) for p in ordered]
+
+    @torch.no_grad()
+    def zero_moment_rows(self, rows):
+        """Zero the moments of rows `rows` (bool [n]) of every parameter with n rows while they are not in a live
+        flat buffer (`live_moments` is None): the moments `replace_params` staged, and the moments a checkpoint
+        restored, which the next `_build` places and then zeroes at those rows.  Exact zeros; nothing else changes."""
+        for s in self._staged or []:
+            for t in s or ():
+                if t.dim() and t.shape[0] == rows.numel():
+                    t.masked_fill_(rows.to(t.device).view((-1,) + (1,) * (t.dim() - 1)), 0.0)
+        resume = getattr(self, "_resume", None)
+        if resume is not None and resume[0] is not None:
+            self._zero_rows = rows.clone() if self._zero_rows is None else self._zero_rows | rows
+
+    @torch.no_grad()
+    def replace_params(self, pairs):
+        """Point `param_groups` at new Parameters, `pairs` = [(old, new)], where the first rows of each new Parameter
+        continue the old one's rows (growth).  The moments of the old rows are staged and the next step's `_build`
+        puts them in the first rows of the new segments and zeroes the rest; `step_count` is kept.  A checkpoint taken
+        before that step saves the staged moments."""
+        old = self._all_params()
+        staged = list(self._staged) if self._staged is not None else [None] * len(old)
+        if self._staged is None and self._flat is not None:
+            flat, m, v, ordered, _, _ = self._flat
+            store = flat.untyped_storage().data_ptr()
+            for k, p in enumerate(old):
+                if any(p is q for q in ordered) and p.data.untyped_storage().data_ptr() == store:
+                    o = p.data.storage_offset()
+                    staged[k] = (m[o:o + p.numel()].view(p.shape), v[o:o + p.numel()].view(p.shape))
+        for g in self.param_groups:
+            g["params"] = [next((nw for od, nw in pairs if od is p), p) for p in g["params"]]
+        self._staged = staged if any(s is not None for s in staged) else None
+        self._flat = None
 
     @torch.no_grad()
     def step(self, visible=None):

@@ -167,6 +167,39 @@ def _check_features(n_features, use_sh_coeff, sh_eval, densify_stats):
         raise ValueError("features are not available with densify_stats='absgrad' (use 'grad')")
 
 
+def _zero_moment_rows(optimizer, params, rows):
+    """Zero the Adam moments of rows `rows` (CUDA bool [n]) of `params`: `torch.optim.Adam`'s per-parameter state, or
+    `optim.FlatAdam`'s moments that are not in a live flat buffer (`FlatAdam.zero_moment_rows`).  masked_fill_ writes
+    exact zeros and leaves other bits alone."""
+    import optim
+    if isinstance(optimizer, optim.FlatAdam):
+        optimizer.zero_moment_rows(rows)
+        return
+    for p in params:
+        for t in optimizer.state.get(p, {}).values():
+            if torch.is_tensor(t) and t.dim() > 0 and t.shape[0] == rows.numel():
+                t.masked_fill_(rows.view((-1,) + (1,) * (t.dim() - 1)), 0.0)
+
+
+def _regrow_optimizer(optimizer, pairs):
+    """Re-point an optimizer from the old Parameters to the grown ones (`pairs` = [(old, new)], the old rows first):
+    `optim.FlatAdam` stages its moments (`replace_params`); `torch.optim.Adam`'s per-parameter state is re-keyed and its
+    row tensors padded with zero rows."""
+    import optim
+    if isinstance(optimizer, optim.FlatAdam):
+        optimizer.replace_params(pairs)
+        return
+    for old, new in pairs:
+        st = optimizer.state.pop(old, None)
+        if st is not None:
+            for k, t in list(st.items()):
+                if torch.is_tensor(t) and t.dim() > 0 and t.shape[0] == old.shape[0]:
+                    st[k] = torch.cat([t, t.new_zeros((new.shape[0] - old.shape[0],) + tuple(t.shape[1:]))])
+            optimizer.state[new] = st
+    for grp in optimizer.param_groups:
+        grp["params"] = [next((nw for od, nw in pairs if od is p), p) for p in grp["params"]]
+
+
 class Tiles:
     """Padded render-target geometry (reference splatter.py:255-272)."""
 
@@ -565,6 +598,95 @@ class Splatter(nn.Module):
         self.n_gaussians = g.pos.shape[0]
         st.reset(self.n_gaussians)
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.n_gaussians)
+
+    # -- MCMC densification (3DGS-MCMC; mcmc.MCMC schedules these) -----------------------------------------------------
+    def _mcmc_params(self):
+        g = self.gaussian_3ds
+        return [g.pos, g.rgb, g.opa, g.quat, g.scale] + ([g.feat] if g.feat is not None else [])
+
+    def _scale_act(self):
+        if self.scale_activation not in ("abs", "exp"):
+            raise ValueError("scale_activation must be 'abs' or 'exp'")
+        return 0 if self.scale_activation == "abs" else 1
+
+    @torch.no_grad()
+    def mcmc_relocate(self, optimizer=None, min_opacity=0.005, generator=None):
+        """Move every dead Gaussian (sigmoid(opa) <= min_opacity) onto a live one drawn with probability proportional
+        to its opacity, and split the drawn ones' opacity and scale among their copies (gsplat's `relocate`;
+        `gaussian.mcmc_relocate`).  In place: the Parameters keep their identity (and `optim.FlatAdam`'s aliasing).
+        The Adam moments of every source and destination row are zeroed (`optim.FlatAdam` or `torch.optim.Adam`; the
+        rows of Parameters the optimizer does not hold have no state to zero); nothing before the optimizer's first
+        step.  The uniforms come from torch's generator (`generator`, default CUDA), so replicas seeded alike stay
+        identical.  Returns the relocated count as a CUDA int32 [1] tensor (no host synchronisation)."""
+        import optim
+        g = self.gaussian_3ds
+        n = g.pos.shape[0]
+        u = torch.rand(n, device=self.device, generator=generator)
+        mom = optimizer.live_moments(self._mcmc_params()) if isinstance(optimizer, optim.FlatAdam) else None
+        touched = None
+        if optimizer is not None and mom is None:
+            touched = torch.zeros(n, device=self.device, dtype=torch.uint8)
+        kw = {}
+        if mom is not None:
+            kw = dict(exp_avg=mom[0], exp_avg_sq=mom[1], seg_starts=mom[2], seg_widths=mom[3])
+        n_rel = gaussian.mcmc_relocate(g.pos.data, g.rgb.data, g.opa.data, g.quat.data, g.scale.data,
+                                       None if g.feat is None else g.feat.data, self._scale_act(), float(min_opacity),
+                                       u, touched=touched, **kw)
+        if touched is not None:
+            _zero_moment_rows(optimizer, self._mcmc_params(), touched.bool())
+        return n_rel
+
+    @torch.no_grad()
+    def mcmc_add(self, cap_max, growth=1.05, optimizer=None, generator=None, min_opacity=0.005):
+        """Grow to min(cap_max, int(growth n)) Gaussians (gsplat's `sample_add`; `gaussian.mcmc_add`): each new one is
+        a copy of a Gaussian drawn with probability proportional to its opacity, and the drawn ones' opacity and scale
+        are split as in `mcmc_relocate`.  New Parameters, like `adaptive_control`; the optimizer (`optim.FlatAdam` or
+        `torch.optim.Adam`) is re-pointed at them and keeps the moments of the existing rows bit for bit, the new rows
+        start at zero.  `densify_stats` and the visible mask re-size from zero.  Returns the number added (host int,
+        computed from the sizes: no synchronisation)."""
+        g = self.gaussian_3ds
+        n = g.pos.shape[0]
+        n_new = max(0, min(int(cap_max), int(float(growth) * n)) - n)
+        if n_new == 0:
+            return 0
+        u = torch.rand(n_new, device=self.device, generator=generator)
+        old = self._mcmc_params()
+        new = gaussian.mcmc_add(g.pos.data, g.rgb.data, g.opa.data, g.quat.data, g.scale.data,
+                                None if g.feat is None else g.feat.data, self._scale_act(), float(min_opacity), u)
+        g._replace(new)
+        if optimizer is not None:
+            _regrow_optimizer(optimizer, list(zip(old, self._mcmc_params())))
+        self.n_gaussians = g.pos.shape[0]
+        self._size_densify_stats()
+        return n_new
+
+    @torch.no_grad()
+    def mcmc_noise(self, scaler, seed=None):
+        """Perturb the positions by scaler g(o) R diag(s^2) R^T z (gsplat's `inject_noise_to_position`;
+        `gaussian.mcmc_noise`), z from a Philox stream keyed by (seed, Gaussian index).  `seed` None draws one from
+        torch's CPU generator, which checkpoints restore.  Writes `pos` only."""
+        g = self.gaussian_3ds
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)))
+        gaussian.mcmc_noise(g.pos.data, g.quat.data, g.scale.data, g.opa.data, self._scale_act(), float(scaler),
+                            int(seed))
+
+    @torch.no_grad()
+    def add_mcmc_regularizer_grads(self, opacity_reg=0.01, scale_reg=0.01):
+        """Add the gradients of MCMC's opacity_reg mean(sigmoid(opa)) + scale_reg mean(s) to `opa.grad` and
+        `scale.grad`, in place: after the backward (and any gradient exchange), before the step, so that they stay
+        views of the flat gradient bucket and every replica adds the same values."""
+        g = self.gaussian_3ds
+        if g.opa.grad is None or g.scale.grad is None:
+            raise RuntimeError("add_mcmc_regularizer_grads: run the backward first (opa.grad / scale.grad are None)")
+        n = g.pos.shape[0]
+        if opacity_reg and n:
+            o = torch.sigmoid(g.opa.detach())
+            g.opa.grad.add_(o * (1 - o), alpha=float(opacity_reg) / n)
+        if scale_reg and n:
+            raw = g.scale.detach()
+            ds = torch.exp(raw) if self._scale_act() == 1 else torch.sign(raw)
+            g.scale.grad.add_(ds, alpha=float(scale_reg) / (3 * n))
 
     @torch.no_grad()
     def visible_mask(self, accumulate=False):

@@ -51,10 +51,14 @@ def make_optimizer(sp, lr=0.003, fused=True):
         {"params": g.scale, "lr": lr}, {"params": g.quat, "lr": lr}], betas=(0.9, 0.99))
 
 
-def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False):
+def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None):
     opt = make_optimizer(sp, lr, fused_adam)
     params = list(sp.gaussian_3ds.parameters())
     bucket = dp.make_grad_bucket(params, average=True)   # peer-memory exchange when available, else NCCL
+    mc = None
+    if cap_max is not None:                                           # MCMC densification, refining every 100 steps
+        import mcmc
+        mc = mcmc.MCMC(sp, opt, cap_max, refine_start=min(500, iters // 4), refine_stop=max(iters - 100, 0))
     hist = []
     torch.cuda.synchronize()
     t0 = time.time()
@@ -65,17 +69,25 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
         loss = (img - gts[view]).abs().mean()                        # train.py:99
         loss.backward()
         bucket.allreduce()
+        if mc is not None:                                            # after the exchange: every rank adds the same
+            mc.after_backward(it)
         if visible_adam:                                              # step only the Gaussians some rank binned
             opt.step(visible=dp.all_reduce_visible(sp.visible_mask()))
         else:
             opt.step()
+        if mc is not None:
+            n = sp.gaussian_3ds.pos.shape[0]
+            mc.after_step(it, lr)
+            if sp.gaussian_3ds.pos.shape[0] != n:                     # grown: the exchange follows the new Parameters
+                bucket.params = list(sp.gaussian_3ds.parameters())
         if it % log_every == 0 or it == iters - 1:
             with torch.no_grad():
                 mse = ((img - gts[view]) ** 2).mean()
                 psnr = float(-10 * torch.log10(mse + 1e-12))
             hist.append((it, float(loss), psnr))
             if rank == 0:
-                print(f"iter {it:5d}  L1 {float(loss):.5f}  PSNR {psnr:6.2f} dB  view {view}", flush=True)
+                print(f"iter {it:5d}  L1 {float(loss):.5f}  PSNR {psnr:6.2f} dB  view {view}  "
+                      f"n {sp.gaussian_3ds.pos.shape[0]}", flush=True)
     torch.cuda.synchronize()
     return hist, iters / (time.time() - t0)
 
@@ -89,9 +101,16 @@ def main():
     ap.add_argument("--torch-adam", action="store_true", help="use torch.optim.Adam instead of the fused flat Adam")
     ap.add_argument("--visible-adam", action="store_true",
                     help="update only the Gaussians binned this step (3DGS sparse Adam); unseen ones stay frozen")
+    ap.add_argument("--mcmc", action="store_true",
+                    help="MCMC densification (3DGS-MCMC, mcmc.MCMC): relocate dead Gaussians and grow to --cap-max "
+                         "every 100 steps, position noise every step; with --visible-adam the opacity and scale "
+                         "regularisers reach only the visible rows, like every other gradient")
+    ap.add_argument("--cap-max", type=int, default=None, help="Gaussian count cap of --mcmc (default 1.5 x --gaussians)")
     args = ap.parse_args()
     if args.visible_adam and args.torch_adam:
         ap.error("--visible-adam is a mode of the fused flat Adam")
+    if args.cap_max is not None and not args.mcmc:
+        ap.error("--cap-max needs --mcmc")
     w, h = (int(x) for x in args.res.split("x"))
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
@@ -101,10 +120,11 @@ def main():
     torch.manual_seed(2023)                                           # identical torch RNG on all ranks
     sp, gts = build(args.gaussians, w, h, args.views, dev)
     hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam,
-                      visible_adam=args.visible_adam)
+                      visible_adam=args.visible_adam,
+                      cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
-              f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB")
+              f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians")
     if world > 1:
         torch.distributed.destroy_process_group()
 

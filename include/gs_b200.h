@@ -513,6 +513,50 @@ int gs_densify_plan_stats(const float* opa, const float* scale, const float* acc
                           int use_split, unsigned char* code, int* dst, void* workspace, size_t workspace_bytes,
                           gs_stream_t stream);
 
+/* MCMC densification (3DGS-MCMC, Kheradmand et al. 2024), an opt-in alternative to prune / clone / split.  o =
+ * sigmoid(opa); s = the activated scale (|raw| + 1e-4 or exp(raw)).  A draw picks source i with probability
+ * proportional to its weight w_i = round(o_i 2^32) (an integer; round half to even; o below 2^-33 weighs 0): with the
+ * caller's uniforms u_j in [0, 1) and C the inclusive integer prefix sum of the weights, t_j = min(floor(u_j C_{n-1}),
+ * C_{n-1} - 1) (the product in fp64) and src_j = min{i : C_i > t_j}.  A source drawn r - 1 times (r clamped to 51) gets
+ *   o' = 1 - (1 - o)^(1/r),  s' = o / den * s,  den = sum_{a=1..r} sum_{b=0..a-1} C(a-1, b) (-1)^b o'^(b+1) / sqrt(b+1)
+ * (fp64), then o' is clamped to [min_opacity, 1 - 2^-23] and stored as its logit; s' is inverted with the activation
+ * (exp: log s'; abs: sign(raw) max(s' - 1e-4, 0), sign(0) = +, so an s' below 1e-4 becomes the raw scale 0).  Every
+ * destination row is a copy of its source with (o', s'), and the source takes the same (o', s').  The prefix sums and
+ * the counts are integer sums, so for the same inputs every call draws the same sources and writes the same bits (on
+ * every data-parallel replica too), whatever order the device adds them in.  No entry synchronises.
+ *   gs_mcmc_workspace_bytes(n): a sampler over n Gaussians with up to n draws.
+ *   gs_mcmc_relocate (gsplat's relocate): in place.  Dead Gaussians (o <= min_opacity) are the destinations, in
+ *     ascending order, with one draw each from the alive ones (u[n]: the first k are used, k = the number of dead).
+ *     With exp_avg / exp_avg_sq (flat buffers and segment table as gs_adam_step_visible takes them, rows = n; NULL =
+ *     no optimizer state) the moment rows of every source and destination are zeroed in every segment: gsplat zeroes
+ *     the sources only, but a relocated row is a new Gaussian that a dead one's moments must not steer.  touched
+ *     (nullable uint8 [n]) gets 1 at those rows and is otherwise left alone.  *n_relocated (DEVICE int) = k, or 0
+ *     when nothing is alive.  Nothing else of the parameters or moments is written.
+ *   gs_mcmc_add (gsplat's sample_add): n_new draws over all n Gaussians with weights o (u[n_new]); out_* are
+ *     caller-allocated [n + n_new] rows: rows 0 .. n-1 are the input with the sources' (o', s'), row n + j the copy of
+ *     src_j.  Workspace: gs_mcmc_workspace_bytes(max(n, n_new)).  feat / out_feat: optional [.., f] feature rows.  When
+ *     every weight is 0 (every opacity below 2^-33) there is nothing to draw from: the n_new appended rows are then
+ *     copies of row 0, unchanged, and row 0 keeps its values.
+ *   gs_mcmc_noise (gsplat's inject_noise_to_position): pos_i += scaler g(o_i) R diag(s^2) R^T z_i with R of the
+ *     normalised quaternion and g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))); z_i = z[i] (nullable [n][3]) or three
+ *     normals of the Philox4x32-10 stream (seed, subsequence i).  Writes pos only; one launch.
+ * GS_ERR_INVALID_ARG, before any launch: n or n_new < 0; a NULL pointer that the call needs with n > 0; d not 3 / 27 /
+ * 48; f not 8 / 16 / 32 with feat; an unknown activation; min_opacity outside (0, 1); a non-finite scaler; a short
+ * workspace; one moment buffer without the other; a segment table gs_adam_step_visible would refuse.  quat (and
+ * out_quat) rows are read and written as float4: the pointers must be 16-byte aligned. */
+size_t gs_mcmc_workspace_bytes(int n);
+int gs_mcmc_relocate(float* pos, float* rgb, float* opa, float* quat, float* scale, float* feat /* nullable */, int f,
+                     int n, int d, int scale_activation, float min_opacity, const float* u, float* exp_avg,
+                     float* exp_avg_sq, long long n_flat, const long long* seg_start_host, const int* seg_width_host,
+                     int n_seg, unsigned char* touched /* nullable */, int* n_relocated, void* workspace,
+                     size_t workspace_bytes, gs_stream_t stream);
+int gs_mcmc_add(const float* pos, const float* rgb, const float* opa, const float* quat, const float* scale,
+                const float* feat /* nullable */, int f, int n, int d, int scale_activation, float min_opacity,
+                int n_new, const float* u, float* out_pos, float* out_rgb, float* out_opa, float* out_quat,
+                float* out_scale, float* out_feat, void* workspace, size_t workspace_bytes, gs_stream_t stream);
+int gs_mcmc_noise(float* pos, const float* quat, const float* scale, const float* opa, int n, int scale_activation,
+                  float scaler, unsigned long long seed, const float* z /* nullable */, gs_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * Next-row widening (SURVEY.md §8 f-3): the training loss of reference train.py:99-107 on the device,
  * forward and backward in two kernels, producing the image gradient in the layout

@@ -7,7 +7,8 @@ true resume needs under the extra key `"resume"`: optimizer moments and step cou
 densification statistics of train.py:82-83, and the RNG states (numpy picks the camera, train.py:93;
 torch samples split positions, utils.py:391-402).  A scene with per-Gaussian features
 (`Splatter(..., n_features=F)`) also stores them under `"feat"` [n, F].  Extra keys are ignored by the reference's
-loader.
+loader.  A scene with Mip-Splatting's 3-D filter (`Splatter(..., filter3d=True)`) stores the filter under
+`"filter3d"` [n], so that a resume renders the same bits; loading a file without it recomputes the filter.
 """
 from __future__ import annotations
 
@@ -42,6 +43,8 @@ def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = N
     ckpt = {k: getattr(g, k).detach().clone() for k in KEYS}
     if g.feat is not None:
         ckpt["feat"] = g.feat.detach().clone()
+    if getattr(splatter, "filter3d", None) is not None:
+        ckpt["filter3d"] = splatter.filter3d.detach().clone()
     ckpt["resume"] = {
         "iteration": iteration,
         "optimizer": _optimizer_state(optimizer),
@@ -86,6 +89,12 @@ def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
             elif g.feat is not None:
                 g.feat = torch.nn.Parameter(torch.zeros(n, splatter.n_features, device=splatter.device))
         splatter.n_gaussians = g.pos.shape[0]
+        if getattr(splatter, "use_filter3d", False):
+            f3 = ckpt.get("filter3d")
+            if f3 is not None and f3.numel() == n:
+                splatter._set_filter3d(f3)
+            else:
+                splatter.compute_filter3d()
     if optimizer is not None and res is not None and res.get("optimizer") is not None:
         st = res["optimizer"]
         if st["kind"] == "torch":

@@ -295,6 +295,78 @@ struct RenderContext {
     check_rc(gs_ctx_set_filter2d(ctx, mode, (float)variance), "gs_ctx_set_filter2d");
   }
 
+  // 3-D smoothing filter (gs_ctx_set_filter3d): a contiguous float32 CUDA tensor [n] on this context's device, or None
+  // (off); applies to the forwards that follow, a backward uses the filter of its forward.  The context keeps the
+  // tensor alive while it is set.
+  torch::Tensor filter3d_ref;
+  void set_filter3d(std::optional<torch::Tensor> f) {
+    if (!f) {
+      check_rc(gs_ctx_set_filter3d(ctx, nullptr, 0), "gs_ctx_set_filter3d");
+      filter3d_ref = torch::Tensor();
+      return;
+    }
+    TORCH_CHECK(f->is_cuda() && f->scalar_type() == at::kFloat && f->is_contiguous() && f->dim() == 1,
+                "set_filter3d: filter3d must be a contiguous 1-D float32 CUDA tensor");
+    TORCH_CHECK(f->device().index() == device, "set_filter3d: filter3d is on another device than the context");
+    TORCH_CHECK(f->numel() < (int64_t(1) << 31), "set_filter3d: n too large");
+    check_rc(gs_ctx_set_filter3d(ctx, fp(*f), (int)f->numel()), "gs_ctx_set_filter3d");
+    filter3d_ref = *f;
+  }
+
+  // gs_filter3d_compute over V views: size [V,2] = (width, height), focal [V,2] = (fx, fy), rot [V,3,3], tran [V,3]
+  // (CPU tensors), one near plane; writes and returns out [n] (allocated when None)
+  torch::Tensor filter3d_compute(torch::Tensor pos, torch::Tensor size, torch::Tensor focal, torch::Tensor rot,
+                                 torch::Tensor tran, double near, double margin, double variance,
+                                 std::optional<torch::Tensor> out) {
+    const char* fn = "filter3d_compute";
+    GS_CHECK_F32(pos);
+    TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && pos.size(0) < (int64_t(1) << 31), fn, ": pos must be [n,3]");
+    TORCH_CHECK(pos.device().index() == device, fn, ": pos is on another device than the context");
+    TORCH_CHECK(!size.is_cuda() && !focal.is_cuda() && !rot.is_cuda() && !tran.is_cuda(), fn,
+                ": size / focal / rot / tran must be CPU tensors (cameras are host data)");
+    const int64_t v = size.dim() == 2 ? size.size(0) : -1;
+    TORCH_CHECK(v >= 1 && v < (int64_t(1) << 31) && size.size(1) == 2 && focal.dim() == 2 && focal.size(0) == v &&
+                    focal.size(1) == 2 && rot.dim() == 3 && rot.size(0) == v && rot.size(1) == 3 && rot.size(2) == 3 &&
+                    tran.dim() == 2 && tran.size(0) == v && tran.size(1) == 3,
+                fn, ": size and focal must be [V,2], rot [V,3,3] and tran [V,3] with V >= 1");
+    const int64_t n = pos.size(0);
+    torch::Tensor f;
+    if (out) {
+      f = *out;
+      TORCH_CHECK(f.is_cuda() && f.scalar_type() == at::kFloat && f.is_contiguous() && f.dim() == 1 && f.numel() == n &&
+                      f.device() == pos.device(),
+                  fn, ": out must be a contiguous float32 CUDA tensor [n] on pos's device");
+    } else {
+      f = torch::empty({n}, pos.options());
+    }
+    auto sz = size.to(at::kLong).contiguous();
+    auto fc = focal.to(at::kFloat).contiguous();
+    auto r = rot.to(at::kFloat).contiguous();
+    auto t = tran.to(at::kFloat).contiguous();
+    auto sa = sz.accessor<int64_t, 2>();
+    auto fa = fc.accessor<float, 2>();
+    std::vector<gs_camera> cams((size_t)v);
+    for (int64_t k = 0; k < v; ++k) {
+      gs_camera& cm = cams[(size_t)k];
+      cm = gs_camera{};
+      TORCH_CHECK(sa[k][0] > 0 && sa[k][0] < (int64_t(1) << 31) && sa[k][1] > 0 && sa[k][1] < (int64_t(1) << 31), fn,
+                  ": bad view size");
+      cm.width = (int)sa[k][0];
+      cm.height = (int)sa[k][1];
+      cm.focal_x = fa[k][0];
+      cm.focal_y = fa[k][1];
+      memcpy(cm.rot, r[k].data_ptr<float>(), sizeof(cm.rot));
+      memcpy(cm.tran, t[k].data_ptr<float>(), sizeof(cm.tran));
+      cm.near_plane = (float)near;
+      cm.tile_thresh = 0.05f;
+    }
+    c10::cuda::CUDAGuard guard(pos.device());
+    check_rc(gs_filter3d_compute(ctx, fp(pos), (int)n, cams.data(), (int)v, (float)margin, (float)variance, fpm(f),
+                                 cur_stream()),
+             "gs_filter3d_compute");
+    return f;
+  }
+
   // screen-space densification statistics (gs_ctx_set_densify_stats): accumulated by every backward that computes
   // parameter gradients until cleared.  The context keeps the tensors alive while they are set.
   std::vector<torch::Tensor> densify_stats_refs;
@@ -1164,6 +1236,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("stats", &RenderContext::stats)
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
+      .def("set_filter3d", &RenderContext::set_filter3d, py::arg("filter3d"))
       .def("set_densify_stats", &RenderContext::set_densify_stats, py::arg("grad2d"), py::arg("count"),
            py::arg("max_radius"), py::arg("absgrad") = py::none())
       .def("clear_densify_stats", &RenderContext::clear_densify_stats)
@@ -1200,6 +1273,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mcmc_noise", &mcmc_noise, "MCMC position noise, in place (gs_mcmc_noise)", py::arg("pos"), py::arg("quat"),
         py::arg("scale"), py::arg("opa"), py::arg("scale_activation"), py::arg("scaler"), py::arg("seed"),
         py::arg("z") = py::none());
+  m.def("filter3d_compute",
+        [](RenderContext& rc, torch::Tensor pos, torch::Tensor size, torch::Tensor focal, torch::Tensor rot,
+           torch::Tensor tran, double near, double margin, double variance, std::optional<torch::Tensor> out) {
+          return rc.filter3d_compute(pos, size, focal, rot, tran, near, margin, variance, out);
+        },
+        "Mip-Splatting's 3-D filter from the sampling rate over V views (gs_filter3d_compute)", py::arg("ctx"),
+        py::arg("pos"), py::arg("size"), py::arg("focal"), py::arg("rot"), py::arg("tran"), py::arg("near"),
+        py::arg("margin") = 0.15, py::arg("variance") = 0.2, py::arg("out") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
   m.def("adam_step_visible", &adam_step_visible,

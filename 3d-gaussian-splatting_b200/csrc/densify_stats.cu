@@ -15,14 +15,19 @@ constexpr int kBlock = 256;
 //   max_radius = max(max_radius, ceil(3 sqrt(lambda_max))) of the 2-D covariance the forward binned, in px^2
 // (sx, sy) = (W / (2 fx), H / (2 fy)) converts dL/d(x/z, y/z) to the NDC convention of 3DGS's viewspace gradient.
 // One thread owns one Gaussian and sums its rows in order: bit-deterministic, no atomics.
-template <bool ABS>
-__global__ void __launch_bounds__(kBlock) densify_stats_kernel(
-    const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n,
-    int scale_act, GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt,
-    const uint32_t* __restrict__ offsets_g, const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
-    int gw, const uint32_t* __restrict__ row_epoch, uint32_t epoch, float sx, float sy, float fx, float fy,
-    float* __restrict__ grad2d, float* __restrict__ absgrad, int* __restrict__ n_views,
-    float* __restrict__ max_radius) {
+// G3: the forward applied the 3-D filter f3d[n]: the covariance is the filtered scale's (gs_filter3d).
+#define GS_STATS_PARAMS                                                                                             \
+  const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n,            \
+      int scale_act, GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt,                      \
+      const uint32_t* __restrict__ offsets_g, const uint32_t* __restrict__ count,                                  \
+      const float* __restrict__ grad_inst, int gw, const uint32_t* __restrict__ row_epoch, uint32_t epoch,         \
+      float sx, float sy, float fx, float fy, float* __restrict__ grad2d, float* __restrict__ absgrad,             \
+      int* __restrict__ n_views, float* __restrict__ max_radius
+#define GS_STATS_ARGS                                                                                             \
+  pos, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, filt, offsets_g, count, grad_inst, gw, row_epoch, \
+      epoch, sx, sy, fx, fy, grad2d, absgrad, n_views, max_radius
+template <bool ABS, bool G3>
+__device__ __forceinline__ void densify_stats_body(GS_STATS_PARAMS, const float* __restrict__ f3d) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   const uint32_t cnt = count[i];
@@ -30,6 +35,10 @@ __global__ void __launch_bounds__(kBlock) densify_stats_kernel(
   float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
   float q[4], s[3], raw_s[3], qn;
   gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+  if constexpr (G3) {
+    float s0[3], dl2o3;
+    gs_filter3d(f3d[i], s, s0, dl2o3);
+  }
   float gx = 0.f, gy = 0.f, ax = 0.f, ay = 0.f;
   const uint32_t o0 = offsets_g[i], o1 = o0 + cnt;
   for (uint32_t r = o0; r < o1; ++r) {
@@ -57,21 +66,41 @@ __global__ void __launch_bounds__(kBlock) densify_stats_kernel(
   max_radius[i] = fmaxf(max_radius[i], rad);
 }
 
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_kernel(GS_STATS_PARAMS) {
+  densify_stats_body<ABS, false>(GS_STATS_ARGS, nullptr);
+}
+
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_filt3_kernel(GS_STATS_PARAMS, const float* __restrict__ f3d) {
+  densify_stats_body<ABS, true>(GS_STATS_ARGS, f3d);
+}
+#undef GS_STATS_ARGS
+#undef GS_STATS_PARAMS
+
 // Batched frame: Gaussian i's views in view order, each one's statistics formed as densify_stats_kernel forms them
 // (pair v n + i, view v's camera, filter and (sx, sy) = (W / (2 fx), H / (2 fy))) and added to running values that are
-// loaded and stored once: the result of B single-view backwards run in view order.
-template <bool ABS>
-__global__ void __launch_bounds__(kBlock) densify_stats_batch_kernel(
-    const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views,
-    int scale_act, const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
-    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, int gw,
-    const uint32_t* __restrict__ row_epoch, uint32_t epoch, int width, int height, float* __restrict__ grad2d,
-    float* __restrict__ absgrad, int* __restrict__ n_views_out, float* __restrict__ max_radius) {
+// loaded and stored once: the result of B single-view backwards run in view order.  G3 as above.
+#define GS_STATS_BATCH_PARAMS                                                                                        \
+  const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, \
+      int scale_act, const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,    \
+      const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, int gw,                              \
+      const uint32_t* __restrict__ row_epoch, uint32_t epoch, int width, int height, float* __restrict__ grad2d,    \
+      float* __restrict__ absgrad, int* __restrict__ n_views_out, float* __restrict__ max_radius
+#define GS_STATS_BATCH_ARGS                                                                                       \
+  pos, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, gw, row_epoch, epoch,   \
+      width, height, grad2d, absgrad, n_views_out, max_radius
+template <bool ABS, bool G3>
+__device__ __forceinline__ void densify_stats_batch_body(GS_STATS_BATCH_PARAMS, const float* __restrict__ f3d) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
   float q[4], s[3], raw_s[3], qn;
   gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+  if constexpr (G3) {
+    float s0[3], dl2o3;
+    gs_filter3d(f3d[i], s, s0, dl2o3);
+  }
   float g2 = grad2d[i], ga = ABS ? absgrad[i] : 0.f, mr = max_radius[i];
   int nv = n_views_out[i];
   bool any = false;
@@ -116,13 +145,26 @@ __global__ void __launch_bounds__(kBlock) densify_stats_batch_kernel(
   max_radius[i] = mr;
 }
 
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_batch_kernel(GS_STATS_BATCH_PARAMS) {
+  densify_stats_batch_body<ABS, false>(GS_STATS_BATCH_ARGS, nullptr);
+}
+
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_batch_filt3_kernel(GS_STATS_BATCH_PARAMS,
+                                                                           const float* __restrict__ f3d) {
+  densify_stats_batch_body<ABS, true>(GS_STATS_BATCH_ARGS, f3d);
+}
+#undef GS_STATS_BATCH_ARGS
+#undef GS_STATS_BATCH_PARAMS
+
 }  // namespace
 
 cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, const float* scale, int n, int n_views,
                                           int scale_act, const GsView* views, float near_plane,
                                           const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
                                           int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
-                                          const gs_densify_stats& s, cudaStream_t st) {
+                                          const gs_densify_stats& s, cudaStream_t st, const float* f3d) {
   if (n == 0) return cudaSuccess;
   const int blocks = (n + kBlock - 1) / kBlock;
 #define GS_LAUNCH_STATS_BATCH(ABS)                                                                                 \
@@ -130,8 +172,15 @@ cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, c
                                                              near_plane, offsets_g, count, grad_inst, gw, row_epoch, \
                                                              epoch, g.width, g.height, s.grad2d, s.absgrad, s.count, \
                                                              s.max_radius)
-  if (s.absgrad) GS_LAUNCH_STATS_BATCH(true);
+#define GS_LAUNCH_STATS_BATCH3(ABS)                                                                                \
+  densify_stats_batch_filt3_kernel<ABS><<<blocks, kBlock, 0, st>>>(                                                 \
+      pos, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, gw, row_epoch, epoch, \
+      g.width, g.height, s.grad2d, s.absgrad, s.count, s.max_radius, f3d)
+  if (f3d && s.absgrad) GS_LAUNCH_STATS_BATCH3(true);
+  else if (f3d) GS_LAUNCH_STATS_BATCH3(false);
+  else if (s.absgrad) GS_LAUNCH_STATS_BATCH(true);
   else GS_LAUNCH_STATS_BATCH(false);
+#undef GS_LAUNCH_STATS_BATCH3
 #undef GS_LAUNCH_STATS_BATCH
   return cudaGetLastError();
 }
@@ -140,7 +189,8 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                     const GsCam& cam, float near_plane, float half_w, float half_h,
                                     const GsFilter2d& filt, const uint32_t* offsets_g, const uint32_t* count,
                                     const float* grad_inst, int gw, const uint32_t* row_epoch, uint32_t epoch,
-                                    const GsFrameGeom& g, const gs_densify_stats& s, cudaStream_t st) {
+                                    const GsFrameGeom& g, const gs_densify_stats& s, cudaStream_t st,
+                                    const float* f3d) {
   if (n == 0) return cudaSuccess;
   const float sx = (float)((double)g.width / (2.0 * (double)g.fx));
   const float sy = (float)((double)g.height / (2.0 * (double)g.fy));
@@ -150,8 +200,16 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                                        half_h, filt, offsets_g, count, grad_inst, gw, row_epoch,   \
                                                        epoch, sx, sy, g.fx, g.fy, s.grad2d, s.absgrad, s.count,    \
                                                        s.max_radius)
-  if (s.absgrad) GS_LAUNCH_STATS(true);
+#define GS_LAUNCH_STATS3(ABS)                                                                                      \
+  densify_stats_filt3_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, scale_act, cam, near_plane,      \
+                                                             half_w, half_h, filt, offsets_g, count, grad_inst, gw, \
+                                                             row_epoch, epoch, sx, sy, g.fx, g.fy, s.grad2d,       \
+                                                             s.absgrad, s.count, s.max_radius, f3d)
+  if (f3d && s.absgrad) GS_LAUNCH_STATS3(true);
+  else if (f3d) GS_LAUNCH_STATS3(false);
+  else if (s.absgrad) GS_LAUNCH_STATS(true);
   else GS_LAUNCH_STATS(false);
+#undef GS_LAUNCH_STATS3
 #undef GS_LAUNCH_STATS
   return cudaGetLastError();
 }

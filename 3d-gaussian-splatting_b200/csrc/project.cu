@@ -57,14 +57,17 @@ __device__ __forceinline__ void sh_logits(const float* coef, const float* Y, flo
 // degree 2 / 3 evaluated once per Gaussian along view_dir (GS_SH_EVAL_GAUSSIAN); the record then carries an RGB colour.
 // F: the 2-D screen-space filter `filt` (gs_filter2d) is applied to the covariance before the tile rectangle and the
 // conic, and its compensation to l2o.
+// G3 (only with F): the 3-D smoothing filter f3d[n] (gs_filter3d) is applied to the activated scale first, and its
+// compensation added to l2o before the 2-D filter's.
 // The batched frame's fused_project_one repeats this arithmetic: a change to it must be made to both.
-template <int KG, bool F = false>
+template <int KG, bool F = false, bool G3 = false>
 __device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
     const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
     uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}) {
+    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr) {
+  static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
   int i = blockIdx.x * kBlock + threadIdx.x;
   bool vis = false;
   uint32_t cnt = 0;
@@ -72,6 +75,12 @@ __device__ __forceinline__ void fused_project_body(
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    float f3 = 0.f, dl2o3 = 0.f;
+    if constexpr (G3) {
+      float s0[3];
+      f3 = f3d[i];
+      gs_filter3d(f3, s, s0, dl2o3);
+    }
     // opacity and RGB logits are issued with the geometry, so that the thread makes one round trip to HBM, not two
     // (a warp almost always has a binned Gaussian, so their sectors are fetched anyway)
     const float opa_raw = opa[i];
@@ -121,7 +130,11 @@ __device__ __forceinline__ void fused_project_body(
           cg = gs_sigmoid(rgb_raw[1]);
           cb = gs_sigmoid(rgb_raw[2]);
         }
-        r->b = make_float4(k.cc, F ? log2f(op) + dl2o : log2f(op), cr, cg);
+        float l2o = log2f(op);
+        if constexpr (G3) {
+          if (f3 != 0.f) l2o += dl2o3;
+        }
+        r->b = make_float4(k.cc, F ? l2o + dl2o : l2o, cr, cg);
         r->c = make_float4(cb, o.depth, __uint_as_float(rc.x), __uint_as_float(rc.y));
         r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
       }
@@ -184,17 +197,31 @@ __global__ void __launch_bounds__(kBlock) fused_project_filt_kernel(
                               rect, count, dkey, mask, n_visible, filt);
 }
 
+// with the 3-D filter f3d[n] and the 2-D filter `filt` (zero when the frame has none)
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_filt3_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible, GsFilter2d filt, const float* __restrict__ f3d) {
+  fused_project_body<K, true, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h,
+                                    rec, rect, count, dkey, mask, n_visible, filt, f3d);
+}
+
 // Batched frames.  Gaussian i (loaded parameters p, q, s, opa_raw, rgb_raw) seen by one view: the arithmetic of
 // fused_project_body, with its record, rectangle, count and depth key going to pair j = v n + i and the rectangle's
 // rows offset by ty_off (the view's first tile row).  Returns the instance count; vis: in the frustum.  (The
 // single-view kernels keep their own copy: routed through this function they compile to different SASS; a change
 // to the arithmetic of either copy must be made to both.)
-template <int KG, bool F>
+// G3: s is the 3-D filtered scale and dl2o3 its compensation (added to l2o when f3 != 0).
+template <int KG, bool F, bool G3 = false>
 __device__ __forceinline__ uint32_t fused_project_one(
     const float* __restrict__ rgb, int i, int d, const GsCam& cam, const GsTileGrid& grid, float near_plane,
     float half_w, float half_h, const GsFilter2d& filt, const float p[3], const float q[4], const float s[3],
     float opa_raw, const float rgb_raw[3], uint32_t ty_off, int j, GsRec* __restrict__ rec, uint2* __restrict__ rect,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis) {
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis,
+    float f3 = 0.f, float dl2o3 = 0.f) {
   uint32_t cnt = 0;
   {
     GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
@@ -237,7 +264,11 @@ __device__ __forceinline__ uint32_t fused_project_one(
           cg = gs_sigmoid(rgb_raw[1]);
           cb = gs_sigmoid(rgb_raw[2]);
         }
-        r->b = make_float4(k.cc, F ? log2f(op) + dl2o : log2f(op), cr, cg);
+        float l2o = log2f(op);
+        if constexpr (G3) {
+          if (f3 != 0.f) l2o += dl2o3;
+        }
+        r->b = make_float4(k.cc, F ? l2o + dl2o : l2o, cr, cg);
         r->c = make_float4(cb, o.depth, __uint_as_float(rc.x), __uint_as_float(rc.y));
         r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
       }
@@ -254,14 +285,14 @@ __device__ __forceinline__ uint32_t fused_project_one(
 
 // Batched frame: one thread per Gaussian loads its parameters once and projects it into each view in turn, writing
 // pair j = v n + i with view v's constants (K, F as in fused_project_filt_kernel; F reads views[v].filt).  The
-// counters receive the frame's totals over the pairs.
-template <int K, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
+// counters receive the frame's totals over the pairs.  G3: the 3-D filter f3d[n] is applied once, before the views.
+template <int K, bool F, bool G3>
+__device__ __forceinline__ void fused_project_batch_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,
     const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible) {
+    unsigned int* __restrict__ n_visible, const float* __restrict__ f3d) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   unsigned int nv = 0;
   unsigned long long c64 = 0;
@@ -269,6 +300,12 @@ __global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    float f3 = 0.f, dl2o3 = 0.f;
+    if constexpr (G3) {
+      float s0[3];
+      f3 = f3d[i];
+      gs_filter3d(f3, s, s0, dl2o3);
+    }
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
     if (K == 0 && d == 3) {
@@ -279,9 +316,9 @@ __global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
     for (int v = 0; v < n_views; ++v) {
       const GsView vw = views[v];
       bool vis = false;
-      c64 += fused_project_one<K, F>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p, q, s,
-                                     opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect, count, dkey,
-                                     mask, vis);
+      c64 += fused_project_one<K, F, G3>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p, q,
+                                         s, opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect, count,
+                                         dkey, mask, vis, f3, dl2o3);
       nv += vis ? 1u : 0u;
     }
   }
@@ -309,6 +346,27 @@ __global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
     if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
   }
 }
+
+#define GS_PBATCH_PARAMS                                                                                            \
+  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                     \
+      const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,   \
+      const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,        \
+      uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,                        \
+      unsigned int* __restrict__ n_visible
+#define GS_PBATCH_ARGS \
+  pos, rgb, opa, quat, scale, n, n_views, d, scale_act, views, near_plane, rec, rect, count, dkey, mask, n_visible
+
+template <int K, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(GS_PBATCH_PARAMS) {
+  fused_project_batch_body<K, F, false>(GS_PBATCH_ARGS, nullptr);
+}
+
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_batch_filt3_kernel(GS_PBATCH_PARAMS,
+                                                                           const float* __restrict__ f3d) {
+  fused_project_batch_body<K, true, true>(GS_PBATCH_ARGS, f3d);
+}
+#undef GS_PBATCH_PARAMS
 
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
 // contiguous rows offsets_g[i] .. + count[i]) and chains them to the RAW parameters.  No
@@ -356,8 +414,11 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
 // the view-direction term of per-Gaussian SH); with all five gradient pointers NULL no parameter gradient is stored.
 // F: the forward applied the 2-D filter `filt` (fused_project_body<KG, true>): the conic is chained with the filtered
 // covariance, and the compensation's gradient is added to dL/dcov.
+// G3 (only with F): the forward applied the 3-D filter f3d[n] (fused_project_body<KG, true, true>): the projection is
+// differentiated at the filtered scale s', and dL/ds' is chained to dL/ds with the compensation's term
+// (gs_filter3d_backward) before the raw-scale chain.
 // The batched frame's fused_project_bwd_one repeats this arithmetic: a change to it must be made to both.
-template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false>
+template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false, bool G3 = false>
 __device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
@@ -365,8 +426,9 @@ __device__ __forceinline__ void fused_project_bwd_body(
     const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
     const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
     float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
-    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}) {
+    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr) {
   static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
+  static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
   static_assert(!CG || (W == 0 && GW == GS_GREC), "camera gradient: RGB gradient rows, no push");
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   int i = blockIdx.x * kBlock + threadIdx.x;
@@ -390,6 +452,12 @@ __device__ __forceinline__ void fused_project_bwd_body(
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    float f3 = 0.f, s0[3];
+    if constexpr (G3) {
+      float dl2o3;
+      f3 = f3d[i];
+      gs_filter3d(f3, s, s0, dl2o3);
+    }
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
     float coef[KG ? D : 1];
@@ -481,6 +549,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     } else {
       gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
     }
+    if constexpr (G3) gs_filter3d_backward(f3, s0, s, acc[5], gsv);
     if constexpr (KG > 0) {
       // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
       // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
@@ -627,6 +696,19 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PB
   fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true>(GS_PBWD_ARGS, nullptr, filt);
 }
 
+// and for a forward that applied the 3-D filter f3d[n] (with `filt`, zero when the frame had no 2-D filter)
+template <int D, int GW, int W, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_filt3_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
+                                                                         const float* __restrict__ f3d) {
+  fused_project_bwd_body<D, GW, W, DT, 0, false, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d);
+}
+
+template <int K, int W, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt3_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
+                                                                            const float* __restrict__ f3d) {
+  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d);
+}
+
 // Batched frames.  One view's share of Gaussian i's parameter gradients, the arithmetic of fused_project_bwd_body for
 // RGB gradient rows without a push or a camera gradient (rows o0 .. o1 - 1 of grad_inst, the loaded parameters p, q,
 // s, raw_s, qn, opa_raw, rgb_raw / coef): acc receives the row sums, then gp, gq_raw, gs_raw, go and the colour
@@ -634,16 +716,23 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PB
 // through this function they compile to different SASS): a change to the arithmetic of either copy must be made to
 // both.  CG: also adds the view's camera terms to cg[12], as fused_project_bwd_body<..., CG = true> does (the parameter
 // gradients are the same bits either way).
-template <int D, bool DT, int KG, bool F, bool CG = false>
+// G3: s is the 3-D filtered scale and f3 the filter; the activated scale is formed again from raw_s (as
+// gs_load_activated forms it) for gs_filter3d_backward, rather than kept live across the caller's view loop.
+template <int D, bool DT, int KG, bool F, bool CG = false, bool G3 = false>
 __device__ __forceinline__ void fused_project_bwd_one(
     GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
     const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
     const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, float opa_raw,
     const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GS_GREC], float (&gsh)[KG ? D : 1],
-    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr) {
+    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr, float f3 = 0.f) {
   constexpr int GW = GS_GREC;
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   {
+    float s0[3];
+    if constexpr (G3) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) s0[k] = (scale_act == GS_SCALE_ABS) ? (fabsf(raw_s[k]) + 1e-4f) : expf(raw_s[k]);
+    }
     // The rows are summed one by one in row order.  For an RGB frame the rows are loaded in groups: the tags of four
     // rows at once, then the live rows among them (48 registers of payload), so that a Gaussian with a few instances
     // waits for two round trips to HBM per group instead of two per row (H100, C3: 0.235 -> 0.230 ms).  Grouping only
@@ -724,6 +813,7 @@ __device__ __forceinline__ void fused_project_bwd_one(
     } else {
       gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
     }
+    if constexpr (G3) gs_filter3d_backward(f3, s0, s, acc[5], gsv);
     if constexpr (KG > 0) {
       // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
       // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
@@ -837,14 +927,19 @@ __device__ __forceinline__ void fused_project_bwd_store(int i, int n, bool valid
 // v n + i with view v's camera, and the shares are added in view order with no contraction into their last products:
 // the sum of B single-view backwards accumulated in view order, to within the FMA contractions the compiler chooses
 // differently inside the view loop (measured: 1e-6 relative at most).
-template <int K, bool DT, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,
-    const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
-    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
-    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
-    float* __restrict__ g_quat, float* __restrict__ g_scale) {
+// G3: the 3-D filter f3d[n] of the forward, applied once before the views.
+#define GS_PBWD_BATCH_PARAMS                                                                                          \
+  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                       \
+      const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,            \
+      const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,                     \
+      const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,                                       \
+      const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb,  \
+      float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale
+#define GS_PBWD_BATCH_ARGS                                                                                          \
+  pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, epoch, \
+      g_pos, g_rgb, g_opa, g_quat, g_scale
+template <int K, bool DT, bool F, bool G3>
+__device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAMS, const float* __restrict__ f3d) {
   constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const bool valid = i < n;
@@ -857,6 +952,12 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
     float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
     float q[4], s[3], raw_s[3], qn;
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    float f3 = 0.f;
+    if constexpr (G3) {
+      float s0[3], dl2o3;
+      f3 = f3d[i];
+      gs_filter3d(f3, s, s0, dl2o3);
+    }
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
     float coef[K ? D : 1];
@@ -876,9 +977,9 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
       float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
 #pragma unroll
       for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      fused_project_bwd_one<D, DT, K, F>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0, o0 + cnt,
-                                         grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw, rgb_raw, coef, acc,
-                                         gsh, vp, vq, vs, vo);
+      fused_project_bwd_one<D, DT, K, F, false, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                                    o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
+                                                    rgb_raw, coef, acc, gsh, vp, vq, vs, vo, nullptr, f3);
       const float* vc = K ? gsh : acc + 6;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
@@ -893,6 +994,17 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
     }
   }
   fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
+}
+
+template <int K, bool DT, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(GS_PBWD_BATCH_PARAMS) {
+  fused_project_bwd_batch_body<K, DT, F, false>(GS_PBWD_BATCH_ARGS, nullptr);
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_filt3_kernel(GS_PBWD_BATCH_PARAMS,
+                                                                               const float* __restrict__ f3d) {
+  fused_project_bwd_batch_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, f3d);
 }
 
 // Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
@@ -923,13 +1035,13 @@ __device__ __forceinline__ void cam_grad_cta_sum(float (&cg)[kCamGrad], float (&
   }
 }
 
-template <int K, bool DT, bool F>
+template <int K, bool DT, bool F, bool G3 = false>
 __device__ __forceinline__ void fused_project_bwd_cam_body(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                           GsFilter2d filt) {
+                                                           GsFilter2d filt, const float* __restrict__ f3d = nullptr) {
   float cg[kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
-  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F>(GS_PBWD_ARGS, cg, filt);
+  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F, G3>(GS_PBWD_ARGS, cg, filt, f3d);
   __shared__ float wsum[kBlock / 32][kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) {
@@ -960,20 +1072,22 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt_kernel(GS_P
   fused_project_bwd_cam_body<K, DT, true>(GS_PBWD_ARGS, cam_part, filt);
 }
 
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt3_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
+                                                                             GsFilter2d filt,
+                                                                             const float* __restrict__ f3d) {
+  fused_project_bwd_cam_body<K, DT, true, true>(GS_PBWD_ARGS, cam_part, filt, f3d);
+}
+
 // Camera gradients of a batched frame (gs_render_backward_batch_cam): fused_project_bwd_batch_kernel's parameter
 // gradients, the same bits, plus the camera terms of each view with that view's camera, filter and SH direction.  Per
 // view v the CTA sums its threads' terms in fused_project_bwd_cam_body's order into row blockIdx.x of
 // cam_part[v][gridDim.x][12].  The view loop and the sums are uniform across the CTA: threads past n and Gaussians
 // without a row in view v take part with zeros, and a CTA without a row in view v stores a zero row (the bits the
 // shuffles would give) without reducing.  With the five gradient pointers NULL only cam_part is written.
-template <int K, bool DT, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,
-    const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
-    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
-    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
-    float* __restrict__ g_quat, float* __restrict__ g_scale, float* __restrict__ cam_part) {
+template <int K, bool DT, bool F, bool G3>
+__device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_PARAMS, float* __restrict__ cam_part,
+                                                                 const float* __restrict__ f3d) {
   constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const bool valid = i < n;
@@ -983,6 +1097,7 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
   for (int k = 0; k < D; ++k) gcol[k] = 0.f;
   float p[3] = {0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, s[3] = {0.f, 0.f, 0.f}, raw_s[3] = {0.f, 0.f, 0.f};
   float qn = 1.f, opa_raw = 0.f, rgb_raw[3] = {0.f, 0.f, 0.f};
+  float f3 = 0.f;
   float coef[K ? D : 1];
 #pragma unroll
   for (int k = 0; k < (K ? D : 1); ++k) coef[k] = 0.f;
@@ -991,6 +1106,11 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
     p[1] = pos[3 * i + 1];
     p[2] = pos[3 * i + 2];
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+    if constexpr (G3) {
+      float s0[3], dl2o3;
+      f3 = f3d[i];
+      gs_filter3d(f3, s, s0, dl2o3);
+    }
     opa_raw = opa[i];
     if constexpr (K > 0) {
 #pragma unroll
@@ -1014,9 +1134,9 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
       float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
 #pragma unroll
       for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      fused_project_bwd_one<D, DT, K, F, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
-                                               o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
-                                               rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg);
+      fused_project_bwd_one<D, DT, K, F, true, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                                   o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
+                                                   rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3);
       const float* vc = K ? gsh : acc + 6;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
@@ -1041,6 +1161,20 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(
   if (!valid && D == 3) return;          // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
   fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
 }
+
+template <int K, bool DT, bool F>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(GS_PBWD_BATCH_PARAMS,
+                                                                             float* __restrict__ cam_part) {
+  fused_project_bwd_batch_cam_body<K, DT, F, false>(GS_PBWD_BATCH_ARGS, cam_part, nullptr);
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_filt3_kernel(GS_PBWD_BATCH_PARAMS,
+                                                                                   float* __restrict__ cam_part,
+                                                                                   const float* __restrict__ f3d) {
+  fused_project_bwd_batch_cam_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, cam_part, f3d);
+}
+#undef GS_PBWD_BATCH_PARAMS
 #undef GS_PBWD_PARAMS
 
 // One CTA: grad_cam[k] = sum over the `rows` rows of cam_part[., k] in fp64, in a fixed order (strided per-thread sums,
@@ -1232,8 +1366,22 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint2* rect, uint32_t* count, uint32_t* dkey, int64_t* mask,
-                                    unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt) {
+                                    unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt,
+                                    const float* f3d) {
   if (n == 0) return cudaSuccess;
+  if (f3d) {
+    const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
+#define GS_LAUNCH_PFILT3(K)                                                                                      \
+  fused_project_filt3_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
+                                                                grid, near_plane, half_w, half_h, rec, rect, count, \
+                                                                dkey, mask, n_visible, f2, f3d)
+    if (sh_gaussian && d == 27) GS_LAUNCH_PFILT3(9);
+    else if (sh_gaussian && d == 48) GS_LAUNCH_PFILT3(16);
+    else if (sh_gaussian) return cudaErrorInvalidValue;
+    else GS_LAUNCH_PFILT3(0);
+#undef GS_LAUNCH_PFILT3
+    return cudaGetLastError();
+  }
   if (filt) {
 #define GS_LAUNCH_PFILT(K)                                                                                      \
   fused_project_filt_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
@@ -1268,10 +1416,13 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
-                                        bool depth_grad, bool sh_gaussian, const GsFilter2d* filt) {
+                                        bool depth_grad, bool sh_gaussian, const GsFilter2d* filt, const float* f3d) {
   if (n == 0) return cudaSuccess;
+  const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
 #define GS_LAUNCH_PBWD(D, GW, W, DT)                                                               \
-  if (filt)                                                                                        \
+  if (f3d)                                                                                         \
+    fused_project_bwd_filt3_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d); \
+  else if (filt)                                                                                   \
     fused_project_bwd_filt_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
   else                                                                                             \
     fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
@@ -1284,7 +1435,9 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
     default: return cudaErrorInvalidValue;           \
   }
 #define GS_LAUNCH_PBWD_SH(K, W, DT)                                                               \
-  if (filt)                                                                                       \
+  if (f3d)                                                                                        \
+    fused_project_bwd_sh_filt3_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d); \
+  else if (filt)                                                                                  \
     fused_project_bwd_sh_filt_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
   else                                                                                            \
     fused_project_bwd_sh_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
@@ -1322,12 +1475,16 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                             uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
-                                            bool depth_grad, bool sh_gaussian, const GsFilter2d* filt) {
+                                            bool depth_grad, bool sh_gaussian, const GsFilter2d* filt,
+                                            const float* f3d) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
   const GsGradPush push{};
+  const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
   if (n > 0) {
 #define GS_LAUNCH_PBWD_CAM(K, DT)                                                                             \
-  if (filt)                                                                                                   \
+  if (f3d)                                                                                                    \
+    fused_project_bwd_cam_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, f2, f3d); \
+  else if (filt)                                                                                              \
     fused_project_bwd_cam_filt_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, *filt); \
   else                                                                                                        \
     fused_project_bwd_cam_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part)
@@ -1348,20 +1505,30 @@ cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, co
                                           const float* scale, int n, int n_views, int d, int scale_act,
                                           const GsView* views, float near_plane, GsRec* rec, uint2* rect,
                                           uint32_t* count, uint32_t* dkey, int64_t* mask, unsigned int* n_visible,
-                                          cudaStream_t st, bool sh_gaussian, bool filt) {
+                                          cudaStream_t st, bool sh_gaussian, bool filt, const float* f3d) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
 #define GS_LAUNCH_PBATCH(K, F)                                                                                    \
   fused_project_batch_kernel<K, F><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,     \
                                                                    scale_act, views, near_plane, rec, rect, count, \
                                                                    dkey, mask, n_visible)
+#define GS_LAUNCH_PBATCH3(K)                                                                                      \
+  fused_project_batch_filt3_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,  \
+                                                                      scale_act, views, near_plane, rec, rect,     \
+                                                                      count, dkey, mask, n_visible, f3d)
   const int k = d == 27 ? 9 : (d == 48 ? 16 : 0);
-  if (k == 9 && filt) GS_LAUNCH_PBATCH(9, true);
+  if (f3d) {
+    if (k == 9) GS_LAUNCH_PBATCH3(9);
+    else if (k == 16) GS_LAUNCH_PBATCH3(16);
+    else GS_LAUNCH_PBATCH3(0);
+  }
+  else if (k == 9 && filt) GS_LAUNCH_PBATCH(9, true);
   else if (k == 9) GS_LAUNCH_PBATCH(9, false);
   else if (k == 16 && filt) GS_LAUNCH_PBATCH(16, true);
   else if (k == 16) GS_LAUNCH_PBATCH(16, false);
   else if (filt) GS_LAUNCH_PBATCH(0, true);
   else GS_LAUNCH_PBATCH(0, false);
+#undef GS_LAUNCH_PBATCH3
 #undef GS_LAUNCH_PBATCH
   return cudaGetLastError();
 }
@@ -1372,15 +1539,19 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
                                               const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                               uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                               float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
-                                              bool filt) {
+                                              bool filt, const float* f3d) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
 #define GS_LAUNCH_PBWD_BATCH(K, DT, F)                                                                              \
   fused_project_bwd_batch_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                         \
       pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
       epoch, g_pos, g_rgb, g_opa, g_quat, g_scale)
-#define GS_LAUNCH_PBWD_BATCH_F(K, DT)       \
-  if (filt) GS_LAUNCH_PBWD_BATCH(K, DT, true); \
+#define GS_LAUNCH_PBWD_BATCH_F(K, DT)                                                                             \
+  if (f3d)                                                                                                        \
+    fused_project_bwd_batch_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                  \
+        pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,        \
+        row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d);                                             \
+  else if (filt) GS_LAUNCH_PBWD_BATCH(K, DT, true);                                                               \
   else GS_LAUNCH_PBWD_BATCH(K, DT, false)
   if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_F(9, true); }
   else if (d == 27) { GS_LAUNCH_PBWD_BATCH_F(9, false); }
@@ -1400,15 +1571,19 @@ cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float*
                                                   const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                                   float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                                   float* g_scale, float* cam_part, float* grad_cams, cudaStream_t st,
-                                                  bool depth_grad, bool sh_gaussian, bool filt) {
+                                                  bool depth_grad, bool sh_gaussian, bool filt, const float* f3d) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
   if (n > 0) {
 #define GS_LAUNCH_PBWD_BATCH_CAM(K, DT, F)                                                                          \
   fused_project_bwd_batch_cam_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                     \
       pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
       epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part)
-#define GS_LAUNCH_PBWD_BATCH_CAM_F(K, DT)          \
-  if (filt) GS_LAUNCH_PBWD_BATCH_CAM(K, DT, true); \
+#define GS_LAUNCH_PBWD_BATCH_CAM_F(K, DT)                                                                         \
+  if (f3d)                                                                                                        \
+    fused_project_bwd_batch_cam_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                              \
+        pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,        \
+        row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part, f3d);                                   \
+  else if (filt) GS_LAUNCH_PBWD_BATCH_CAM(K, DT, true);                                                           \
   else GS_LAUNCH_PBWD_BATCH_CAM(K, DT, false)
     if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, true); }
     else if (d == 27) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, false); }

@@ -250,6 +250,46 @@ __device__ __forceinline__ GsFilter2dOut gs_filter2d(const GsFilter2d& f, float 
   return o;
 }
 
+// 3-D smoothing filter of the fused frame path (gs_ctx_set_filter3d; Mip-Splatting's 3D filter): with Gaussian i's
+// filter std f >= 0 (world units), its activated scale s becomes s' = sqrt(s^2 + f^2) and l2o gains
+// dl2o = 0.5 sum_k log2(s_k^2 / s'_k^2), i.e. sigma' = sigma prod_k s_k / s'_k, which keeps sigma sqrt(det Sigma3), the
+// Gaussian's 3-D integral.  f == 0 keeps s and dl2o = 0 by selection, so a zero filter gives the unfiltered bits.  A
+// scale of 0 (exp underflow) gives dl2o = -inf: opacity 0.
+// s: the activated scale on entry, s' on return; s0: the activated scale.
+__device__ __forceinline__ void gs_filter3d(float f, float s[3], float s0[3], float& dl2o) {
+  dl2o = 0.f;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) s0[k] = s[k];
+  if (f != 0.f) {
+    const float f2 = f * f;
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float s2 = s0[k] * s0[k];
+      const float t = s2 + f2;
+      s[k] = sqrtf(t);
+      acc += log2f(s2 / t);
+    }
+    dl2o = 0.5f * acc;
+  }
+}
+
+// Backward of gs_filter3d (f is a constant): gs = dL/ds' on entry, dL/ds on return,
+//   dL/ds_k = dL/ds'_k s_k / s'_k + g_l2o f^2 / (ln 2 s_k (s_k^2 + f^2)).
+// The second term is taken as 0 where g_l2o == 0 or s_k == 0 (a Gaussian whose opacity underflowed has no blend
+// gradient, and 0 * inf must not reach the parameters).
+__device__ __forceinline__ void gs_filter3d_backward(float f, const float s0[3], const float sf[3], float g_l2o,
+                                                     float gs[3]) {
+  if (f == 0.f) return;
+  const float f2 = f * f;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float s = s0[k];
+    const float comp = (g_l2o != 0.f && s > 0.f) ? g_l2o * f2 / (GS_LN2 * s * (s * s + f2)) : 0.f;
+    gs[k] = gs[k] * (s / sf[k]) + comp;
+  }
+}
+
 // Tile rectangle covered by a Gaussian, method 2 "prob2" (gaussian.cu:226-242): axis aligned
 // bbox of the `thresh` iso-probability ellipse; float->uint32 casts truncate / saturate.
 struct GsTileGrid {

@@ -174,6 +174,14 @@ struct gs_ctx {
   GsFilter2d filt{};
   bool stats_on = false;                  // gs_ctx_set_densify_stats: accumulated by the backwards that follow
   gs_densify_stats stats{};
+  const float* filter3d = nullptr;        // gs_ctx_set_filter3d: applies to the forwards that follow (the caller's [n])
+  int filter3d_n = 0;
+  const float* f3d = nullptr;             // the last forward's 3-D filter (its backward uses it); NULL: none
+  // gs_filter3d_compute: the view table (after a 16-byte slot for the smallest seen rate) and its pinned staging
+  DevBuf f3_dev;
+  GsF3View* f3_host = nullptr;
+  int f3_host_cap = 0;
+  cudaEvent_t ev_f3 = nullptr;            // marks the completion of the view table's upload from f3_host
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -210,13 +218,15 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
-                    &c->grad_feat_inst, &c->views};
+                    &c->grad_feat_inst, &c->views, &c->f3_dev};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
   if (c->host_views) cudaFreeHost(c->host_views);
   if (c->ev_m) cudaEventDestroy(c->ev_m);
   if (c->ev_views) cudaEventDestroy(c->ev_views);
+  if (c->f3_host) cudaFreeHost(c->f3_host);
+  if (c->ev_f3) cudaEventDestroy(c->ev_f3);
   if (c->ev_ok)
     for (cudaEvent_t e : c->ev) cudaEventDestroy(e);
   if (switched) cudaSetDevice(cur);
@@ -307,7 +317,7 @@ static int begin_forward(gs_ctx* c, const char* who) {
 // what the backward of a completed forward needs; v: the constants of its (first) view
 static void commit_forward(gs_ctx* c, int n, int d, int scale_activation, long long m, const GsFrameGeom& g,
                            const GsView& v, float near_plane, int n_views, bool sh_gaussian, bool gather, bool filt_on,
-                           const GsAuxOut& aux_out, const gs_render_feat* ft) {
+                           const GsAuxOut& aux_out, const gs_render_feat* ft, const float* f3d) {
   c->ev_fwd_valid = c->timing && c->ev_ok;
   c->have_forward = true;
   c->have_aux = aux_out.aux != nullptr;
@@ -316,6 +326,7 @@ static void commit_forward(gs_ctx* c, int n, int d, int scale_activation, long l
   c->feat = ft ? ft->feat : nullptr;
   c->filt_on = filt_on;
   c->filt = v.filt;
+  c->f3d = f3d;
   c->gather = gather;
   c->n = n;
   c->d = d;
@@ -522,6 +533,8 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
     if (!gather)
       return gs_fail(GS_ERR_UNSUPPORTED, who, "the packed path (gs_tune(\"gather\", 0)) has no feature kernel");
   }
+  const float* f3d = c->filter3d;
+  if (f3d && c->filter3d_n != n) return gs_fail(GS_ERR_INVALID_ARG, who, "the 3-D filter is sized for another n");
   if (int rc = begin_forward(c, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   GsFrameGeom g;
@@ -570,7 +583,7 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
   GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
                                       half_w, half_h, c->rec.as<GsRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
                                       c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
-                                      sh_gaussian, filt_on ? &filt : nullptr));
+                                      sh_gaussian, filt_on ? &filt : nullptr, f3d));
   if (n > 0) gs_count_launch();
   long long m = 0;
   if (int rc = bin_frame(c, n, g, gather, blend_d, d, rgb, st, m)) return rc;
@@ -597,7 +610,8 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
   }
   gs_count_launch();   // blend forward
   gs_mark(c, 6, st);
-  commit_forward(c, n, d, scale_activation, m, g, vw, cam->near_plane, 0, sh_gaussian, gather, filt_on, aux_out, ft);
+  commit_forward(c, n, d, scale_activation, m, g, vw, cam->near_plane, 0, sh_gaussian, gather, filt_on, aux_out, ft,
+                 f3d);
   return 0;
 }
 
@@ -736,7 +750,7 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                       c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                                       grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
                                                       c->cam_part.as<float>(), grad_cam, st, grad_aux != nullptr,
-                                                      c->sh_gaussian, c->filt_on));
+                                                      c->sh_gaussian, c->filt_on, c->f3d));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sums
   } else if (grad_cam) {
     GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
@@ -745,7 +759,8 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                 c->count.as<uint32_t>(), c->grad_inst.as<float>(),
                                                 c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
                                                 grad_quat, grad_scale, c->cam_part.as<float>(), grad_cam, st,
-                                                grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
+                                                grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr,
+                                                c->f3d));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sum (always: grad_cam is always written)
   } else if (c->n_views > 1) {
     // B views: the batched kernels, which take each Gaussian's views in order.  One view: the pairs are the Gaussians,
@@ -755,14 +770,15 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                   c->count.as<uint32_t>(), c->grad_inst.as<float>(),
                                                   c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
                                                   grad_quat, grad_scale, st, grad_aux != nullptr, c->sh_gaussian,
-                                                  c->filt_on));
+                                                  c->filt_on, c->f3d));
     if (c->n > 0) gs_count_launch();
   } else {
     GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
                                             c->half_w, c->half_h, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                             c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                             grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
-                                            grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr));
+                                            grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr,
+                                            c->f3d));
     if (c->n > 0) gs_count_launch();
   }
   if (grad_map) {
@@ -775,12 +791,12 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
       GS_CUDA_TRY(gs_launch_densify_stats_batch(pos, quat, scale, c->n, c->n_views, c->scale_act, c->views.as<GsView>(),
                                                 c->near_plane, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                                 c->grad_inst.as<float>(), (int)(grow / 4), c->row_epoch.as<uint32_t>(),
-                                                c->epoch, c->geom, c->stats, st));
+                                                c->epoch, c->geom, c->stats, st, c->f3d));
     else
       GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
                                           c->half_h, c->filt_on ? c->filt : GsFilter2d{}, c->offsets_g.as<uint32_t>(),
                                           c->count.as<uint32_t>(), c->grad_inst.as<float>(), (int)(grow / 4),
-                                          c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st));
+                                          c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st, c->f3d));
     if (c->n > 0) gs_count_launch();
   }
   gs_mark(c, 9, st);
@@ -913,6 +929,8 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
     return gs_fail(GS_ERR_UNSUPPORTED, who, "SH colour evaluated per pixel has no batched kernel (use GS_SH_EVAL_GAUSSIAN)");
   if (int rc = gs_blend_batch_supported()) return rc;
   if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
+  const float* f3d = c->filter3d;
+  if (f3d && c->filter3d_n != n) return gs_fail(GS_ERR_INVALID_ARG, who, "the 3-D filter is sized for another n");
   GsAuxOut aux_out;
   bool use_aux;
   if (int rc = parse_aux(ax, final_img, aux_out, use_aux, who)) return rc;
@@ -935,7 +953,8 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   GS_CUDA_TRY(gs_launch_fused_project_batch(pos, rgb, opa, quat, scale, n, n_views, d, scale_activation,
                                             c->views.as<GsView>(), c0.near_plane, c->rec.as<GsRec>(),
                                             c->rect.as<uint2>(), c->count.as<uint32_t>(), c->dkey_in.as<uint32_t>(),
-                                            culling_mask, c->counters.as<unsigned int>(), st, sh_gaussian, filt_on));
+                                            culling_mask, c->counters.as<unsigned int>(), st, sh_gaussian, filt_on,
+                                            f3d));
   if (n > 0) gs_count_launch();
   long long m = 0;
   if (int rc = bin_frame(c, nb, g, true, 3, d, rgb, st, m)) return rc;
@@ -948,7 +967,7 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   gs_mark(c, 6, st);
   // view 0's constants: a one-view batch is differentiated by the single-view projection backward
   commit_forward(c, n, d, scale_activation, m, g, c->host_views[0], c0.near_plane, n_views, sh_gaussian, true, filt_on,
-                 aux_out, nullptr);
+                 aux_out, nullptr, f3d);
   return 0;
 }
 
@@ -1028,6 +1047,75 @@ extern "C" int gs_ctx_set_filter2d(gs_ctx* c, int mode, float variance_px2) {
     return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter2d: variance must be finite and > 0");
   c->filter2d = mode;
   c->filter2d_var = variance_px2;
+  return 0;
+}
+
+extern "C" int gs_ctx_set_filter3d(gs_ctx* c, const float* filter3d, int n) {
+  if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter3d: null ctx");
+  if (n < 0) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_ctx_set_filter3d: n < 0");
+  c->filter3d = filter3d;
+  c->filter3d_n = filter3d ? n : 0;
+  return 0;
+}
+
+extern "C" int gs_filter3d_compute(gs_ctx* c, const float* pos, int n, const gs_camera* cams_host, int n_cams,
+                                   float margin, float variance, float* filter3d, gs_stream_t stream) {
+  const char* who = "gs_filter3d_compute";
+  if (!c || !cams_host || (n > 0 && (!pos || !filter3d))) return gs_fail(GS_ERR_INVALID_ARG, who, "null argument");
+  if (n < 0 || n_cams < 1) return gs_fail(GS_ERR_INVALID_ARG, who, "n must be >= 0 and n_cams >= 1");
+  if (!std::isfinite(variance) || !(variance > 0.f))
+    return gs_fail(GS_ERR_INVALID_ARG, who, "variance must be finite and > 0");
+  if (!std::isfinite(margin) || !(margin >= 0.f)) return gs_fail(GS_ERR_INVALID_ARG, who, "margin must be finite and >= 0");
+  for (int v = 0; v < n_cams; ++v) {
+    const gs_camera& cm = cams_host[v];
+    if (cm.width <= 0 || cm.height <= 0 || !std::isfinite(cm.focal_x) || !(cm.focal_x > 0.f) ||
+        !std::isfinite(cm.focal_y) || !(cm.focal_y > 0.f))
+      return gs_fail(GS_ERR_INVALID_ARG, who, "bad camera (size and focal lengths must be positive and finite)");
+    if (!std::isfinite(cm.near_plane) || cm.near_plane < 0.f)
+      return gs_fail(GS_ERR_INVALID_ARG, who, "bad camera (near_plane must be finite and >= 0)");
+  }
+  if (n == 0) return 0;
+  if (int rc = gs_check_device(c->device, who)) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!c->ev_f3) GS_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_f3, cudaEventDisableTiming));
+  // the previous upload from the pinned staging may still be pending
+  GS_CUDA_TRY(cudaEventSynchronize(c->ev_f3));
+  if (c->f3_host_cap < n_cams) {
+    if (c->f3_host) cudaFreeHost(c->f3_host);
+    c->f3_host = nullptr;
+    c->f3_host_cap = 0;
+    GS_CUDA_TRY(cudaMallocHost(reinterpret_cast<void**>(&c->f3_host), sizeof(GsF3View) * (size_t)n_cams));
+    c->f3_host_cap = n_cams;
+  }
+  for (int v = 0; v < n_cams; ++v) {
+    const gs_camera& cm = cams_host[v];
+    GsF3View& o = c->f3_host[v];
+    o = GsF3View{};
+    for (int k = 0; k < 3; ++k) o.rz[k] = cm.rot[6 + k];
+    o.tz = cm.tran[2];
+    o.fxd = cm.focal_x;
+    for (int k = 0; k < 6; ++k) o.r[k] = cm.rot[k];
+    o.t[0] = cm.tran[0];
+    o.t[1] = cm.tran[1];
+    o.fx = cm.focal_x;
+    o.fy = cm.focal_y;
+    o.cx = (float)(cm.width / 2.0);
+    o.cy = (float)(cm.height / 2.0);
+    o.ulo = (float)(-(double)margin * cm.width);
+    o.uhi = (float)((1.0 + (double)margin) * cm.width);
+    o.wlo = (float)(-(double)margin * cm.height);
+    o.whi = (float)((1.0 + (double)margin) * cm.height);
+    o.near = cm.near_plane;
+  }
+  GS_CUDA_TRY(c->f3_dev.reserve(16 + sizeof(GsF3View) * (size_t)n_cams, st));
+  unsigned int* min_rate = c->f3_dev.as<unsigned int>();
+  GsF3View* views = reinterpret_cast<GsF3View*>(c->f3_dev.as<char>() + 16);
+  GS_CUDA_TRY(cudaMemsetAsync(min_rate, 0xff, 4, st));
+  GS_CUDA_TRY(cudaMemcpyAsync(views, c->f3_host, sizeof(GsF3View) * (size_t)n_cams, cudaMemcpyHostToDevice, st));
+  GS_CUDA_TRY(cudaEventRecord(c->ev_f3, st));
+  GS_CUDA_TRY(gs_launch_filter3d(pos, n, views, n_cams, variance, filter3d, min_rate, st));
+  gs_count_launch(2);
   return 0;
 }
 

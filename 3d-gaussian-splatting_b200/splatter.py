@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import math
 import os
+import weakref
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -226,7 +227,8 @@ class Splatter(nn.Module):
                  tile_culling_method="prob2", tile_culling_dist_thresh=0.5, tile_culling_prob_thresh=0.1,
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
-                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none", n_features=0):
+                 sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none", n_features=0,
+                 filter3d=False, filter3d_variance=0.2):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -247,6 +249,16 @@ class Splatter(nn.Module):
         sqrt(det / det'), keeping each Gaussian's screen-space integral (Mip-Splatting's 2-D filter, gsplat's
         "antialiased").  Every frame of this Splatter follows it, with gradients.  A scene renders differently under
         another mode: train and render with the same one.
+
+        `filter3d`: Mip-Splatting's 3-D smoothing filter (default off, the reference).  Each Gaussian's scale is
+        bounded from below by the finest sampling interval the training views have at it, s' = sqrt(s^2 + f^2) with
+        f = sqrt(`filter3d_variance`) z / fx over the view that samples it most finely, and its opacity is scaled by
+        prod s / s' (the 3-D integral is kept): no needle-like artefacts when the scene is rendered closer or at a longer
+        focal length than it was trained.  The filter lives in `self.filter3d` [n] (a buffer, not a Parameter), is
+        computed by `compute_filter3d`, and is recomputed after every densification and whenever the Gaussians were
+        replaced; Mip-Splatting also recomputes it every 100 steps (call `compute_filter3d()`).  Densification, MCMC
+        noise and regularisers keep using the unfiltered scale and opacity.  Mip-Splatting's configuration:
+        filter2d="antialias", filter3d=True, filter3d_variance=0.1 (the default 0.2 is its filter's own default).
 
         `densify_stats`: "none" (default); "grad" accumulates the screen-space densification statistics of 3D
         Gaussian Splatting in `self.densify_stats` (a `DensifyStats`: view-space gradient norm, view count, largest
@@ -276,6 +288,12 @@ class Splatter(nn.Module):
             raise ValueError(f"filter2d_variance must be a number, not {filter2d_variance!r}") from None
         if not (math.isfinite(filter2d_variance) and filter2d_variance > 0):
             raise ValueError(f"filter2d_variance must be finite and > 0, not {filter2d_variance!r}")
+        try:
+            filter3d_variance = float(filter3d_variance)
+        except (TypeError, ValueError):
+            raise ValueError(f"filter3d_variance must be a number, not {filter3d_variance!r}") from None
+        if not (math.isfinite(filter3d_variance) and filter3d_variance > 0):
+            raise ValueError(f"filter3d_variance must be finite and > 0, not {filter3d_variance!r}")
         if densify_stats not in DENSIFY_STATS:
             raise ValueError(f"densify_stats must be one of {DENSIFY_STATS}, not {densify_stats!r}")
         if densify_stats == "absgrad" and use_sh_coeff and sh_eval == "pixel":
@@ -285,6 +303,10 @@ class Splatter(nn.Module):
         _check_features(n_features, use_sh_coeff, sh_eval, densify_stats)
         self.sh_eval = sh_eval
         self.filter2d, self.filter2d_variance = filter2d, filter2d_variance
+        self.use_filter3d, self.filter3d_variance = bool(filter3d), filter3d_variance
+        self.filter3d = None                                        # [n] once computed (compute_filter3d)
+        self._filter3d_of = None                                    # weakref to the pos Parameter it was computed for
+        ckpt_filter3d = None
         self.use_sh_coeff = bool(use_sh_coeff)
         self.near = near
         self.render_downsample = render_downsample
@@ -306,6 +328,7 @@ class Splatter(nn.Module):
         if load_ckpt is not None:                                   # reference splatter.py:417-424
             ckpt = torch.load(load_ckpt, map_location="cpu", weights_only=False)   # nn.Parameters, train.py:284-290
             params = {k: ckpt[k].detach() for k in ("pos", "rgb", "opa", "quat", "scale")}
+            ckpt_filter3d = ckpt.get("filter3d")
             if ckpt.get("feat") is not None:                       # a checkpoint with features (checkpoint.py)
                 params["feat"] = ckpt["feat"].detach()
                 if not n_features:
@@ -332,6 +355,8 @@ class Splatter(nn.Module):
         if densify_stats != "none":
             self.densify_stats = DensifyStats(self.gaussian_3ds.pos.shape[0], densify_stats == "absgrad", self.device,
                                               self._rctx)
+        if self.use_filter3d and ckpt_filter3d is not None and ckpt_filter3d.numel() == self.gaussian_3ds.pos.shape[0]:
+            self._set_filter3d(ckpt_filter3d)
         self._visible = None                                        # visible_mask()'s buffer
         self.ground_truth = None
         self.culling_mask = None
@@ -436,6 +461,7 @@ class Splatter(nn.Module):
         """Padded, un-clamped image (what reference `render` returns, splatter.py:563-634)."""
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
+        self._size_filter3d()
         image, mask = render_frame(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                    v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                    self.tile_culling_prob_thresh, self.scale_activation)
@@ -449,6 +475,7 @@ class Splatter(nn.Module):
         self.set_camera(camera_id, extrinsics, intrinsics)
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
+        self._size_filter3d()
         image, mask = render_frame_final(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                          v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                          self.tile_culling_prob_thresh, self.scale_activation)
@@ -464,6 +491,7 @@ class Splatter(nn.Module):
         self.set_camera(camera_id, extrinsics, intrinsics)
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
+        self._size_filter3d()
         image, depth, alpha, mask = render_frame_aux(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], v["rot"], v["tran"],
                                                      self.near, self.tile_culling_prob_thresh, self.scale_activation,
@@ -501,6 +529,7 @@ class Splatter(nn.Module):
             rots, trans = torch.stack([v["rot"] for v in vs]), torch.stack([v["tran"] for v in vs])
         g = self.gaussian_3ds
         self._size_densify_stats()
+        self._size_filter3d()
         image, depth, alpha, mask = render(
             self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, vs[0]["width"], vs[0]["height"],
             [v["focal_x"] for v in vs], [v["focal_y"] for v in vs], rots, trans, self.near,
@@ -525,6 +554,7 @@ class Splatter(nn.Module):
         self.set_camera(camera_id, extrinsics, intrinsics)
         v = self.current_view
         self._size_densify_stats()
+        self._size_filter3d()
         image, features, depth, alpha, mask = render_frame_feat(
             self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, g.feat, v["width"], v["height"], v["focal_x"],
             v["focal_y"], v["rot"], v["tran"], self.near, self.tile_culling_prob_thresh, self.scale_activation,
@@ -547,6 +577,7 @@ class Splatter(nn.Module):
             raise ValueError("render_at_pose: no current view; pass camera_id")
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
+        self._size_filter3d()
         image, depth, alpha, mask = render_frame_cam(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], rot, tran, self.near,
                                                      self.tile_culling_prob_thresh, self.scale_activation,
@@ -561,6 +592,66 @@ class Splatter(nn.Module):
         self.set_camera(camera_id, extrinsics, intrinsics)
         padded = self.render_padded()
         return self.tile_info.crop(torch.clamp(padded, 0, 1))
+
+    # -- 3-D smoothing filter (Mip-Splatting) ----------------------------------------------------
+    @torch.no_grad()
+    def compute_filter3d(self, views=None, margin=0.15):
+        """(Re)compute `self.filter3d` [n] on the device (`gaussian.filter3d_compute`) from the sampling rate of
+        `views` (default: the training views, with their current focal lengths; dicts with width, height, focal_x,
+        focal_y, rot, tran) at this Splatter's near plane: f_i = sqrt(filter3d_variance) / max over the views that see
+        Gaussian i (in front of the near plane, inside the image widened by `margin` on every side) of fx / z; a
+        Gaussian no view sees gets the largest filter.  The same bits for any order of the views, so data-parallel
+        replicas that hold the same views agree.  Returns the buffer."""
+        if not self.use_filter3d:
+            raise RuntimeError("compute_filter3d needs Splatter(..., filter3d=True)")
+        vs = list(self.views if views is None else views)
+        if not vs:
+            raise ValueError("compute_filter3d: no views")
+        g = self.gaussian_3ds
+        size = torch.tensor([[int(v["width"]), int(v["height"])] for v in vs], dtype=torch.int64)
+        focal = torch.tensor([[float(v["focal_x"]), float(v["focal_y"])] for v in vs], dtype=torch.float32)
+        rot = torch.stack([torch.as_tensor(np.asarray(v["rot"]), dtype=torch.float32).reshape(3, 3) for v in vs])
+        tran = torch.stack([torch.as_tensor(np.asarray(v["tran"]), dtype=torch.float32).reshape(3) for v in vs])
+        n = g.pos.shape[0]
+        out = self.filter3d if self.filter3d is not None and self.filter3d.numel() == n else None
+        f = gaussian.filter3d_compute(self._rctx, g.pos.detach().contiguous(), size, focal, rot, tran, float(self.near),
+                                      float(margin), self.filter3d_variance, out)
+        self._set_filter3d(f)
+        return f
+
+    def _set_filter3d(self, f):
+        self.filter3d = f.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        self._filter3d_of = weakref.ref(self.gaussian_3ds.pos)
+        self._rctx.set_filter3d(self.filter3d)
+
+    def _size_filter3d(self):
+        # the filter follows the scene: recomputed when its Gaussians were replaced (a densification, a checkpoint)
+        if not self.use_filter3d:
+            return
+        if (self.filter3d is None or self.filter3d.numel() != self.gaussian_3ds.pos.shape[0] or
+                self._filter3d_of is None or self._filter3d_of() is not self.gaussian_3ds.pos):
+            self.compute_filter3d()
+
+    @torch.no_grad()
+    def bake_filter3d(self):
+        """Raw (opa [n], scale [n, 3]) with the 3-D filter folded in, for renderers without one: the logit of
+        sigma prod s / s' formed in fp64, and s' = sqrt(s^2 + f^2) inverted through the scale activation.  Rows with a
+        zero filter keep their parameters.  Rendered without a 3-D filter they give the filtered frame."""
+        if not self.use_filter3d:
+            raise RuntimeError("bake_filter3d needs Splatter(..., filter3d=True)")
+        self._size_filter3d()
+        g = self.gaussian_3ds
+        raw = g.scale.detach().double()
+        s = raw.abs() + EPS if self._scale_act() == 0 else torch.exp(raw)
+        f = self.filter3d.double().unsqueeze(1)
+        sf = torch.sqrt(s * s + f * f)
+        sig = torch.sigmoid(g.opa.detach().double()) * torch.prod(s / sf, dim=1)
+        opa = torch.log(sig) - torch.log1p(-sig)
+        scale = (sf - EPS) if self._scale_act() == 0 else torch.log(sf)
+        keep = self.filter3d == 0
+        opa = torch.where(keep, g.opa.detach(), opa.float())
+        scale = torch.where(keep.unsqueeze(1), g.scale.detach(), scale.float())
+        return opa.contiguous(), scale.contiguous()
 
     # -- densification from screen-space statistics ----------------------------------------------
     def _size_densify_stats(self):
@@ -597,6 +688,7 @@ class Splatter(nn.Module):
         g._replace(new)
         self.n_gaussians = g.pos.shape[0]
         st.reset(self.n_gaussians)
+        self._size_filter3d()
         return dict(deleted=int(n_deleted), cloned=int(n_clone), split=int(n_split), total=self.n_gaussians)
 
     # -- MCMC densification (3DGS-MCMC; mcmc.MCMC schedules these) -----------------------------------------------------
@@ -634,6 +726,8 @@ class Splatter(nn.Module):
                                        u, touched=touched, **kw)
         if touched is not None:
             _zero_moment_rows(optimizer, self._mcmc_params(), touched.bool())
+        if self.use_filter3d:                                       # in place: the Parameters kept their identity
+            self.compute_filter3d()
         return n_rel
 
     @torch.no_grad()
@@ -658,6 +752,7 @@ class Splatter(nn.Module):
             _regrow_optimizer(optimizer, list(zip(old, self._mcmc_params())))
         self.n_gaussians = g.pos.shape[0]
         self._size_densify_stats()
+        self._size_filter3d()
         return n_new
 
     @torch.no_grad()

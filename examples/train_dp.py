@@ -27,7 +27,7 @@ import splatter  # noqa: E402
 import synthetic as S  # noqa: E402
 
 
-def build(n, w, h, n_views, dev, seed=0):
+def build(n, w, h, n_views, dev, seed=0, student_kw=None):
     teacher = S.make_gaussians(n, w, h, seed)
     views = [S.make_view(w, h, k) for k in range(n_views)]
     vd = [dict(width=v.width, height=v.height, focal_x=v.fx, focal_y=v.fy, rot=v.rot, tran=v.tran) for v in views]
@@ -40,7 +40,7 @@ def build(n, w, h, n_views, dev, seed=0):
     student["rgb"] = torch.zeros_like(teacher["rgb"])
     student["opa"] = torch.full_like(teacher["opa"], -2.0)
     student["scale"] = teacher["scale"] * (1 + 0.2 * torch.randn(n, 3, generator=g)).clamp(0.5, 1.5)
-    return splatter.Splatter.from_tensors(student, vd, device=dev), gts
+    return splatter.Splatter.from_tensors(student, vd, device=dev, **(student_kw or {})), gts
 
 
 def make_optimizer(sp, lr=0.003, fused=True):
@@ -51,7 +51,8 @@ def make_optimizer(sp, lr=0.003, fused=True):
         {"params": g.scale, "lr": lr}, {"params": g.quat, "lr": lr}], betas=(0.9, 0.99))
 
 
-def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None):
+def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None,
+          filter3d_every=0):
     opt = make_optimizer(sp, lr, fused_adam)
     params = list(sp.gaussian_3ds.parameters())
     bucket = dp.make_grad_bucket(params, average=True)   # peer-memory exchange when available, else NCCL
@@ -75,6 +76,8 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
             opt.step(visible=dp.all_reduce_visible(sp.visible_mask()))
         else:
             opt.step()
+        if filter3d_every and it % filter3d_every == 0:                 # Mip-Splatting: over all training views
+            sp.compute_filter3d()
         if mc is not None:
             n = sp.gaussian_3ds.pos.shape[0]
             mc.after_step(it, lr)
@@ -106,6 +109,9 @@ def main():
                          "every 100 steps, position noise every step; with --visible-adam the opacity and scale "
                          "regularisers reach only the visible rows, like every other gradient")
     ap.add_argument("--cap-max", type=int, default=None, help="Gaussian count cap of --mcmc (default 1.5 x --gaussians)")
+    ap.add_argument("--filter3d", action="store_true",
+                    help="Mip-Splatting's configuration: the 2-D antialias filter and the 3-D filter (variance 0.1), "
+                         "recomputed every 100 steps over all training views on every rank")
     args = ap.parse_args()
     if args.visible_adam and args.torch_adam:
         ap.error("--visible-adam is a mode of the fused flat Adam")
@@ -118,10 +124,12 @@ def main():
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=dev)
     torch.manual_seed(2023)                                           # identical torch RNG on all ranks
-    sp, gts = build(args.gaussians, w, h, args.views, dev)
+    kw = dict(filter2d="antialias", filter3d=True, filter3d_variance=0.1) if args.filter3d else None
+    sp, gts = build(args.gaussians, w, h, args.views, dev, student_kw=kw)
     hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam,
                       visible_adam=args.visible_adam,
-                      cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None)
+                      cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None,
+                      filter3d_every=100 if args.filter3d else 0)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
               f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians")

@@ -370,6 +370,40 @@ int gs_ctx_set_sh_eval(gs_ctx* ctx, int mode);
 #define GS_FILTER2D_ANTIALIAS 2
 int gs_ctx_set_filter2d(gs_ctx* ctx, int mode, float variance_px2);
 
+/* 3-D smoothing filter of the Gaussians (additive; default off, the reference, which has none): Mip-Splatting's 3D
+ * filter, which bounds every Gaussian's 3-D scale from below by the finest sampling interval any training view has at
+ * it, so that a scene rendered closer or at a longer focal length than it was trained shows no needle-like artefacts.
+ * With filter3d[i] = f_i >= 0 (world units) and the activated scale s (|raw| + 1e-4 or exp(raw)), every fused frame
+ * uses
+ *   s'_k = sqrt(s_k^2 + f_i^2)                 for the 3-D covariance (the conic, the det <= 0 test, the tile
+ *                                              rectangle and the 2-D filter, if one is set, follow it);
+ *   sigma' = sigma prod_k s_k / s'_k           the opacity, which keeps sigma sqrt(det Sigma3), the 3-D integral.
+ * A row with f_i == 0 takes the unfiltered arithmetic by selection: a zero filter renders, and differentiates, the bits
+ * of a frame without one.  A scale that underflows to 0 gets opacity 0 and zero gradients.  Backward: filter3d is a
+ * constant (no gradient); dL/ds_k = dL/ds'_k s_k / s'_k + dL/dl2o f^2 / (ln 2 s_k (s_k^2 + f^2)) joins the raw-scale
+ * chain; the opacity-logit gradient is unchanged; the camera gradient uses s' (f does not depend on the camera).
+ * gs_ctx_set_filter3d: a context setting, like gs_ctx_set_densify_stats: the DEVICE pointer [n] is the caller's and
+ * must stay alive while it is set; NULL turns the filter off.  It applies to every fused forward that follows (plain,
+ * final, aux, feat, batch, the packed path, gs_render_forward_backward_host); a forward records the pointer and its
+ * backward (plain, final, aux, cam, batch, batch cam, feat, with or without a gradient push, the densification
+ * statistics' max_radius) uses the recorded one.  A forward whose n differs from the filter's n is refused
+ * (GS_ERR_INVALID_ARG) before any launch.  No launch or synchronisation is added.  Null ctx or n < 0:
+ * GS_ERR_INVALID_ARG. */
+int gs_ctx_set_filter3d(gs_ctx* ctx, const float* filter3d /* DEVICE [n]; NULL: off */, int n);
+/* The filter of Mip-Splatting's sampling rate over the views cams_host[n_cams] (e.g. all training views), into
+ * filter3d[n] (DEVICE):  view c (W, H, fx, fy, R, t, near = near_plane) sees Gaussian i when, with p_c = R pos_i + t,
+ * u = fx x / z + W / 2 and w = fy y / z + H / 2:  z > near, -margin W <= u <= (1 + margin) W and
+ * -margin H <= w <= (1 + margin) H.  nu_i = max over the views that see i of fx / z (the maximal sampling rate), and
+ * filter3d[i] = sqrt(variance) / nu_i.  A Gaussian no view sees gets the largest filter, that of the smallest nu over
+ * the seen ones; none seen at all: 0 everywhere.  Mip-Splatting's defaults: margin 0.15, variance 0.2.  The rates are
+ * fp64 divisions and max / min are order-independent: the same bits on every call and for any order of the views, so
+ * data-parallel replicas agree without an exchange.  Two launches when n > 0, no host synchronisation; the context
+ * keeps 112 bytes of device workspace and pinned staging per view.  Refused before any launch (GS_ERR_INVALID_ARG):
+ * a null ctx or cams_host, a null pos or filter3d with n > 0; n < 0 or n_cams < 1; a variance that is not finite and > 0; a margin that is not finite and
+ * >= 0; a camera whose size or focal lengths are not positive and finite, or whose near_plane is not finite and >= 0. */
+int gs_filter3d_compute(gs_ctx* ctx, const float* pos /* [n,3] */, int n, const gs_camera* cams_host, int n_cams,
+                        float margin, float variance, float* filter3d /* [n] */, gs_stream_t stream);
+
 /* Screen-space densification statistics (additive; default off).  While a context has them set, every backward that
  * computes parameter gradients (plain, final, aux, cam with parameter gradients, gs_render_forward_backward_host, with
  * or without a gradient push) accumulates, for every Gaussian i with count[i] > 0 in its forward (i.e. binned into at

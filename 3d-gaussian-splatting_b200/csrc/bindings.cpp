@@ -313,6 +313,32 @@ struct RenderContext {
     filter3d_ref = *f;
   }
 
+  // camera lenses (gs_ctx_set_lens): models a sequence of n GS_LENS_* codes and params a CPU float32 tensor [n, 6] =
+  // (cx, cy, k0, k1, k2, k3) per lens, or None (off); applies to the forwards that follow, a backward uses the lenses
+  // of its forward
+  void set_lens(std::optional<std::vector<int>> models, std::optional<torch::Tensor> params) {
+    if (!models || !params) {
+      TORCH_CHECK(!models && !params, "set_lens: give both models and params, or neither");
+      check_rc(gs_ctx_set_lens(ctx, nullptr, 0), "gs_ctx_set_lens");
+      return;
+    }
+    const int64_t n = (int64_t)models->size();
+    TORCH_CHECK(!params->is_cuda() && params->scalar_type() == at::kFloat && params->dim() == 2 &&
+                    params->size(0) == n && params->size(1) == 6,
+                "set_lens: params must be a CPU float32 tensor [n, 6] with n = len(models)");
+    TORCH_CHECK(n <= GS_MAX_VIEWS, "set_lens: more than GS_MAX_VIEWS lenses");
+    const torch::Tensor pc = params->contiguous();
+    const float* pp = pc.data_ptr<float>();
+    std::vector<gs_lens> lenses((size_t)n);
+    for (int64_t v = 0; v < n; ++v) {
+      lenses[v].model = (*models)[v];
+      lenses[v].cx = pp[6 * v];
+      lenses[v].cy = pp[6 * v + 1];
+      for (int k = 0; k < 4; ++k) lenses[v].k[k] = pp[6 * v + 2 + k];
+    }
+    check_rc(gs_ctx_set_lens(ctx, lenses.data(), (int)n), "gs_ctx_set_lens");
+  }
+
   // gs_filter3d_compute over V views: size [V,2] = (width, height), focal [V,2] = (fx, fy), rot [V,3,3], tran [V,3]
   // (CPU tensors), one near plane; writes and returns out [n] (allocated when None)
   torch::Tensor filter3d_compute(torch::Tensor pos, torch::Tensor size, torch::Tensor focal, torch::Tensor rot,
@@ -1237,6 +1263,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
       .def("set_filter3d", &RenderContext::set_filter3d, py::arg("filter3d"))
+      .def("set_lens", &RenderContext::set_lens, py::arg("models"), py::arg("params"))
       .def("set_densify_stats", &RenderContext::set_densify_stats, py::arg("grad2d"), py::arg("count"),
            py::arg("max_radius"), py::arg("absgrad") = py::none())
       .def("clear_densify_stats", &RenderContext::clear_densify_stats)
@@ -1295,4 +1322,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("FILTER2D_NONE") = GS_FILTER2D_NONE;
   m.attr("FILTER2D_DILATE") = GS_FILTER2D_DILATE;
   m.attr("FILTER2D_ANTIALIAS") = GS_FILTER2D_ANTIALIAS;
+  m.attr("LENS_PINHOLE") = GS_LENS_PINHOLE;
+  m.attr("LENS_OPENCV") = GS_LENS_OPENCV;
+  m.attr("LENS_FISHEYE") = GS_LENS_FISHEYE;
 }

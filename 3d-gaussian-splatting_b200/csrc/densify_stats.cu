@@ -7,6 +7,7 @@
 namespace {
 
 constexpr int kBlock = 256;
+constexpr float kInf = __builtin_huge_valf();   // gs_project's frustum half-widths in a lens frame (gs_lens_project)
 
 // Gaussian i with count[i] > 0 (it got at least one tile instance in the forward):
 //   grad2d  += |(gx sx, gy sy)|, (gx, gy) = sum of columns 0, 1 over its rows tagged with this backward's epoch
@@ -16,6 +17,8 @@ constexpr int kBlock = 256;
 // (sx, sy) = (W / (2 fx), H / (2 fy)) converts dL/d(x/z, y/z) to the NDC convention of 3DGS's viewspace gradient.
 // One thread owns one Gaussian and sums its rows in order: bit-deterministic, no atomics.
 // G3: the forward applied the 3-D filter f3d[n]: the covariance is the filtered scale's (gs_filter3d).
+// L (only with G3): the forward applied the lens `lens`: the covariance is the lensed one (gs_lens_project); f3d may be
+// NULL.  (x, y) stays the stored mean's gradient.
 #define GS_STATS_PARAMS                                                                                             \
   const float* __restrict__ pos, const float* __restrict__ quat, const float* __restrict__ scale, int n,            \
       int scale_act, GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt,                      \
@@ -26,8 +29,9 @@ constexpr int kBlock = 256;
 #define GS_STATS_ARGS                                                                                             \
   pos, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, filt, offsets_g, count, grad_inst, gw, row_epoch, \
       epoch, sx, sy, fx, fy, grad2d, absgrad, n_views, max_radius
-template <bool ABS, bool G3>
-__device__ __forceinline__ void densify_stats_body(GS_STATS_PARAMS, const float* __restrict__ f3d) {
+template <bool ABS, bool G3, bool L = false>
+__device__ __forceinline__ void densify_stats_body(GS_STATS_PARAMS, const float* __restrict__ f3d,
+                                                   GsLens lens = GsLens{}) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   const uint32_t cnt = count[i];
@@ -37,7 +41,7 @@ __device__ __forceinline__ void densify_stats_body(GS_STATS_PARAMS, const float*
   gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
   if constexpr (G3) {
     float s0[3], dl2o3;
-    gs_filter3d(f3d[i], s, s0, dl2o3);
+    gs_filter3d((L && !f3d) ? 0.f : f3d[i], s, s0, dl2o3);
   }
   float gx = 0.f, gy = 0.f, ax = 0.f, ay = 0.f;
   const uint32_t o0 = offsets_g[i], o1 = o0 + cnt;
@@ -54,7 +58,11 @@ __device__ __forceinline__ void densify_stats_body(GS_STATS_PARAMS, const float*
     }
   }
   // the covariance the forward binned: with the filter its dilated one (a zero filter leaves it as it is)
-  GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+  GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
+  if constexpr (L) {
+    float J[4];
+    gs_lens_project(lens, o, half_w, half_h, J);
+  }
   const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
   const double A = (double)fo.a * fx * fx, B = (double)o.b * fx * fy, D = (double)fo.d * fy * fy;
   const double h = 0.5 * (A - D);
@@ -75,6 +83,12 @@ template <bool ABS>
 __global__ void __launch_bounds__(kBlock) densify_stats_filt3_kernel(GS_STATS_PARAMS, const float* __restrict__ f3d) {
   densify_stats_body<ABS, true>(GS_STATS_ARGS, f3d);
 }
+
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_lens_kernel(GS_STATS_PARAMS, const float* __restrict__ f3d,
+                                                                    GsLens lens) {
+  densify_stats_body<ABS, true, true>(GS_STATS_ARGS, f3d, lens);
+}
 #undef GS_STATS_ARGS
 #undef GS_STATS_PARAMS
 
@@ -90,8 +104,9 @@ __global__ void __launch_bounds__(kBlock) densify_stats_filt3_kernel(GS_STATS_PA
 #define GS_STATS_BATCH_ARGS                                                                                       \
   pos, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, gw, row_epoch, epoch,   \
       width, height, grad2d, absgrad, n_views_out, max_radius
-template <bool ABS, bool G3>
-__device__ __forceinline__ void densify_stats_batch_body(GS_STATS_BATCH_PARAMS, const float* __restrict__ f3d) {
+template <bool ABS, bool G3, bool L = false>
+__device__ __forceinline__ void densify_stats_batch_body(GS_STATS_BATCH_PARAMS, const float* __restrict__ f3d,
+                                                         const GsLens* __restrict__ lenses = nullptr) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   if (i >= n) return;
   float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
@@ -99,7 +114,7 @@ __device__ __forceinline__ void densify_stats_batch_body(GS_STATS_BATCH_PARAMS, 
   gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
   if constexpr (G3) {
     float s0[3], dl2o3;
-    gs_filter3d(f3d[i], s, s0, dl2o3);
+    gs_filter3d((L && !f3d) ? 0.f : f3d[i], s, s0, dl2o3);
   }
   float g2 = grad2d[i], ga = ABS ? absgrad[i] : 0.f, mr = max_radius[i];
   int nv = n_views_out[i];
@@ -126,7 +141,11 @@ __device__ __forceinline__ void densify_stats_batch_body(GS_STATS_BATCH_PARAMS, 
         ay += a.y;
       }
     }
-    GsProj o = gs_project(vw.cam, p, q, s, near_plane, vw.half_w, vw.half_h);
+    GsProj o = gs_project(vw.cam, p, q, s, near_plane, L ? kInf : vw.half_w, L ? kInf : vw.half_h);
+    if constexpr (L) {
+      float J[4];
+      gs_lens_project(lenses[v], o, vw.half_w, vw.half_h, J);
+    }
     const GsFilter2dOut fo = gs_filter2d(vw.filt, o.a, o.b, o.c, o.d);
     const float fx = vw.fx, fy = vw.fy;
     const double A = (double)fo.a * fx * fx, B = (double)o.b * fx * fy, D = (double)fo.d * fy * fy;
@@ -155,6 +174,13 @@ __global__ void __launch_bounds__(kBlock) densify_stats_batch_filt3_kernel(GS_ST
                                                                            const float* __restrict__ f3d) {
   densify_stats_batch_body<ABS, true>(GS_STATS_BATCH_ARGS, f3d);
 }
+
+template <bool ABS>
+__global__ void __launch_bounds__(kBlock) densify_stats_batch_lens_kernel(GS_STATS_BATCH_PARAMS,
+                                                                          const float* __restrict__ f3d,
+                                                                          const GsLens* __restrict__ lenses) {
+  densify_stats_batch_body<ABS, true, true>(GS_STATS_BATCH_ARGS, f3d, lenses);
+}
 #undef GS_STATS_BATCH_ARGS
 #undef GS_STATS_BATCH_PARAMS
 
@@ -164,9 +190,20 @@ cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, c
                                           int scale_act, const GsView* views, float near_plane,
                                           const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
                                           int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
-                                          const gs_densify_stats& s, cudaStream_t st, const float* f3d) {
+                                          const gs_densify_stats& s, cudaStream_t st, const float* f3d,
+                                          const GsLens* lenses) {
   if (n == 0) return cudaSuccess;
   const int blocks = (n + kBlock - 1) / kBlock;
+  if (lenses) {
+#define GS_LAUNCH_STATS_BATCHL(ABS)                                                                                \
+  densify_stats_batch_lens_kernel<ABS><<<blocks, kBlock, 0, st>>>(                                                  \
+      pos, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, gw, row_epoch, epoch, \
+      g.width, g.height, s.grad2d, s.absgrad, s.count, s.max_radius, f3d, lenses)
+    if (s.absgrad) GS_LAUNCH_STATS_BATCHL(true);
+    else GS_LAUNCH_STATS_BATCHL(false);
+#undef GS_LAUNCH_STATS_BATCHL
+    return cudaGetLastError();
+  }
 #define GS_LAUNCH_STATS_BATCH(ABS)                                                                                 \
   densify_stats_batch_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, n_views, scale_act, views,       \
                                                              near_plane, offsets_g, count, grad_inst, gw, row_epoch, \
@@ -190,11 +227,22 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                     const GsFilter2d& filt, const uint32_t* offsets_g, const uint32_t* count,
                                     const float* grad_inst, int gw, const uint32_t* row_epoch, uint32_t epoch,
                                     const GsFrameGeom& g, const gs_densify_stats& s, cudaStream_t st,
-                                    const float* f3d) {
+                                    const float* f3d, const GsLens* lens) {
   if (n == 0) return cudaSuccess;
   const float sx = (float)((double)g.width / (2.0 * (double)g.fx));
   const float sy = (float)((double)g.height / (2.0 * (double)g.fy));
   const int blocks = (n + kBlock - 1) / kBlock;
+  if (lens) {
+#define GS_LAUNCH_STATSL(ABS)                                                                                      \
+  densify_stats_lens_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, scale_act, cam, near_plane,       \
+                                                            half_w, half_h, filt, offsets_g, count, grad_inst, gw,  \
+                                                            row_epoch, epoch, sx, sy, g.fx, g.fy, s.grad2d,        \
+                                                            s.absgrad, s.count, s.max_radius, f3d, *lens)
+    if (s.absgrad) GS_LAUNCH_STATSL(true);
+    else GS_LAUNCH_STATSL(false);
+#undef GS_LAUNCH_STATSL
+    return cudaGetLastError();
+  }
 #define GS_LAUNCH_STATS(ABS)                                                                                       \
   densify_stats_kernel<ABS><<<blocks, kBlock, 0, st>>>(pos, quat, scale, n, scale_act, cam, near_plane, half_w,    \
                                                        half_h, filt, offsets_g, count, grad_inst, gw, row_epoch,   \

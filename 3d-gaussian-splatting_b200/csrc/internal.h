@@ -135,7 +135,8 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     uint32_t* count, uint32_t* dkey, int64_t* mask, unsigned int* n_visible, cudaStream_t st,
                                     bool sh_gaussian = false /*d = 27 / 48: SH evaluated per Gaussian into rec's RGB*/,
                                     const GsFilter2d* filt = nullptr /*non-null: 2-D screen-space filter*/,
-                                    const float* f3d = nullptr /*non-null: 3-D filter [n] (with filt, or a zero one)*/);
+                                    const float* f3d = nullptr /*non-null: 3-D filter [n] (with filt, or a zero one)*/,
+                                    const GsLens* lens = nullptr /*non-null: the lens (with the 2-D and 3-D filter paths)*/);
 
 // One view of a batched frame (gs_render_forward_batch): the per-view constants of the projection, the blend, the
 // projection backward and the densification statistics, formed on the host exactly as a single-view frame forms them
@@ -154,7 +155,8 @@ cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, co
                                           uint2* rect /*[B n]*/, uint32_t* count /*[B n]*/, uint32_t* dkey /*[B n]*/,
                                           int64_t* mask /*[B, n], nullable*/, unsigned int* n_visible,
                                           cudaStream_t st, bool sh_gaussian, bool filt,
-                                          const float* f3d = nullptr /*non-null: 3-D filter [n]*/);
+                                          const float* f3d = nullptr /*non-null: 3-D filter [n]*/,
+                                          const GsLens* lenses = nullptr /*non-null: DEVICE [n_views] lenses*/);
 
 // Data-parallel gradient push (device view of gs_grad_push): world == 0 disables it.
 struct GsGradPush {
@@ -173,7 +175,8 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         bool depth_grad = false /*rows carry dL/d|p_c| in the column after the colour*/,
                                         bool sh_gaussian = false /*d = 27 / 48 coefficients, RGB gradient rows*/,
                                         const GsFilter2d* filt = nullptr /*the forward's 2-D filter*/,
-                                        const float* f3d = nullptr /*the forward's 3-D filter [n]*/);
+                                        const float* f3d = nullptr /*the forward's 3-D filter [n]*/,
+                                        const GsLens* lens = nullptr /*the forward's lens (no push)*/);
 // The same without a push, for RGB and per-Gaussian SH, plus the camera gradient: the projection backward leaves one
 // 12-float partial sum per CTA in cam_part (gs_cam_grad_workspace_bytes(n)), and a one-CTA kernel sums them in fp64
 // into grad_cam[12] = {dL/drot row-major, dL/dtran} (zeros when n == 0).  The five gradient pointers may all be NULL
@@ -186,7 +189,8 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
                                             bool depth_grad, bool sh_gaussian, const GsFilter2d* filt = nullptr,
-                                            const float* f3d = nullptr);
+                                            const float* f3d = nullptr,
+                                            const GsLens* lens = nullptr);
 
 // Batched frame: one thread per Gaussian sums, view by view in view order, the rows of pair v n + i exactly as
 // gs_launch_fused_project_bwd does for one view, chains them with view v's camera and filter, and writes the sum over
@@ -197,7 +201,8 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
                                               const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                               uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                               float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
-                                              bool filt, const float* f3d = nullptr);
+                                              bool filt, const float* f3d = nullptr,
+                                              const GsLens* lenses = nullptr);
 // The same plus each view's camera gradient (RGB and per-Gaussian SH): the projection backward leaves view v's per-CTA
 // partial sums in cam_part[v][grid][12] (n_views * gs_cam_grad_workspace_bytes(n)), and one CTA per view sums them in
 // fp64 into grad_cams[v][12] (zeros when n == 0).  The five gradient pointers may all be NULL (camera only).  Two
@@ -210,7 +215,8 @@ cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float*
                                                   float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                                   float* g_scale, float* cam_part, float* grad_cams, cudaStream_t st,
                                                   bool depth_grad, bool sh_gaussian, bool filt,
-                                                  const float* f3d = nullptr);
+                                                  const float* f3d = nullptr,
+                                                  const GsLens* lenses = nullptr);
 
 // ---- densify_stats.cu ------------------------------------------------------------------
 // Accumulates the screen-space densification statistics of the backward that just wrote grad_inst (rows of gw floats;
@@ -221,13 +227,15 @@ cudaError_t gs_launch_densify_stats(const float* pos, const float* quat, const f
                                     const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst, int gw,
                                     const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
                                     const gs_densify_stats& s, cudaStream_t st,
-                                    const float* f3d = nullptr /*the forward's 3-D filter [n]*/);
+                                    const float* f3d = nullptr /*the forward's 3-D filter [n]*/,
+                                    const GsLens* lens = nullptr /*the forward's lens*/);
 // The same for a batched frame: each view's statistics are added in view order (g: the per-view width and height)
 cudaError_t gs_launch_densify_stats_batch(const float* pos, const float* quat, const float* scale, int n, int n_views,
                                           int scale_act, const GsView* views, float near_plane,
                                           const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
                                           int gw, const uint32_t* row_epoch, uint32_t epoch, const GsFrameGeom& g,
-                                          const gs_densify_stats& s, cudaStream_t st, const float* f3d = nullptr);
+                                          const gs_densify_stats& s, cudaStream_t st, const float* f3d = nullptr,
+                                          const GsLens* lenses = nullptr);
 
 // ---- filter3d.cu -----------------------------------------------------------------------
 // One view of gs_filter3d_compute, formed on the host: the depth and the rate in fp64, the margin test in fp32.
@@ -235,15 +243,17 @@ struct GsF3View {
   double rz[3], tz;            // row 2 of R and t_z: z = rz . p + tz
   double fxd;                  // fx: the rate fx / z
   float r[6], t[2];            // rows 0, 1 of R and t_x, t_y
-  float fx, fy, cx, cy;        // cx = W / 2, cy = H / 2
+  float fx, fy, cx, cy;        // cx = W / 2, cy = H / 2 (with a lens: its principal point)
   float ulo, uhi, wlo, whi;    // -m W, (1 + m) W, -m H, (1 + m) H
   double near;                 // seen only where z > near
 };
 // f3d[n] = sqrt(variance) / (the largest fx / z among the views that see Gaussian i), or that of the smallest seen
 // rate for a Gaussian no view sees (0 everywhere when none is seen).  min_rate: one u32 set to 0xffffffff by the
 // caller.  Two launches when n > 0.
+// lenses (DEVICE [n_views], nullable): the lens variant of the rate and the visibility test (gs_ctx_set_lens).
 cudaError_t gs_launch_filter3d(const float* pos, int n, const GsF3View* views /*DEVICE [n_views]*/, int n_views,
-                               float variance, float* f3d, unsigned int* min_rate, cudaStream_t st);
+                               float variance, float* f3d, unsigned int* min_rate, cudaStream_t st,
+                               const GsLens* lenses = nullptr);
 
 // ---- optim.cu --------------------------------------------------------------------------
 // visible[n] (uint8) = count[v n + i] > 0 in any of the n_views views, OR-ed into visible when accumulate is set

@@ -7,6 +7,8 @@
 namespace {
 
 constexpr int kBlock = 256;
+// gs_project's frustum half-widths in a lens frame: the lens tests the stored mean itself (gs_lens_project)
+constexpr float kInf = __builtin_huge_valf();
 
 __global__ void __launch_bounds__(kBlock) jacobian_kernel(const float* __restrict__ pc, int n,
                                                            float* __restrict__ jac) {
@@ -59,15 +61,19 @@ __device__ __forceinline__ void sh_logits(const float* coef, const float* Y, flo
 // conic, and its compensation to l2o.
 // G3 (only with F): the 3-D smoothing filter f3d[n] (gs_filter3d) is applied to the activated scale first, and its
 // compensation added to l2o before the 2-D filter's.
+// L (only with F and G3): the lens `lens` (gs_lens_project) is applied to the projection before the 2-D filter; f3d may
+// be NULL (no 3-D filter: the f == 0 bits).
 // The batched frame's fused_project_one repeats this arithmetic: a change to it must be made to both.
-template <int KG, bool F = false, bool G3 = false>
+template <int KG, bool F = false, bool G3 = false, bool L = false>
 __device__ __forceinline__ void fused_project_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
     const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
     uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr) {
+    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr,
+    GsLens lens = GsLens{}) {
   static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
+  static_assert(!L || G3, "the lens runs in the 3-D filter's kernels");
   int i = blockIdx.x * kBlock + threadIdx.x;
   bool vis = false;
   uint32_t cnt = 0;
@@ -78,7 +84,7 @@ __device__ __forceinline__ void fused_project_body(
     float f3 = 0.f, dl2o3 = 0.f;
     if constexpr (G3) {
       float s0[3];
-      f3 = f3d[i];
+      f3 = (L && !f3d) ? 0.f : f3d[i];
       gs_filter3d(f3, s, s0, dl2o3);
     }
     // opacity and RGB logits are issued with the geometry, so that the thread makes one round trip to HBM, not two
@@ -90,7 +96,11 @@ __device__ __forceinline__ void fused_project_body(
       rgb_raw[1] = rgb[3 * i + 1];
       rgb_raw[2] = rgb[3 * i + 2];
     }
-    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
+    if constexpr (L) {
+      float J[4];
+      gs_lens_project(lens, o, half_w, half_h, J);
+    }
     vis = o.visible;
     if (mask) mask[i] = o.visible ? 1 : 0;
     bool keep = o.visible;
@@ -209,22 +219,38 @@ __global__ void __launch_bounds__(kBlock) fused_project_filt3_kernel(
                                     rec, rect, count, dkey, mask, n_visible, filt, f3d);
 }
 
+// with a lens: the 2-D and 3-D filter paths unconditionally (zero filters, f3d NULL without one, give their bits)
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_lens_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible, GsFilter2d filt, const float* __restrict__ f3d, GsLens lens) {
+  fused_project_body<K, true, true, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w,
+                                          half_h, rec, rect, count, dkey, mask, n_visible, filt, f3d, lens);
+}
+
 // Batched frames.  Gaussian i (loaded parameters p, q, s, opa_raw, rgb_raw) seen by one view: the arithmetic of
 // fused_project_body, with its record, rectangle, count and depth key going to pair j = v n + i and the rectangle's
 // rows offset by ty_off (the view's first tile row).  Returns the instance count; vis: in the frustum.  (The
 // single-view kernels keep their own copy: routed through this function they compile to different SASS; a change
 // to the arithmetic of either copy must be made to both.)
-// G3: s is the 3-D filtered scale and dl2o3 its compensation (added to l2o when f3 != 0).
-template <int KG, bool F, bool G3 = false>
+// G3: s is the 3-D filtered scale and dl2o3 its compensation (added to l2o when f3 != 0).  L: the view's lens *lens.
+template <int KG, bool F, bool G3 = false, bool L = false>
 __device__ __forceinline__ uint32_t fused_project_one(
     const float* __restrict__ rgb, int i, int d, const GsCam& cam, const GsTileGrid& grid, float near_plane,
     float half_w, float half_h, const GsFilter2d& filt, const float p[3], const float q[4], const float s[3],
     float opa_raw, const float rgb_raw[3], uint32_t ty_off, int j, GsRec* __restrict__ rec, uint2* __restrict__ rect,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis,
-    float f3 = 0.f, float dl2o3 = 0.f) {
+    float f3 = 0.f, float dl2o3 = 0.f, const GsLens* __restrict__ lens = nullptr) {
   uint32_t cnt = 0;
   {
-    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
+    if constexpr (L) {
+      float J[4];
+      gs_lens_project(*lens, o, half_w, half_h, J);
+    }
     vis = o.visible;
     if (mask) mask[j] = o.visible ? 1 : 0;
     bool keep = o.visible;
@@ -286,13 +312,14 @@ __device__ __forceinline__ uint32_t fused_project_one(
 // Batched frame: one thread per Gaussian loads its parameters once and projects it into each view in turn, writing
 // pair j = v n + i with view v's constants (K, F as in fused_project_filt_kernel; F reads views[v].filt).  The
 // counters receive the frame's totals over the pairs.  G3: the 3-D filter f3d[n] is applied once, before the views.
-template <int K, bool F, bool G3>
+// L (only with F and G3): view v's lens lenses[v]; f3d may be NULL.
+template <int K, bool F, bool G3, bool L = false>
 __device__ __forceinline__ void fused_project_batch_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,
     const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, const float* __restrict__ f3d) {
+    unsigned int* __restrict__ n_visible, const float* __restrict__ f3d, const GsLens* __restrict__ lenses = nullptr) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   unsigned int nv = 0;
   unsigned long long c64 = 0;
@@ -303,7 +330,7 @@ __device__ __forceinline__ void fused_project_batch_body(
     float f3 = 0.f, dl2o3 = 0.f;
     if constexpr (G3) {
       float s0[3];
-      f3 = f3d[i];
+      f3 = (L && !f3d) ? 0.f : f3d[i];
       gs_filter3d(f3, s, s0, dl2o3);
     }
     const float opa_raw = opa[i];
@@ -316,9 +343,9 @@ __device__ __forceinline__ void fused_project_batch_body(
     for (int v = 0; v < n_views; ++v) {
       const GsView vw = views[v];
       bool vis = false;
-      c64 += fused_project_one<K, F, G3>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p, q,
-                                         s, opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect, count,
-                                         dkey, mask, vis, f3, dl2o3);
+      c64 += fused_project_one<K, F, G3, L>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p,
+                                            q, s, opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect,
+                                            count, dkey, mask, vis, f3, dl2o3, lenses + v);
       nv += vis ? 1u : 0u;
     }
   }
@@ -365,6 +392,13 @@ template <int K>
 __global__ void __launch_bounds__(kBlock) fused_project_batch_filt3_kernel(GS_PBATCH_PARAMS,
                                                                            const float* __restrict__ f3d) {
   fused_project_batch_body<K, true, true>(GS_PBATCH_ARGS, f3d);
+}
+
+template <int K>
+__global__ void __launch_bounds__(kBlock) fused_project_batch_lens_kernel(GS_PBATCH_PARAMS,
+                                                                          const float* __restrict__ f3d,
+                                                                          const GsLens* __restrict__ lenses) {
+  fused_project_batch_body<K, true, true, true>(GS_PBATCH_ARGS, f3d, lenses);
 }
 #undef GS_PBATCH_PARAMS
 
@@ -417,8 +451,11 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
 // G3 (only with F): the forward applied the 3-D filter f3d[n] (fused_project_body<KG, true, true>): the projection is
 // differentiated at the filtered scale s', and dL/ds' is chained to dL/ds with the compensation's term
 // (gs_filter3d_backward) before the raw-scale chain.
+// L (only with G3, W = 0): the forward applied the lens `lens` (fused_project_body<KG, true, true, true>): the conic's
+// gradient is that of the lensed covariance, and gs_lens_backward takes the mean and covariance gradients back through
+// the lens before the projection backward; f3d may be NULL.
 // The batched frame's fused_project_bwd_one repeats this arithmetic: a change to it must be made to both.
-template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false, bool G3 = false>
+template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false, bool G3 = false, bool L = false>
 __device__ __forceinline__ void fused_project_bwd_body(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
@@ -426,9 +463,11 @@ __device__ __forceinline__ void fused_project_bwd_body(
     const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
     const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
     float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
-    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr) {
+    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr,
+    GsLens lens = GsLens{}) {
   static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
   static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
+  static_assert(!L || (G3 && W == 0), "the lens runs in the 3-D filter's kernels, without a push");
   static_assert(!CG || (W == 0 && GW == GS_GREC), "camera gradient: RGB gradient rows, no push");
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   int i = blockIdx.x * kBlock + threadIdx.x;
@@ -455,7 +494,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     float f3 = 0.f, s0[3];
     if constexpr (G3) {
       float dl2o3;
-      f3 = f3d[i];
+      f3 = (L && !f3d) ? 0.f : f3d[i];
       gs_filter3d(f3, s, s0, dl2o3);
     }
     const float opa_raw = opa[i];
@@ -515,7 +554,9 @@ __device__ __forceinline__ void fused_project_bwd_body(
         }
       }
     }
-    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
+    float J[4];                                                // L: the lens Jacobian
+    if constexpr (L) gs_lens_project(lens, o, half_w, half_h, J);
     float fk[4];                                               // F: d l2o / d cov of the compensation
     if constexpr (F) {
       const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
@@ -541,6 +582,7 @@ __device__ __forceinline__ void fused_project_bwd_body(
     }
     static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
     float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
+    if constexpr (L) gs_lens_backward(J, gxyd, gcov);
     float gq[4], gsv[3];
     if constexpr (CG) {
       float gc[3], gjw[6];
@@ -709,6 +751,16 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt3_kernel(GS_P
   fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d);
 }
 
+// and for a forward with a lens (fused_project_lens_kernel<K>): K = 0 with the parameter width D (RGB or per-pixel SH
+// rows of width GW), K = 9 / 16 per-Gaussian SH; no push
+template <int D, int GW, int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_lens_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
+                                                                        const float* __restrict__ f3d, GsLens lens) {
+  // per-pixel SH takes a principal point only (the host refuses a distortion): the lens map folds to the identity
+  if (K == 0 && D != 3) lens.model = GS_LENS_PINHOLE;
+  fused_project_bwd_body<D, GW, 0, DT, K, false, true, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d, lens);
+}
+
 // Batched frames.  One view's share of Gaussian i's parameter gradients, the arithmetic of fused_project_bwd_body for
 // RGB gradient rows without a push or a camera gradient (rows o0 .. o1 - 1 of grad_inst, the loaded parameters p, q,
 // s, raw_s, qn, opa_raw, rgb_raw / coef): acc receives the row sums, then gp, gq_raw, gs_raw, go and the colour
@@ -718,13 +770,15 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt3_kernel(GS_P
 // gradients are the same bits either way).
 // G3: s is the 3-D filtered scale and f3 the filter; the activated scale is formed again from raw_s (as
 // gs_load_activated forms it) for gs_filter3d_backward, rather than kept live across the caller's view loop.
-template <int D, bool DT, int KG, bool F, bool CG = false, bool G3 = false>
+// L: the view's lens `lens`, as in fused_project_bwd_body.
+template <int D, bool DT, int KG, bool F, bool CG = false, bool G3 = false, bool L = false>
 __device__ __forceinline__ void fused_project_bwd_one(
     GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
     const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
     const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, float opa_raw,
     const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GS_GREC], float (&gsh)[KG ? D : 1],
-    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr, float f3 = 0.f) {
+    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr, float f3 = 0.f,
+    const GsLens& lens = GsLens{}) {
   constexpr int GW = GS_GREC;
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
   {
@@ -779,7 +833,9 @@ __device__ __forceinline__ void fused_project_bwd_one(
         }
       }
     }
-    GsProj o = gs_project(cam, p, q, s, near_plane, half_w, half_h);
+    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
+    float J[4];                                                // L: the lens Jacobian
+    if constexpr (L) gs_lens_project(lens, o, half_w, half_h, J);
     float fk[4];                                               // F: d l2o / d cov of the compensation
     if constexpr (F) {
       const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
@@ -805,6 +861,7 @@ __device__ __forceinline__ void fused_project_bwd_one(
     }
     static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
     float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
+    if constexpr (L) gs_lens_backward(J, gxyd, gcov);
     float gq[4], gsv[3];
     if constexpr (CG) {
       float gc[3], gjw[6];
@@ -938,8 +995,9 @@ __device__ __forceinline__ void fused_project_bwd_store(int i, int n, bool valid
 #define GS_PBWD_BATCH_ARGS                                                                                          \
   pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, epoch, \
       g_pos, g_rgb, g_opa, g_quat, g_scale
-template <int K, bool DT, bool F, bool G3>
-__device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAMS, const float* __restrict__ f3d) {
+template <int K, bool DT, bool F, bool G3, bool L = false>
+__device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAMS, const float* __restrict__ f3d,
+                                                             const GsLens* __restrict__ lenses = nullptr) {
   constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const bool valid = i < n;
@@ -955,7 +1013,7 @@ __device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAM
     float f3 = 0.f;
     if constexpr (G3) {
       float s0[3], dl2o3;
-      f3 = f3d[i];
+      f3 = (L && !f3d) ? 0.f : f3d[i];
       gs_filter3d(f3, s, s0, dl2o3);
     }
     const float opa_raw = opa[i];
@@ -977,9 +1035,17 @@ __device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAM
       float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
 #pragma unroll
       for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      fused_project_bwd_one<D, DT, K, F, false, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
-                                                    o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
-                                                    rgb_raw, coef, acc, gsh, vp, vq, vs, vo, nullptr, f3);
+      if constexpr (L) {
+        const GsLens ln = lenses[v];
+        fused_project_bwd_one<D, DT, K, F, false, G3, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt,
+                                                            scale_act, o0, o0 + cnt, grad_inst, row_epoch, epoch, p, q,
+                                                            s, raw_s, qn, opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs,
+                                                            vo, nullptr, f3, ln);
+      } else {
+        fused_project_bwd_one<D, DT, K, F, false, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                                      o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn,
+                                                      opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs, vo, nullptr, f3);
+      }
       const float* vc = K ? gsh : acc + 6;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
@@ -1005,6 +1071,13 @@ template <int K, bool DT>
 __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_filt3_kernel(GS_PBWD_BATCH_PARAMS,
                                                                                const float* __restrict__ f3d) {
   fused_project_bwd_batch_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, f3d);
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_lens_kernel(GS_PBWD_BATCH_PARAMS,
+                                                                              const float* __restrict__ f3d,
+                                                                              const GsLens* __restrict__ lenses) {
+  fused_project_bwd_batch_body<K, DT, true, true, true>(GS_PBWD_BATCH_ARGS, f3d, lenses);
 }
 
 // Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
@@ -1035,13 +1108,14 @@ __device__ __forceinline__ void cam_grad_cta_sum(float (&cg)[kCamGrad], float (&
   }
 }
 
-template <int K, bool DT, bool F, bool G3 = false>
+template <int K, bool DT, bool F, bool G3 = false, bool L = false>
 __device__ __forceinline__ void fused_project_bwd_cam_body(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                           GsFilter2d filt, const float* __restrict__ f3d = nullptr) {
+                                                           GsFilter2d filt, const float* __restrict__ f3d = nullptr,
+                                                           GsLens lens = GsLens{}) {
   float cg[kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
-  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F, G3>(GS_PBWD_ARGS, cg, filt, f3d);
+  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F, G3, L>(GS_PBWD_ARGS, cg, filt, f3d, lens);
   __shared__ float wsum[kBlock / 32][kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) {
@@ -1079,15 +1153,23 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt3_kernel(GS_
   fused_project_bwd_cam_body<K, DT, true, true>(GS_PBWD_ARGS, cam_part, filt, f3d);
 }
 
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_lens_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
+                                                                            GsFilter2d filt,
+                                                                            const float* __restrict__ f3d, GsLens lens) {
+  fused_project_bwd_cam_body<K, DT, true, true, true>(GS_PBWD_ARGS, cam_part, filt, f3d, lens);
+}
+
 // Camera gradients of a batched frame (gs_render_backward_batch_cam): fused_project_bwd_batch_kernel's parameter
 // gradients, the same bits, plus the camera terms of each view with that view's camera, filter and SH direction.  Per
 // view v the CTA sums its threads' terms in fused_project_bwd_cam_body's order into row blockIdx.x of
 // cam_part[v][gridDim.x][12].  The view loop and the sums are uniform across the CTA: threads past n and Gaussians
 // without a row in view v take part with zeros, and a CTA without a row in view v stores a zero row (the bits the
 // shuffles would give) without reducing.  With the five gradient pointers NULL only cam_part is written.
-template <int K, bool DT, bool F, bool G3>
+template <int K, bool DT, bool F, bool G3, bool L = false>
 __device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_PARAMS, float* __restrict__ cam_part,
-                                                                 const float* __restrict__ f3d) {
+                                                                 const float* __restrict__ f3d,
+                                                                 const GsLens* __restrict__ lenses = nullptr) {
   constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const bool valid = i < n;
@@ -1108,7 +1190,7 @@ __device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_P
     gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
     if constexpr (G3) {
       float s0[3], dl2o3;
-      f3 = f3d[i];
+      f3 = (L && !f3d) ? 0.f : f3d[i];
       gs_filter3d(f3, s, s0, dl2o3);
     }
     opa_raw = opa[i];
@@ -1134,9 +1216,16 @@ __device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_P
       float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
 #pragma unroll
       for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      fused_project_bwd_one<D, DT, K, F, true, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
-                                                   o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
-                                                   rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3);
+      if constexpr (L) {
+        const GsLens ln = lenses[v];
+        fused_project_bwd_one<D, DT, K, F, true, G3, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act,
+                                                           o0, o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn,
+                                                           opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3, ln);
+      } else {
+        fused_project_bwd_one<D, DT, K, F, true, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                                     o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
+                                                     rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3);
+      }
       const float* vc = K ? gsh : acc + 6;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
@@ -1173,6 +1262,14 @@ __global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_filt3_kern
                                                                                    float* __restrict__ cam_part,
                                                                                    const float* __restrict__ f3d) {
   fused_project_bwd_batch_cam_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, cam_part, f3d);
+}
+
+template <int K, bool DT>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_lens_kernel(GS_PBWD_BATCH_PARAMS,
+                                                                                  float* __restrict__ cam_part,
+                                                                                  const float* __restrict__ f3d,
+                                                                                  const GsLens* __restrict__ lenses) {
+  fused_project_bwd_batch_cam_body<K, DT, true, true, true>(GS_PBWD_BATCH_ARGS, cam_part, f3d, lenses);
 }
 #undef GS_PBWD_BATCH_PARAMS
 #undef GS_PBWD_PARAMS
@@ -1367,8 +1464,21 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
                                     GsRec* rec, uint2* rect, uint32_t* count, uint32_t* dkey, int64_t* mask,
                                     unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt,
-                                    const float* f3d) {
+                                    const float* f3d, const GsLens* lens) {
   if (n == 0) return cudaSuccess;
+  if (lens) {
+    const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
+#define GS_LAUNCH_PLENS(K)                                                                                      \
+  fused_project_lens_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
+                                                               grid, near_plane, half_w, half_h, rec, rect, count, \
+                                                               dkey, mask, n_visible, f2, f3d, *lens)
+    if (sh_gaussian && d == 27) GS_LAUNCH_PLENS(9);
+    else if (sh_gaussian && d == 48) GS_LAUNCH_PLENS(16);
+    else if (sh_gaussian) return cudaErrorInvalidValue;
+    else GS_LAUNCH_PLENS(0);
+#undef GS_LAUNCH_PLENS
+    return cudaGetLastError();
+  }
   if (f3d) {
     const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
 #define GS_LAUNCH_PFILT3(K)                                                                                      \
@@ -1416,9 +1526,26 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                         float* g_pos, float* g_rgb, float* g_opa,
                                         float* g_quat, float* g_scale, const GsGradPush& push, cudaStream_t st,
-                                        bool depth_grad, bool sh_gaussian, const GsFilter2d* filt, const float* f3d) {
+                                        bool depth_grad, bool sh_gaussian, const GsFilter2d* filt, const float* f3d,
+                                        const GsLens* lens) {
   if (n == 0) return cudaSuccess;
   const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
+  if (lens) {
+    if (push.world) return cudaErrorInvalidValue;
+#define GS_LAUNCH_PBWD_LENS(D, GW, K)                                                                              \
+  if (depth_grad)                                                                                                  \
+    fused_project_bwd_lens_kernel<D, GW, K, true><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d, *lens);  \
+  else                                                                                                             \
+    fused_project_bwd_lens_kernel<D, GW, K, false><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d, *lens)
+    if (sh_gaussian && d == 27) { GS_LAUNCH_PBWD_LENS(27, GS_GREC, 9); }
+    else if (sh_gaussian && d == 48) { GS_LAUNCH_PBWD_LENS(48, GS_GREC, 16); }
+    else if (sh_gaussian) return cudaErrorInvalidValue;
+    else if (d == 3) { GS_LAUNCH_PBWD_LENS(3, GS_GREC, 0); }
+    else if (d == 27) { GS_LAUNCH_PBWD_LENS(27, 36, 0); }
+    else { GS_LAUNCH_PBWD_LENS(48, 56, 0); }
+#undef GS_LAUNCH_PBWD_LENS
+    return cudaGetLastError();
+  }
 #define GS_LAUNCH_PBWD(D, GW, W, DT)                                                               \
   if (f3d)                                                                                         \
     fused_project_bwd_filt3_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d); \
@@ -1476,13 +1603,16 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                             float* g_scale, float* cam_part, float* grad_cam, cudaStream_t st,
                                             bool depth_grad, bool sh_gaussian, const GsFilter2d* filt,
-                                            const float* f3d) {
+                                            const float* f3d, const GsLens* lens) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
   const GsGradPush push{};
   const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
   if (n > 0) {
 #define GS_LAUNCH_PBWD_CAM(K, DT)                                                                             \
-  if (f3d)                                                                                                    \
+  if (lens)                                                                                                   \
+    fused_project_bwd_cam_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, f2, f3d, \
+                                                                             *lens);                          \
+  else if (f3d)                                                                                                    \
     fused_project_bwd_cam_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, f2, f3d); \
   else if (filt)                                                                                              \
     fused_project_bwd_cam_filt_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, *filt); \
@@ -1505,9 +1635,21 @@ cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, co
                                           const float* scale, int n, int n_views, int d, int scale_act,
                                           const GsView* views, float near_plane, GsRec* rec, uint2* rect,
                                           uint32_t* count, uint32_t* dkey, int64_t* mask, unsigned int* n_visible,
-                                          cudaStream_t st, bool sh_gaussian, bool filt, const float* f3d) {
+                                          cudaStream_t st, bool sh_gaussian, bool filt, const float* f3d,
+                                          const GsLens* lenses) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+#define GS_LAUNCH_PBATCHL(K)                                                                                     \
+  fused_project_batch_lens_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,  \
+                                                                     scale_act, views, near_plane, rec, rect,     \
+                                                                     count, dkey, mask, n_visible, f3d, lenses)
+  if (lenses) {
+    if (d == 27) GS_LAUNCH_PBATCHL(9);
+    else if (d == 48) GS_LAUNCH_PBATCHL(16);
+    else GS_LAUNCH_PBATCHL(0);
+#undef GS_LAUNCH_PBATCHL
+    return cudaGetLastError();
+  }
 #define GS_LAUNCH_PBATCH(K, F)                                                                                    \
   fused_project_batch_kernel<K, F><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,     \
                                                                    scale_act, views, near_plane, rec, rect, count, \
@@ -1539,9 +1681,23 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
                                               const uint32_t* count, const float* grad_inst, const uint32_t* row_epoch,
                                               uint32_t epoch, float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                               float* g_scale, cudaStream_t st, bool depth_grad, bool sh_gaussian,
-                                              bool filt, const float* f3d) {
+                                              bool filt, const float* f3d, const GsLens* lenses) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
+  if (lenses) {
+#define GS_LAUNCH_PBWD_BATCHL(K, DT)                                                                                \
+  fused_project_bwd_batch_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                       \
+      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
+      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d, lenses)
+    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_BATCHL(9, true);
+    else if (d == 27) GS_LAUNCH_PBWD_BATCHL(9, false);
+    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_BATCHL(16, true);
+    else if (d == 48) GS_LAUNCH_PBWD_BATCHL(16, false);
+    else if (depth_grad) GS_LAUNCH_PBWD_BATCHL(0, true);
+    else GS_LAUNCH_PBWD_BATCHL(0, false);
+#undef GS_LAUNCH_PBWD_BATCHL
+    return cudaGetLastError();
+  }
 #define GS_LAUNCH_PBWD_BATCH(K, DT, F)                                                                              \
   fused_project_bwd_batch_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                         \
       pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
@@ -1571,9 +1727,22 @@ cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float*
                                                   const float* grad_inst, const uint32_t* row_epoch, uint32_t epoch,
                                                   float* g_pos, float* g_rgb, float* g_opa, float* g_quat,
                                                   float* g_scale, float* cam_part, float* grad_cams, cudaStream_t st,
-                                                  bool depth_grad, bool sh_gaussian, bool filt, const float* f3d) {
+                                                  bool depth_grad, bool sh_gaussian, bool filt, const float* f3d,
+                                                  const GsLens* lenses) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
-  if (n > 0) {
+  if (n > 0 && lenses) {
+#define GS_LAUNCH_PBWD_BATCH_CAML(K, DT)                                                                            \
+  fused_project_bwd_batch_cam_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                   \
+      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
+      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part, f3d, lenses)
+    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(9, true);
+    else if (d == 27) GS_LAUNCH_PBWD_BATCH_CAML(9, false);
+    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(16, true);
+    else if (d == 48) GS_LAUNCH_PBWD_BATCH_CAML(16, false);
+    else if (depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(0, true);
+    else GS_LAUNCH_PBWD_BATCH_CAML(0, false);
+#undef GS_LAUNCH_PBWD_BATCH_CAML
+  } else if (n > 0) {
 #define GS_LAUNCH_PBWD_BATCH_CAM(K, DT, F)                                                                          \
   fused_project_bwd_batch_cam_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                     \
       pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \

@@ -290,6 +290,101 @@ __device__ __forceinline__ void gs_filter3d_backward(float f, const float s0[3],
   }
 }
 
+// Lens of the fused frame path (gs_ctx_set_lens): a 2-D map D of the undistorted image-plane position (a, b) =
+// (x/z, y/z), COLMAP's OPENCV or OPENCV_FISHEYE model, applied after the pinhole.  The stored mean is D(a, b) + (ox, oy),
+// (ox, oy) = ((cx - W/2) / fx, (cy - H/2) / fy), and the 2-D covariance J_D Sigma J_D^T with J_D the map's Jacobian.
+// rho2_max: the squared undistorted radius past which the polynomial folds back (+inf: none); farther Gaussians are
+// culled.  model is GS_LENS_PINHOLE (D = identity), GS_LENS_OPENCV (k = k1, k2, p1, p2) or GS_LENS_FISHEYE (k1..k4).
+struct GsLens {
+  int model;
+  float ox, oy, rho2_max;
+  float k[4];
+};
+
+// (a, b) -> (ad, bd) = D(a, b) and J = dD/d(a, b) row-major {d ad/da, d ad/db, d bd/da, d bd/db}
+__device__ __forceinline__ void gs_lens_map(const GsLens& L, float a, float b, float& ad, float& bd, float J[4]) {
+  const float r2 = a * a + b * b;
+  if (L.model == GS_LENS_OPENCV) {
+    const float k1 = L.k[0], k2 = L.k[1], p1 = L.k[2], p2 = L.k[3];
+    const float rad = 1.f + r2 * (k1 + k2 * r2);
+    const float drad = 2.f * k1 + 4.f * k2 * r2;   // d rad / d a = drad a
+    ad = a * rad + 2.f * p1 * a * b + p2 * (r2 + 2.f * a * a);
+    bd = b * rad + p1 * (r2 + 2.f * b * b) + 2.f * p2 * a * b;
+    J[0] = rad + drad * a * a + 2.f * p1 * b + 6.f * p2 * a;
+    J[1] = drad * a * b + 2.f * p1 * a + 2.f * p2 * b;
+    J[2] = J[1];
+    J[3] = rad + drad * b * b + 6.f * p1 * b + 2.f * p2 * a;
+  } else if (L.model == GS_LENS_FISHEYE) {
+    // (ad, bd) = f (a, b), f = theta_d / rho, theta = atan(rho); J = f I + g (a, b)^T (a, b) with g = f'(rho) / rho.
+    // Near the axis f and g come from their series in rho^2 (the closed forms are 0 / 0 there).
+    const float k1 = L.k[0], k2 = L.k[1], k3 = L.k[2], k4 = L.k[3];
+    float f, g;
+    if (r2 < 1e-4f) {
+      f = 1.f + (k1 - 1.f / 3.f) * r2 + (0.2f - k1 + k2) * r2 * r2;
+      g = 2.f * (k1 - 1.f / 3.f) + 4.f * (0.2f - k1 + k2) * r2;
+    } else {
+      const float rho = sqrtf(r2);
+      const float th = atanf(rho), t2 = th * th;
+      const float poly = 1.f + t2 * (k1 + t2 * (k2 + t2 * (k3 + t2 * k4)));
+      const float dpoly = 1.f + t2 * (3.f * k1 + t2 * (5.f * k2 + t2 * (7.f * k3 + t2 * 9.f * k4)));   // d theta_d / d theta
+      const float thd = th * poly;
+      f = thd / rho;
+      g = (dpoly * rho / (1.f + r2) - thd) / (r2 * rho);
+    }
+    ad = f * a;
+    bd = f * b;
+    J[0] = f + g * a * a;
+    J[1] = g * a * b;
+    J[2] = J[1];
+    J[3] = f + g * b * b;
+  } else {
+    ad = a;
+    bd = b;
+    J[0] = 1.f;
+    J[1] = 0.f;
+    J[2] = 0.f;
+    J[3] = 1.f;
+  }
+}
+
+// The lens on a projection of gs_project taken without its frustum test (half_w = half_h = +inf): o.visible on entry is
+// z > near.  It becomes z > near, rho^2 < rho2_max and the stored mean inside the 1.2x frustum (half_w, half_h); a
+// visible o gets the stored mean and J_D Sigma J_D^T, and J the Jacobian (the backward's detached J_D).
+__device__ __forceinline__ void gs_lens_project(const GsLens& L, GsProj& o, float half_w, float half_h, float J[4]) {
+  if (!o.visible) return;
+  const float r2 = o.x * o.x + o.y * o.y;
+  float ad, bd;
+  gs_lens_map(L, o.x, o.y, ad, bd, J);
+  o.x = ad + L.ox;
+  o.y = bd + L.oy;
+  if (!(r2 < L.rho2_max) || fabsf(o.x) >= half_w || fabsf(o.y) >= half_h) {
+    o.visible = false;
+    return;
+  }
+  // Sigma' = J Sigma J^T, Sigma = [[a, b], [c, d]] symmetric
+  const float t00 = J[0] * o.a + J[1] * o.c, t01 = J[0] * o.b + J[1] * o.d;
+  const float t10 = J[2] * o.a + J[3] * o.c, t11 = J[2] * o.b + J[3] * o.d;
+  o.a = t00 * J[0] + t01 * J[1];
+  o.b = t00 * J[2] + t01 * J[3];
+  o.c = o.b;
+  o.d = t10 * J[2] + t11 * J[3];
+}
+
+// Backward of gs_lens_project with J_D detached in the covariance: g_xyd[0..1] = dL/d(stored mean) becomes
+// J_D^T dL/dmean = dL/d(x/z, y/z), and g_cov = dL/dSigma' becomes J_D^T (dL/dSigma') J_D = dL/dSigma.
+__device__ __forceinline__ void gs_lens_backward(const float J[4], float g_xyd[3], float g_cov[4]) {
+  const float gx = g_xyd[0], gy = g_xyd[1];
+  g_xyd[0] = J[0] * gx + J[2] * gy;
+  g_xyd[1] = J[1] * gx + J[3] * gy;
+  // G = J^T G' J, G' = [[g0, g1], [g2, g3]]
+  const float u00 = g_cov[0] * J[0] + g_cov[1] * J[2], u01 = g_cov[0] * J[1] + g_cov[1] * J[3];
+  const float u10 = g_cov[2] * J[0] + g_cov[3] * J[2], u11 = g_cov[2] * J[1] + g_cov[3] * J[3];
+  g_cov[0] = J[0] * u00 + J[2] * u10;
+  g_cov[1] = J[0] * u01 + J[2] * u11;
+  g_cov[2] = J[1] * u00 + J[3] * u10;
+  g_cov[3] = J[1] * u01 + J[3] * u11;
+}
+
 // Tile rectangle covered by a Gaussian, method 2 "prob2" (gaussian.cu:226-242): axis aligned
 // bbox of the `thresh` iso-probability ellipse; float->uint32 casts truncate / saturate.
 struct GsTileGrid {

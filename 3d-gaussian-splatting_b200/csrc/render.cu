@@ -141,8 +141,10 @@ struct gs_ctx {
   DevBuf tile_accum, tile_neff, tile_neff_b, cub_tmp, counters, img_dev, gimg_dev, rays;
   DevBuf cam_part;                        // per-CTA partial sums of the camera gradient (gs_render_backward_cam)
   DevBuf views;                           // GsView[n_views] of the last batched forward (gs_render_forward_batch)
+  DevBuf lenses;                          // GsLens[n_views] of the last batched forward with a lens
   float* host_rays = nullptr;             // pinned: rays_o, lefttop, dx, dy (SH colour only)
   GsView* host_views = nullptr;           // pinned: staging of the view table (GS_MAX_VIEWS entries)
+  GsLens* host_lenses = nullptr;          // pinned: staging of the lens table (GS_MAX_VIEWS entries, with the views)
   unsigned long long* host_m = nullptr;   // pinned: {M}
   cudaEvent_t ev_m = nullptr;             // marks the completion of the M read-back
   cudaEvent_t ev_views = nullptr;         // marks the completion of the view table's upload from host_views
@@ -182,6 +184,10 @@ struct gs_ctx {
   GsF3View* f3_host = nullptr;
   int f3_host_cap = 0;
   cudaEvent_t ev_f3 = nullptr;            // marks the completion of the view table's upload from f3_host
+  gs_lens lens_set[GS_MAX_VIEWS] = {};    // gs_ctx_set_lens: applies to the forwards that follow
+  int lens_n = 0;                         //   0: off
+  bool lens_on = false;                   // the last forward ran the lens kernels (its backward uses them)
+  GsLens lens{};                          //   with the lens of its (first) view
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -199,6 +205,7 @@ extern "C" int gs_ctx_create(gs_ctx** out) {
   cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&c->host_m), 64);
   if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->host_rays), 64);
   if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->host_views), GS_MAX_VIEWS * sizeof(GsView));
+  if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->host_lenses), GS_MAX_VIEWS * sizeof(GsLens));
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_m, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_views, cudaEventDisableTiming);
   if (e != cudaSuccess) {
@@ -218,11 +225,12 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
-                    &c->grad_feat_inst, &c->views, &c->f3_dev};
+                    &c->grad_feat_inst, &c->views, &c->f3_dev, &c->lenses};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
   if (c->host_views) cudaFreeHost(c->host_views);
+  if (c->host_lenses) cudaFreeHost(c->host_lenses);
   if (c->ev_m) cudaEventDestroy(c->ev_m);
   if (c->ev_views) cudaEventDestroy(c->ev_views);
   if (c->f3_host) cudaFreeHost(c->f3_host);
@@ -317,7 +325,10 @@ static int begin_forward(gs_ctx* c, const char* who) {
 // what the backward of a completed forward needs; v: the constants of its (first) view
 static void commit_forward(gs_ctx* c, int n, int d, int scale_activation, long long m, const GsFrameGeom& g,
                            const GsView& v, float near_plane, int n_views, bool sh_gaussian, bool gather, bool filt_on,
-                           const GsAuxOut& aux_out, const gs_render_feat* ft, const float* f3d) {
+                           const GsAuxOut& aux_out, const gs_render_feat* ft, const float* f3d, bool lens_on,
+                           const GsLens& lens) {
+  c->lens_on = lens_on;
+  c->lens = lens;
   c->ev_fwd_valid = c->timing && c->ev_ok;
   c->have_forward = true;
   c->have_aux = aux_out.aux != nullptr;
@@ -339,6 +350,91 @@ static void commit_forward(gs_ctx* c, int n, int d, int scale_activation, long l
   c->half_w = v.half_w;
   c->half_h = v.half_h;
   c->n_views = n_views;
+}
+
+// The smallest t in (0, hi] with sum_j c[j] t^j <= 0 (c[0] = 1 > 0), or +inf: a scan to the first sample at or below
+// zero, then bisection of that interval (fp64).
+static double first_nonpositive(const double* c, int deg, double hi) {
+  auto p = [&](double t) {
+    double v = 0.0;
+    for (int j = deg; j >= 0; --j) v = v * t + c[j];
+    return v;
+  };
+  const int steps = 1 << 14;
+  double a = 0.0;
+  for (int s = 1; s <= steps; ++s) {
+    double b = hi * s / steps;
+    if (p(b) > 0.0) {
+      a = b;
+      continue;
+    }
+    for (int it = 0; it < 200; ++it) {
+      const double m = 0.5 * (a + b);
+      if (!(m > a && m < b)) break;
+      (p(m) <= 0.0 ? b : a) = m;
+    }
+    return b;
+  }
+  return INFINITY;
+}
+
+// The squared undistorted radius past which a lens folds back (GS_LENS_* in gs_b200.h), +inf without a limit.
+//   OPENCV: the smallest rho^2 > 0 with 1 + 3 k1 rho^2 + 5 k2 rho^4 <= 0 (d(rho rad)/d rho, the radial part only).
+//   FISHEYE: tan^2 of the smallest theta in (0, pi/2) with d theta_d / d theta <= 0.
+static double lens_rho2_max(const gs_lens& l) {
+  if (l.model == GS_LENS_OPENCV) {
+    const double b = 3.0 * l.k[0], a = 5.0 * l.k[1];   // the quadratic a u^2 + b u + 1 in u = rho^2
+    if (a == 0.0) return b < 0.0 ? -1.0 / b : INFINITY;
+    const double disc = b * b - 4.0 * a;
+    if (disc < 0.0) return INFINITY;
+    const double q = -0.5 * (b + (b >= 0.0 ? 1.0 : -1.0) * sqrt(disc));   // roots q / a and 1 / q
+    double best = INFINITY;
+    const double r0 = q / a, r1 = q != 0.0 ? 1.0 / q : INFINITY;
+    if (r0 > 0.0) best = r0;
+    if (r1 > 0.0 && r1 < best) best = r1;
+    return best;
+  }
+  if (l.model == GS_LENS_FISHEYE) {
+    const double c[5] = {1.0, 3.0 * l.k[0], 5.0 * l.k[1], 7.0 * l.k[2], 9.0 * l.k[3]};   // in t = theta^2
+    const double half_pi = 1.5707963267948966;
+    const double t = first_nonpositive(c, 4, half_pi * half_pi);
+    if (!(t < half_pi * half_pi)) return INFINITY;
+    const double r = tan(sqrt(t));
+    return r * r;
+  }
+  return INFINITY;
+}
+
+static bool lens_is_centre_pinhole(const gs_lens& l, const gs_camera& cam) {
+  return l.model == GS_LENS_PINHOLE && (double)l.cx == cam.width / 2.0 && (double)l.cy == cam.height / 2.0;
+}
+
+// The device constants of lens l on camera cam: (ox, oy) = ((cx - W/2) / fx, (cy - H/2) / fy) and rho2_max, in fp64
+// then narrowed.
+static GsLens lens_constants(const gs_lens& l, const gs_camera& cam) {
+  GsLens L{};
+  L.model = l.model;
+  L.ox = (float)(((double)l.cx - cam.width / 2.0) / (double)cam.focal_x);
+  L.oy = (float)(((double)l.cy - cam.height / 2.0) / (double)cam.focal_y);
+  L.rho2_max = (float)lens_rho2_max(l);
+  if (l.model != GS_LENS_PINHOLE)
+    for (int k = 0; k < 4; ++k) L.k[k] = l.k[k];
+  return L;
+}
+
+// The lenses of a forward of n_views views: out[v] for view v, and on = false when none is set or every view's is the
+// image-centre pinhole (the frame then runs the kernels of a frame without a lens).
+static int resolve_lenses(const gs_ctx* c, const gs_camera* cams, int n_views, GsLens* out, bool& on, const char* who) {
+  on = false;
+  if (c->lens_n == 0) return 0;
+  if (c->lens_n != 1 && c->lens_n != n_views)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the context's lenses are set for another number of views (n must be 1 or B)");
+  for (int v = 0; v < n_views; ++v) {
+    const gs_lens& l = c->lens_set[c->lens_n == 1 ? 0 : v];
+    if (!lens_is_centre_pinhole(l, cams[v])) on = true;
+    out[v] = lens_constants(l, cams[v]);
+  }
+  return 0;
 }
 
 // The per-camera constants of a frame of padded size g.wp x g.hp, formed from host scalars in double then narrowed, like
@@ -535,6 +631,12 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
   }
   const float* f3d = c->filter3d;
   if (f3d && c->filter3d_n != n) return gs_fail(GS_ERR_INVALID_ARG, who, "the 3-D filter is sized for another n");
+  GsLens lens{};
+  bool lens_on;
+  if (int rc = resolve_lenses(c, cam, 1, &lens, lens_on, who)) return rc;
+  if (lens_on && blend_d != 3 && lens.model != GS_LENS_PINHOLE)
+    return gs_fail(GS_ERR_UNSUPPORTED, who,
+                   "SH colour evaluated per pixel takes a principal point but no distortion (use GS_SH_EVAL_GAUSSIAN)");
   if (int rc = begin_forward(c, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   GsFrameGeom g;
@@ -551,7 +653,8 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
 
   if (blend_d != 3) {
     // world-space ray set-up for per-pixel SH, reference splatter.py:305-321 (RayInfo):
-    // c2w = inverse(w2c); rays_o = -c2w t; lefttop = c2w (((-Wp/2+.5)/fx, (-Hp/2+.5)/fy, 1) - t)
+    // c2w = inverse(w2c); rays_o = -c2w t; lefttop = c2w (((-Wp/2+.5)/fx, (-Hp/2+.5)/fy, 1) - t), with a lens's
+    // principal point shifting the first two components by -((cx - W/2) / fx, (cy - H/2) / fy)
     GS_CUDA_TRY(c->rays.reserve(64, st));
     double m3[9], inv[9];
     for (int k = 0; k < 9; ++k) m3[k] = cam->rot[k];
@@ -568,6 +671,11 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
     inv[8] = (m3[0] * m3[4] - m3[1] * m3[3]) / det3;
     double lt[3] = {(-(double)g.wp / 2 + 0.5) / cam->focal_x - cam->tran[0],
                     (-(double)g.hp / 2 + 0.5) / cam->focal_y - cam->tran[1], 1.0 - cam->tran[2]};
+    if (lens_on) {
+      const gs_lens& l = c->lens_set[0];
+      lt[0] -= ((double)l.cx - cam->width / 2.0) / cam->focal_x;
+      lt[1] -= ((double)l.cy - cam->height / 2.0) / cam->focal_y;
+    }
     for (int k = 0; k < 3; ++k) {
       c->host_rays[k] = (float)(-(inv[3 * k] * cam->tran[0] + inv[3 * k + 1] * cam->tran[1] + inv[3 * k + 2] * cam->tran[2]));
       c->host_rays[3 + k] = (float)(inv[3 * k] * lt[0] + inv[3 * k + 1] * lt[1] + inv[3 * k + 2] * lt[2]);
@@ -583,7 +691,7 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
   GS_CUDA_TRY(gs_launch_fused_project(pos, rgb, opa, quat, scale, n, d, scale_activation, dc, grid, cam->near_plane,
                                       half_w, half_h, c->rec.as<GsRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
                                       c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st,
-                                      sh_gaussian, filt_on ? &filt : nullptr, f3d));
+                                      sh_gaussian, filt_on ? &filt : nullptr, f3d, lens_on ? &lens : nullptr));
   if (n > 0) gs_count_launch();
   long long m = 0;
   if (int rc = bin_frame(c, n, g, gather, blend_d, d, rgb, st, m)) return rc;
@@ -611,7 +719,7 @@ static int render_forward_impl(gs_ctx* c, const char* who, const float* pos, con
   gs_count_launch();   // blend forward
   gs_mark(c, 6, st);
   commit_forward(c, n, d, scale_activation, m, g, vw, cam->near_plane, 0, sh_gaussian, gather, filt_on, aux_out, ft,
-                 f3d);
+                 f3d, lens_on, lens);
   return 0;
 }
 
@@ -682,6 +790,8 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
     if (absgrad)
       if (int rc = gs_blend_absgrad_supported(blend_d, c->gather)) return rc;
   }
+  if (c->push.world && c->lens_on)
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "a frame with a lens has no gradient push (all-reduce the gradients instead)");
   if (c->push.world) {
     // every gradient segment must lie inside the sliced bucket, quaternions on 16-byte offsets
     const float* lo = c->push.bucket;
@@ -750,7 +860,8 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                       c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                                       grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale,
                                                       c->cam_part.as<float>(), grad_cam, st, grad_aux != nullptr,
-                                                      c->sh_gaussian, c->filt_on, c->f3d));
+                                                      c->sh_gaussian, c->filt_on, c->f3d,
+                                                      c->lens_on ? c->lenses.as<GsLens>() : nullptr));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sums
   } else if (grad_cam) {
     GS_CUDA_TRY(c->cam_part.reserve(gs_cam_grad_workspace_bytes(c->n) + 16, st));
@@ -760,7 +871,7 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                 c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
                                                 grad_quat, grad_scale, c->cam_part.as<float>(), grad_cam, st,
                                                 grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr,
-                                                c->f3d));
+                                                c->f3d, c->lens_on ? &c->lens : nullptr));
     gs_count_launch(c->n > 0 ? 2 : 1);   // projection backward + the finishing sum (always: grad_cam is always written)
   } else if (c->n_views > 1) {
     // B views: the batched kernels, which take each Gaussian's views in order.  One view: the pairs are the Gaussians,
@@ -770,7 +881,7 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                                   c->count.as<uint32_t>(), c->grad_inst.as<float>(),
                                                   c->row_epoch.as<uint32_t>(), c->epoch, grad_pos, grad_rgb, grad_opa,
                                                   grad_quat, grad_scale, st, grad_aux != nullptr, c->sh_gaussian,
-                                                  c->filt_on, c->f3d));
+                                                  c->filt_on, c->f3d, c->lens_on ? c->lenses.as<GsLens>() : nullptr));
     if (c->n > 0) gs_count_launch();
   } else {
     GS_CUDA_TRY(gs_launch_fused_project_bwd(pos, rgb, opa, quat, scale, c->n, d, c->scale_act, c->cam, c->near_plane,
@@ -778,7 +889,7 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
                                             c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch,
                                             grad_pos, grad_rgb, grad_opa, grad_quat, grad_scale, c->push, st,
                                             grad_aux != nullptr, c->sh_gaussian, c->filt_on ? &c->filt : nullptr,
-                                            c->f3d));
+                                            c->f3d, c->lens_on ? &c->lens : nullptr));
     if (c->n > 0) gs_count_launch();
   }
   if (grad_map) {
@@ -791,12 +902,14 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
       GS_CUDA_TRY(gs_launch_densify_stats_batch(pos, quat, scale, c->n, c->n_views, c->scale_act, c->views.as<GsView>(),
                                                 c->near_plane, c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
                                                 c->grad_inst.as<float>(), (int)(grow / 4), c->row_epoch.as<uint32_t>(),
-                                                c->epoch, c->geom, c->stats, st, c->f3d));
+                                                c->epoch, c->geom, c->stats, st, c->f3d,
+                                                c->lens_on ? c->lenses.as<GsLens>() : nullptr));
     else
       GS_CUDA_TRY(gs_launch_densify_stats(pos, quat, scale, c->n, c->scale_act, c->cam, c->near_plane, c->half_w,
                                           c->half_h, c->filt_on ? c->filt : GsFilter2d{}, c->offsets_g.as<uint32_t>(),
                                           c->count.as<uint32_t>(), c->grad_inst.as<float>(), (int)(grow / 4),
-                                          c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st, c->f3d));
+                                          c->row_epoch.as<uint32_t>(), c->epoch, c->geom, c->stats, st, c->f3d,
+                                          c->lens_on ? &c->lens : nullptr));
     if (c->n > 0) gs_count_launch();
   }
   gs_mark(c, 9, st);
@@ -934,6 +1047,9 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   GsAuxOut aux_out;
   bool use_aux;
   if (int rc = parse_aux(ax, final_img, aux_out, use_aux, who)) return rc;
+  GsLens lenses[GS_MAX_VIEWS] = {};
+  bool lens_on;
+  if (int rc = resolve_lenses(c, cams, n_views, lenses, lens_on, who)) return rc;
   if (int rc = begin_forward(c, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
 
@@ -944,6 +1060,11 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   GS_CUDA_TRY(cudaEventSynchronize(c->ev_views));
   for (int v = 0; v < n_views; ++v) c->host_views[v] = view_constants(c, &cams[v], g);
   GS_CUDA_TRY(cudaMemcpyAsync(c->views.p, c->host_views, sizeof(GsView) * n_views, cudaMemcpyHostToDevice, st));
+  if (lens_on) {
+    GS_CUDA_TRY(c->lenses.reserve(sizeof(GsLens) * GS_MAX_VIEWS, st));
+    for (int v = 0; v < n_views; ++v) c->host_lenses[v] = lenses[v];
+    GS_CUDA_TRY(cudaMemcpyAsync(c->lenses.p, c->host_lenses, sizeof(GsLens) * n_views, cudaMemcpyHostToDevice, st));
+  }
   GS_CUDA_TRY(cudaEventRecord(c->ev_views, st));
   const bool filt_on = c->filter2d != GS_FILTER2D_NONE;
 
@@ -954,7 +1075,7 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
                                             c->views.as<GsView>(), c0.near_plane, c->rec.as<GsRec>(),
                                             c->rect.as<uint2>(), c->count.as<uint32_t>(), c->dkey_in.as<uint32_t>(),
                                             culling_mask, c->counters.as<unsigned int>(), st, sh_gaussian, filt_on,
-                                            f3d));
+                                            f3d, lens_on ? c->lenses.as<GsLens>() : nullptr));
   if (n > 0) gs_count_launch();
   long long m = 0;
   if (int rc = bin_frame(c, nb, g, true, 3, d, rgb, st, m)) return rc;
@@ -967,7 +1088,7 @@ extern "C" int gs_render_forward_batch(gs_ctx* c, const float* pos, const float*
   gs_mark(c, 6, st);
   // view 0's constants: a one-view batch is differentiated by the single-view projection backward
   commit_forward(c, n, d, scale_activation, m, g, c->host_views[0], c0.near_plane, n_views, sh_gaussian, true, filt_on,
-                 aux_out, nullptr, f3d);
+                 aux_out, nullptr, f3d, lens_on, lenses[0]);
   return 0;
 }
 
@@ -1058,6 +1179,25 @@ extern "C" int gs_ctx_set_filter3d(gs_ctx* c, const float* filter3d, int n) {
   return 0;
 }
 
+extern "C" int gs_ctx_set_lens(gs_ctx* c, const gs_lens* lenses, int n) {
+  const char* who = "gs_ctx_set_lens";
+  if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
+  if (n < 0 || n > GS_MAX_VIEWS) return gs_fail(GS_ERR_INVALID_ARG, who, "n must be in 0 .. GS_MAX_VIEWS");
+  if (!lenses && n > 0) return gs_fail(GS_ERR_INVALID_ARG, who, "NULL lenses with n > 0");
+  const int m = lenses ? n : 0;
+  for (int v = 0; v < m; ++v) {
+    const gs_lens& l = lenses[v];
+    if (l.model != GS_LENS_PINHOLE && l.model != GS_LENS_OPENCV && l.model != GS_LENS_FISHEYE)
+      return gs_fail(GS_ERR_INVALID_ARG, who, "model must be GS_LENS_PINHOLE, GS_LENS_OPENCV or GS_LENS_FISHEYE");
+    bool finite = std::isfinite(l.cx) && std::isfinite(l.cy);
+    for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(l.k[k]);
+    if (!finite) return gs_fail(GS_ERR_INVALID_ARG, who, "cx, cy and k must be finite");
+  }
+  for (int v = 0; v < m; ++v) c->lens_set[v] = lenses[v];
+  c->lens_n = m;
+  return 0;
+}
+
 extern "C" int gs_filter3d_compute(gs_ctx* c, const float* pos, int n, const gs_camera* cams_host, int n_cams,
                                    float margin, float variance, float* filter3d, gs_stream_t stream) {
   const char* who = "gs_filter3d_compute";
@@ -1075,6 +1215,13 @@ extern "C" int gs_filter3d_compute(gs_ctx* c, const float* pos, int n, const gs_
       return gs_fail(GS_ERR_INVALID_ARG, who, "bad camera (near_plane must be finite and >= 0)");
   }
   if (n == 0) return 0;
+  if (c->lens_n && c->lens_n != 1 && c->lens_n != n_cams)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the context's lenses are set for another number of views (n must be 1 or n_cams)");
+  // the lens variant unless no lens is set or every view's is the image-centre pinhole (then the rate, the test and
+  // the bits are those without a lens)
+  bool lens_on = false;
+  for (int v = 0; v < n_cams && c->lens_n; ++v)
+    if (!lens_is_centre_pinhole(c->lens_set[c->lens_n == 1 ? 0 : v], cams_host[v])) lens_on = true;
   if (int rc = gs_check_device(c->device, who)) return rc;
   g_cur_alloc = &c->allocator;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1085,9 +1232,12 @@ extern "C" int gs_filter3d_compute(gs_ctx* c, const float* pos, int n, const gs_
     if (c->f3_host) cudaFreeHost(c->f3_host);
     c->f3_host = nullptr;
     c->f3_host_cap = 0;
-    GS_CUDA_TRY(cudaMallocHost(reinterpret_cast<void**>(&c->f3_host), sizeof(GsF3View) * (size_t)n_cams));
+    // the view table, then the lens table (GsLens[cap])
+    GS_CUDA_TRY(cudaMallocHost(reinterpret_cast<void**>(&c->f3_host),
+                               (sizeof(GsF3View) + sizeof(GsLens)) * (size_t)n_cams));
     c->f3_host_cap = n_cams;
   }
+  GsLens* lens_host = reinterpret_cast<GsLens*>(c->f3_host + c->f3_host_cap);
   for (int v = 0; v < n_cams; ++v) {
     const gs_camera& cm = cams_host[v];
     GsF3View& o = c->f3_host[v];
@@ -1107,14 +1257,23 @@ extern "C" int gs_filter3d_compute(gs_ctx* c, const float* pos, int n, const gs_
     o.wlo = (float)(-(double)margin * cm.height);
     o.whi = (float)((1.0 + (double)margin) * cm.height);
     o.near = cm.near_plane;
+    if (lens_on) {
+      const gs_lens& l = c->lens_set[c->lens_n == 1 ? 0 : v];
+      o.cx = l.cx;
+      o.cy = l.cy;
+      lens_host[v] = lens_constants(l, cm);
+    }
   }
-  GS_CUDA_TRY(c->f3_dev.reserve(16 + sizeof(GsF3View) * (size_t)n_cams, st));
+  const size_t vbytes = sizeof(GsF3View) * (size_t)n_cams, lbytes = lens_on ? sizeof(GsLens) * (size_t)n_cams : 0;
+  GS_CUDA_TRY(c->f3_dev.reserve(16 + vbytes + lbytes, st));
   unsigned int* min_rate = c->f3_dev.as<unsigned int>();
   GsF3View* views = reinterpret_cast<GsF3View*>(c->f3_dev.as<char>() + 16);
+  GsLens* lenses = lens_on ? reinterpret_cast<GsLens*>(c->f3_dev.as<char>() + 16 + vbytes) : nullptr;
   GS_CUDA_TRY(cudaMemsetAsync(min_rate, 0xff, 4, st));
-  GS_CUDA_TRY(cudaMemcpyAsync(views, c->f3_host, sizeof(GsF3View) * (size_t)n_cams, cudaMemcpyHostToDevice, st));
+  GS_CUDA_TRY(cudaMemcpyAsync(views, c->f3_host, vbytes, cudaMemcpyHostToDevice, st));
+  if (lens_on) GS_CUDA_TRY(cudaMemcpyAsync(lenses, lens_host, lbytes, cudaMemcpyHostToDevice, st));
   GS_CUDA_TRY(cudaEventRecord(c->ev_f3, st));
-  GS_CUDA_TRY(gs_launch_filter3d(pos, n, views, n_cams, variance, filter3d, min_rate, st));
+  GS_CUDA_TRY(gs_launch_filter3d(pos, n, views, n_cams, variance, filter3d, min_rate, st, lenses));
   gs_count_launch(2);
   return 0;
 }

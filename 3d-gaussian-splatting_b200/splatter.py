@@ -221,6 +221,36 @@ class Tiles:
         return image[top:top + self.height, left:left + self.width, :]
 
 
+CAMERA_MODELS = ("reference", "colmap")
+# COLMAP camera models the fused path renders: name -> (lens model, focal params, cx/cy index, distortion mapping)
+_COLMAP_LENSES = {
+    "SIMPLE_PINHOLE": ("PINHOLE", 1, 1, ()),
+    "PINHOLE": ("PINHOLE", 2, 2, ()),
+    "SIMPLE_RADIAL": ("OPENCV", 1, 1, (3,)),            # k -> k1; k2 = p1 = p2 = 0
+    "RADIAL": ("OPENCV", 1, 1, (3, 4)),
+    "OPENCV": ("OPENCV", 2, 2, (4, 5, 6, 7)),
+    "OPENCV_FISHEYE": ("FISHEYE", 2, 2, (4, 5, 6, 7)),
+    "SIMPLE_RADIAL_FISHEYE": ("FISHEYE", 1, 1, (3,)),   # the missing k are 0
+    "RADIAL_FISHEYE": ("FISHEYE", 1, 1, (3, 4)),
+}
+LENS_MODELS = {"PINHOLE": gaussian.LENS_PINHOLE, "OPENCV": gaussian.LENS_OPENCV, "FISHEYE": gaussian.LENS_FISHEYE}
+
+
+def colmap_intrinsics(model, params, downsample=1):
+    """(focal_x, focal_y, lens) of a COLMAP camera at 1 / `downsample` resolution, lens = dict(model="PINHOLE" |
+    "OPENCV" | "FISHEYE", cx, cy, k=[4]) for `Splatter(camera_model="colmap")`.  Focal lengths and the principal
+    point scale with the resolution; the distortion coefficients do not.  ValueError for a model the fused path does
+    not render (FULL_OPENCV, FOV, THIN_PRISM_FISHEYE)."""
+    if model not in _COLMAP_LENSES:
+        raise ValueError(f"COLMAP camera model {model} is not supported (supported: {sorted(_COLMAP_LENSES)})")
+    lens_model, nf, ic, ik = _COLMAP_LENSES[model]
+    fx = float(params[0]) / downsample
+    fy = float(params[nf - 1]) / downsample
+    k = [float(params[j]) for j in ik] + [0.0] * (4 - len(ik))
+    return fx, fy, dict(model=lens_model, cx=float(params[ic]) / downsample, cy=float(params[ic + 1]) / downsample,
+                        k=k)
+
+
 class Splatter(nn.Module):
     def __init__(self, colmap_path, image_path, near=0.3, jacobian_calc="cuda", render_downsample=1,
                  use_sh_coeff=False, render_weight_normalize=False, opa_init_value=0.1, scale_init_value=0.02,
@@ -228,7 +258,7 @@ class Splatter(nn.Module):
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
                  sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none", n_features=0,
-                 filter3d=False, filter3d_variance=0.2):
+                 filter3d=False, filter3d_variance=0.2, camera_model="reference"):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -268,8 +298,22 @@ class Splatter(nn.Module):
         `n_features`: 0 (default) or F = 8, 16, 32 raw per-Gaussian features in `gaussian_3ds.feat` (an nn.Parameter
         [n, F], zero-initialised; `from_tensors` / a checkpoint may provide a "feat" tensor, whose width then sets F),
         blended with the image's weights by `render_features` and carried through densification and checkpoints.
-        Not available with per-pixel SH colour, nor with densify_stats="absgrad"."""
+        Not available with per-pixel SH colour, nor with densify_stats="absgrad".
+
+        `camera_model`: "reference" (default) renders every camera as an undistorted pinhole whose principal point is
+        the image centre, keeping only the focal lengths of `cameras.bin`, as the reference does.  "colmap" renders
+        through each COLMAP camera's own intrinsics (`colmap_intrinsics`): the principal point of PINHOLE and
+        SIMPLE_PINHOLE, the radial / tangential distortion of SIMPLE_RADIAL, RADIAL and OPENCV, and the fisheye
+        distortion of OPENCV_FISHEYE, SIMPLE_RADIAL_FISHEYE and RADIAL_FISHEYE, with gradients (gs_ctx_set_lens).  The
+        view dicts then carry a "lens" (dict(model, cx, cy, k)); view dicts given directly and the free-camera
+        `intrinsics` may carry one too (or cx, cy, model, k) under either setting.  FULL_OPENCV, FOV and
+        THIN_PRISM_FISHEYE raise a ValueError.  Per-pixel SH colour takes a principal point but no distortion.
+        `compute_filter3d` uses the views' lenses (the distorted image for visibility, the fisheye's magnification for
+        the rate)."""
         super().__init__()
+        if camera_model not in CAMERA_MODELS:
+            raise ValueError(f"camera_model must be one of {CAMERA_MODELS}, not {camera_model!r}")
+        self.camera_model = camera_model
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
             raise NotImplementedError("render_weight_normalize is not supported (the reference never enables it)")
@@ -387,6 +431,9 @@ class Splatter(nn.Module):
         from scipy.spatial import cKDTree
         self.colmap_path, self.image_path = colmap_path, image_path
         self.cameras = colmap_io.read_cameras_binary(os.path.join(colmap_path, "cameras.bin"))
+        if self.camera_model == "colmap":
+            for cam in self.cameras.values():
+                colmap_intrinsics(cam.model, cam.params)        # refuses an unsupported model before any image is read
         self.images_info = colmap_io.read_images_binary(os.path.join(colmap_path, "images.bin"))
         pts = colmap_io.read_points3d_binary(os.path.join(colmap_path, "points3D.bin"))
         if not self.test:
@@ -425,9 +472,12 @@ class Splatter(nn.Module):
             im = cv2.cvtColor(cv2.imread(fn), cv2.COLOR_BGR2RGB)
             self.imgs.append(torch.from_numpy(im).to(torch.uint8).to(self.device))
             fy = cam.params[1] if cam.model != "SIMPLE_PINHOLE" else cam.params[0]
-            views.append(dict(width=im.shape[1], height=im.shape[0], focal_x=cam.params[0] / self.render_downsample,
-                              focal_y=fy / self.render_downsample, rot=colmap_io.qvec_to_rotmat(info.qvec),
-                              tran=np.asarray(info.tvec), camera_id=info.camera_id))
+            v = dict(width=im.shape[1], height=im.shape[0], focal_x=cam.params[0] / self.render_downsample,
+                     focal_y=fy / self.render_downsample, rot=colmap_io.qvec_to_rotmat(info.qvec),
+                     tran=np.asarray(info.tvec), camera_id=info.camera_id)
+            if self.camera_model == "colmap":
+                v["focal_x"], v["focal_y"], v["lens"] = colmap_intrinsics(cam.model, cam.params, self.render_downsample)
+            views.append(v)
         self._set_views(views)
 
     def switch_resolution(self, downsample_factor):                 # reference splatter.py:454-463
@@ -447,6 +497,12 @@ class Splatter(nn.Module):
                      focal_x=float(intrinsics["focal_x"]), focal_y=float(intrinsics["focal_y"]),
                      rot=torch.as_tensor(np.asarray(extrinsics["rot"]), dtype=torch.float32).cpu().contiguous(),
                      tran=torch.as_tensor(np.asarray(extrinsics["tran"]), dtype=torch.float32).cpu().contiguous())
+            if intrinsics.get("lens") is not None:
+                v["lens"] = dict(intrinsics["lens"])
+            elif any(intrinsics.get(key) is not None for key in ("cx", "cy", "model", "k")):
+                v["lens"] = dict(model=intrinsics.get("model", "PINHOLE"),
+                                 cx=float(intrinsics.get("cx", v["width"] / 2)),
+                                 cy=float(intrinsics.get("cy", v["height"] / 2)), k=list(intrinsics.get("k", [0.0] * 4)))
             self.ground_truth = None
         else:
             v = self.views[idx]
@@ -462,6 +518,7 @@ class Splatter(nn.Module):
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens([v])
         image, mask = render_frame(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                    v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                    self.tile_culling_prob_thresh, self.scale_activation)
@@ -476,6 +533,7 @@ class Splatter(nn.Module):
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens([v])
         image, mask = render_frame_final(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
                                          v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
                                          self.tile_culling_prob_thresh, self.scale_activation)
@@ -492,6 +550,7 @@ class Splatter(nn.Module):
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens([v])
         image, depth, alpha, mask = render_frame_aux(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], v["rot"], v["tran"],
                                                      self.near, self.tile_culling_prob_thresh, self.scale_activation,
@@ -530,6 +589,7 @@ class Splatter(nn.Module):
         g = self.gaussian_3ds
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens(vs)
         image, depth, alpha, mask = render(
             self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, vs[0]["width"], vs[0]["height"],
             [v["focal_x"] for v in vs], [v["focal_y"] for v in vs], rots, trans, self.near,
@@ -555,6 +615,7 @@ class Splatter(nn.Module):
         v = self.current_view
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens([v])
         image, features, depth, alpha, mask = render_frame_feat(
             self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, g.feat, v["width"], v["height"], v["focal_x"],
             v["focal_y"], v["rot"], v["tran"], self.near, self.tile_culling_prob_thresh, self.scale_activation,
@@ -578,6 +639,7 @@ class Splatter(nn.Module):
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
         self._size_filter3d()
+        self._set_lens([v])
         image, depth, alpha, mask = render_frame_cam(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"],
                                                      v["height"], v["focal_x"], v["focal_y"], rot, tran, self.near,
                                                      self.tile_culling_prob_thresh, self.scale_activation,
@@ -593,6 +655,28 @@ class Splatter(nn.Module):
         padded = self.render_padded()
         return self.tile_info.crop(torch.clamp(padded, 0, 1))
 
+    def _set_lens(self, views):
+        """The context's lenses for a frame (or a sampling-rate pass) over `views`: off when no view has a "lens",
+        one for every view when they all share one, else one per view (a view without one gets the image-centre
+        pinhole; at most 64 distinct per call)."""
+        if all(v.get("lens") is None for v in views):
+            self._rctx.set_lens(None, None)
+            return
+        first = views[0].get("lens")
+        if first is not None and all(v.get("lens") == first for v in views):
+            views = views[:1]
+        models, params = [], []
+        for v in views:
+            ln = v.get("lens") or dict(model="PINHOLE", cx=v["width"] / 2, cy=v["height"] / 2, k=[0.0] * 4)
+            if ln["model"] not in LENS_MODELS:
+                raise ValueError(f"lens model must be one of {sorted(LENS_MODELS)}, not {ln['model']!r}")
+            k = list(ln.get("k", [0.0] * 4))
+            if len(k) != 4:
+                raise ValueError(f"lens k must have 4 coefficients, not {len(k)}")
+            models.append(LENS_MODELS[ln["model"]])
+            params.append([float(ln["cx"]), float(ln["cy"])] + [float(x) for x in k])
+        self._rctx.set_lens(models, torch.tensor(params, dtype=torch.float32))
+
     # -- 3-D smoothing filter (Mip-Splatting) ----------------------------------------------------
     @torch.no_grad()
     def compute_filter3d(self, views=None, margin=0.15):
@@ -607,6 +691,7 @@ class Splatter(nn.Module):
         vs = list(self.views if views is None else views)
         if not vs:
             raise ValueError("compute_filter3d: no views")
+        self._set_lens(vs)                                          # the lens variant of the rate and the test
         g = self.gaussian_3ds
         size = torch.tensor([[int(v["width"]), int(v["height"])] for v in vs], dtype=torch.int64)
         focal = torch.tensor([[float(v["focal_x"]), float(v["focal_y"])] for v in vs], dtype=torch.float32)

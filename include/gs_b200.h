@@ -404,6 +404,47 @@ int gs_ctx_set_filter3d(gs_ctx* ctx, const float* filter3d /* DEVICE [n]; NULL: 
 int gs_filter3d_compute(gs_ctx* ctx, const float* pos /* [n,3] */, int n, const gs_camera* cams_host, int n_cams,
                         float margin, float variance, float* filter3d /* [n] */, gs_stream_t stream);
 
+/* COLMAP camera intrinsics on the fused frame path (additive; default off: every camera is an undistorted pinhole whose
+ * principal point is the image centre, as in the reference).  With (a, b) = (x/z, y/z) and rho = |(a, b)|, a lens maps
+ * (a, b) to (a_d, b_d) by COLMAP's formulas:
+ *   GS_LENS_PINHOLE : (a_d, b_d) = (a, b)                                               (k unused)
+ *   GS_LENS_OPENCV  : a_d = a rad + 2 p1 a b + p2 (rho^2 + 2 a^2), b_d = b rad + p1 (rho^2 + 2 b^2) + 2 p2 a b,
+ *                     rad = 1 + k1 rho^2 + k2 rho^4                                     (k = k1, k2, p1, p2)
+ *   GS_LENS_FISHEYE : (a_d, b_d) = (theta_d / rho) (a, b), theta = atan(rho),
+ *                     theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8)  (COLMAP OPENCV_FISHEYE)
+ * and pixel u of the image (centre u + 0.5) sits at u + 0.5 = fx a_d + cx, v + 0.5 = fy b_d + cy, as COLMAP projects.
+ * The 2-D covariance is J_D (J Sigma3 J^T) J_D^T with J_D the lens map's Jacobian.  Backward: the mean chain is live
+ * through the lens; J_D, like the pinhole Jacobian, is detached in the covariance; the camera gradient uses J_D J;
+ * depth, the SH view direction, the 2-D and 3-D filters and the opacity are unchanged; the intrinsics get no gradient.
+ * Culling: z > near, the 1.2x frustum test on the stored (distorted, principal-point shifted) mean, and rho < rho_max,
+ * where the radial polynomial folds back: OPENCV the smallest rho > 0 with 1 + 3 k1 rho^2 + 5 k2 rho^4 <= 0, FISHEYE
+ * tan of the smallest theta in (0, pi/2) with d theta_d / d theta <= 0 (none: no limit).  A Gaussian past it gets no
+ * instances and its culling_mask entry reports it culled.  Fields of view beyond 180 degrees are not supported.
+ * gs_ctx_set_lens: a context setting, like gs_ctx_set_filter2d: it applies to every fused forward that follows (plain,
+ * final, aux, feat, batch, the packed path, gs_render_forward_backward_host), and a backward (plain, final, aux, cam,
+ * batch, batch cam, feat, the densification statistics' max_radius) uses the lenses its forward recorded.  n == 1: one
+ * lens for every view; n == B: lens v for view v of a batched frame; any other n at a forward is GS_ERR_INVALID_ARG
+ * before any launch.  A PINHOLE lens at exactly (W/2, H/2) in every view runs the kernels of a frame without a lens, so
+ * it renders and differentiates the same bits.  No launch or synchronisation is added.
+ * Refused:  gs_ctx_set_lens (GS_ERR_INVALID_ARG): a null ctx; n < 0 or n > GS_MAX_VIEWS; NULL lenses with n > 0; an
+ * unknown model; a cx, cy or k that is not finite.  Before any launch (GS_ERR_UNSUPPORTED): a forward of SH colour
+ * evaluated per pixel with any lens but a pinhole (a principal point alone is supported: its rays shift with it); a
+ * backward with a gradient push configured (train data-parallel through an all-reduce instead).
+ * gs_filter3d_compute uses the context's lenses too (n == 1 or n == n_cams, GS_ERR_INVALID_ARG otherwise): view c sees
+ * a Gaussian when z > near, rho < rho_max and the distorted pixel position (fx a_d + cx, fy b_d + cy) lies inside the
+ * widened image; the rate stays fx / z for PINHOLE and OPENCV (Mip-Splatting's rate, which ignores distortion) and is
+ * fx max(theta_d'(theta), theta_d(theta) / sin theta) / |p_c| for FISHEYE (the larger of the radial and tangential
+ * magnifications; fx / z on the axis), in fp64.  The legacy per-stage API is not affected. */
+#define GS_LENS_PINHOLE 0
+#define GS_LENS_OPENCV 1  /* k = k1, k2, p1, p2 */
+#define GS_LENS_FISHEYE 2 /* k = k1, k2, k3, k4 (COLMAP OPENCV_FISHEYE) */
+typedef struct gs_lens {
+  int model;
+  float cx, cy; /* principal point in pixels, COLMAP convention (the image centre is (W/2, H/2)) */
+  float k[4];
+} gs_lens;
+int gs_ctx_set_lens(gs_ctx* ctx, const gs_lens* lenses /* HOST [n]; NULL: off */, int n);
+
 /* Screen-space densification statistics (additive; default off).  While a context has them set, every backward that
  * computes parameter gradients (plain, final, aux, cam with parameter gradients, gs_render_forward_backward_host, with
  * or without a gradient push) accumulates, for every Gaussian i with count[i] > 0 in its forward (i.e. binned into at

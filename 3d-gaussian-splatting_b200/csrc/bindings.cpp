@@ -808,6 +808,52 @@ struct RenderContext {
              fn);
   }
 
+  // 2D Gaussian surfels (gs_render_forward_surfel): maps = the GS_SURFEL_MAP_CH map channels (alpha, depth, median,
+  // distortion, normal xyz, 0); returns (final[H,W,3] or None, raw padded[Hp,Wp,3], maps padded[Hp,Wp,8] or None,
+  // maps_final[H,W,8] or None, mask)
+  py::tuple forward_surfel(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                           torch::Tensor scale, int width, int height, float fx, float fy, torch::Tensor rot,
+                           torch::Tensor tran, float near, float thresh, int scale_activation,
+                           std::optional<std::vector<double>> background, bool maps, bool final, double dist_near,
+                           double dist_far) {
+    const char* fn = "RenderContext.forward_surfel";
+    const int64_t n = check_params(fn, pos, rgb, opa, quat, scale);
+    const Background bg = background_of(fn, background);
+    c10::cuda::CUDAGuard guard(pos.device());
+    gs_camera cam = make_cam(width, height, fx, fy, rot, tran, near, thresh);
+    Outputs o = alloc_outputs(pos, 0, n, height, width, false, maps ? GS_SURFEL_MAP_CH : 0, final);
+    gs_render_surfel sf{bg.ptr(), fpm_or_null(o.map), fpm_or_null(o.map_fin), (float)dist_near, (float)dist_far};
+    rendered(gs_render_forward_surfel(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), (int)n, (int)rgb.size(1),
+                                      scale_activation, &cam, fpm(o.raw), fpm_or_null(o.fin),
+                                      o.mask.data_ptr<int64_t>(), &sf, cur_stream()),
+             fn);
+    return py::make_tuple(or_none(o.fin), o.raw, or_none(o.map), or_none(o.map_fin), o.mask);
+  }
+
+  // backward of forward_surfel; grad_maps = None: zero map gradients (the kernels without the map terms)
+  void backward_surfel_into(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa, torch::Tensor quat,
+                            torch::Tensor scale, torch::Tensor raw, torch::Tensor grad_image, bool grad_is_final,
+                            std::optional<torch::Tensor> grad_maps, torch::Tensor g_pos, torch::Tensor g_rgb,
+                            torch::Tensor g_opa, torch::Tensor g_quat, torch::Tensor g_scale, int64_t expected_frame) {
+    const char* fn = "RenderContext.backward_surfel_into";
+    check_backward(fn, expected_frame, false, grad_is_final, pos, rgb, opa, quat, scale, raw, grad_image, nullptr,
+                   nullptr);
+    if (grad_maps) {
+      const std::vector<int64_t> pixels = grad_is_final ? std::vector<int64_t>{grad_image.size(0), grad_image.size(1)}
+                                                        : std::vector<int64_t>{raw.size(0), raw.size(1)};
+      check_image(fn, "grad_maps", *grad_maps, pixels, GS_SURFEL_MAP_CH, false);
+    }
+    check_grads(fn, {pos, rgb, opa, quat, scale}, {g_pos, g_rgb, g_opa, g_quat, g_scale});
+    c10::cuda::CUDAGuard guard(pos.device());
+    auto gi = grad_image.contiguous();
+    torch::Tensor gm;
+    if (grad_maps) gm = grad_maps->contiguous();
+    check_rc(gs_render_backward_surfel(ctx, fp(pos), fp(rgb), fp(opa), fp(quat), fp(scale), fp(raw), fp(gi),
+                                       grad_is_final ? 1 : 0, fpm_or_null(gm), fpm(g_pos), fpm(g_rgb), fpm(g_opa),
+                                       fpm(g_quat), fpm(g_scale), cur_stream()),
+             fn);
+  }
+
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
   // mask[n] (uint8) = the Gaussians the last forward binned (gs_frame_visible); accumulate: OR into mask
@@ -1251,6 +1297,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("quat"), py::arg("scale"), py::arg("feat"), py::arg("width"), py::arg("height"), py::arg("fx"),
            py::arg("fy"), py::arg("rot"), py::arg("tran"), py::arg("near"), py::arg("thresh"),
            py::arg("scale_activation"), py::arg("background") = py::none(), py::arg("final") = true)
+      .def("forward_surfel", &RenderContext::forward_surfel, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
+           py::arg("quat"), py::arg("scale"), py::arg("width"), py::arg("height"), py::arg("fx"), py::arg("fy"),
+           py::arg("rot"), py::arg("tran"), py::arg("near"), py::arg("thresh"), py::arg("scale_activation"),
+           py::arg("background"), py::arg("maps"), py::arg("final"), py::arg("dist_near") = 0.2,
+           py::arg("dist_far") = 100.0)
+      .def("backward_surfel_into", &RenderContext::backward_surfel_into, py::arg("pos"), py::arg("rgb"),
+           py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("raw"), py::arg("grad_image"),
+           py::arg("grad_is_final"), py::arg("grad_maps"), py::arg("g_pos"), py::arg("g_rgb"), py::arg("g_opa"),
+           py::arg("g_quat"), py::arg("g_scale"), py::arg("expected_frame") = -1)
       .def("backward_feat_into", &RenderContext::backward_feat_into, py::arg("pos"), py::arg("rgb"), py::arg("opa"),
            py::arg("quat"), py::arg("scale"), py::arg("feat"), py::arg("raw"), py::arg("grad_image"),
            py::arg("grad_is_final"), py::arg("aux"), py::arg("grad_aux"), py::arg("map"), py::arg("grad_map"),
@@ -1319,6 +1374,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("abi_version") = gs_abi_version();
   m.attr("SH_EVAL_PIXEL") = GS_SH_EVAL_PIXEL;
   m.attr("SH_EVAL_GAUSSIAN") = GS_SH_EVAL_GAUSSIAN;
+  m.attr("SURFEL_MAP_CH") = GS_SURFEL_MAP_CH;
   m.attr("FILTER2D_NONE") = GS_FILTER2D_NONE;
   m.attr("FILTER2D_DILATE") = GS_FILTER2D_DILATE;
   m.attr("FILTER2D_ANTIALIAS") = GS_FILTER2D_ANTIALIAS;

@@ -282,6 +282,48 @@ cudaError_t gs_launch_feat_grad(const uint32_t* offsets_g, const uint32_t* count
                                 const uint32_t* row_epoch, uint32_t epoch, int n, int f, float* grad_feat,
                                 cudaStream_t st);
 
+// ---- surfel.cu / blend_surfel.cu (2D Gaussian surfels: gs_render_forward_surfel) ----------------------------------
+// One surfel's record (64 bytes), written by the surfel projection and gathered by the surfel blend kernels:
+//   M = [s_u R r0 | s_v R r1 | p_c] row-major (rows m_x, m_y, m_z), op = sigmoid(opa), the activated colour, and the
+//   camera-frame normal R r2 flipped to face the camera.
+struct __align__(16) GsSurfelRec {
+  float M[9];
+  float op;
+  float rgb[3];
+  float nrm[3];
+};
+// Per padded pixel, written by the surfel forward for its backward: ws[p] = {sum w c (3), T_f}; with maps also
+// wsm[2p] = {sum w z, sum w, sum w m, sum w m^2} (m relative to the first blended instance) and wsm[2p + 1] = {sum w n (3), median instance (int bits, -1: none)}.
+// The map channels of gs_render_surfel: GS_SURFEL_MAP_CH floats per pixel.
+struct GsSurfelMaps {
+  float* maps;         // [Hp, Wp, 8] or NULL
+  float* maps_final;   // [height, width, 8] or NULL
+  float dist_near, dist_far;
+};
+// KG = 0: RGB logits (d = 3); 9 / 16: per-Gaussian SH of degree 2 / 3.  One launch when n > 0.
+cudaError_t gs_launch_surfel_project(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                     const float* scale, int n, int kg, int scale_act, const GsCam& cam,
+                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h, float fx,
+                                     float fy, GsSurfelRec* rec, uint2* rect, uint32_t* count, uint32_t* dkey,
+                                     int64_t* mask, unsigned int* n_visible, cudaStream_t st);
+// Chains the epoch-tagged GS_SURFEL_GREC rows of each surfel to the raw parameters.  One launch when n > 0.
+#define GS_SURFEL_GREC 16
+cudaError_t gs_launch_surfel_project_bwd(const float* pos, const float* rgb, const float* opa, const float* quat,
+                                         const float* scale, int n, int kg, int scale_act, const GsCam& cam,
+                                         const uint32_t* offsets_g, const uint32_t* count, const float* grad_inst,
+                                         const uint32_t* row_epoch, uint32_t epoch, float* g_pos, float* g_rgb,
+                                         float* g_opa, float* g_quat, float* g_scale, cudaStream_t st);
+cudaError_t gs_launch_blend_surfel_fwd(const GsSurfelRec* rec, const uint32_t* ids, const int* tile_accum,
+                                       const GsFrameGeom& g, const float* bg /*3 floats, by value*/, float* image,
+                                       float* final_img, const GsCrop& crop, const GsSurfelMaps* maps /*nullable*/,
+                                       float near /*hits at z <= near are skipped*/, float4* ws, float4* wsm, int* tile_neff, cudaStream_t st);
+cudaError_t gs_launch_blend_surfel_bwd(const GsSurfelRec* rec, const uint32_t* ids, const uint2* rect,
+                                       const uint32_t* goff, const int* tile_accum, const GsFrameGeom& g,
+                                       const float* bg, const float* image, const float* grad_image, int grad_is_final,
+                                       const GsCrop& crop, const float* grad_maps /*nullable*/, float dist_near,
+                                       float dist_far, float near, const float4* ws, const float4* wsm, float* grad_inst,
+                                       uint32_t* row_epoch, uint32_t epoch, int* tile_neff_b, cudaStream_t st);
+
 // ---- binning.cu ------------------------------------------------------------------------
 cudaError_t gs_launch_emit_keys(const uint2* rect, const uint32_t* perm, const uint32_t* offsets_sorted, int n, int ntx,
                                 void* keys, int key_bytes, uint32_t* vals, cudaStream_t st);

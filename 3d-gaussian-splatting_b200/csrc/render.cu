@@ -188,6 +188,13 @@ struct gs_ctx {
   int lens_n = 0;                         //   0: off
   bool lens_on = false;                   // the last forward ran the lens kernels (its backward uses them)
   GsLens lens{};                          //   with the lens of its (first) view
+  // 2D Gaussian surfels (gs_render_forward_surfel): the last forward's records, per-pixel workspaces and settings
+  DevBuf srec, sws, swsm;
+  bool surfel = false;                    // the last forward rendered surfels
+  bool surfel_maps = false;               //   and wrote maps (swsm holds their sums)
+  int surfel_kg = 0;                      //   its colour: 0 RGB, 9 / 16 per-Gaussian SH
+  float surfel_bg[3] = {0.f, 0.f, 0.f};
+  float dist_near = 0.2f, dist_far = 100.f;
 };
 
 // stage boundaries: event i is recorded BEFORE stage i; stage i lasts ev[i+1]-ev[i]
@@ -225,7 +232,7 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
-                    &c->grad_feat_inst, &c->views, &c->f3_dev, &c->lenses};
+                    &c->grad_feat_inst, &c->views, &c->f3_dev, &c->lenses, &c->srec, &c->sws, &c->swsm};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
@@ -318,6 +325,7 @@ static int begin_forward(gs_ctx* c, const char* who) {
   c->have_backward = false;
   c->have_aux = false;
   c->n_views = 0;
+  c->surfel = false;
   c->ev_fwd_valid = false;
   return 0;
 }
@@ -765,6 +773,8 @@ static int render_backward_impl(gs_ctx* c, const char* who, bool batch, const fl
   if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
   if (c->n_views && !batch)
     return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was batched (use gs_render_backward_batch)");
+  if (c->surfel)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward rendered surfels (use gs_render_backward_surfel)");
   // camera only (grad_cam, the five parameter gradients all NULL: the caller has checked the set is not mixed)
   const bool cam_only = grad_cam && !grad_pos;
   if (!image || !grad_image || (!cam_only && (!grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale)) ||
@@ -985,6 +995,9 @@ extern "C" int gs_render_backward_feat(gs_ctx* c, const float* pos, const float*
                                        float* grad_quat, float* grad_scale, float* grad_feat, gs_stream_t stream) {
   if (!c) return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: null ctx");
   if (!c->have_forward) return gs_set_error_msg(GS_ERR_NO_FORWARD, "gs_render_backward_feat: no forward on this ctx");
+  if (c->surfel)
+    return gs_set_error_msg(GS_ERR_INVALID_ARG, "gs_render_backward_feat: the last forward rendered surfels (use "
+                                                "gs_render_backward_surfel)");
   if (c->n_views)
     return gs_set_error_msg(GS_ERR_INVALID_ARG,
                             "gs_render_backward_feat: the last forward was batched (use gs_render_backward_batch)");
@@ -1100,6 +1113,8 @@ extern "C" int gs_render_backward_batch(gs_ctx* c, const float* pos, const float
   const char* who = "gs_render_backward_batch";
   if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
   if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (c->surfel)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward rendered surfels (use gs_render_backward_surfel)");
   if (!c->n_views) return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was not batched");
   if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
   if (int rc = gs_blend_batch_supported()) return rc;
@@ -1120,6 +1135,8 @@ extern "C" int gs_render_backward_batch_cam(gs_ctx* c, const float* pos, const f
     return gs_fail(GS_ERR_INVALID_ARG, who, "the five parameter gradients must be all NULL or all non-NULL");
   if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
   if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (c->surfel)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward rendered surfels (use gs_render_backward_surfel)");
   if (!c->n_views) return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward was not batched");
   if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "not available with a gradient push configured");
   if (int rc = gs_blend_batch_supported()) return rc;
@@ -1429,5 +1446,136 @@ extern "C" int gs_frame_stage_ms(gs_ctx* c, float* out, gs_stream_t stream) {
     for (int i = 0; i < 6; ++i) GS_CUDA_TRY(cudaEventElapsedTime(&out[i], c->ev[i], c->ev[i + 1]));
   if (c->ev_bwd_valid)
     for (int i = 6; i < 8; ++i) GS_CUDA_TRY(cudaEventElapsedTime(&out[i], c->ev[i + 1], c->ev[i + 2]));
+  return 0;
+}
+
+// ---- 2D Gaussian surfels ----------------------------------------------------------------
+// Stage 1 is the surfel projection (surfel.cu), stages 2-5 the 3DGS frame's bin_frame on the gather path, stage 6 the
+// surfel blend (blend_surfel.cu); the backward is the surfel blend backward and projection backward.
+extern "C" int gs_render_forward_surfel(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                        const float* quat, const float* scale, int n, int d, int scale_activation,
+                                        const gs_camera* cam, float* image, float* final_img, int64_t* culling_mask,
+                                        const gs_render_surfel* s, gs_stream_t stream) {
+  const char* who = "gs_render_forward_surfel";
+  if (!c || !cam || n < 0) return gs_fail(GS_ERR_INVALID_ARG, who, "bad arguments");
+  if (d != 3 && gs_sh_basis_count(d) == 0)
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "colour width must be 3 (RGB), 27 (SH deg 2) or 48 (SH deg 3)");
+  if (int rc = check_camera(*cam, who)) return rc;
+  if (!image || (n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
+    return gs_fail(GS_ERR_INVALID_ARG, who, "null tensor pointer");
+  if (scale_activation != GS_SCALE_ABS && scale_activation != GS_SCALE_EXP)
+    return gs_fail(GS_ERR_INVALID_ARG, who, "unknown scale activation");
+  float bg[3] = {0.f, 0.f, 0.f};
+  GsSurfelMaps mp{nullptr, nullptr, 0.2f, 100.f};
+  if (s) {
+    if (s->background)
+      for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(s->background[k])) return gs_fail(GS_ERR_INVALID_ARG, who, "background must be finite");
+        bg[k] = s->background[k];
+      }
+    if (!(std::isfinite(s->dist_near) && std::isfinite(s->dist_far) && s->dist_near > 0.f && s->dist_far > s->dist_near))
+      return gs_fail(GS_ERR_INVALID_ARG, who, "dist_near and dist_far must be finite with 0 < dist_near < dist_far");
+    if (s->maps_final && (!s->maps || !final_img))
+      return gs_fail(GS_ERR_INVALID_ARG, who, "maps_final needs maps and image_final");
+    if ((reinterpret_cast<uintptr_t>(s->maps) | reinterpret_cast<uintptr_t>(s->maps_final)) % 16)
+      return gs_fail(GS_ERR_INVALID_ARG, who, "maps and maps_final must be 16-byte aligned");
+    mp = GsSurfelMaps{s->maps, s->maps_final, s->dist_near, s->dist_far};
+  }
+  if (d != 3 && c->sh_eval != GS_SH_EVAL_GAUSSIAN)
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "SH colour evaluated per pixel has no surfel kernel (use GS_SH_EVAL_GAUSSIAN)");
+  if (c->filter2d != GS_FILTER2D_NONE || c->filter3d)
+    return gs_fail(GS_ERR_UNSUPPORTED, who, "the 2-D and 3-D filters have no surfel kernel");
+  if (c->stats_on) return gs_fail(GS_ERR_UNSUPPORTED, who, "densification statistics have no surfel kernel");
+  if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "a gradient push has no surfel kernel");
+  if (!gs_tuning().gather) return gs_fail(GS_ERR_UNSUPPORTED, who, "the packed path (gs_tune(\"gather\", 0)) has no surfel kernel");
+  GsLens lens{};
+  bool lens_on;
+  if (int rc = resolve_lenses(c, cam, 1, &lens, lens_on, who)) return rc;
+  if (lens_on) return gs_fail(GS_ERR_UNSUPPORTED, who, "lenses have no surfel kernel (image-centre pinhole only)");
+  if (int rc = begin_forward(c, who)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  GsFrameGeom g;
+  if (int rc = frame_geom(*cam, 1, g, who)) return rc;
+  const GsView vw = view_constants(c, cam, g);
+  const size_t N = (size_t)n, P = (size_t)g.wp * g.hp;
+  if (int rc = reserve_frame(c, N, g.n_tiles, st)) return rc;
+  GS_CUDA_TRY(c->srec.reserve(N * sizeof(GsSurfelRec) + 64, st));
+  GS_CUDA_TRY(c->sws.reserve(P * sizeof(float4), st));
+  if (mp.maps) GS_CUDA_TRY(c->swsm.reserve(2 * P * sizeof(float4), st));
+  const int kg = d == 3 ? 0 : gs_sh_basis_count(d);
+
+  gs_mark(c, 0, st);
+  GS_CUDA_TRY(cudaMemsetAsync(c->counters.p, 0, 64, st));
+  GS_CUDA_TRY(cudaMemsetAsync(c->count.as<uint32_t>() + N, 0, 4, st));
+  GS_CUDA_TRY(gs_launch_surfel_project(pos, rgb, opa, quat, scale, n, kg, scale_activation, vw.cam, vw.grid,
+                                       cam->near_plane, vw.half_w, vw.half_h, cam->focal_x, cam->focal_y,
+                                       c->srec.as<GsSurfelRec>(), c->rect.as<uint2>(), c->count.as<uint32_t>(),
+                                       c->dkey_in.as<uint32_t>(), culling_mask, c->counters.as<unsigned int>(), st));
+  if (n > 0) gs_count_launch();
+  long long m = 0;
+  if (int rc = bin_frame(c, n, g, true, 3, 3, rgb, st, m)) return rc;
+  GsCrop crop{(g.wp - g.width) / 2, (g.hp - g.height) / 2, g.width, g.height};
+  gs_mark(c, 5, st);
+  GS_CUDA_TRY(gs_launch_blend_surfel_fwd(c->srec.as<GsSurfelRec>(), c->vals_out.as<uint32_t>(), c->tile_accum.as<int>(),
+                                         g, bg, image, final_img, crop, mp.maps ? &mp : nullptr, cam->near_plane,
+                                         c->sws.as<float4>(),
+                                         mp.maps ? c->swsm.as<float4>() : nullptr, c->tile_neff.as<int>(), st));
+  gs_count_launch();
+  gs_mark(c, 6, st);
+  commit_forward(c, n, d, scale_activation, m, g, vw, cam->near_plane, 0, kg > 0, true, false, GsAuxOut{}, nullptr,
+                 nullptr, false, lens);
+  c->surfel = true;
+  c->surfel_maps = mp.maps != nullptr;
+  c->surfel_kg = kg;
+  memcpy(c->surfel_bg, bg, sizeof(bg));
+  c->dist_near = mp.dist_near;
+  c->dist_far = mp.dist_far;
+  return 0;
+}
+
+extern "C" int gs_render_backward_surfel(gs_ctx* c, const float* pos, const float* rgb, const float* opa,
+                                         const float* quat, const float* scale, const float* image,
+                                         const float* grad_image, int grad_is_final, const float* grad_maps,
+                                         float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat,
+                                         float* grad_scale, gs_stream_t stream) {
+  const char* who = "gs_render_backward_surfel";
+  if (!c) return gs_fail(GS_ERR_INVALID_ARG, who, "null ctx");
+  if (!c->have_forward) return gs_fail(GS_ERR_NO_FORWARD, who, "no forward on this ctx");
+  if (!c->surfel) return gs_fail(GS_ERR_INVALID_ARG, who, "the last forward did not render surfels");
+  if (!image || !grad_image || !grad_pos || !grad_rgb || !grad_opa || !grad_quat || !grad_scale ||
+      (c->n > 0 && (!pos || !rgb || !opa || !quat || !scale)))
+    return gs_fail(GS_ERR_INVALID_ARG, who, "null tensor pointer");
+  if (grad_maps && !c->surfel_maps) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_maps given but the forward wrote no maps");
+  if (reinterpret_cast<uintptr_t>(grad_maps) % 16) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_maps must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(grad_quat) % 16) return gs_fail(GS_ERR_INVALID_ARG, who, "grad_quat must be 16-byte aligned");
+  if (c->push.world) return gs_fail(GS_ERR_UNSUPPORTED, who, "a gradient push has no surfel kernel");
+  if (c->stats_on) return gs_fail(GS_ERR_UNSUPPORTED, who, "densification statistics have no surfel kernel");
+  if (int rc = gs_check_device(c->device, who)) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t M = (size_t)c->m;
+  GS_CUDA_TRY(c->grad_inst.reserve(M * GS_SURFEL_GREC * 4 + 16, st));
+  if (int rc = next_row_epoch(c, M, st)) return rc;
+  c->ev_bwd_valid = false;
+  GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
+  gs_mark(c, 7, st);
+  if (c->m > 0) {
+    GS_CUDA_TRY(gs_launch_blend_surfel_bwd(c->srec.as<GsSurfelRec>(), c->vals_out.as<uint32_t>(), c->rect.as<uint2>(),
+                                           c->offsets_g.as<uint32_t>(), c->tile_accum.as<int>(), c->geom, c->surfel_bg,
+                                           image, grad_image, grad_is_final, crop, grad_maps, c->dist_near,
+                                           c->dist_far, c->near_plane, c->sws.as<float4>(),
+                                           c->surfel_maps ? c->swsm.as<float4>() : nullptr, c->grad_inst.as<float>(),
+                                           c->row_epoch.as<uint32_t>(), c->epoch, c->tile_neff_b.as<int>(), st));
+    gs_count_launch();
+    c->have_backward = true;
+  }
+  gs_mark(c, 8, st);
+  GS_CUDA_TRY(gs_launch_surfel_project_bwd(pos, rgb, opa, quat, scale, c->n, c->surfel_kg, c->scale_act, c->cam,
+                                           c->offsets_g.as<uint32_t>(), c->count.as<uint32_t>(),
+                                           c->grad_inst.as<float>(), c->row_epoch.as<uint32_t>(), c->epoch, grad_pos,
+                                           grad_rgb, grad_opa, grad_quat, grad_scale, st));
+  if (c->n > 0) gs_count_launch();
+  gs_mark(c, 9, st);
+  c->ev_bwd_valid = c->timing && c->ev_ok;
   return 0;
 }

@@ -64,3 +64,23 @@ def psnr(image, target, data_range=None):
     mse = torch.mean((image - t) ** 2)
     dr = (t.max() - t.min()) if data_range is None else torch.as_tensor(float(data_range), device=image.device)
     return 10.0 * torch.log10(dr * dr / mse)
+
+
+def surfel_normal_consistency(normal, depth, alpha, fx, fy, eps=1e-8):
+    """2DGS's normal-consistency term on the maps of a surfel frame (renderer.render_frame_surfel): the mean over the
+    interior pixels of 1 - alpha n . n_d, where n = normal [H,W,3] (sum w n, camera frame) and n_d is the unit normal of
+    the surface back-projected from the expected depth depth / alpha through the pixel rays
+    ((x + 0.5 - W/2) / fx, (y + 0.5 - H/2) / fy, 1), from central differences, turned to face the camera.  As in 2DGS,
+    the gradient reaches both sides: the normal map, and the depth and alpha maps through n_d; the alpha weight is a
+    constant."""
+    h, w = depth.shape
+    d = depth / alpha.clamp_min(eps)
+    xs = (torch.arange(w, dtype=d.dtype, device=d.device) + 0.5 - w / 2) / fx
+    ys = (torch.arange(h, dtype=d.dtype, device=d.device) + 0.5 - h / 2) / fy
+    P = torch.stack([xs[None, :].expand(h, w) * d, ys[:, None].expand(h, w) * d, d], dim=-1)
+    dx = P[1:-1, 2:] - P[1:-1, :-2]
+    dy = P[2:, 1:-1] - P[:-2, 1:-1]
+    nd = torch.linalg.cross(dy, dx, dim=-1)
+    nd = nd / nd.norm(dim=-1, keepdim=True).clamp_min(eps)
+    a = alpha[1:-1, 1:-1].detach()
+    return (1.0 - a * (normal[1:-1, 1:-1] * nd).sum(-1)).mean()

@@ -345,6 +345,73 @@ def render_frame_aux(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, f
                                  near, tile_thresh, scale_activation, background, final)
 
 
+SURFEL_MAPS = ("alpha", "depth", "median", "distortion", "normal")
+
+
+class _RenderFrameSurfel(torch.autograd.Function):
+    """2D Gaussian surfels (gs_render_forward_surfel): the five parameters rendered as flat disks evaluated at the
+    ray-disk intersection.  Outputs: the image (final: clamped + cropped [H,W,3]; else padded, un-clamped), and with
+    maps the alpha, depth (sum w z, camera z), median depth, distortion and camera-frame normal (sum w n) maps, then
+    the culling mask.  Every map is differentiable; maps no loss uses pass no gradient."""
+
+    @staticmethod
+    def forward(ctx, rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                near, tile_thresh, scale_activation, background, final, maps, dist_near, dist_far):
+        params = _params(pos, rgb, opa, quat, scale)
+        bg = None if background is None else [float(v) for v in background]
+        fin, raw, m, m_fin, mask = rctx.forward_surfel(
+            *params, int(width), int(height), float(focal_x), float(focal_y), rot.detach().cpu(),
+            tran.detach().cpu(), float(near), float(tile_thresh), SCALE_ACTIVATIONS[scale_activation], bg,
+            bool(maps), bool(final), float(dist_near), float(dist_far))
+        image = fin if final else raw
+        _save_frame(ctx, rctx, mask, params + (raw,), final, image.shape[:2])
+        ctx.maps = bool(maps)
+        if not maps:
+            return image, mask
+        mp = m_fin if final else m
+        return (image, mp[..., 0].contiguous(), mp[..., 1].contiguous(), mp[..., 2].contiguous(),
+                mp[..., 3].contiguous(), mp[..., 4:7].contiguous(), mask)
+
+    @staticmethod
+    def backward(ctx, grad_image, *grads):
+        *params, raw = ctx.saved_tensors
+        shape = ctx.map_shape
+        if grad_image is None:
+            grad_image = raw.new_zeros(*shape, 3)
+        grad_maps = None
+        gm = grads[:-1]                                           # the last is the mask's
+        if ctx.maps and any(g is not None for g in gm):
+            grad_maps = raw.new_zeros(*shape, 8)
+            for k, g in enumerate(gm[:4]):
+                if g is not None:
+                    grad_maps[..., k] = g
+            if gm[4] is not None:
+                grad_maps[..., 4:7] = gm[4]
+        outs, push = _flat_grads(params)
+        if push is not None:
+            raise RuntimeError("render_frame_surfel: surfel frames have no data-parallel gradient push; exchange the "
+                               "gradients with an all-reduce (dp.py's NCCL bucket) instead")
+        _apply_push(ctx.rctx, None)
+        ctx.rctx.backward_surfel_into(*params, raw, _f32(grad_image), ctx.final, grad_maps, *outs, ctx.frame)
+        return (None, *outs) + (None,) * 14
+
+
+def render_frame_surfel(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran, near,
+                        tile_thresh, scale_activation, background=None, final=True, maps=True, dist_near=0.2,
+                        dist_far=100.0):
+    """-> (image, maps, culling_mask) of a frame of 2D Gaussian surfels (include/gs_b200.h, gs_render_forward_surfel).
+    maps: {} without maps, else {"alpha", "depth", "median", "distortion": [rows, cols], "normal": [rows, cols, 3]}
+    over the same pixels as the image (final: the [H,W] crop, not clamped; else [Hp,Wp]).  depth is accumulated
+    (expected depth = depth / alpha); the normal is in the camera frame (world: rot^T n).  Only scale[:, :2] is used.
+    Per-Gaussian SH colour (d = 27 / 48) needs rctx.set_sh_eval(SH_EVAL_GAUSSIAN)."""
+    out = _RenderFrameSurfel.apply(rctx, pos, rgb, opa, quat, scale, width, height, focal_x, focal_y, rot, tran,
+                                   near, tile_thresh, scale_activation, background, final, maps, dist_near,
+                                   dist_far)
+    if not maps:
+        return out[0], {}, out[1]
+    return out[0], dict(zip(SURFEL_MAPS, out[1:6])), out[6]
+
+
 MAX_VIEWS = 64
 
 

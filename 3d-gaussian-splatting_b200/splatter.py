@@ -29,7 +29,8 @@ import torch.nn as nn
 
 import gaussian
 from renderer import (FEATURE_WIDTHS, FILTER2D, SH_EVAL, render_frame, render_frame_aux, render_frame_batch,
-                      render_frame_batch_cam, render_frame_cam, render_frame_feat, render_frame_final)
+                      render_frame_batch_cam, render_frame_cam, render_frame_feat, render_frame_final,
+                      render_frame_surfel)
 
 EPS = 1e-4
 SH_C0 = 0.28209479177387814
@@ -222,6 +223,7 @@ class Tiles:
 
 
 CAMERA_MODELS = ("reference", "colmap")
+PRIMITIVES = ("gaussian", "surfel")
 # COLMAP camera models the fused path renders: name -> (lens model, focal params, cx/cy index, distortion mapping)
 _COLMAP_LENSES = {
     "SIMPLE_PINHOLE": ("PINHOLE", 1, 1, ()),
@@ -258,7 +260,7 @@ class Splatter(nn.Module):
                  debug=0, scale_activation="abs", cudaculling=1, load_ckpt=None, debug_align=False,
                  fast_drawing=True, test=False, images: Optional[List[torch.Tensor]] = None, device=None, *,
                  sh_eval="pixel", filter2d="none", filter2d_variance=0.3, densify_stats="none", n_features=0,
-                 filter3d=False, filter3d_variance=0.2, camera_model="reference"):
+                 filter3d=False, filter3d_variance=0.2, camera_model="reference", primitive="gaussian"):
         """Reference signature (splatter.py:324-345).  `colmap_path` may also be a dict of raw
         parameter tensors (pos, rgb, opa, quat, scale) with `image_path` a list of view dicts
         (width, height, focal_x, focal_y, rot[3,3], tran[3]) - see `from_tensors`.
@@ -309,11 +311,30 @@ class Splatter(nn.Module):
         `intrinsics` may carry one too (or cx, cy, model, k) under either setting.  FULL_OPENCV, FOV and
         THIN_PRISM_FISHEYE raise a ValueError.  Per-pixel SH colour takes a principal point but no distortion.
         `compute_filter3d` uses the views' lenses (the distorted image for visibility, the fisheye's magnification for
-        the rate)."""
+        the rate).
+
+        `primitive`: "gaussian" (default) renders 3-D Gaussians; "surfel" renders each Gaussian as the flat disk of 2D
+        Gaussian Splatting (Huang et al. 2024), spanned by its first two scale axes and evaluated where the pixel ray
+        meets it (`renderer.render_frame_surfel`).  `forward` then returns the surfel image and `render_surfel_maps`
+        the image with alpha, depth, median-depth, distortion and normal maps.  scale[:, 2] is set to the activation's
+        floor (raw 0 for "abs", log 1e-4 for "exp") and gets no gradient, so densification and MCMC keep every
+        Gaussian flat; checkpoints keep the five-key schema.  Surfels take RGB colour or sh_eval="gaussian", the
+        image-centre pinhole ("reference" cameras), and none of the filters, densify_stats or features."""
         super().__init__()
         if camera_model not in CAMERA_MODELS:
             raise ValueError(f"camera_model must be one of {CAMERA_MODELS}, not {camera_model!r}")
         self.camera_model = camera_model
+        if primitive not in PRIMITIVES:
+            raise ValueError(f"primitive must be one of {PRIMITIVES}, not {primitive!r}")
+        if primitive == "surfel":
+            if use_sh_coeff and sh_eval != "gaussian":
+                raise ValueError("primitive='surfel' with SH colour needs sh_eval='gaussian'")
+            for name, value, default in (("filter2d", filter2d, "none"), ("filter3d", bool(filter3d), False),
+                                         ("densify_stats", densify_stats, "none"), ("n_features", n_features, 0),
+                                         ("camera_model", camera_model, "reference")):
+                if value != default:
+                    raise ValueError(f"primitive='surfel' does not take {name}={value!r}")
+        self.primitive = primitive
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if render_weight_normalize:
             raise NotImplementedError("render_weight_normalize is not supported (the reference never enables it)")
@@ -378,6 +399,9 @@ class Splatter(nn.Module):
                 if not n_features:
                     n_features = int(params["feat"].shape[1])
                     _check_features(n_features, use_sh_coeff, sh_eval, densify_stats)
+        if self.primitive == "surfel":                             # flat: the third axis at the activation's floor
+            params["scale"] = params["scale"].clone()
+            params["scale"][:, 2] = 0.0 if scale_activation == "abs" else math.log(EPS)
         if self.use_sh_coeff != (params["rgb"].shape[1] != 3):
             raise ValueError("use_sh_coeff must match the colour width (3 = RGB logits, 27 / 48 = SH)")
         n = params["pos"].shape[0]
@@ -513,9 +537,40 @@ class Splatter(nn.Module):
         self.tile_info = Tiles(v["width"], v["height"], v["focal_x"], v["focal_y"])
 
     # -- frame ------------------------------------------------------------------------------
+    def _surfel_frame(self, final, maps, background=None, dist_near=0.2, dist_far=100.0):
+        g, v = self.gaussian_3ds, self.current_view
+        image, mp, mask = render_frame_surfel(self._rctx, g.pos, g.rgb, g.opa, g.quat, g.scale, v["width"], v["height"],
+                                              v["focal_x"], v["focal_y"], v["rot"], v["tran"], self.near,
+                                              self.tile_culling_prob_thresh, self.scale_activation,
+                                              background=background, final=final, maps=maps, dist_near=dist_near,
+                                              dist_far=dist_far)
+        self.culling_mask = mask
+        self.n_gaussians = g.pos.shape[0]
+        self.n_tile_gaussians = self._rctx.last_instances()
+        return image, mp
+
+    def _gaussian_only(self, who):
+        if self.primitive != "gaussian":
+            raise ValueError(f"{who} renders 3-D Gaussians; a Splatter with primitive='surfel' renders with forward, "
+                             "render_padded and render_surfel_maps")
+
+    def render_surfel_maps(self, camera_id=None, extrinsics=None, intrinsics=None, background=None, dist_near=0.2,
+                           dist_far=100.0):
+        """primitive='surfel': dict(image [H,W,3] (clamped, cropped, over `background`), alpha, depth (sum w z, camera
+        z: divide by alpha for the expected depth), median, distortion (m(z) = far / (far - near) (1 - near / z) with
+        near, far = `dist_near`, `dist_far`) [H,W], normal [H,W,3] (sum w n, camera frame; rot^T n in the world)).  All
+        are differentiable (`renderer.render_frame_surfel`)."""
+        if self.primitive != "surfel":
+            raise ValueError("render_surfel_maps needs primitive='surfel'")
+        self.set_camera(camera_id, extrinsics, intrinsics)
+        image, mp = self._surfel_frame(True, True, background, dist_near, dist_far)
+        return dict(image=image, **mp)
+
     def render_padded(self):
         """Padded, un-clamped image (what reference `render` returns, splatter.py:563-634)."""
         g, v = self.gaussian_3ds, self.current_view
+        if self.primitive == "surfel":
+            return self._surfel_frame(False, False)[0]
         self._size_densify_stats()
         self._size_filter3d()
         self._set_lens([v])
@@ -530,6 +585,8 @@ class Splatter(nn.Module):
         """reference splatter.py:643-655; clamp(0,1) + centre crop (:652-653) run inside the blend
         kernels (`render_frame_final`)."""
         self.set_camera(camera_id, extrinsics, intrinsics)
+        if self.primitive == "surfel":
+            return self._surfel_frame(True, False)[0]
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
         self._size_filter3d()
@@ -546,6 +603,7 @@ class Splatter(nn.Module):
         """`forward` plus per-pixel maps: dict(image [H,W,3] (clamped, cropped, over `background`, default black),
         depth [H,W] (accumulated sum w |p_c|: divide by alpha for the expected Euclidean distance), alpha [H,W]).
         All three are differentiable (`renderer.render_frame_aux`)."""
+        self._gaussian_only("render_maps")
         self.set_camera(camera_id, extrinsics, intrinsics)
         g, v = self.gaussian_3ds, self.current_view
         self._size_densify_stats()
@@ -566,6 +624,7 @@ class Splatter(nn.Module):
         holds images.  Each view is what `render_maps` returns for it; the gradients are SUMS over the views (divide
         the loss by B for a mean).  Sets `culling_mask` to the [n] sum over the views and `n_tile_gaussians` to the
         batch's instance count.  The views must share their size (ValueError otherwise)."""
+        self._gaussian_only("render_batch")
         return self._render_batch("render_batch", render_frame_batch, camera_ids, None, None, background)
 
     def render_batch_at_poses(self, rots, trans, camera_ids, background=None):
@@ -575,6 +634,7 @@ class Splatter(nn.Module):
         The intrinsics and `ground_truth` come from `camera_ids` (B ids).  Returns `render_batch`'s dict and sets the
         same attributes; backward gives rots and trans their gradients (`renderer.render_frame_batch_cam`), and runs
         camera only when no scene parameter needs a gradient.  Costs one host synchronisation (the 12 B pose floats)."""
+        self._gaussian_only("render_batch_at_poses")
         return self._render_batch("render_batch_at_poses", render_frame_batch_cam, camera_ids, rots, trans, background)
 
     def _render_batch(self, who, render, camera_ids, rots, trans, background):
@@ -608,6 +668,7 @@ class Splatter(nn.Module):
         f_i,k with the image's weights, composited over zero (the background applies to the image only; divide by
         alpha for the expected feature), not clamped.  All four are differentiable (`renderer.render_frame_feat`);
         the feature loss reaches `gaussian_3ds.feat` and, through alpha, the geometry.  Needs n_features > 0."""
+        self._gaussian_only("render_features")
         g = self.gaussian_3ds
         if g.feat is None:
             raise RuntimeError("render_features needs Splatter(..., n_features=8, 16 or 32)")
@@ -632,6 +693,7 @@ class Splatter(nn.Module):
         `ground_truth` come from view `camera_id` (default: the current view).  Returns dict(image, depth, alpha) like
         `render_maps`; backward gives rot and tran their gradients (`renderer.render_frame_cam`), and runs camera
         only when no scene parameter needs a gradient.  Costs one extra host synchronisation (the 12 pose floats)."""
+        self._gaussian_only("render_at_pose")
         if camera_id is not None:
             self.set_camera(camera_id)
         if self.current_view is None:

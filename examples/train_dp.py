@@ -7,6 +7,7 @@ rank renders a different view and the gradients are all-reduced (one flat bucket
 
   python examples/train_dp.py --gaussians 200000 --res 640x360 --iters 300
   python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_dp.py ...
+  python examples/train_dp.py --surfel --lambda-normal 0.05 --lambda-dist 100    # 2D Gaussian Splatting
 
 Ground truth = renders of a "teacher" Gaussian set; the student starts from perturbed positions,
 grey colours and low opacity.  Prints loss / PSNR and iterations per second.
@@ -22,6 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "3d-gaussian-splatting_b200"))
 
 import dp  # noqa: E402
+import loss as L  # noqa: E402
 import optim  # noqa: E402
 import splatter  # noqa: E402
 import synthetic as S  # noqa: E402
@@ -31,7 +33,8 @@ def build(n, w, h, n_views, dev, seed=0, student_kw=None):
     teacher = S.make_gaussians(n, w, h, seed)
     views = [S.make_view(w, h, k) for k in range(n_views)]
     vd = [dict(width=v.width, height=v.height, focal_x=v.fx, focal_y=v.fy, rot=v.rot, tran=v.tran) for v in views]
-    sp_t = splatter.Splatter.from_tensors(teacher, vd, device=dev)
+    prim = (student_kw or {}).get("primitive", "gaussian")        # the teacher renders the student's primitive
+    sp_t = splatter.Splatter.from_tensors(teacher, vd, device=dev, primitive=prim)
     with torch.no_grad():
         gts = [sp_t(k).clone() for k in range(n_views)]
     g = torch.Generator().manual_seed(seed + 100)          # identical on every rank: replicas start equal
@@ -52,10 +55,13 @@ def make_optimizer(sp, lr=0.003, fused=True):
 
 
 def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None,
-          filter3d_every=0):
+          filter3d_every=0, lambda_normal=0.0, lambda_dist=0.0):
     opt = make_optimizer(sp, lr, fused_adam)
     params = list(sp.gaussian_3ds.parameters())
-    bucket = dp.make_grad_bucket(params, average=True)   # peer-memory exchange when available, else NCCL
+    surfel = sp.primitive == "surfel"
+    # peer-memory exchange when available, else NCCL; surfel frames have no gradient push, so they all-reduce
+    bucket = dp.make_grad_bucket(params, average=True, exchange="nccl" if surfel else "auto")
+    maps = surfel and (lambda_normal > 0 or lambda_dist > 0)
     mc = None
     if cap_max is not None:                                           # MCMC densification, refining every 100 steps
         import mcmc
@@ -66,8 +72,17 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
     for it in range(iters):
         opt.zero_grad(set_to_none=True)
         view = dp.view_for_rank(it, rank, world, len(gts))
-        img = sp(view)
-        loss = (img - gts[view]).abs().mean()                        # train.py:99
+        if maps:                                                      # 2DGS: L1 + normal consistency + distortion
+            out = sp.render_surfel_maps(view)
+            img = out["image"]
+            v = sp.current_view
+            loss = ((img - gts[view]).abs().mean()
+                    + lambda_normal * L.surfel_normal_consistency(out["normal"], out["depth"], out["alpha"],
+                                                                  v["focal_x"], v["focal_y"])
+                    + lambda_dist * out["distortion"].mean())
+        else:
+            img = sp(view)
+            loss = (img - gts[view]).abs().mean()                    # train.py:99
         loss.backward()
         bucket.allreduce()
         if mc is not None:                                            # after the exchange: every rank adds the same
@@ -112,7 +127,15 @@ def main():
     ap.add_argument("--filter3d", action="store_true",
                     help="Mip-Splatting's configuration: the 2-D antialias filter and the 3-D filter (variance 0.1), "
                          "recomputed every 100 steps over all training views on every rank")
+    ap.add_argument("--surfel", action="store_true",
+                    help="2D Gaussian Splatting: train (and render the ground truth with) surfels")
+    ap.add_argument("--lambda-normal", type=float, default=0.0, help="--surfel: weight of the normal-consistency loss")
+    ap.add_argument("--lambda-dist", type=float, default=0.0, help="--surfel: weight of the depth-distortion loss")
     args = ap.parse_args()
+    if (args.lambda_normal or args.lambda_dist) and not args.surfel:
+        ap.error("--lambda-normal / --lambda-dist need --surfel")
+    if args.surfel and args.filter3d:
+        ap.error("--surfel takes no --filter3d")
     if args.visible_adam and args.torch_adam:
         ap.error("--visible-adam is a mode of the fused flat Adam")
     if args.cap_max is not None and not args.mcmc:
@@ -125,11 +148,14 @@ def main():
         torch.distributed.init_process_group("nccl", device_id=dev)
     torch.manual_seed(2023)                                           # identical torch RNG on all ranks
     kw = dict(filter2d="antialias", filter3d=True, filter3d_variance=0.1) if args.filter3d else None
+    if args.surfel:
+        kw = dict(primitive="surfel")
     sp, gts = build(args.gaussians, w, h, args.views, dev, student_kw=kw)
     hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam,
                       visible_adam=args.visible_adam,
                       cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None,
-                      filter3d_every=100 if args.filter3d else 0)
+                      filter3d_every=100 if args.filter3d else 0, lambda_normal=args.lambda_normal,
+                      lambda_dist=args.lambda_dist)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
               f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians")

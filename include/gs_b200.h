@@ -224,6 +224,61 @@ int gs_render_backward_aux(gs_ctx* ctx, const float* pos, const float* rgb, cons
                            float* grad_pos, float* grad_rgb, float* grad_opa, float* grad_quat, float* grad_scale,
                            gs_stream_t stream);
 
+/* 2D Gaussian surfels (additive; Huang et al., "2D Gaussian Splatting", SIGGRAPH 2024).  The five parameter tensors
+ * are those of gs_render_forward; only scale columns 0 and 1 are used (grad_scale[:, 2] is written as 0).  A surfel is
+ * the flat disk spanned by u = s_u R r0 and v = s_v R r1 (r0, r1, r2: the columns of the normalised quaternion's
+ * rotation, s the activated scale, R the camera rotation) at p_c = R pos + tran, evaluated exactly at the ray-disk
+ * intersection (a, b): rho = a^2 + b^2, or 2DGS's screen filter rho = 2 |q - centre|^2 in px^2 where that is smaller
+ * (then z = the centre's camera z).  alpha = min(0.99, sigmoid(opa) exp(-rho / 2)); alpha < 1/255 is skipped, and so is a
+ * hit whose depth z is not beyond the near plane (a disk whose plane crosses the camera plane can be met behind the
+ * camera just past its 3-sigma edge; without this the depth and distortion of that pixel would be negative or
+ * infinite); the 1e-4 early stop applies.  Culling and the 1.2x frustum test are on the centre, the sort key is the centre's camera z,
+ * and the tile rectangle is the box of the projected 3-sigma disk joined with a sqrt(2)/2 px box around the centre
+ * (a disk that reaches the camera plane gets no instances).  Colour: RGB logits (d = 3), or SH of degree 2 / 3
+ * (d = 27 / 48) evaluated once per Gaussian, which requires GS_SH_EVAL_GAUSSIAN on the context.
+ * Per pixel, with instances in (tile, depth) order and w_i = alpha_i T_i:
+ *   image = sum w c + T_f background;  maps (GS_SURFEL_MAP_CH floats per pixel, in this order):
+ *   0 alpha = 1 - T_f;  1 depth = sum w z (camera z; expected depth = depth / alpha);  2 median = z of the last blended
+ *   instance with T > 0.5 before it (0: none);  3 distortion = sum_i w_i sum_{j<i} w_j (m_i - m_j)^2 with
+ *   m(z) = far / (far - near) (1 - near / z);  4..6 normal = sum w n, n = R r2 flipped to face the camera (camera frame;
+ *   the world normal is rot^T normal);  7 zero.
+ *   background : HOST float[3]; NULL = black.  Must be finite.  It has no gradient.
+ *   maps       : DEVICE [Hp, Wp, GS_SURFEL_MAP_CH], 16-byte aligned; NULL: no maps (the kernels that skip them run).
+ *   maps_final : DEVICE [height, width, GS_SURFEL_MAP_CH] centre crop of maps (not clamped), or NULL; needs maps and
+ *                image_final.
+ *   dist_near, dist_far : the distortion's m(z); 0 < dist_near < dist_far, finite.
+ * s == NULL: black background, no maps.  The context keeps 16 bytes per padded pixel of workspace (48 with maps).
+ * Refused before any launch, GS_ERR_UNSUPPORTED: SH colour evaluated per pixel (d != 3 without GS_SH_EVAL_GAUSSIAN); a
+ * lens other than the image-centre pinhole; the 2-D or 3-D filter; densification statistics; a gradient push; the
+ * packed path (gs_tune("gather", 0)).  GS_ERR_INVALID_ARG: bad arguments as gs_render_forward_aux, misaligned or
+ * inconsistent map pointers, a bad dist_near / dist_far.  Batched views, feature maps and camera gradients have no
+ * surfel entry; every existing backward after a surfel forward is GS_ERR_INVALID_ARG, and so is
+ * gs_render_backward_surfel after any other forward.  gs_frame_stats, gs_frame_visible and the stage timer report
+ * surfel frames as they report 3DGS ones. */
+#define GS_SURFEL_MAP_CH 8
+typedef struct gs_render_surfel {
+  const float* background;
+  float* maps;
+  float* maps_final;
+  float dist_near, dist_far;
+} gs_render_surfel;
+int gs_render_forward_surfel(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                             const float* scale, int n, int d, int scale_activation, const gs_camera* cam_host,
+                             float* image_raw_padded, float* image_final, int64_t* culling_mask,
+                             const gs_render_surfel* s /* nullable */, gs_stream_t stream);
+/* Backward of gs_render_forward_surfel.  grad_image is [Hp,Wp,3] (grad_is_final == 0) or [height,width,3] of the final
+ * image (grad_is_final != 0: clamp mask from image_raw_padded, zero outside the crop).  grad_maps: [Hp,Wp,8] or
+ * [height,width,8] (per grad_is_final; maps are not clamped, only the crop masks them), 16-byte aligned, or NULL (zero
+ * map gradients, which runs the kernels without the map terms); channel 7 is ignored.  grad_maps needs a forward that
+ * wrote maps (GS_ERR_INVALID_ARG).  The median's gradient reaches only the median instance's z.  Deterministic (fixed
+ * order sums, no atomics).  Refused before any launch: no surfel forward on ctx (GS_ERR_INVALID_ARG after a 3DGS
+ * forward, GS_ERR_NO_FORWARD without one), a gradient push or densification statistics configured
+ * (GS_ERR_UNSUPPORTED). */
+int gs_render_backward_surfel(gs_ctx* ctx, const float* pos, const float* rgb, const float* opa, const float* quat,
+                              const float* scale, const float* image_raw_padded, const float* grad_image,
+                              int grad_is_final, const float* grad_maps, float* grad_pos, float* grad_rgb,
+                              float* grad_opa, float* grad_quat, float* grad_scale, gs_stream_t stream);
+
 /* gs_render_backward_aux plus the gradient with respect to the camera of the last forward, p_c = rot p + tran (rot
  * used as given, not re-orthonormalised): grad_cam (DEVICE float[12]) receives dL/drot row-major [9], then dL/dtran [3].
  * It follows the semantics of pos: the projection Jacobian is constant, rot stays live in the 2-D covariance

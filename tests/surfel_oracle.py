@@ -110,14 +110,38 @@ def surfel_rects(M, cam: O.Camera, visible):
     return tx0, tx1, ty0, ty1
 
 
+def without_branch_ties(g, cam, tol=1e-5):
+    """g without the surfels that have a pixel where the screen filter and the intersection tie (|rho2 - rho3| <
+    tol rho3) at an alpha above the skip threshold.  The model's gradient jumps where the branch changes, so at such a
+    pixel an fp32 and an fp64 evaluation may take different branches and both be right; a surfel with a projected std
+    near sqrt(2)/2 px has them."""
+    p = {k: v.double() for k, v in g.items()}
+    M, _, _ = surfel_matrix(p["pos"], p["quat"], p["scale"], cam)
+    ys, xs = torch.meshgrid(torch.arange(cam.Hp, dtype=torch.float64), torch.arange(cam.Wp, dtype=torch.float64),
+                            indexing="ij")
+    qx = ((xs + 0.5 - cam.Wp // 2) / cam.fx).reshape(-1, 1)
+    qy = ((ys + 0.5 - cam.Hp // 2) / cam.fy).reshape(-1, 1)
+    _, _, _, araw = pixel_eval(M, p["opa"].sigmoid(), qx, qy, cam.fx, cam.fy)
+    h = ray_hit(M.unsqueeze(0), qx, qy)
+    h2 = torch.where(h[..., 2] != 0, h[..., 2], torch.ones_like(h[..., 2]))
+    rho3 = (h[..., 0] ** 2 + h[..., 1] ** 2) / h2 ** 2
+    cx, cy = M[:, 0, 2] / M[:, 2, 2], M[:, 1, 2] / M[:, 2, 2]
+    rho2 = 2.0 * (((qx - cx[None]) * cam.fx) ** 2 + ((qy - cy[None]) * cam.fy) ** 2)
+    tie = ((rho2 - rho3).abs() < tol * rho3) & (araw >= ALPHA_MIN) & (h[..., 2] != 0)
+    keep = ~tie.any(0)
+    return {k: v[keep].contiguous() for k, v in g.items()}
+
+
 def distortion_m(z, near, far):
     return far / (far - near) * (1.0 - near / z)
 
 
 def render(pos, rgb, opa, quat, scale, cam: O.Camera, thresh=0.05, scale_activation="abs", background=None,
-           dist_near=0.2, dist_far=100.0):
+           dist_near=0.2, dist_far=100.0, tiles=None, depth_key=None):
     """-> (image [Hp,Wp,3] padded, un-clamped; maps dict of [Hp,Wp] / normal [Hp,Wp,3]; info dict).  rgb [n,3]
-    logits or [n,27|48] per-Gaussian SH coefficients."""
+    logits or [n,27|48] per-Gaussian SH coefficients.  tiles: blend only those tile indices (the others stay 0, with
+    no gradient); binning and order are those of the whole frame.  depth_key [n]: the sort key (default: the float32
+    camera z of each centre)."""
     dt = pos.dtype
     M, nrm, pc = surfel_matrix(pos, quat, scale, cam, scale_activation)
     op = opa.sigmoid()
@@ -127,7 +151,7 @@ def render(pos, rgb, opa, quat, scale, cam: O.Camera, thresh=0.05, scale_activat
     zs = torch.where(zc > cam.near, zc, torch.ones_like(zc))
     visible = (zc > cam.near) & ((pcd[:, 0] / zs).abs() < cam.half_w) & ((pcd[:, 1] / zs).abs() < cam.half_h)
     rects = surfel_rects(M, cam, visible)
-    key = (pos.detach().float() @ cam.rot.float().T + cam.tran.float())[:, 2]
+    key = (pos.detach().float() @ cam.rot.float().T + cam.tran.float())[:, 2] if depth_key is None else depth_key
     gi, accum = O.bin_and_sort(torch.stack([key, key, key], -1), None, rects, cam.ntx, cam.nty, depth_key=key)
     bg = torch.zeros(3, dtype=dt) if background is None else torch.tensor(background, dtype=dt)
     Hp, Wp = cam.Hp, cam.Wp
@@ -137,7 +161,7 @@ def render(pos, rgb, opa, quat, scale, cam: O.Camera, thresh=0.05, scale_activat
     mp["normal"] = torch.zeros(cam.nty, cam.ntx, 256, 3, dtype=dt)
     acc = accum.to(torch.int64)
     r16 = torch.arange(16, dtype=dt)
-    for t in range(cam.ntx * cam.nty):
+    for t in range(cam.ntx * cam.nty) if tiles is None else tiles:
         s, e = int(acc[t]), int(acc[t + 1])
         ty, tx = divmod(t, cam.ntx)
         ix = (tx * 16 + r16).reshape(1, 16).expand(16, 16).reshape(-1, 1)

@@ -52,29 +52,7 @@ def _scene(n=400, w=80, h=64, seed=0, sh=0, extra=True):
         # a saturated tile: a stack of opaque surfels in front of everything
         add([[0.2 * z0, 0.2 * z0, 0.5 * z0 + 0.01 * k] for k in range(12)], [[1.0, 0.0, 0.0, 0.0]] * 12,
             [(0.03 * z0, 0.03 * z0)] * 12, [6.0] * 12)
-    return _without_branch_ties(g, cam), cam
-
-
-def _without_branch_ties(g, cam, tol=1e-5):
-    """g without the surfels that have a pixel where the screen filter and the intersection tie (|rho2 - rho3| <
-    tol rho3) at an alpha above the skip threshold.  The model's gradient jumps where the branch changes, so at such a
-    pixel an fp32 and an fp64 evaluation may take different branches and both be right; a surfel with a projected std
-    near sqrt(2)/2 px has them."""
-    p = {k: v.double() for k, v in g.items()}
-    M, _, _ = SO.surfel_matrix(p["pos"], p["quat"], p["scale"], cam)
-    ys, xs = torch.meshgrid(torch.arange(cam.Hp, dtype=torch.float64), torch.arange(cam.Wp, dtype=torch.float64),
-                            indexing="ij")
-    qx = ((xs + 0.5 - cam.Wp // 2) / cam.fx).reshape(-1, 1)
-    qy = ((ys + 0.5 - cam.Hp // 2) / cam.fy).reshape(-1, 1)
-    _, _, _, araw = SO.pixel_eval(M, p["opa"].sigmoid(), qx, qy, cam.fx, cam.fy)
-    h = SO.ray_hit(M.unsqueeze(0), qx, qy)
-    h2 = torch.where(h[..., 2] != 0, h[..., 2], torch.ones_like(h[..., 2]))
-    rho3 = (h[..., 0] ** 2 + h[..., 1] ** 2) / h2 ** 2
-    cx, cy = M[:, 0, 2] / M[:, 2, 2], M[:, 1, 2] / M[:, 2, 2]
-    rho2 = 2.0 * (((qx - cx[None]) * cam.fx) ** 2 + ((qy - cy[None]) * cam.fy) ** 2)
-    tie = ((rho2 - rho3).abs() < tol * rho3) & (araw >= SO.ALPHA_MIN) & (h[..., 2] != 0)
-    keep = ~tie.any(0)
-    return {k: v[keep].contiguous() for k, v in g.items()}
+    return SO.without_branch_ties(g, cam), cam
 
 
 def _device(g, dev):
@@ -199,7 +177,7 @@ def test_a_tile_longer_than_a_staging_chunk():
     extra = dict(pos=(pc - t) @ R, quat=torch.randn(n, 4, generator=gen),
                  scale=torch.cat([torch.rand(n, 2, generator=gen) * 0.2 + 0.1, torch.zeros(n, 1)], -1),
                  opa=torch.full((n,), -3.5), rgb=torch.randn(n, 3, generator=gen))
-    g = _without_branch_ties({k: torch.cat([g[k], extra[k]]) for k in KEYS}, cam)
+    g = SO.without_branch_ties({k: torch.cat([g[k], extra[k]]) for k in KEYS}, cam)
     w = _weights((cam.height, cam.width), ("image",) + MAPS, seed=7)
     gpu = _run(g, cam, background=BG, weights=w)[:3]
     ref, info = _oracle(g, cam, background=BG, weights=w)[:3], None

@@ -24,7 +24,7 @@ CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CU_SOURCES = ["project.cu", "binning.cu", "blend.cu", "blend_sh.cu", "blend_sh_tc.cu", "render.cu", "optim.cu", "collective.cu", "loss.cu", "densify.cu",
-              "densify_stats.cu", "blend_feat.cu", "mcmc.cu", "filter3d.cu", "surfel.cu", "blend_surfel.cu"]
+              "densify_stats.cu", "blend_feat.cu", "mcmc.cu", "filter3d.cu", "surfel.cu", "blend_surfel.cu", "scores.cu"]
 HEADERS = ["gs_common.cuh", "sh_common.cuh", "tc_common.cuh", "project.cuh", "internal.h", os.path.join(ROOT, "include", "gs_b200.h")]
 LIB = os.path.join(HERE, "libgs_b200.so")
 EXT = os.path.join(HERE, "gaussian" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))

@@ -856,6 +856,25 @@ struct RenderContext {
 
   int64_t last_instances() { return (int64_t)gs_frame_instances(ctx); }
 
+  // weight_sum[n] += sum of the last forward's blend weights per Gaussian, weight_max[n] = max with its largest one
+  // (gs_frame_scores)
+  void scores_into(torch::Tensor weight_sum, torch::Tensor weight_max) {
+    for (auto* t : {&weight_sum, &weight_max}) {
+      TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == at::kFloat && t->dim() == 1,
+                  "RenderContext.scores_into: weight_sum and weight_max must be contiguous 1-D CUDA float32 tensors");
+      TORCH_CHECK(t->device().index() == device,
+                  "RenderContext.scores_into: weight_sum / weight_max is on another device than the context");
+    }
+    TORCH_CHECK(weight_sum.numel() == weight_max.numel(), "RenderContext.scores_into: weight_sum and weight_max differ in size");
+    TORCH_CHECK(weight_sum.numel() < (int64_t(1) << 31), "RenderContext.scores_into: too many Gaussians");
+    c10::cuda::CUDAGuard guard(weight_sum.device());
+    struct gs_frame_scores sc{};
+    sc.n = (int)weight_sum.numel();
+    sc.weight_sum = weight_sum.data_ptr<float>();
+    sc.weight_max = weight_max.data_ptr<float>();
+    check_rc(gs_frame_scores(ctx, &sc, cur_stream()), "gs_frame_scores");
+  }
+
   // mask[n] (uint8) = the Gaussians the last forward binned (gs_frame_visible); accumulate: OR into mask
   void visible_into(torch::Tensor mask, bool accumulate) {
     TORCH_CHECK(mask.is_cuda() && mask.is_contiguous() && mask.scalar_type() == at::kByte && mask.dim() == 1,
@@ -1006,6 +1025,34 @@ static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_appl
              "gs_densify_apply_rows");
   }
   return {out, {n - nk, nc, nsp}};
+}
+
+// keep-only densification plan: the rows with keep[i] set, in order (code = keep bit, dst[0] = its exclusive scan, no
+// clones or splits); returns the new parameter tensors (+ feat) and the number removed
+std::tuple<std::vector<torch::Tensor>, int64_t> prune(torch::Tensor pos, torch::Tensor rgb, torch::Tensor opa,
+                                                      torch::Tensor quat, torch::Tensor scale, torch::Tensor keep,
+                                                      c10::optional<torch::Tensor> feat) {
+  GS_CHECK_F32(pos); GS_CHECK_F32(rgb); GS_CHECK_F32(opa); GS_CHECK_F32(quat); GS_CHECK_F32(scale);
+  const int64_t n = pos.size(0);
+  TORCH_CHECK(pos.dim() == 2 && pos.size(1) == 3 && rgb.dim() == 2 && rgb.size(0) == n && opa.numel() == n &&
+                  quat.dim() == 2 && quat.size(0) == n && quat.size(1) == 4 && scale.dim() == 2 && scale.size(0) == n &&
+                  scale.size(1) == 3,
+              "prune: bad shapes");
+  TORCH_CHECK(n < (int64_t(1) << 31), "prune: too many Gaussians");
+  TORCH_CHECK(keep.is_cuda() && keep.scalar_type() == at::kBool && keep.dim() == 1 && keep.numel() == n &&
+                  keep.device() == pos.device(),
+              "prune: keep must be a 1-D CUDA bool tensor [n] on the parameters' device");
+  if (feat) {
+    GS_CHECK_F32(*feat);
+    TORCH_CHECK(feat->dim() == 2 && feat->size(0) == n && feat->size(1) > 0, "prune: feat must be [n, f]");
+  }
+  c10::cuda::CUDAGuard guard(pos.device());
+  auto code = torch::zeros({n + 1}, keep.options().dtype(at::kByte));
+  code.narrow(0, 0, n).copy_(keep);
+  auto dst = torch::zeros({3, n + 1}, keep.options().dtype(at::kInt));
+  if (n > 0) dst[0].narrow(0, 1, n).copy_(torch::cumsum(keep, 0, at::kInt));
+  auto [out, counts] = densify_apply(pos, rgb, opa, quat, scale, nullptr, 0, 0.0, c10::nullopt, code, dst, feat);
+  return {out, counts[0]};
 }
 
 // densification (SURVEY.md §8 f-2): returns the five new parameter tensors + (n_deleted, n_clone, n_split)
@@ -1314,6 +1361,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("frame_id", &RenderContext::frame_id)
       .def("last_instances", &RenderContext::last_instances)
       .def("visible_into", &RenderContext::visible_into, py::arg("mask"), py::arg("accumulate") = false)
+      .def("scores_into", &RenderContext::scores_into, py::arg("weight_sum"), py::arg("weight_max"))
       .def("stats", &RenderContext::stats)
       .def("set_sh_eval", &RenderContext::set_sh_eval, py::arg("mode"))
       .def("set_filter2d", &RenderContext::set_filter2d, py::arg("mode"), py::arg("variance") = 0.3)
@@ -1338,6 +1386,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("opa_logit_min"), py::arg("delete_thresh"), py::arg("grad_thresh"), py::arg("grad_agg_max"), py::arg("tau"),
         py::arg("use_clone"), py::arg("use_split"), py::arg("clone_dt"), py::arg("generator") = py::none(),
         py::arg("feat") = py::none());
+  m.def("prune", &prune, "keep the rows with keep[i] set (gs_densify_apply with a keep-only plan)", py::arg("pos"),
+        py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("keep"), py::arg("feat") = py::none());
   m.def("densify_stats", &densify_stats,
         "prune / clone / split on the device from screen-space densification statistics (gs_densify_plan_stats)",
         py::arg("pos"), py::arg("rgb"), py::arg("opa"), py::arg("quat"), py::arg("scale"), py::arg("accum"),

@@ -261,6 +261,16 @@ cudaError_t gs_launch_filter3d(const float* pos, int n, const GsF3View* views /*
 cudaError_t gs_launch_frame_visible(const uint32_t* count, int n, int n_views, int accumulate, unsigned char* visible,
                                     cudaStream_t st);
 
+// ---- scores.cu -------------------------------------------------------------------------
+// gs_frame_scores: the blend-weight rows of the last gather-path forward (views: its DEVICE view table when batched,
+// else NULL) to rows[M] / row_epoch[M] tagged with `epoch`, then added into weight_sum / weight_max [n].  Two
+// launches when n > 0.
+cudaError_t gs_launch_frame_scores(const GsRec* grec, const uint32_t* ids, const uint32_t* offsets_g,
+                                   const uint32_t* count, const int* tile_accum, const GsFrameGeom& g,
+                                   const GsView* views, int n, int n_views, const GsCrop& crop, float2* rows,
+                                   uint32_t* row_epoch, uint32_t epoch, float* weight_sum, float* weight_max,
+                                   cudaStream_t st);
+
 // ---- blend_feat.cu ---------------------------------------------------------------------
 // Feature maps (gs_render_forward_feat / gs_render_backward_feat), gather path only.  f: 8, 16 or 32.
 bool gs_feat_width_ok(int f);

@@ -137,6 +137,8 @@ struct gs_ctx {
   DevBuf keys_in, keys_out, vals_in, vals_out, pA, pB, pC, grad_inst, row_epoch;
   DevBuf grad_feat_inst;                  // [M][f] per-instance feature gradients (gs_render_backward_feat)
   uint32_t epoch = 0;                      // tag of the current backward in row_epoch[]
+  DevBuf score_rows, score_epoch;         // [M] (sum w, max w) rows of gs_frame_scores and their tags
+  uint32_t score_ep = 0;                  // tag of the current score pass in score_epoch[]
   // per tile / misc
   DevBuf tile_accum, tile_neff, tile_neff_b, cub_tmp, counters, img_dev, gimg_dev, rays;
   DevBuf cam_part;                        // per-CTA partial sums of the camera gradient (gs_render_backward_cam)
@@ -232,7 +234,8 @@ extern "C" void gs_ctx_destroy(gs_ctx* c) {
   DevBuf* bufs[] = {&c->rec, &c->rect, &c->count, &c->offsets, &c->dkey_in, &c->dkey_out, &c->perm, &c->iota, &c->offsets_g, &c->keys_in, &c->keys_out,
                     &c->vals_in, &c->vals_out, &c->pA, &c->pB, &c->pC, &c->grad_inst, &c->row_epoch, &c->tile_accum, &c->tile_neff,
                     &c->tile_neff_b, &c->cub_tmp, &c->counters, &c->img_dev, &c->gimg_dev, &c->rays, &c->cam_part,
-                    &c->grad_feat_inst, &c->views, &c->f3_dev, &c->lenses, &c->srec, &c->sws, &c->swsm};
+                    &c->grad_feat_inst, &c->views, &c->f3_dev, &c->lenses, &c->srec, &c->sws, &c->swsm,
+                    &c->score_rows, &c->score_epoch};
   for (DevBuf* b : bufs) b->release();
   if (c->host_m) cudaFreeHost(c->host_m);
   if (c->host_rays) cudaFreeHost(c->host_rays);
@@ -1392,6 +1395,36 @@ extern "C" int gs_frame_visible(gs_ctx* c, unsigned char* visible, int n, int ac
   GS_CUDA_TRY(gs_launch_frame_visible(c->count.as<uint32_t>(), n, c->n_views ? c->n_views : 1, accumulate, visible,
                                       (cudaStream_t)stream));
   if (n > 0) gs_count_launch();
+  return 0;
+}
+
+extern "C" int gs_frame_scores(gs_ctx* c, const struct gs_frame_scores* s, gs_stream_t stream) {
+  const char* who = "gs_frame_scores";
+  if (!c || !s || !s->weight_sum || !s->weight_max) return gs_fail(GS_ERR_INVALID_ARG, who, "null argument");
+  if (!c->have_forward) return gs_fail(GS_ERR_INVALID_ARG, who, "no forward on this ctx");
+  if (c->surfel) return gs_fail(GS_ERR_UNSUPPORTED, who, "the last forward rendered surfels");
+  if (!c->gather) return gs_fail(GS_ERR_UNSUPPORTED, who, "the last forward ran the packed path (gs_tune(\"gather\", 0))");
+  if (s->n != c->n) return gs_fail(GS_ERR_INVALID_ARG, who, "n differs from the last forward's");
+  if (int rc = gs_check_device(c->device, who)) return rc;
+  g_cur_alloc = &c->allocator;
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t M = (size_t)c->m;
+  // the pass's own tags, as next_row_epoch keeps the backward's
+  GS_CUDA_TRY(c->score_rows.reserve(M * sizeof(float2) + 16, st));
+  const size_t before = c->score_epoch.cap;
+  GS_CUDA_TRY(c->score_epoch.reserve(M * 4 + 16, st));
+  if (c->score_epoch.cap != before || c->score_ep == 0xffffffffu) {
+    GS_CUDA_TRY(cudaMemsetAsync(c->score_epoch.p, 0, c->score_epoch.cap, st));
+    c->score_ep = 0;
+  }
+  ++c->score_ep;
+  GsCrop crop{(c->geom.wp - c->geom.width) / 2, (c->geom.hp - c->geom.height) / 2, c->geom.width, c->geom.height};
+  GS_CUDA_TRY(gs_launch_frame_scores(c->rec.as<GsRec>(), c->vals_out.as<uint32_t>(), c->offsets_g.as<uint32_t>(),
+                                     c->count.as<uint32_t>(), c->tile_accum.as<int>(), c->geom,
+                                     c->n_views ? c->views.as<GsView>() : nullptr, c->n, c->n_views ? c->n_views : 1,
+                                     crop, c->score_rows.as<float2>(), c->score_epoch.as<uint32_t>(), c->score_ep,
+                                     s->weight_sum, s->weight_max, st));
+  if (c->n > 0) gs_count_launch(2);
   return 0;
 }
 

@@ -23,6 +23,14 @@ import torch
 import gaussian
 
 
+def _keep_rows(t, keep):
+    """Rows keep[i] of t, t zero-padded to keep.numel() rows first."""
+    n = keep.numel()
+    if t.shape[0] < n:
+        t = torch.cat([t, t.new_zeros((n - t.shape[0],) + tuple(t.shape[1:]))])
+    return t[keep.to(t.device)]
+
+
 class FlatAdam:
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.99), eps=1e-8):
         groups = list(params)
@@ -127,11 +135,13 @@ class FlatAdam:
             self._zero_rows = rows.clone() if self._zero_rows is None else self._zero_rows | rows
 
     @torch.no_grad()
-    def replace_params(self, pairs):
+    def replace_params(self, pairs, keep=None):
         """Point `param_groups` at new Parameters, `pairs` = [(old, new)], where the first rows of each new Parameter
         continue the old one's rows (growth).  The moments of the old rows are staged and the next step's `_build`
         puts them in the first rows of the new segments and zeroes the rest; `step_count` is kept.  A checkpoint taken
-        before that step saves the staged moments."""
+        before that step saves the staged moments.  `keep` (bool [n_old]): the new Parameters hold the old rows keep[i]
+        selects, in order (pruning), and the staged moments are those rows' (rows staged by an earlier growth without
+        a step in between count as zero rows)."""
         old = self._all_params()
         staged = list(self._staged) if self._staged is not None else [None] * len(old)
         if self._staged is None and self._flat is not None:
@@ -141,6 +151,8 @@ class FlatAdam:
                 if any(p is q for q in ordered) and p.data.untyped_storage().data_ptr() == store:
                     o = p.data.storage_offset()
                     staged[k] = (m[o:o + p.numel()].view(p.shape), v[o:o + p.numel()].view(p.shape))
+        if keep is not None:
+            staged = [None if s is None else tuple(_keep_rows(t, keep) for t in s) for s in staged]
         for g in self.param_groups:
             g["params"] = [next((nw for od, nw in pairs if od is p), p) for p in g["params"]]
         self._staged = staged if any(s is not None for s in staged) else None

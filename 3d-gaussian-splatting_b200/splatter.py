@@ -160,6 +160,43 @@ class DensifyStats:
         dist.all_reduce(self.max_radius, op=dist.ReduceOp.MAX, group=group)
 
 
+class ContributionScores:
+    """Per-Gaussian blend-weight scores of the fused frame path, accumulated on the device by
+    `Splatter.score_views` / `Splatter.accumulate_scores` (`gaussian.RenderContext.scores_into`, gs_frame_scores):
+
+    - `weight_sum[n]`: the sum over the scored frames' pixels of w = alpha T, the weight each pixel blended the
+      Gaussian's colour with (LightGaussian's and Mini-Splatting's importance);
+    - `weight_max[n]`: its largest w on any scored pixel (RadSplat's score).
+
+    Only pixels inside the rendered images count.  A Gaussian no scored frame binned keeps 0 in both."""
+
+    def __init__(self, n, device=None):
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.weight_sum = self.weight_max = None
+        self.reset(n)
+
+    @property
+    def n(self):
+        return self.weight_sum.numel()
+
+    def reset(self, n):
+        """Zero the scores, sized for n Gaussians."""
+        n = int(n)
+        if self.weight_sum is not None and self.n == n:
+            self.weight_sum.zero_()
+            self.weight_max.zero_()
+            return
+        self.weight_sum = torch.zeros(n, device=self.device, dtype=torch.float32)
+        self.weight_max = torch.zeros(n, device=self.device, dtype=torch.float32)
+
+    def all_reduce(self, group=None):
+        """Combine the scores of all ranks of `group`: the sum of weight_sum, the max of weight_max.  Under data
+        parallel every rank scores other views: call this on every rank before selecting."""
+        import torch.distributed as dist
+        dist.all_reduce(self.weight_sum, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(self.weight_max, op=dist.ReduceOp.MAX, group=group)
+
+
 def _check_features(n_features, use_sh_coeff, sh_eval, densify_stats):
     if n_features != 0 and n_features not in FEATURE_WIDTHS:
         raise ValueError(f"n_features must be 0 or one of {FEATURE_WIDTHS} (pad with zero channels), not {n_features!r}")
@@ -183,23 +220,32 @@ def _zero_moment_rows(optimizer, params, rows):
                 t.masked_fill_(rows.view((-1,) + (1,) * (t.dim() - 1)), 0.0)
 
 
-def _regrow_optimizer(optimizer, pairs):
-    """Re-point an optimizer from the old Parameters to the grown ones (`pairs` = [(old, new)], the old rows first):
-    `optim.FlatAdam` stages its moments (`replace_params`); `torch.optim.Adam`'s per-parameter state is re-keyed and its
-    row tensors padded with zero rows."""
+def _regrow_optimizer(optimizer, pairs, keep=None):
+    """Re-point an optimizer from the old Parameters to the new ones (`pairs` = [(old, new)]): grown ones (the old rows
+    first), or with `keep` (bool [n_old]) the old rows keep[i] selects, in order.  `optim.FlatAdam` stages its moments
+    (`replace_params`); `torch.optim.Adam`'s per-parameter state is re-keyed and its row tensors padded with zero rows
+    or row-selected."""
     import optim
     if isinstance(optimizer, optim.FlatAdam):
-        optimizer.replace_params(pairs)
+        optimizer.replace_params(pairs, keep=keep)
         return
     for old, new in pairs:
         st = optimizer.state.pop(old, None)
         if st is not None:
             for k, t in list(st.items()):
                 if torch.is_tensor(t) and t.dim() > 0 and t.shape[0] == old.shape[0]:
-                    st[k] = torch.cat([t, t.new_zeros((new.shape[0] - old.shape[0],) + tuple(t.shape[1:]))])
+                    if keep is not None:
+                        st[k] = t[keep]
+                    else:
+                        st[k] = torch.cat([t, t.new_zeros((new.shape[0] - old.shape[0],) + tuple(t.shape[1:]))])
             optimizer.state[new] = st
     for grp in optimizer.param_groups:
         grp["params"] = [next((nw for od, nw in pairs if od is p), p) for p in grp["params"]]
+
+
+# what a frame rendered through a Splatter leaves on it (set_camera and the frame entry points)
+_FRAME_ATTRS = ("culling_mask", "n_tile_gaussians", "current_view", "current_camera", "current_w2c_rot",
+                "current_w2c_tran", "tile_info", "ground_truth")
 
 
 class Tiles:
@@ -901,6 +947,106 @@ class Splatter(nn.Module):
         self._size_densify_stats()
         self._size_filter3d()
         return n_new
+
+    # -- contribution scores and pruning ---------------------------------------------------------------------------
+    def _scores_only(self, who):
+        if self.primitive != "gaussian":
+            raise ValueError(f"{who} scores 3-D Gaussian frames; a Splatter with primitive='surfel' has no score pass")
+
+    def _check_scores(self, who, scores):
+        n = self.gaussian_3ds.pos.shape[0]
+        if not isinstance(scores, ContributionScores):
+            raise TypeError(f"{who}: scores must be a ContributionScores")
+        if scores.n != n:
+            raise ValueError(f"{who}: scores are sized for {scores.n} Gaussians, the scene has {n}")
+
+    @torch.no_grad()
+    def score_views(self, camera_ids=None, batch_size=8, scores=None):
+        """Blend-weight scores (`ContributionScores`) of the views `camera_ids` (default: every training view):
+        the views are rendered forward only, in batches of up to `batch_size` views of equal size through the batched
+        frame (one view at a time with per-pixel SH colour, which has no batched frame), and each frame is scored on the
+        device (gs_frame_scores).  `scores` is zeroed first unless given, in which case the views are added to it.
+        Per Gaussian, weight_sum is the sum and weight_max the largest of its weights w = alpha T over the views' pixels.
+
+        The score frames replace the context's last frame: call this between a training frame's backward and the next
+        forward, not between a forward and its backward.  A data-parallel gradient push configured by earlier
+        backwards is cleared first (batched frames take none; the next backward sets it again).  The Splatter's
+        attributes of the last frame (`culling_mask`, `n_tile_gaussians`, the current view and `ground_truth`) are left
+        as they were.  Under data parallel, each rank can score its share of the views (`camera_ids=range(rank,
+        n_views, world)`) and `scores.all_reduce()` combines them.
+
+        Keeping a budget of the k Gaussians with the largest weight_sum is one line; the stable sort breaks ties by
+        index, so data-parallel replicas (after `scores.all_reduce()`) keep the same rows:
+
+            keep = torch.zeros(n, dtype=torch.bool, device=dev).index_fill_(
+                0, torch.sort(scores.weight_sum, descending=True, stable=True).indices[:k], True)
+            splatter.prune(keep, optimizer)
+        """
+        self._scores_only("score_views")
+        ids = list(range(len(self.views))) if camera_ids is None else [int(i) for i in camera_ids]
+        if int(batch_size) < 1:
+            raise ValueError(f"score_views: batch_size must be >= 1, not {batch_size!r}")
+        if scores is None:
+            scores = ContributionScores(self.gaussian_3ds.pos.shape[0], self.device)
+        else:
+            self._check_scores("score_views", scores)
+        saved = {k: getattr(self, k, None) for k in _FRAME_ATTRS}
+        self._rctx.clear_grad_push()
+        try:
+            if self.use_sh_coeff and self.sh_eval == "pixel":
+                for i in ids:
+                    self.forward(i)
+                    self._rctx.scores_into(scores.weight_sum, scores.weight_max)
+                return scores
+            by_size = {}
+            for i in ids:
+                by_size.setdefault((self.views[i]["width"], self.views[i]["height"]), []).append(i)
+            for group in by_size.values():
+                for k in range(0, len(group), int(batch_size)):
+                    self._render_batch("score_views", render_frame_batch, group[k:k + int(batch_size)], None, None,
+                                       None)
+                    self._rctx.scores_into(scores.weight_sum, scores.weight_max)
+            return scores
+        finally:
+            for k, v in saved.items():
+                setattr(self, k, v)
+
+    @torch.no_grad()
+    def accumulate_scores(self, scores):
+        """Add the blend-weight scores of the last frame rendered through this Splatter (`forward`, `render_maps`,
+        `render_batch`, `render_features`, `render_at_pose`) to `scores` (a `ContributionScores` sized for the scene):
+        a trainer collects them from its training frames without extra forwards.  Returns `scores`."""
+        self._scores_only("accumulate_scores")
+        self._check_scores("accumulate_scores", scores)
+        self._rctx.scores_into(scores.weight_sum, scores.weight_max)
+        return scores
+
+    @torch.no_grad()
+    def prune(self, keep, optimizer=None):
+        """Keep the Gaussians with keep[i] set (CUDA bool [n]), in order, and remove the others (`gaussian.prune`: a
+        keep-only `gs_densify_apply` plan; feature rows follow).  New Parameters, like `mcmc_add`; the optimizer
+        (`optim.FlatAdam` or `torch.optim.Adam`) is re-pointed at them and keeps the kept rows' moments bit for bit and
+        its step count.  `densify_stats` and the visible mask re-size from zero, and the 3-D filter is recomputed.
+        Returns the number removed.  ValueError when keep selects nothing."""
+        g = self.gaussian_3ds
+        n = g.pos.shape[0]
+        if not (torch.is_tensor(keep) and keep.is_cuda and keep.dtype == torch.bool and keep.dim() == 1):
+            raise TypeError("prune: keep must be a 1-D CUDA bool tensor")
+        if keep.numel() != n:
+            raise ValueError(f"prune: keep has {keep.numel()} entries, the scene has {n} Gaussians")
+        if not bool(keep.any()):
+            raise ValueError("prune: keep selects no Gaussian")
+        keep = keep.to(self.device).contiguous()
+        old = self._mcmc_params()
+        new, n_removed = gaussian.prune(*(t.detach().contiguous() for t in (g.pos, g.rgb, g.opa, g.quat, g.scale)),
+                                        keep, g._feat_arg())
+        g._replace(new)
+        if optimizer is not None:
+            _regrow_optimizer(optimizer, list(zip(old, self._mcmc_params())), keep)
+        self.n_gaussians = g.pos.shape[0]
+        self._size_densify_stats()
+        self._size_filter3d()
+        return int(n_removed)
 
     @torch.no_grad()
     def mcmc_noise(self, scaler, seed=None):

@@ -8,6 +8,7 @@ rank renders a different view and the gradients are all-reduced (one flat bucket
   python examples/train_dp.py --gaussians 200000 --res 640x360 --iters 300
   python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_dp.py ...
   python examples/train_dp.py --surfel --lambda-normal 0.05 --lambda-dist 100    # 2D Gaussian Splatting
+  python examples/train_dp.py --prune-at 100 --prune-keep 0.5     # keep the half that blends the most weight
 
 Ground truth = renders of a "teacher" Gaussian set; the student starts from perturbed positions,
 grey colours and low opacity.  Prints loss / PSNR and iterations per second.
@@ -55,7 +56,7 @@ def make_optimizer(sp, lr=0.003, fused=True):
 
 
 def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None,
-          filter3d_every=0, lambda_normal=0.0, lambda_dist=0.0):
+          filter3d_every=0, lambda_normal=0.0, lambda_dist=0.0, prune_at=None, prune_keep=1.0):
     opt = make_optimizer(sp, lr, fused_adam)
     params = list(sp.gaussian_3ds.parameters())
     surfel = sp.primitive == "surfel"
@@ -93,6 +94,14 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
             opt.step()
         if filter3d_every and it % filter3d_every == 0:                 # Mip-Splatting: over all training views
             sp.compute_filter3d()
+        if it == prune_at:                                            # LightGaussian-style: by summed blend weight
+            scores = sp.score_views(range(rank, len(gts), world))     # this rank's share of the training views
+            if world > 1:                                             # summed over the shares: every view once
+                scores.all_reduce()
+            n = sp.gaussian_3ds.pos.shape[0]
+            top = torch.sort(scores.weight_sum, descending=True, stable=True).indices[:max(1, int(prune_keep * n))]
+            sp.prune(torch.zeros(n, dtype=torch.bool, device=top.device).index_fill_(0, top, True), opt)
+            bucket.params = list(sp.gaussian_3ds.parameters())
         if mc is not None:
             n = sp.gaussian_3ds.pos.shape[0]
             mc.after_step(it, lr)
@@ -131,7 +140,16 @@ def main():
                     help="2D Gaussian Splatting: train (and render the ground truth with) surfels")
     ap.add_argument("--lambda-normal", type=float, default=0.0, help="--surfel: weight of the normal-consistency loss")
     ap.add_argument("--lambda-dist", type=float, default=0.0, help="--surfel: weight of the depth-distortion loss")
+    ap.add_argument("--prune-at", type=int, default=None,
+                    help="at this step, score every training view (each rank its share, all-reduced) and keep the "
+                         "--prune-keep fraction of the Gaussians with the largest summed blend weight "
+                         "(Splatter.score_views / prune)")
+    ap.add_argument("--prune-keep", type=float, default=0.5, help="--prune-at: fraction of the Gaussians kept")
     args = ap.parse_args()
+    if args.prune_at is not None and args.surfel:
+        ap.error("--prune-at scores 3-D Gaussian frames; it does not take --surfel")
+    if not 0.0 < args.prune_keep <= 1.0:
+        ap.error("--prune-keep must be in (0, 1]")
     if (args.lambda_normal or args.lambda_dist) and not args.surfel:
         ap.error("--lambda-normal / --lambda-dist need --surfel")
     if args.surfel and args.filter3d:
@@ -155,7 +173,7 @@ def main():
                       visible_adam=args.visible_adam,
                       cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None,
                       filter3d_every=100 if args.filter3d else 0, lambda_normal=args.lambda_normal,
-                      lambda_dist=args.lambda_dist)
+                      lambda_dist=args.lambda_dist, prune_at=args.prune_at, prune_keep=args.prune_keep)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
               f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians")

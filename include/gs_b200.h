@@ -567,6 +567,31 @@ int gs_frame_tile_consumed(gs_ctx* ctx, int* tile_consumed, gs_stream_t stream);
  * GS_ERR_INVALID_ARG: a null ctx or pointer, no forward on ctx yet, n different from the last forward's. */
 int gs_frame_visible(gs_ctx* ctx, unsigned char* visible, int n, int accumulate, gs_stream_t stream);
 
+/* Blend-weight scores of the last forward on ctx (additive; for pruning a scene by contribution): for every Gaussian
+ * i, with w_{i,p} = alpha_{i,p} T_{i,p} the weight the gather forward blended Gaussian i's colour with at pixel p (0
+ * once T_{i,p} <= GS_T_STOP: the forward's alpha, T recurrence, instance order and early stop), over the pixels p of
+ * the rendered image (the crop, not the padding) and, for a batched forward, over its views v:
+ *   weight_sum[i] += sum_v sum_p w_{i,p}                        (LightGaussian / Mini-Splatting's score)
+ *   weight_max[i]  = max(weight_max[i], max_v max_p w_{i,p})    (RadSplat's score)
+ * The weights depend on geometry and opacity only, so RGB, per-Gaussian and per-pixel SH, feature frames, both 2-D
+ * filters, the 3-D filter and lenses are all covered.  The caller zeroes the buffers (all DEVICE float32 [n]); a call
+ * adds, so two calls after one forward add twice.  A batched forward adds view by view: B views give the bits of B
+ * single-view forwards each followed by a call, in view order.  Bit-deterministic: one thread per Gaussian sums its
+ * rows in row order, no atomics.
+ * Valid after gs_render_forward, _final, _aux, _feat, _batch and gs_render_forward_backward_host; reads only what
+ * that forward left in ctx and writes nothing a backward reads (forward, scores, backward gives the gradients and
+ * densification statistics of forward, backward).  The per-instance rows (12 bytes per tile instance) live in a
+ * workspace of their own, grown on the first call.  Two launches when n > 0, no synchronisation.
+ * Refused before any launch: a null ctx, s, weight_sum or weight_max, no forward on ctx yet, s->n different from the
+ * forward's n (GS_ERR_INVALID_ARG); a surfel forward, a packed-path forward (gs_tune("gather", 0)) (GS_ERR_UNSUPPORTED).
+ * The struct has no typedef: its tag is also the entry's name. */
+struct gs_frame_scores {
+  int n;               /* must equal the n of the last forward */
+  float* weight_sum;   /* [n] */
+  float* weight_max;   /* [n] */
+};
+int gs_frame_scores(gs_ctx* ctx, const struct gs_frame_scores* s, gs_stream_t stream);
+
 /* End-to-end convenience with HOST buffers (bench `e2e` leg and plain-C callers): copies
  * the camera + grad_image from host, runs forward + backward on device-resident parameters,
  * copies the padded image back.  Host buffers should be pinned.  Synchronises. */

@@ -81,7 +81,8 @@ __device__ __forceinline__ GsProj gs_project(const GsCam& cam, const float p[3],
   o.x = pc[0] / pc[2];
   o.y = pc[1] / pc[2];
   o.depth = sqrtf(pc[0] * pc[0] + pc[1] * pc[1] + pc[2] * pc[2]);
-  if (fabsf(o.x) >= half_w || fabsf(o.y) >= half_h) return o;  // :1220
+  // :1220, written so that a NaN x/z or y/z (p_c.x and p_c.z both overflowed to inf) is culled too
+  if (!(fabsf(o.x) < half_w) || !(fabsf(o.y) < half_h)) return o;
   o.visible = true;
   float jw0[3], jw1[3];
   gs_jw_rows(cam, pc, jw0, jw1);
@@ -357,7 +358,7 @@ __device__ __forceinline__ void gs_lens_project(const GsLens& L, GsProj& o, floa
   gs_lens_map(L, o.x, o.y, ad, bd, J);
   o.x = ad + L.ox;
   o.y = bd + L.oy;
-  if (!(r2 < L.rho2_max) || fabsf(o.x) >= half_w || fabsf(o.y) >= half_h) {
+  if (!(r2 < L.rho2_max) || !(fabsf(o.x) < half_w) || !(fabsf(o.y) < half_h)) {
     o.visible = false;
     return;
   }

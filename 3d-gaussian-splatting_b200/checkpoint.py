@@ -8,7 +8,9 @@ densification statistics of train.py:82-83, and the RNG states (numpy picks the 
 torch samples split positions, utils.py:391-402).  A scene with per-Gaussian features
 (`Splatter(..., n_features=F)`) also stores them under `"feat"` [n, F].  Extra keys are ignored by the reference's
 loader.  A scene with Mip-Splatting's 3-D filter (`Splatter(..., filter3d=True)`) stores the filter under
-`"filter3d"` [n], so that a resume renders the same bits; loading a file without it recomputes the filter.
+`"filter3d"` [n], so that a resume renders the same bits; loading a file without it recomputes the filter.  Per-view
+bilateral grids (`bilagrid.BilateralGrids`) and their optimizer go under `"bilagrid"` (`grids` and the optimizer's
+state dict), so that a resume restores the grids and their Adam moments.
 """
 from __future__ import annotations
 
@@ -37,7 +39,8 @@ def _optimizer_state(opt):
                                                    for s in staged]}
 
 
-def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = None, trainer_state: Optional[dict] = None):
+def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = None, trainer_state: Optional[dict] = None,
+                    bilagrid=None, bilagrid_optimizer=None):
     """`path` is the checkpoint file (train.py writes `<exp>/ckpt.pth`)."""
     g = splatter.gaussian_3ds
     ckpt = {k: getattr(g, k).detach().clone() for k in KEYS}
@@ -45,6 +48,9 @@ def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = N
         ckpt["feat"] = g.feat.detach().clone()
     if getattr(splatter, "filter3d", None) is not None:
         ckpt["filter3d"] = splatter.filter3d.detach().clone()
+    if bilagrid is not None:
+        ckpt["bilagrid"] = {"grids": bilagrid.grids.detach().cpu().clone(),
+                            "optimizer": None if bilagrid_optimizer is None else bilagrid_optimizer.state_dict()}
     ckpt["resume"] = {
         "iteration": iteration,
         "optimizer": _optimizer_state(optimizer),
@@ -62,11 +68,13 @@ def save_checkpoint(splatter, path, optimizer=None, iteration: Optional[int] = N
     return path
 
 
-def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
+def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True, bilagrid=None, bilagrid_optimizer=None):
     """Returns the dict; with `splatter` the parameters are replaced in place (new nn.Parameters, like
     adaptive_control - rebuild torch optimizers before passing them here), the features too when the file has them
     (a splatter with features loading a file without them gets zero features); with `optimizer` its state is restored.
-    A reference-written file (five keys only) loads the parameters and returns `resume == None`."""
+    A reference-written file (five keys only) loads the parameters and returns `resume == None`.  With `bilagrid` (a
+    BilateralGrids of the saved shape) the grids are copied into its Parameter in place, so optimizers over it stay
+    valid, and `bilagrid_optimizer` gets their saved state; a file without grids leaves both as they are."""
     ckpt = torch.load(path, map_location="cpu", weights_only=False)
     missing = [k for k in KEYS if k not in ckpt]
     if missing:
@@ -106,6 +114,15 @@ def load_checkpoint(path, splatter=None, optimizer=None, restore_rng=True):
             optimizer._resume = (st["exp_avg"], st["exp_avg_sq"])      # consumed by FlatAdam._build
             if st.get("staged") is not None:
                 optimizer._staged = st["staged"]
+    bl = ckpt.get("bilagrid")
+    if bilagrid is not None and bl is not None:
+        if tuple(bl["grids"].shape) != tuple(bilagrid.grids.shape):
+            raise ValueError(f"{path}: bilateral grids {list(bl['grids'].shape)} do not fit "
+                             f"{list(bilagrid.grids.shape)}")
+        with torch.no_grad():
+            bilagrid.grids.copy_(bl["grids"])
+        if bilagrid_optimizer is not None and bl.get("optimizer") is not None:
+            bilagrid_optimizer.load_state_dict(bl["optimizer"])
     if restore_rng and res is not None:
         torch.set_rng_state(res["torch_rng"])
         if res.get("cuda_rng") is not None and splatter is not None:

@@ -994,6 +994,60 @@ std::tuple<torch::Tensor, torch::Tensor> loss_l1_ssim(torch::Tensor image, torch
   return {out3, grad};
 }
 
+// bilateral-grid slice (gs_bilagrid_slice_fwd / _bwd): image [B, H, W, 3] (or [H, W, 3], B = 1), grids
+// [V, GH, GW, GL, 12], view_ids: B host ints
+static std::vector<int> bilagrid_check(const char* fn, const torch::Tensor& image, const torch::Tensor& grids,
+                                       const std::vector<int64_t>& view_ids) {
+  GS_CHECK_F32(image); GS_CHECK_F32(grids);
+  TORCH_CHECK((image.dim() == 4 || image.dim() == 3) && image.size(-1) == 3, fn, ": image must be [B, H, W, 3] or [H, W, 3]");
+  TORCH_CHECK(grids.dim() == 5 && grids.size(4) == 12, fn, ": grids must be [V, GH, GW, GL, 12]");
+  TORCH_CHECK(grids.device() == image.device(), fn, ": image and grids are on different devices");
+  const int64_t b = image.dim() == 4 ? image.size(0) : 1;
+  TORCH_CHECK((int64_t)view_ids.size() == b, fn, ": one view id per image");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(grids.data_ptr()) % 16 == 0, fn, ": grids must be 16-byte aligned");
+  std::vector<int> ids;
+  for (int64_t v : view_ids) {
+    TORCH_CHECK(v >= 0 && v < grids.size(0), fn, ": view id ", v, " outside [0, ", grids.size(0), ")");
+    ids.push_back((int)v);
+  }
+  return ids;
+}
+
+torch::Tensor bilagrid_slice(torch::Tensor image, torch::Tensor grids, std::vector<int64_t> view_ids) {
+  auto ids = bilagrid_check("bilagrid_slice", image, grids, view_ids);
+  c10::cuda::CUDAGuard guard(image.device());
+  const int h = (int)image.size(-3), w = (int)image.size(-2);
+  auto out = torch::empty_like(image);
+  check_rc(gs_bilagrid_slice_fwd(fp(image), fp(grids), ids.data(), (int)ids.size(), h, w, (int)grids.size(0),
+                                 (int)grids.size(1), (int)grids.size(2), (int)grids.size(3), fpm(out), cur_stream()),
+           "gs_bilagrid_slice_fwd");
+  return out;
+}
+
+// returns (grad_image or an undefined tensor, grad_grids [V, GH, GW, GL, 12] with the rows of views outside the batch
+// zero, or an undefined tensor)
+std::tuple<torch::Tensor, torch::Tensor> bilagrid_slice_backward(torch::Tensor image, torch::Tensor grids,
+                                                                 std::vector<int64_t> view_ids, torch::Tensor grad_out,
+                                                                 bool want_image, bool want_grids) {
+  auto ids = bilagrid_check("bilagrid_slice_backward", image, grids, view_ids);
+  GS_CHECK_F32(grad_out);
+  TORCH_CHECK(grad_out.sizes() == image.sizes() && grad_out.device() == image.device(),
+              "bilagrid_slice_backward: grad_out must match image");
+  c10::cuda::CUDAGuard guard(image.device());
+  const int b = (int)ids.size(), h = (int)image.size(-3), w = (int)image.size(-2);
+  const int v = (int)grids.size(0), gh = (int)grids.size(1), gw = (int)grids.size(2), gl = (int)grids.size(3);
+  torch::Tensor gi = want_image ? torch::empty_like(image) : torch::Tensor();
+  torch::Tensor gg = want_grids ? torch::zeros_like(grids) : torch::Tensor();
+  if (!want_image && !want_grids) return {gi, gg};
+  auto ws = torch::empty({(int64_t)std::max<size_t>(gs_bilagrid_workspace_bytes(b, h, w, v, gh, gw, gl), 1)},
+                         image.options().dtype(at::kByte));
+  check_rc(gs_bilagrid_slice_bwd(fp(image), fp(grids), ids.data(), b, h, w, v, gh, gw, gl, fp(grad_out),
+                                 want_image ? fpm(gi) : nullptr, want_grids ? fpm(gg) : nullptr, ws.data_ptr(),
+                                 (size_t)ws.numel(), cur_stream()),
+           "gs_bilagrid_slice_bwd");
+  return {gi, gg};
+}
+
 // the apply half of densify / densify_stats: reads the plan's totals (the one host sync), draws the split samples and
 // writes the five new parameter tensors; returns them + (n_deleted, n_clone, n_split)
 static std::tuple<std::vector<torch::Tensor>, std::vector<int64_t>> densify_apply(
@@ -1414,6 +1468,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("pos"), py::arg("size"), py::arg("focal"), py::arg("rot"), py::arg("tran"), py::arg("near"),
         py::arg("margin") = 0.15, py::arg("variance") = 0.2, py::arg("out") = py::none());
   m.def("loss_l1_ssim", &loss_l1_ssim, "fused L1 + SSIM loss, forward + image gradient (CUDA)");
+  m.def("bilagrid_slice", &bilagrid_slice, "slice images through their views' bilateral grids (gs_bilagrid_slice_fwd)",
+        py::arg("image"), py::arg("grids"), py::arg("view_ids"));
+  m.def("bilagrid_slice_backward", &bilagrid_slice_backward,
+        "image and grid gradients of bilagrid_slice (gs_bilagrid_slice_bwd, deterministic)", py::arg("image"),
+        py::arg("grids"), py::arg("view_ids"), py::arg("grad_out"), py::arg("want_image") = true,
+        py::arg("want_grids") = true);
   m.def("adam_step", &adam_step, "fused Adam over flat parameter / gradient buffers (CUDA)");
   m.def("adam_step_visible", &adam_step_visible,
         "Adam over the rows of the visible Gaussians of flat parameter / gradient buffers (CUDA)");

@@ -79,3 +79,18 @@ def make_grad_output(height: int, width: int, seed: int = 0):
     """Upstream gradient of the (cropped) image: U(-1,1)/P, generator seeded seed+1."""
     g = torch.Generator("cpu").manual_seed(seed + 1)
     return ((torch.rand(height, width, 3, generator=g) * 2 - 1) / float(height * width)).float()
+
+
+def appearance_jitter(images, strength: float, seed: int = 0):
+    """Per-view photometric differences of strength S, as a camera that sets exposure and white balance per shot
+    would make them: image k becomes clamp(e_k * wb_k * x, 0, 1) ** gamma_k with log e_k ~ N(0, (0.5 S)^2),
+    log wb_k ~ N(0, (0.2 S)^2) per channel and log gamma_k ~ N(0, (0.3 S)^2), drawn from one CPU generator seeded
+    `seed` in view order.  images: list of [H, W, 3] tensors; returns a new list."""
+    g = torch.Generator("cpu").manual_seed(seed)
+    out = []
+    for x in images:
+        e = math.exp(0.5 * strength * float(torch.randn(1, generator=g)))
+        wb = torch.exp(0.2 * strength * torch.randn(3, generator=g))
+        gamma = math.exp(0.3 * strength * float(torch.randn(1, generator=g)))
+        out.append((x * (e * wb).to(x.device, x.dtype)).clamp(0.0, 1.0) ** gamma)
+    return out

@@ -9,9 +9,11 @@ rank renders a different view and the gradients are all-reduced (one flat bucket
   python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_dp.py ...
   python examples/train_dp.py --surfel --lambda-normal 0.05 --lambda-dist 100    # 2D Gaussian Splatting
   python examples/train_dp.py --prune-at 100 --prune-keep 0.5     # keep the half that blends the most weight
+  python examples/train_dp.py --bilagrid --appearance-jitter 0.3  # per-view bilateral grids on jittered views
 
 Ground truth = renders of a "teacher" Gaussian set; the student starts from perturbed positions,
-grey colours and low opacity.  Prints loss / PSNR and iterations per second.
+grey colours and low opacity.  Prints loss / PSNR and iterations per second, and the colour-corrected PSNR of the
+final renders against the clean teacher renders.
 """
 import argparse
 import os
@@ -23,6 +25,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "3d-gaussian-splatting_b200"))
 
+import bilagrid  # noqa: E402
 import dp  # noqa: E402
 import loss as L  # noqa: E402
 import optim  # noqa: E402
@@ -55,9 +58,23 @@ def make_optimizer(sp, lr=0.003, fused=True):
         {"params": g.scale, "lr": lr}, {"params": g.quat, "lr": lr}], betas=(0.9, 0.99))
 
 
+def cc_psnr(sp, clean):
+    """Mean over the views of the PSNR of the raw render (no grid) after a least-squares colour fit to the clean
+    teacher render: the evaluation metric of appearance-corrected training."""
+    with torch.no_grad():
+        vals = []
+        for k, gt in enumerate(clean):
+            mse = ((bilagrid.color_correct(sp(k), gt) - gt) ** 2).mean()
+            vals.append(float(-10 * torch.log10(mse + 1e-12)))
+    return sum(vals) / len(vals)
+
+
 def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, visible_adam=False, cap_max=None,
-          filter3d_every=0, lambda_normal=0.0, lambda_dist=0.0, prune_at=None, prune_keep=1.0):
+          filter3d_every=0, lambda_normal=0.0, lambda_dist=0.0, prune_at=None, prune_keep=1.0, bilagrid_module=None,
+          bilagrid_lr=2e-3, bilagrid_tv=10.0):
     opt = make_optimizer(sp, lr, fused_adam)
+    bg = bilagrid_module                                              # per-view appearance grids, their own Adam
+    bg_opt = torch.optim.Adam(bg.parameters(), lr=bilagrid_lr, eps=1e-15) if bg is not None else None
     params = list(sp.gaussian_3ds.parameters())
     surfel = sp.primitive == "surfel"
     # peer-memory exchange when available, else NCCL; surfel frames have no gradient push, so they all-reduce
@@ -73,19 +90,28 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
     for it in range(iters):
         opt.zero_grad(set_to_none=True)
         view = dp.view_for_rank(it, rank, world, len(gts))
+        if bg is not None:
+            bg_opt.zero_grad(set_to_none=True)
         if maps:                                                      # 2DGS: L1 + normal consistency + distortion
             out = sp.render_surfel_maps(view)
-            img = out["image"]
+            img = out["image"] if bg is None else bg(out["image"], view)
             v = sp.current_view
             loss = ((img - gts[view]).abs().mean()
                     + lambda_normal * L.surfel_normal_consistency(out["normal"], out["depth"], out["alpha"],
                                                                   v["focal_x"], v["focal_y"])
                     + lambda_dist * out["distortion"].mean())
         else:
-            img = sp(view)
+            img = sp(view) if bg is None else bg(sp(view), view)
             loss = (img - gts[view]).abs().mean()                    # train.py:99
+        l1 = loss.detach()
+        if bg is not None:
+            loss = loss + bilagrid_tv * bg.tv_loss([view])
         loss.backward()
         bucket.allreduce()
+        if bg is not None:
+            if world > 1:                                             # every view's row comes from one rank: SUM
+                bg.all_reduce_grad([dp.view_for_rank(it, r, world, len(gts)) for r in range(world)])
+            bg_opt.step()
         if mc is not None:                                            # after the exchange: every rank adds the same
             mc.after_backward(it)
         if visible_adam:                                              # step only the Gaussians some rank binned
@@ -111,9 +137,9 @@ def train(sp, gts, iters, world, rank, log_every=50, lr=0.003, fused_adam=True, 
             with torch.no_grad():
                 mse = ((img - gts[view]) ** 2).mean()
                 psnr = float(-10 * torch.log10(mse + 1e-12))
-            hist.append((it, float(loss), psnr))
+            hist.append((it, float(l1), psnr))
             if rank == 0:
-                print(f"iter {it:5d}  L1 {float(loss):.5f}  PSNR {psnr:6.2f} dB  view {view}  "
+                print(f"iter {it:5d}  L1 {float(l1):.5f}  PSNR {psnr:6.2f} dB  view {view}  "
                       f"n {sp.gaussian_3ds.pos.shape[0]}", flush=True)
     torch.cuda.synchronize()
     return hist, iters / (time.time() - t0)
@@ -145,6 +171,14 @@ def main():
                          "--prune-keep fraction of the Gaussians with the largest summed blend weight "
                          "(Splatter.score_views / prune)")
     ap.add_argument("--prune-keep", type=float, default=0.5, help="--prune-at: fraction of the Gaussians kept")
+    ap.add_argument("--bilagrid", action="store_true",
+                    help="one bilateral grid (16x16x8 affine colour transforms) per training view, sliced over the "
+                         "render before the loss and trained with its own Adam (bilagrid.BilateralGrids)")
+    ap.add_argument("--bilagrid-lr", type=float, default=2e-3, help="--bilagrid: learning rate of the grids")
+    ap.add_argument("--bilagrid-tv", type=float, default=10.0, help="--bilagrid: weight of the grids' total variation")
+    ap.add_argument("--appearance-jitter", type=float, default=0.0, metavar="S",
+                    help="give each ground-truth view a seeded exposure, white-balance gain and gamma of strength S "
+                         "(synthetic.appearance_jitter)")
     args = ap.parse_args()
     if args.prune_at is not None and args.surfel:
         ap.error("--prune-at scores 3-D Gaussian frames; it does not take --surfel")
@@ -169,14 +203,20 @@ def main():
     if args.surfel:
         kw = dict(primitive="surfel")
     sp, gts = build(args.gaussians, w, h, args.views, dev, student_kw=kw)
+    clean = gts
+    if args.appearance_jitter > 0:
+        gts = S.appearance_jitter(clean, args.appearance_jitter, seed=1)
+    bg = bilagrid.BilateralGrids(args.views, device=dev) if args.bilagrid else None
     hist, ips = train(sp, gts, args.iters, world, rank, fused_adam=not args.torch_adam,
                       visible_adam=args.visible_adam,
                       cap_max=(args.cap_max or int(1.5 * args.gaussians)) if args.mcmc else None,
                       filter3d_every=100 if args.filter3d else 0, lambda_normal=args.lambda_normal,
-                      lambda_dist=args.lambda_dist, prune_at=args.prune_at, prune_keep=args.prune_keep)
+                      lambda_dist=args.lambda_dist, prune_at=args.prune_at, prune_keep=args.prune_keep,
+                      bilagrid_module=bg, bilagrid_lr=args.bilagrid_lr, bilagrid_tv=args.bilagrid_tv)
     if rank == 0:
         print(f"done: {ips:.1f} it/s ({ips * world:.1f} views/s on {world} GPU), L1 {hist[0][1]:.5f} -> {hist[-1][1]:.5f}, "
-              f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians")
+              f"PSNR {hist[0][2]:.2f} -> {hist[-1][2]:.2f} dB, {sp.gaussian_3ds.pos.shape[0]} Gaussians, "
+              f"colour-corrected PSNR vs clean views {cc_psnr(sp, clean):.2f} dB")
     if world > 1:
         torch.distributed.destroy_process_group()
 

@@ -731,6 +731,46 @@ int gs_loss_l1_ssim(const float* image, const void* target, int target_is_half, 
                     size_t workspace_bytes, gs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Per-view bilateral grids for appearance correction (additive; Wang et al., "Bilateral Guided Radiance Field
+ * Processing", SIGGRAPH Asia 2024): a rendered image is "sliced" through its training view's grid of 3x4 affine colour
+ * transforms before the loss, so per-image exposure, white balance and tone end up in the grids, not in the scene.
+ *   grids     : DEVICE float32 [V, GH, GW, GL, 12], one row per training view, the 12 coefficients innermost (a node's
+ *               affine is three float4 loads: pointers 16-byte aligned).  Row-major affine A:
+ *               out_i = sum_j A[i][j] rgb_j + A[i][3].  grid_sample's [V, 12, GL, GH, GW] is grids.permute(0, 4, 3, 1, 2).
+ *               Identity initialisation: A = [I | 0] at every node.
+ *   image/out : DEVICE float32 [B, H, W, 3];  view_ids_host : HOST int[B] in [0, V), repeats allowed.
+ * Pixel (x, y) of image b samples row view_ids_host[b] at
+ *   gx = (x + 0.5) / W (GW - 1),  gy = (y + 0.5) / H (GH - 1),  gz = clamp(z, 0, 1) (GL - 1),
+ *   z  = fmaf(0.114f, b, fmaf(0.587f, g, 0.299f * r))   (fp32 luminance of the INPUT pixel)
+ * trilinearly with border clamping: value and gradients equal
+ *   grid_sample(grids_ncdhw[ids], coords * 2 - 1, mode="bilinear", align_corners=True, padding_mode="border")
+ * followed by the affine, including grid_sample's knot convention: dz is 0 at z <= 0 and z >= 1, and an interior knot
+ * takes the upper cell's slope.  The output is not clamped; inputs outside [0, 1] are accepted (only z is clamped).
+ * Bounds: 2 <= GH, GW <= GS_BILAGRID_MAX_HW; 2 <= GL <= GS_BILAGRID_MAX_L (the backward keeps one accumulator per
+ * z knot in registers); B <= 65535; H * W <= 2^30.
+ * gs_bilagrid_slice_fwd: one kernel launch per 64 images.
+ * gs_bilagrid_slice_bwd: from grad_out = dL/dout [B, H, W, 3] in one pass over the pixels,
+ *   grad_image (nullable) = dL/dimage, through the affine and through the guide z;
+ *   grad_grids (nullable) : the rows of the views in the batch are WRITTEN (repeated views' contributions added); the
+ *               other rows are left as they are (callers zero them).
+ * The grid gradient is bit-deterministic without floating-point atomics: per-CTA partials of one spatial cell, written
+ * once, then summed per node in index order (images of the view ascending, adjacent cells, row slices).  Two launches
+ * (one without grad_grids) after one that writes the view table into the workspace (one per 960 table entries; the
+ * table has at most 2B).  No allocation, no synchronisation.
+ * Refused before any launch (GS_ERR_INVALID_ARG, gs_last_error set): a null image, grids, view_ids_host, out / grad_out
+ * or workspace; B, H, W or V <= 0; a grid dimension outside the bounds; a view id outside [0, V); a workspace shorter
+ * than gs_bilagrid_workspace_bytes (0 for invalid shapes).  Nothing to compute (both gradients NULL) returns 0. */
+#define GS_BILAGRID_MAX_HW 256
+#define GS_BILAGRID_MAX_L 16
+size_t gs_bilagrid_workspace_bytes(int B, int H, int W, int V, int GH, int GW, int GL);
+int gs_bilagrid_slice_fwd(const float* image, const float* grids, const int* view_ids_host, int B, int H, int W,
+                          int V, int GH, int GW, int GL, float* out, gs_stream_t stream);
+int gs_bilagrid_slice_bwd(const float* image, const float* grids, const int* view_ids_host, int B, int H, int W,
+                          int V, int GH, int GW, int GL, const float* grad_out, float* grad_image /* nullable */,
+                          float* grad_grids /* nullable */, void* workspace, size_t workspace_bytes,
+                          gs_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * Multi-GPU exchange step (SURVEY.md §8e; new - the reference is single-GPU): in-place SUM of
  * the flat gradient bucket across `world` GPUs of one NVSwitch domain through an NVLS multicast
  * mapping.  `multicast_ptr` is the multicast address of a symmetric buffer holding each rank's

@@ -4,6 +4,8 @@
 #include "internal.h"
 #include "sh_common.cuh"
 
+#include <type_traits>
+
 namespace {
 
 constexpr int kBlock = 256;
@@ -55,195 +57,25 @@ __device__ __forceinline__ void sh_logits(const float* coef, const float* Y, flo
   }
 }
 
+// Gaussian i (loaded parameters p, q, s, opa_raw, rgb_raw) seen by one view: its record, rectangle, count and depth key
+// go to pair j (j = i in a single-view frame, v n + i for view v of a batched one) with the rectangle's rows offset by
+// ty_off (the view's first tile row).  Returns the instance count; vis: in the frustum.
 // KG = 0: colour from the rgb[n, 3] logits when d == 3 (per-pixel SH leaves it to the blend).  KG = 9 / 16: SH of
 // degree 2 / 3 evaluated once per Gaussian along view_dir (GS_SH_EVAL_GAUSSIAN); the record then carries an RGB colour.
-// F: the 2-D screen-space filter `filt` (gs_filter2d) is applied to the covariance before the tile rectangle and the
-// conic, and its compensation to l2o.
-// G3 (only with F): the 3-D smoothing filter f3d[n] (gs_filter3d) is applied to the activated scale first, and its
-// compensation added to l2o before the 2-D filter's.
-// L (only with F and G3): the lens `lens` (gs_lens_project) is applied to the projection before the 2-D filter; f3d may
-// be NULL (no 3-D filter: the f == 0 bits).
-// The batched frame's fused_project_one repeats this arithmetic: a change to it must be made to both.
-template <int KG, bool F = false, bool G3 = false, bool L = false>
-__device__ __forceinline__ void fused_project_body(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, const GsCam& cam,
-    const GsTileGrid& grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr,
-    GsLens lens = GsLens{}) {
-  static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
-  static_assert(!L || G3, "the lens runs in the 3-D filter's kernels");
-  int i = blockIdx.x * kBlock + threadIdx.x;
-  bool vis = false;
-  uint32_t cnt = 0;
-  if (i < n) {
-    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
-    float q[4], s[3], raw_s[3], qn;
-    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
-    float f3 = 0.f, dl2o3 = 0.f;
-    if constexpr (G3) {
-      float s0[3];
-      f3 = (L && !f3d) ? 0.f : f3d[i];
-      gs_filter3d(f3, s, s0, dl2o3);
-    }
-    // opacity and RGB logits are issued with the geometry, so that the thread makes one round trip to HBM, not two
-    // (a warp almost always has a binned Gaussian, so their sectors are fetched anyway)
-    const float opa_raw = opa[i];
-    float rgb_raw[3] = {0.f, 0.f, 0.f};
-    if (KG == 0 && d == 3) {
-      rgb_raw[0] = rgb[3 * i];
-      rgb_raw[1] = rgb[3 * i + 1];
-      rgb_raw[2] = rgb[3 * i + 2];
-    }
-    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
-    if constexpr (L) {
-      float J[4];
-      gs_lens_project(lens, o, half_w, half_h, J);
-    }
-    vis = o.visible;
-    if (mask) mask[i] = o.visible ? 1 : 0;
-    bool keep = o.visible;
-    float dl2o = 0.f;
-    if constexpr (F) {
-      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
-      o.a = fo.a;
-      o.d = fo.d;
-      dl2o = fo.dl2o;
-      keep = keep && fo.keep;
-    }
-    uint2 rc = make_uint2(0u, 0u);
-    if (keep) {
-      uint32_t tx0, tx1, ty0, ty1;
-      if (gs_tile_rect(grid, o.x, o.y, o.a, o.b, o.c, o.d, tx0, tx1, ty0, ty1)) {
-        cnt = (tx1 - tx0) * (ty1 - ty0);
-        rc = make_uint2(tx0 | (ty0 << 16), (tx1 - tx0) | ((ty1 - ty0) << 16));
-        GsConic k = gs_make_conic(o.a, o.b, o.c, o.d);
-        float op = gs_sigmoid(opa_raw);
-        GsRec* r = rec + i;
-        r->a = make_float4(o.x, o.y, k.ca, k.cb);
-        // RGB colour = sigmoid(logit) (splatter.py:539); per-pixel SH coefficients stay raw and are gathered
-        // from the parameter tensor by the pack pass
-        float cr = 0.f, cg = 0.f, cb = 0.f;
-        if constexpr (KG > 0) {
-          float coef[3 * KG], dir[3], il, Y[KG], l[3];
-#pragma unroll
-          for (int k = 0; k < 3 * KG; ++k) coef[k] = rgb[(size_t)i * (3 * KG) + k];
-          view_dir(cam, p, dir, il);
-          gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
-          sh_logits<KG>(coef, Y, l);
-          cr = gs_sigmoid(l[0]);
-          cg = gs_sigmoid(l[1]);
-          cb = gs_sigmoid(l[2]);
-        } else if (d == 3) {
-          cr = gs_sigmoid(rgb_raw[0]);
-          cg = gs_sigmoid(rgb_raw[1]);
-          cb = gs_sigmoid(rgb_raw[2]);
-        }
-        float l2o = log2f(op);
-        if constexpr (G3) {
-          if (f3 != 0.f) l2o += dl2o3;
-        }
-        r->b = make_float4(k.cc, F ? l2o + dl2o : l2o, cr, cg);
-        r->c = make_float4(cb, o.depth, __uint_as_float(rc.x), __uint_as_float(rc.y));
-        r->d = make_uint4(0u, 0u, 0u, 0u);   // whole 32-byte sectors: a half-written sector is a DRAM read-modify-write (ECC)
-      }
-    }
-    // the tile rectangle again, densely (zero without instances: whole sectors), for the instance emission: an 8-byte
-    // read from a 19 MB array at C3 instead of a 16-byte gather from the 154 MB records
-    rect[i] = rc;
-    count[i] = cnt;
-    // depth sort key: positive float bits order like the floats; Gaussians without instances last
-    dkey[i] = cnt ? __float_as_uint(o.depth) : 0xffffffffu;
-  }
-  // 64-bit instance total next to the visible count (counters[2..3]): the u32 scans that follow
-  // would wrap silently for M >= 2^32 (e.g. diverged scales: every Gaussian on every tile); the
-  // host sizes the frame from this total and refuses instead
-  __shared__ unsigned long long wsum[kBlock / 32];
-  unsigned long long c64 = cnt;
-#pragma unroll
-  for (int o = 16; o; o >>= 1) c64 += __shfl_xor_sync(0xffffffffu, c64, o);
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c64;
-  int nv = __syncthreads_count(vis);
-  if (threadIdx.x == 0) {
-    unsigned long long tot = 0;
-#pragma unroll
-    for (int w = 0; w < kBlock / 32; ++w) tot += wsum[w];
-    if (nv) atomicAdd(n_visible, (unsigned int)nv);
-    if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
-  }
-}
-
-__global__ void __launch_bounds__(kBlock) fused_project_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible) {
-  fused_project_body<0>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec, rect,
-                        count, dkey, mask, n_visible);
-}
-
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_sh_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible) {
-  fused_project_body<K>(pos, rgb, opa, quat, scale, n, 3 * K, scale_act, cam, grid, near_plane, half_w, half_h, rec,
-                        rect, count, dkey, mask, n_visible);
-}
-
-// with the 2-D filter: K = 0 is fused_project_kernel's colour rule, K = 9 / 16 fused_project_sh_kernel<K>'s
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_filt_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt) {
-  fused_project_body<K, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h, rec,
-                              rect, count, dkey, mask, n_visible, filt);
-}
-
-// with the 3-D filter f3d[n] and the 2-D filter `filt` (zero when the frame has none)
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_filt3_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt, const float* __restrict__ f3d) {
-  fused_project_body<K, true, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w, half_h,
-                                    rec, rect, count, dkey, mask, n_visible, filt, f3d);
-}
-
-// with a lens: the 2-D and 3-D filter paths unconditionally (zero filters, f3d NULL without one, give their bits)
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_lens_kernel(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
-    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
-    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, GsFilter2d filt, const float* __restrict__ f3d, GsLens lens) {
-  fused_project_body<K, true, true, true>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid, near_plane, half_w,
-                                          half_h, rec, rect, count, dkey, mask, n_visible, filt, f3d, lens);
-}
-
-// Batched frames.  Gaussian i (loaded parameters p, q, s, opa_raw, rgb_raw) seen by one view: the arithmetic of
-// fused_project_body, with its record, rectangle, count and depth key going to pair j = v n + i and the rectangle's
-// rows offset by ty_off (the view's first tile row).  Returns the instance count; vis: in the frustum.  (The
-// single-view kernels keep their own copy: routed through this function they compile to different SASS; a change
-// to the arithmetic of either copy must be made to both.)
-// G3: s is the 3-D filtered scale and dl2o3 its compensation (added to l2o when f3 != 0).  L: the view's lens *lens.
-template <int KG, bool F, bool G3 = false, bool L = false>
+// TIER (GsTier, cumulative):
+//   >= GS_TIER_FILT2D: the 2-D screen-space filter `filt` (gs_filter2d) is applied to the covariance before the tile
+//     rectangle and the conic, and its compensation to l2o.
+//   >= GS_TIER_FILT3D: s is the 3-D filtered scale (gs_filter3d) and dl2o3 its compensation, added to l2o before the
+//     2-D filter's when f3 != 0.
+//   GS_TIER_LENS: the lens *lens (gs_lens_project) is applied to the projection before the 2-D filter.
+template <int KG, int TIER>
 __device__ __forceinline__ uint32_t fused_project_one(
     const float* __restrict__ rgb, int i, int d, const GsCam& cam, const GsTileGrid& grid, float near_plane,
     float half_w, float half_h, const GsFilter2d& filt, const float p[3], const float q[4], const float s[3],
     float opa_raw, const float rgb_raw[3], uint32_t ty_off, int j, GsRec* __restrict__ rec, uint2* __restrict__ rect,
-    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis,
-    float f3 = 0.f, float dl2o3 = 0.f, const GsLens* __restrict__ lens = nullptr) {
+    uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask, bool& vis, float f3,
+    float dl2o3, const GsLens* __restrict__ lens) {
+  constexpr bool F = TIER >= GS_TIER_FILT2D, G3 = TIER >= GS_TIER_FILT3D, L = TIER == GS_TIER_LENS;
   uint32_t cnt = 0;
   {
     GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
@@ -309,30 +141,85 @@ __device__ __forceinline__ uint32_t fused_project_one(
   return cnt;
 }
 
-// Batched frame: one thread per Gaussian loads its parameters once and projects it into each view in turn, writing
-// pair j = v n + i with view v's constants (K, F as in fused_project_filt_kernel; F reads views[v].filt).  The
-// counters receive the frame's totals over the pairs.  G3: the 3-D filter f3d[n] is applied once, before the views.
-// L (only with F and G3): view v's lens lenses[v]; f3d may be NULL.
-template <int K, bool F, bool G3, bool L = false>
-__device__ __forceinline__ void fused_project_batch_body(
+// Gaussian i's parameters as the projection and its backward load them: position, normalised quaternion (and the raw
+// one's norm), activated scale s and raw scale.  TIER >= GS_TIER_FILT3D: s is 3-D filtered (f3, compensation dl2o3)
+// and s0 keeps the activated scale.  A lens frame without a 3-D filter passes f3d NULL (the f == 0 bits).
+template <int TIER>
+__device__ __forceinline__ void fused_project_load(const float* __restrict__ pos, const float* __restrict__ quat,
+                                                   const float* __restrict__ scale, const float* __restrict__ f3d,
+                                                   int i, int scale_act, float p[3], float q[4], float s[3],
+                                                   float raw_s[3], float& qn, float s0[3], float& f3, float& dl2o3) {
+  p[0] = pos[3 * i];
+  p[1] = pos[3 * i + 1];
+  p[2] = pos[3 * i + 2];
+  gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
+  f3 = 0.f;
+  dl2o3 = 0.f;
+  if constexpr (TIER >= GS_TIER_FILT3D) {
+    f3 = (TIER == GS_TIER_LENS && !f3d) ? 0.f : f3d[i];
+    gs_filter3d(f3, s, s0, dl2o3);
+  }
+}
+
+// Single-view frame: pair j = i.  The opacity and RGB logits are issued with the geometry, so that the thread makes one
+// round trip to HBM, not two (a warp almost always has a binned Gaussian, so their sectors are fetched anyway).
+template <int KG, int TIER>
+__global__ void __launch_bounds__(kBlock) fused_project_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int d, int scale_act, GsCam cam,
+    GsTileGrid grid, float near_plane, float half_w, float half_h, GsRec* __restrict__ rec,
+    uint2* __restrict__ rect, uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
+    unsigned int* __restrict__ n_visible, GsFilter2d filt, const float* __restrict__ f3d, GsLens lens) {
+  int i = blockIdx.x * kBlock + threadIdx.x;
+  bool vis = false;
+  uint32_t cnt = 0;
+  if (i < n) {
+    float p[3], q[4], s[3], raw_s[3], qn, s0[3], f3, dl2o3;
+    fused_project_load<TIER>(pos, quat, scale, f3d, i, scale_act, p, q, s, raw_s, qn, s0, f3, dl2o3);
+    const float opa_raw = opa[i];
+    float rgb_raw[3] = {0.f, 0.f, 0.f};
+    if (KG == 0 && d == 3) {
+      rgb_raw[0] = rgb[3 * i];
+      rgb_raw[1] = rgb[3 * i + 1];
+      rgb_raw[2] = rgb[3 * i + 2];
+    }
+    cnt = fused_project_one<KG, TIER>(rgb, i, d, cam, grid, near_plane, half_w, half_h, filt, p, q, s, opa_raw,
+                                      rgb_raw, 0u, i, rec, rect, count, dkey, mask, vis, f3, dl2o3, &lens);
+  }
+  // 64-bit instance total next to the visible count (counters[2..3]): the u32 scans that follow
+  // would wrap silently for M >= 2^32 (e.g. diverged scales: every Gaussian on every tile); the
+  // host sizes the frame from this total and refuses instead
+  __shared__ unsigned long long wsum[kBlock / 32];
+  unsigned long long c64 = cnt;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) c64 += __shfl_xor_sync(0xffffffffu, c64, o);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c64;
+  int nv = __syncthreads_count(vis);
+  if (threadIdx.x == 0) {
+    unsigned long long tot = 0;
+#pragma unroll
+    for (int w = 0; w < kBlock / 32; ++w) tot += wsum[w];
+    if (nv) atomicAdd(n_visible, (unsigned int)nv);
+    if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
+  }
+}
+
+// Batched frame: one thread per Gaussian loads its parameters once (the 3-D filter applied once, before the views) and
+// projects it into each view in turn, writing pair j = v n + i with view v's constants: camera, grid, filter
+// views[v].filt and lens lenses[v].  The counters receive the frame's totals over the pairs.
+template <int K, int TIER>
+__global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(
     const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
     const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,
     const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,
     uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,
-    unsigned int* __restrict__ n_visible, const float* __restrict__ f3d, const GsLens* __restrict__ lenses = nullptr) {
+    unsigned int* __restrict__ n_visible, const float* __restrict__ f3d, const GsLens* __restrict__ lenses) {
   const int i = blockIdx.x * kBlock + threadIdx.x;
   unsigned int nv = 0;
   unsigned long long c64 = 0;
   if (i < n) {
-    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
-    float q[4], s[3], raw_s[3], qn;
-    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
-    float f3 = 0.f, dl2o3 = 0.f;
-    if constexpr (G3) {
-      float s0[3];
-      f3 = (L && !f3d) ? 0.f : f3d[i];
-      gs_filter3d(f3, s, s0, dl2o3);
-    }
+    float p[3], q[4], s[3], raw_s[3], qn, s0[3], f3, dl2o3;
+    fused_project_load<TIER>(pos, quat, scale, f3d, i, scale_act, p, q, s, raw_s, qn, s0, f3, dl2o3);
     const float opa_raw = opa[i];
     float rgb_raw[3] = {0.f, 0.f, 0.f};
     if (K == 0 && d == 3) {
@@ -343,9 +230,9 @@ __device__ __forceinline__ void fused_project_batch_body(
     for (int v = 0; v < n_views; ++v) {
       const GsView vw = views[v];
       bool vis = false;
-      c64 += fused_project_one<K, F, G3, L>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p,
-                                            q, s, opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect,
-                                            count, dkey, mask, vis, f3, dl2o3, lenses + v);
+      c64 += fused_project_one<K, TIER>(rgb, i, d, vw.cam, vw.grid, near_plane, vw.half_w, vw.half_h, vw.filt, p, q,
+                                        s, opa_raw, rgb_raw, (uint32_t)(v * vw.grid.nty), v * n + i, rec, rect, count,
+                                        dkey, mask, vis, f3, dl2o3, lenses + v);
       nv += vis ? 1u : 0u;
     }
   }
@@ -373,34 +260,6 @@ __device__ __forceinline__ void fused_project_batch_body(
     if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(n_visible + 2), tot);
   }
 }
-
-#define GS_PBATCH_PARAMS                                                                                            \
-  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                     \
-      const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int d, int scale_act,   \
-      const GsView* __restrict__ views, float near_plane, GsRec* __restrict__ rec, uint2* __restrict__ rect,        \
-      uint32_t* __restrict__ count, uint32_t* __restrict__ dkey, int64_t* __restrict__ mask,                        \
-      unsigned int* __restrict__ n_visible
-#define GS_PBATCH_ARGS \
-  pos, rgb, opa, quat, scale, n, n_views, d, scale_act, views, near_plane, rec, rect, count, dkey, mask, n_visible
-
-template <int K, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_batch_kernel(GS_PBATCH_PARAMS) {
-  fused_project_batch_body<K, F, false>(GS_PBATCH_ARGS, nullptr);
-}
-
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_batch_filt3_kernel(GS_PBATCH_PARAMS,
-                                                                           const float* __restrict__ f3d) {
-  fused_project_batch_body<K, true, true>(GS_PBATCH_ARGS, f3d);
-}
-
-template <int K>
-__global__ void __launch_bounds__(kBlock) fused_project_batch_lens_kernel(GS_PBATCH_PARAMS,
-                                                                          const float* __restrict__ f3d,
-                                                                          const GsLens* __restrict__ lenses) {
-  fused_project_batch_body<K, true, true, true>(GS_PBATCH_ARGS, f3d, lenses);
-}
-#undef GS_PBATCH_PARAMS
 
 // Segment-sums the per-instance gradient records of each Gaussian (its instances occupy the
 // contiguous rows offsets_g[i] .. + count[i]) and chains them to the RAW parameters.  No
@@ -438,76 +297,37 @@ __device__ __forceinline__ void push_store(const GsGradPush& P, float* local, co
   }
 }
 
+// One view's share of Gaussian i's parameter gradients over its rows o0 .. o1 - 1 of grad_inst (GW floats each), with
+// the loaded parameters p, q, s, raw_s, qn, opa_raw and rgb_raw (D == 3) or coef (KG > 0): acc receives the row sums,
+// then gp, gq_raw, gs_raw, go and the colour gradients (acc + 6 for D == 3 and per-pixel SH, gsh for KG > 0) are formed.
 // DT: the blend backward stored dL/d|p_c| in the row's pad column 6 + DC (aux depth gradient); it enters as g_xyd[2]
 // and reaches pos through p_c / |p_c|.  Without it depth is only a sort key.
-// KG = 9 / 16: SH evaluated once per Gaussian (fused_project_body<KG>): the rows carry dL/d(colour) like RGB rows
+// KG = 9 / 16: SH evaluated once per Gaussian (fused_project_one<KG>): the rows carry dL/d(colour) like RGB rows
 // (GW = GS_GREC); the D = 3 KG coefficient gradients and the view-direction term are formed here.
-// (cam and push are taken by value, as the kernel parameters they are: by reference, the KG = 0 instantiations would
+// (cam and filt are taken by value, as the kernel parameters they are: by reference, the KG = 0 instantiations would
 // no longer compile to the code fused_project_bwd_kernel had before the body was shared.)
-// CG (camera gradient, W = 0 only): also adds this Gaussian's share of dL/d(rot, tran) to cg[12] (gs_cam_grad_add plus
-// the view-direction term of per-Gaussian SH); with all five gradient pointers NULL no parameter gradient is stored.
-// F: the forward applied the 2-D filter `filt` (fused_project_body<KG, true>): the conic is chained with the filtered
-// covariance, and the compensation's gradient is added to dL/dcov.
-// G3 (only with F): the forward applied the 3-D filter f3d[n] (fused_project_body<KG, true, true>): the projection is
-// differentiated at the filtered scale s', and dL/ds' is chained to dL/ds with the compensation's term
-// (gs_filter3d_backward) before the raw-scale chain.
-// L (only with G3, W = 0): the forward applied the lens `lens` (fused_project_body<KG, true, true, true>): the conic's
-// gradient is that of the lensed covariance, and gs_lens_backward takes the mean and covariance gradients back through
-// the lens before the projection backward; f3d may be NULL.
-// The batched frame's fused_project_bwd_one repeats this arithmetic: a change to it must be made to both.
-template <int D, int GW, int W, bool DT, int KG, bool CG = false, bool F = false, bool G3 = false, bool L = false>
-__device__ __forceinline__ void fused_project_bwd_body(
-    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
-    const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
-    float near_plane, float half_w, float half_h, const uint32_t* __restrict__ offsets_g,
-    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,
-    const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,
-    float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale,
-    GsGradPush push, float* cg = nullptr, GsFilter2d filt = GsFilter2d{}, const float* __restrict__ f3d = nullptr,
-    GsLens lens = GsLens{}) {
+// CG (camera gradient): also adds this view's share of dL/d(rot, tran) to cg[12] (gs_cam_grad_add plus the
+// view-direction term of per-Gaussian SH); the parameter gradients are the same bits either way.
+// TIER, the forward's (fused_project_one):
+//   >= GS_TIER_FILT2D: the conic is chained with the filtered covariance, and the compensation's gradient is added to
+//     dL/dcov.
+//   >= GS_TIER_FILT3D: s is the 3-D filtered scale s', s0 the activated one and f3 the filter: dL/ds' is chained to
+//     dL/ds with the compensation's term (gs_filter3d_backward) before the raw-scale chain.
+//   GS_TIER_LENS: the conic's gradient is that of the lensed covariance, and gs_lens_backward takes the mean and
+//     covariance gradients back through the lens `lens` before the projection backward.
+template <int D, int GW, bool DT, int KG, int TIER, bool CG>
+__device__ __forceinline__ void fused_project_bwd_one(
+    GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
+    const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
+    const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, const float (&s0)[3], float f3,
+    float opa_raw, const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GW],
+    float (&gsh)[KG ? D : 1], float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg,
+    const GsLens& lens) {
   static_assert(KG == 0 || (D == 3 * KG && GW == GS_GREC), "per-Gaussian SH: 3K coefficients, RGB gradient rows");
-  static_assert(!G3 || F, "the 3-D filter runs in the 2-D filter's kernels");
-  static_assert(!L || (G3 && W == 0), "the lens runs in the 3-D filter's kernels, without a push");
-  static_assert(!CG || (W == 0 && GW == GS_GREC), "camera gradient: RGB gradient rows, no push");
+  static_assert(!CG || GW == GS_GREC, "camera gradient: RGB gradient rows");
+  constexpr bool F = TIER >= GS_TIER_FILT2D, G3 = TIER >= GS_TIER_FILT3D, L = TIER == GS_TIER_LENS;
   constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
-  int i = blockIdx.x * kBlock + threadIdx.x;
-  // SH colour on one GPU: the warp writes its coefficient gradients together (below), so threads past n stay
-  constexpr bool kStagedRgb = (D != 3) && (W == 0);
-  const bool valid = i < n;
-  if (!valid && !kStagedRgb) return;
-  float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f};
-  float go = 0.f;
-  float acc[GW];
-#pragma unroll
-  for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-  float gsh[KG ? D : 1];                    // KG: coefficient gradients
-#pragma unroll
-  for (int k = 0; k < (KG ? D : 1); ++k) gsh[k] = 0.f;
-  const uint32_t cnt = valid ? count[i] : 0u;
-  const uint32_t o0 = valid ? offsets_g[i] : 0u;      // loaded with the count: one round trip, not two
-  if (cnt > 0) {
-    const uint32_t o1 = o0 + cnt;                      // this Gaussian's contiguous gradient rows
-    // issue the parameter loads BEFORE the row loop so that both round trips to HBM overlap
-    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
-    float q[4], s[3], raw_s[3], qn;
-    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
-    float f3 = 0.f, s0[3];
-    if constexpr (G3) {
-      float dl2o3;
-      f3 = (L && !f3d) ? 0.f : f3d[i];
-      gs_filter3d(f3, s, s0, dl2o3);
-    }
-    const float opa_raw = opa[i];
-    float rgb_raw[3] = {0.f, 0.f, 0.f};
-    float coef[KG ? D : 1];
-    if constexpr (KG > 0) {
-#pragma unroll
-      for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
-    } else if (D == 3) {
-      rgb_raw[0] = rgb[3 * i];
-      rgb_raw[1] = rgb[3 * i + 1];
-      rgb_raw[2] = rgb[3 * i + 2];
-    }
+  {
     // The rows are summed one by one in row order.  For an RGB frame the rows are loaded in groups: the tags of four
     // rows at once, then the live rows among them (48 registers of payload), so that a Gaussian with a few instances
     // waits for two round trips to HBM per group instead of two per row (H100, C3: 0.235 -> 0.230 ms).  Grouping only
@@ -651,283 +471,6 @@ __device__ __forceinline__ void fused_project_bwd_body(
       }
     }
   }
-  const float* gcol = KG ? gsh : acc + 6;   // the D gradients of this Gaussian's rgb row
-  if (CG && !g_pos) return;                 // camera only (the pointers are all NULL or all set: uniform)
-  if (W == 0) {
-    if constexpr (kStagedRgb) {
-      // The 32 Gaussians of a warp own 32 * D contiguous floats of g_rgb.  One strided 4-byte store per coefficient
-      // makes every store a partial-sector write (read-modify-write under ECC: 8x the bytes): the rows go through
-      // shared memory and leave as whole sectors.
-      // D = 48: two passes of 24 floats (96-byte, sector-aligned pieces); D = 27: the whole 32 x 108-byte span.
-      constexpr int HW = (D % 8 == 0) ? D / 2 : D;
-      __shared__ float stage[kBlock / 32][32][HW + 1];
-      const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-      const int i0 = blockIdx.x * kBlock + warp * 32;
-      const int nrow = min(32, n - i0);
-#pragma unroll
-      for (int pass = 0; pass < D / HW; ++pass) {
-        __syncwarp();
-#pragma unroll
-        for (int k = 0; k < HW; ++k) stage[warp][lane][k] = gcol[pass * HW + k];
-        __syncwarp();
-        if (HW == D) {
-          float* dst = g_rgb + (size_t)i0 * D;
-          for (int t = lane; t < nrow * D; t += 32) dst[t] = stage[warp][t / D][t % D];
-        } else {
-          for (int t = lane; t < nrow * HW; t += 32) {
-            const int g = t / HW, c = t % HW;
-            g_rgb[(size_t)(i0 + g) * D + pass * HW + c] = stage[warp][g][c];
-          }
-        }
-      }
-      if (!valid) return;
-    } else {
-#pragma unroll
-      for (int k = 0; k < D; ++k) g_rgb[(size_t)i * D + k] = gcol[k];
-    }
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      g_pos[3 * i + k] = gp[k];
-      g_scale[3 * i + k] = gs_raw[k];
-    }
-    reinterpret_cast<float4*>(g_quat)[i] = make_float4(gq_raw[0], gq_raw[1], gq_raw[2], gq_raw[3]);
-    g_opa[i] = go;
-  } else {
-    push_store<W, 3>(push, g_pos + 3 * (size_t)i, gp);
-    push_store<W, 3>(push, g_scale + 3 * (size_t)i, gs_raw);
-    push_store<W, D>(push, g_rgb + (size_t)i * D, gcol);
-    // a quaternion is 4 floats at a 16-byte aligned bucket offset and `per` is a multiple of 4:
-    // it never straddles two slices
-    *reinterpret_cast<float4*>(push_dst<W>(push, g_quat + 4 * (size_t)i, 1)) =
-        make_float4(gq_raw[0], gq_raw[1], gq_raw[2], gq_raw[3]);
-    push_store<W, 1>(push, g_opa + i, &go);
-  }
-}
-
-#define GS_PBWD_PARAMS                                                                                             \
-  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                      \
-      const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,             \
-      float near_plane, float half_w, float half_h, const uint32_t* __restrict__ offsets_g,                         \
-      const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,                                      \
-      const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos,                            \
-      float* __restrict__ g_rgb, float* __restrict__ g_opa, float* __restrict__ g_quat,                             \
-      float* __restrict__ g_scale, GsGradPush push
-#define GS_PBWD_ARGS                                                                                               \
-  pos, rgb, opa, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, offsets_g, count, grad_inst, row_epoch, \
-      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, push
-
-template <int D, int GW, int W, bool DT = false>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(GS_PBWD_PARAMS) {
-  fused_project_bwd_body<D, GW, W, DT, 0>(GS_PBWD_ARGS);
-}
-
-// per-Gaussian SH of K basis functions (fused_project_sh_kernel<K>)
-template <int K, int W, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_kernel(GS_PBWD_PARAMS) {
-  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K>(GS_PBWD_ARGS);
-}
-
-// the same two families for a forward that applied the 2-D filter
-template <int D, int GW, int W, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_filt_kernel(GS_PBWD_PARAMS, GsFilter2d filt) {
-  fused_project_bwd_body<D, GW, W, DT, 0, false, true>(GS_PBWD_ARGS, nullptr, filt);
-}
-
-template <int K, int W, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt_kernel(GS_PBWD_PARAMS, GsFilter2d filt) {
-  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true>(GS_PBWD_ARGS, nullptr, filt);
-}
-
-// and for a forward that applied the 3-D filter f3d[n] (with `filt`, zero when the frame had no 2-D filter)
-template <int D, int GW, int W, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_filt3_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
-                                                                         const float* __restrict__ f3d) {
-  fused_project_bwd_body<D, GW, W, DT, 0, false, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d);
-}
-
-template <int K, int W, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_sh_filt3_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
-                                                                            const float* __restrict__ f3d) {
-  fused_project_bwd_body<3 * K, GS_GREC, W, DT, K, false, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d);
-}
-
-// and for a forward with a lens (fused_project_lens_kernel<K>): K = 0 with the parameter width D (RGB or per-pixel SH
-// rows of width GW), K = 9 / 16 per-Gaussian SH; no push
-template <int D, int GW, int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_lens_kernel(GS_PBWD_PARAMS, GsFilter2d filt,
-                                                                        const float* __restrict__ f3d, GsLens lens) {
-  // per-pixel SH takes a principal point only (the host refuses a distortion): the lens map folds to the identity
-  if (K == 0 && D != 3) lens.model = GS_LENS_PINHOLE;
-  fused_project_bwd_body<D, GW, 0, DT, K, false, true, true, true>(GS_PBWD_ARGS, nullptr, filt, f3d, lens);
-}
-
-// Batched frames.  One view's share of Gaussian i's parameter gradients, the arithmetic of fused_project_bwd_body for
-// RGB gradient rows without a push or a camera gradient (rows o0 .. o1 - 1 of grad_inst, the loaded parameters p, q,
-// s, raw_s, qn, opa_raw, rgb_raw / coef): acc receives the row sums, then gp, gq_raw, gs_raw, go and the colour
-// gradients (acc + 6 for D == 3, gsh for KG > 0) are formed.  The single-view kernels keep their own copy (routed
-// through this function they compile to different SASS): a change to the arithmetic of either copy must be made to
-// both.  CG: also adds the view's camera terms to cg[12], as fused_project_bwd_body<..., CG = true> does (the parameter
-// gradients are the same bits either way).
-// G3: s is the 3-D filtered scale and f3 the filter; the activated scale is formed again from raw_s (as
-// gs_load_activated forms it) for gs_filter3d_backward, rather than kept live across the caller's view loop.
-// L: the view's lens `lens`, as in fused_project_bwd_body.
-template <int D, bool DT, int KG, bool F, bool CG = false, bool G3 = false, bool L = false>
-__device__ __forceinline__ void fused_project_bwd_one(
-    GsCam cam, float near_plane, float half_w, float half_h, GsFilter2d filt, int scale_act, uint32_t o0, uint32_t o1,
-    const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch, uint32_t epoch, const float (&p)[3],
-    const float (&q)[4], const float (&s)[3], const float (&raw_s)[3], float qn, float opa_raw,
-    const float (&rgb_raw)[3], const float (&coef)[KG ? D : 1], float (&acc)[GS_GREC], float (&gsh)[KG ? D : 1],
-    float (&gp)[3], float (&gq_raw)[4], float (&gs_raw)[3], float& go, float* cg = nullptr, float f3 = 0.f,
-    const GsLens& lens = GsLens{}) {
-  constexpr int GW = GS_GREC;
-  constexpr int DC = KG ? 3 : D;   // colour columns of a gradient row
-  {
-    float s0[3];
-    if constexpr (G3) {
-#pragma unroll
-      for (int k = 0; k < 3; ++k) s0[k] = (scale_act == GS_SCALE_ABS) ? (fabsf(raw_s[k]) + 1e-4f) : expf(raw_s[k]);
-    }
-    // The rows are summed one by one in row order.  For an RGB frame the rows are loaded in groups: the tags of four
-    // rows at once, then the live rows among them (48 registers of payload), so that a Gaussian with a few instances
-    // waits for two round trips to HBM per group instead of two per row (H100, C3: 0.235 -> 0.230 ms).  Grouping only
-    // the tags and loading the rows one at a time was slower (RGB 0.245 ms; per-pixel SH, D = 27: 0.496 -> 0.526 ms),
-    // and so was the grouped loop with per-Gaussian SH of degree 2 (80 -> 99 registers, 0.409 -> 0.464 ms): those
-    // kernels keep the plain loop.  An instance its (saturated) tile did not reach has a stale tag and contributes
-    // nothing.
-    if constexpr (KG > 0) {
-      for (uint32_t r = o0; r < o1; ++r) {
-        if (row_epoch[r] != epoch) continue;
-        const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)r * GW);
-#pragma unroll
-        for (int qq = 0; qq < GW / 4; ++qq) {
-          const float4 v = row[qq];
-          acc[4 * qq] += v.x;
-          acc[4 * qq + 1] += v.y;
-          acc[4 * qq + 2] += v.z;
-          acc[4 * qq + 3] += v.w;
-        }
-      }
-    } else {
-      constexpr int kGroup = 4;
-      for (uint32_t r0 = o0; r0 < o1; r0 += kGroup) {
-        bool live[kGroup];
-#pragma unroll
-        for (int j = 0; j < kGroup; ++j) live[j] = r0 + j < o1 && row_epoch[r0 + j] == epoch;
-        float4 v[kGroup][GW / 4];
-#pragma unroll
-        for (int j = 0; j < kGroup; ++j) {
-          const float4* row = reinterpret_cast<const float4*>(grad_inst + (size_t)(r0 + j) * GW);
-#pragma unroll
-          for (int qq = 0; qq < GW / 4; ++qq) v[j][qq] = live[j] ? row[qq] : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int j = 0; j < kGroup; ++j) {
-          if (!live[j]) continue;
-#pragma unroll
-          for (int qq = 0; qq < GW / 4; ++qq) {
-            acc[4 * qq] += v[j][qq].x;
-            acc[4 * qq + 1] += v[j][qq].y;
-            acc[4 * qq + 2] += v[j][qq].z;
-            acc[4 * qq + 3] += v[j][qq].w;
-          }
-        }
-      }
-    }
-    GsProj o = gs_project(cam, p, q, s, near_plane, L ? kInf : half_w, L ? kInf : half_h);
-    float J[4];                                                // L: the lens Jacobian
-    if constexpr (L) gs_lens_project(lens, o, half_w, half_h, J);
-    float fk[4];                                               // F: d l2o / d cov of the compensation
-    if constexpr (F) {
-      const GsFilter2dOut fo = gs_filter2d(filt, o.a, o.b, o.c, o.d);
-      o.a = fo.a;
-      o.d = fo.d;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) fk[j] = fo.k[j];
-    }
-    // conic (ca, cb, cc) = (d, b+c, a) * sc,  sc = log2e / (2 det + 1e-14)
-    float det = o.a * o.d - o.b * o.c;
-    double pn = 2.0 * (double)det + 1e-14;
-    float sc = (float)((double)GS_LOG2E / pn);
-    float kk = 2.f * sc * sc / GS_LOG2E;                      // d sc / d det = -kk
-    float gsc = acc[2] * o.d + acc[3] * (o.b + o.c) + acc[4] * o.a;
-    float gcov[4];
-    gcov[0] = acc[4] * sc - gsc * kk * o.d;                   // d det/da =  d
-    gcov[1] = acc[3] * sc + gsc * kk * o.c;                   // d det/db = -c
-    gcov[2] = acc[3] * sc + gsc * kk * o.b;                   // d det/dc = -b
-    gcov[3] = acc[2] * sc - gsc * kk * o.a;                   // d det/dd =  a
-    if constexpr (F) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) gcov[j] += acc[5] * fk[j];
-    }
-    static_assert(!DT || 6 + DC < GW, "no pad column for the depth gradient");
-    float gxyd[3] = {acc[0], acc[1], DT ? acc[6 + DC] : 0.f};   // without DT depth is only a sort key
-    if constexpr (L) gs_lens_backward(J, gxyd, gcov);
-    float gq[4], gsv[3];
-    if constexpr (CG) {
-      float gc[3], gjw[6];
-      gs_project_backward_cam(cam, p, q, s, gxyd, gcov, gp, gq, gsv, gc, gjw);
-      gs_cam_grad_add(cam, p, gc, gjw, cg);
-    } else {
-      gs_project_backward(cam, p, q, s, gxyd, gcov, gp, gq, gsv);
-    }
-    if constexpr (G3) gs_filter3d_backward(f3, s0, s, acc[5], gsv);
-    if constexpr (KG > 0) {
-      // c = sigmoid(l), l_c = sum_k Y_k(dir) coef[c*K + k]: dL/dcoef = g_l,c Y_k; dL/ddir = sum_k w_k dY_k/ddir with
-      // w_k = sum_c g_l,c coef[c*K + k]; ddir/dpos = (I - dir dir^T) / |pos - C|
-      float dir[3], il, Y[KG], l[3], gl[3], w[KG], gd[3];
-      view_dir(cam, p, dir, il);
-      gs_sh::sh_basis<KG>(dir[0], dir[1], dir[2], Y);
-      sh_logits<KG>(coef, Y, l);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const float sg = gs_sigmoid(l[c]);
-        gl[c] = acc[6 + c] * sg * (1.f - sg);
-      }
-#pragma unroll
-      for (int k = 0; k < KG; ++k) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) gsh[c * KG + k] = gl[c] * Y[k];
-        w[k] = gl[0] * coef[k] + gl[1] * coef[KG + k] + gl[2] * coef[2 * KG + k];
-      }
-      gs_sh::sh_basis_grad<KG>(dir[0], dir[1], dir[2], w, gd);
-      const float dd = dir[0] * gd[0] + dir[1] * gd[1] + dir[2] * gd[2];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) gp[j] += (gd[j] - dir[j] * dd) * il;
-      if constexpr (CG) {
-        // the direction term of fused_project_bwd_body, with il applied last for the same reason (gp keeps its bits)
-        float v[3];
-#pragma unroll
-        for (int j = 0; j < 3; ++j) v[j] = gd[j] - dir[j] * dd;
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-#pragma unroll
-          for (int j = 0; j < 3; ++j) cg[3 * r + j] += (cam.t[r] * v[j]) * il;
-          cg[9 + r] += (cam.r[3 * r] * v[0] + cam.r[3 * r + 1] * v[1] + cam.r[3 * r + 2] * v[2]) * il;
-        }
-      }
-    }
-    // quat normalisation backward: q = r/|r|
-    float dot = q[0] * gq[0] + q[1] * gq[1] + q[2] * gq[2] + q[3] * gq[3];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) gq_raw[k] = (gq[k] - q[k] * dot) / qn;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      if (scale_act == GS_SCALE_ABS)
-        gs_raw[k] = gsv[k] * (raw_s[k] > 0.f ? 1.f : (raw_s[k] < 0.f ? -1.f : 0.f));
-      else
-        gs_raw[k] = gsv[k] * expf(fminf(fmaxf(raw_s[k], -1.f), 1.f));   // renderer.py:98-100
-    }
-    float op = gs_sigmoid(opa_raw);
-    // l2o = log2(op):  d/d logit = d_l2o / (op ln2) * op (1-op) = d_l2o (1-op) / ln2
-    go = acc[5] * (1.f - op) / GS_LN2;
-    if (D == 3) {
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        float c = gs_sigmoid(rgb_raw[k]);
-        acc[6 + k] *= c * (1.f - c);
-      }
-    }
-  }
 }
 
 // The parameter gradients of Gaussian i to the caller's tensors (no push).  Per-Gaussian and per-pixel SH colour (D != 3)
@@ -979,115 +522,11 @@ __device__ __forceinline__ void fused_project_bwd_store(int i, int n, bool valid
   g_opa[i] = go;
 }
 
-// Batched frame: K = 0 RGB, 9 / 16 per-Gaussian SH; DT, F as above (F reads views[v].filt).  Thread i loads Gaussian
-// i's parameters once and takes its views in order: view v's share is fused_project_bwd_one over the rows of pair
-// v n + i with view v's camera, and the shares are added in view order with no contraction into their last products:
-// the sum of B single-view backwards accumulated in view order, to within the FMA contractions the compiler chooses
-// differently inside the view loop (measured: 1e-6 relative at most).
-// G3: the 3-D filter f3d[n] of the forward, applied once before the views.
-#define GS_PBWD_BATCH_PARAMS                                                                                          \
-  const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,                       \
-      const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,            \
-      const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,                     \
-      const uint32_t* __restrict__ count, const float* __restrict__ grad_inst,                                       \
-      const uint32_t* __restrict__ row_epoch, uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb,  \
-      float* __restrict__ g_opa, float* __restrict__ g_quat, float* __restrict__ g_scale
-#define GS_PBWD_BATCH_ARGS                                                                                          \
-  pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, epoch, \
-      g_pos, g_rgb, g_opa, g_quat, g_scale
-template <int K, bool DT, bool F, bool G3, bool L = false>
-__device__ __forceinline__ void fused_project_bwd_batch_body(GS_PBWD_BATCH_PARAMS, const float* __restrict__ f3d,
-                                                             const GsLens* __restrict__ lenses = nullptr) {
-  constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
-  const int i = blockIdx.x * kBlock + threadIdx.x;
-  const bool valid = i < n;
-  if (!valid && D == 3) return;   // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
-  float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f}, go = 0.f;
-  float gcol[D];
-#pragma unroll
-  for (int k = 0; k < D; ++k) gcol[k] = 0.f;
-  if (valid) {
-    float p[3] = {pos[3 * i], pos[3 * i + 1], pos[3 * i + 2]};
-    float q[4], s[3], raw_s[3], qn;
-    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
-    float f3 = 0.f;
-    if constexpr (G3) {
-      float s0[3], dl2o3;
-      f3 = (L && !f3d) ? 0.f : f3d[i];
-      gs_filter3d(f3, s, s0, dl2o3);
-    }
-    const float opa_raw = opa[i];
-    float rgb_raw[3] = {0.f, 0.f, 0.f};
-    float coef[K ? D : 1];
-    if constexpr (K > 0) {
-#pragma unroll
-      for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
-    } else {
-      rgb_raw[0] = rgb[3 * i];
-      rgb_raw[1] = rgb[3 * i + 1];
-      rgb_raw[2] = rgb[3 * i + 2];
-    }
-    for (int v = 0; v < n_views; ++v) {
-      const int j = v * n + i;
-      const uint32_t cnt = count[j], o0 = offsets_g[j];
-      if (cnt == 0) continue;
-      const GsView vw = views[v];
-      float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
-#pragma unroll
-      for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      if constexpr (L) {
-        const GsLens ln = lenses[v];
-        fused_project_bwd_one<D, DT, K, F, false, G3, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt,
-                                                            scale_act, o0, o0 + cnt, grad_inst, row_epoch, epoch, p, q,
-                                                            s, raw_s, qn, opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs,
-                                                            vo, nullptr, f3, ln);
-      } else {
-        fused_project_bwd_one<D, DT, K, F, false, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
-                                                      o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn,
-                                                      opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs, vo, nullptr, f3);
-      }
-      const float* vc = K ? gsh : acc + 6;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        gp[k] = __fadd_rn(gp[k], vp[k]);
-        gs_raw[k] = __fadd_rn(gs_raw[k], vs[k]);
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) gq_raw[k] = __fadd_rn(gq_raw[k], vq[k]);
-      go = __fadd_rn(go, vo);
-#pragma unroll
-      for (int k = 0; k < D; ++k) gcol[k] = __fadd_rn(gcol[k], vc[k]);
-    }
-  }
-  fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
-}
-
-template <int K, bool DT, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(GS_PBWD_BATCH_PARAMS) {
-  fused_project_bwd_batch_body<K, DT, F, false>(GS_PBWD_BATCH_ARGS, nullptr);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_filt3_kernel(GS_PBWD_BATCH_PARAMS,
-                                                                               const float* __restrict__ f3d) {
-  fused_project_bwd_batch_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, f3d);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_lens_kernel(GS_PBWD_BATCH_PARAMS,
-                                                                              const float* __restrict__ f3d,
-                                                                              const GsLens* __restrict__ lenses) {
-  fused_project_bwd_batch_body<K, DT, true, true, true>(GS_PBWD_BATCH_ARGS, f3d, lenses);
-}
-
-// Camera gradient (gs_render_backward_cam), K = 0: RGB, K = 9 / 16: per-Gaussian SH.  The CTA sums its threads'
-// 12-float shares in a fixed order (butterfly shuffles, then the 8 warp sums in warp order) into row blockIdx.x of
-// cam_part[gridDim.x][12]; cam_grad_finish_kernel adds the rows.  No atomics: the result is bit-deterministic.
-// F: with the 2-D filter of the forward (fused_project_bwd_cam_filt_kernel).
+// Camera gradient: the CTA sums its threads' 12-float shares in a fixed order (butterfly shuffles, then the 8 warp sums
+// in warp order) into row[12]; cam_grad_finish_kernel adds the rows.  No atomics: the result is bit-deterministic.  Every
+// thread of the CTA calls it.
 constexpr int kCamGrad = 12;
 
-// The CTA's sum of its threads' cg[12] into row[12], in fused_project_bwd_cam_body's order (that kernel keeps its own
-// copy: routed through this function it compiles to different SASS).  Every thread of the CTA calls it.
 __device__ __forceinline__ void cam_grad_cta_sum(float (&cg)[kCamGrad], float (&wsum)[kBlock / 32][kCamGrad],
                                                  float* __restrict__ row) {
 #pragma unroll
@@ -1108,91 +547,118 @@ __device__ __forceinline__ void cam_grad_cta_sum(float (&cg)[kCamGrad], float (&
   }
 }
 
-template <int K, bool DT, bool F, bool G3 = false, bool L = false>
-__device__ __forceinline__ void fused_project_bwd_cam_body(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                           GsFilter2d filt, const float* __restrict__ f3d = nullptr,
-                                                           GsLens lens = GsLens{}) {
+// Single-view frame: fused_project_bwd_one over Gaussian i's rows.  (KG, D, GW): RGB (0, 3, 12), per-pixel SH
+// (0, 27 / 48, 36 / 56), per-Gaussian SH (9 / 16, 27 / 48, 12).  W == 0: the gradients go to the caller's tensors
+// (fused_project_bwd_store); W > 0: through the data-parallel push (push_store).  TIER: the forward's; a lens frame has
+// no push.
+// CG (camera gradient, gs_render_backward_cam; W = 0, RGB rows): the CTA's sum of its Gaussians' camera terms goes to
+// row blockIdx.x of cam_part[gridDim.x][12]; with all five gradient pointers NULL no parameter gradient is stored.
+template <int KG, int D, int GW, int W, bool DT, int TIER, bool CG>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int scale_act, GsCam cam,
+    float near_plane, float half_w, float half_h, const uint32_t* __restrict__ offsets_g,
+    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
+    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
+    float* __restrict__ g_quat, float* __restrict__ g_scale, GsGradPush push, GsFilter2d filt,
+    const float* __restrict__ f3d, GsLens lens, float* __restrict__ cam_part) {
+  static_assert(TIER != GS_TIER_LENS || W == 0, "the lens runs without a push");
+  static_assert(!CG || W == 0, "camera gradient: no push");
+  // per-pixel SH takes a principal point only (the host refuses a distortion): the lens map folds to the identity
+  if constexpr (KG == 0 && D != 3) lens.model = GS_LENS_PINHOLE;
+  const int i = blockIdx.x * kBlock + threadIdx.x;
+  const bool valid = i < n;
   float cg[kCamGrad];
 #pragma unroll
   for (int k = 0; k < kCamGrad; ++k) cg[k] = 0.f;
-  fused_project_bwd_body<K ? 3 * K : 3, GS_GREC, 0, DT, K, true, F, G3, L>(GS_PBWD_ARGS, cg, filt, f3d, lens);
-  __shared__ float wsum[kBlock / 32][kCamGrad];
+  // SH colour on one GPU: the warp writes its coefficient gradients together (fused_project_bwd_store), so threads past
+  // n stay
+  if (valid || (D != 3 && W == 0)) {
+    float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f};
+    float go = 0.f;
+    float acc[GW];
 #pragma unroll
-  for (int k = 0; k < kCamGrad; ++k) {
+    for (int k = 0; k < GW; ++k) acc[k] = 0.f;
+    float gsh[KG ? D : 1];                    // KG: coefficient gradients
 #pragma unroll
-    for (int o = 16; o; o >>= 1) cg[k] += __shfl_xor_sync(0xffffffffu, cg[k], o);
+    for (int k = 0; k < (KG ? D : 1); ++k) gsh[k] = 0.f;
+    const uint32_t cnt = valid ? count[i] : 0u;
+    const uint32_t o0 = valid ? offsets_g[i] : 0u;      // loaded with the count: one round trip, not two
+    if (cnt > 0) {
+      // issue the parameter loads BEFORE the row loop so that both round trips to HBM overlap
+      float p[3], q[4], s[3], raw_s[3], qn, s0[3], f3, dl2o3;
+      fused_project_load<TIER>(pos, quat, scale, f3d, i, scale_act, p, q, s, raw_s, qn, s0, f3, dl2o3);
+      const float opa_raw = opa[i];
+      float rgb_raw[3] = {0.f, 0.f, 0.f};
+      float coef[KG ? D : 1];
+      if constexpr (KG > 0) {
+#pragma unroll
+        for (int k = 0; k < D; ++k) coef[k] = rgb[(size_t)i * D + k];
+      } else if (D == 3) {
+        rgb_raw[0] = rgb[3 * i];
+        rgb_raw[1] = rgb[3 * i + 1];
+        rgb_raw[2] = rgb[3 * i + 2];
+      }
+      fused_project_bwd_one<D, GW, DT, KG, TIER, CG>(cam, near_plane, half_w, half_h, filt, scale_act, o0, o0 + cnt,
+                                                     grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, s0, f3, opa_raw,
+                                                     rgb_raw, coef, acc, gsh, gp, gq_raw, gs_raw, go, cg, lens);
+    }
+    const float* gcol = KG ? gsh : acc + 6;   // the D gradients of this Gaussian's rgb row
+    if (!CG || g_pos) {                       // camera only: the pointers are all NULL or all set (uniform)
+      if constexpr (W == 0) {
+        fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
+      } else {
+        push_store<W, 3>(push, g_pos + 3 * (size_t)i, gp);
+        push_store<W, 3>(push, g_scale + 3 * (size_t)i, gs_raw);
+        push_store<W, D>(push, g_rgb + (size_t)i * D, gcol);
+        // a quaternion is 4 floats at a 16-byte aligned bucket offset and `per` is a multiple of 4:
+        // it never straddles two slices
+        *reinterpret_cast<float4*>(push_dst<W>(push, g_quat + 4 * (size_t)i, 1)) =
+            make_float4(gq_raw[0], gq_raw[1], gq_raw[2], gq_raw[3]);
+        push_store<W, 1>(push, g_opa + i, &go);
+      }
+    }
   }
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < kCamGrad; ++k) wsum[threadIdx.x >> 5][k] = cg[k];
-  }
-  __syncthreads();
-  if (threadIdx.x < kCamGrad) {
-    float s = 0.f;
-#pragma unroll
-    for (int w = 0; w < kBlock / 32; ++w) s += wsum[w][threadIdx.x];
-    cam_part[(size_t)blockIdx.x * kCamGrad + threadIdx.x] = s;
+  if constexpr (CG) {
+    __shared__ float wsum[kBlock / 32][kCamGrad];
+    cam_grad_cta_sum(cg, wsum, cam_part + (size_t)blockIdx.x * kCamGrad);
   }
 }
 
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part) {
-  fused_project_bwd_cam_body<K, DT, false>(GS_PBWD_ARGS, cam_part, GsFilter2d{});
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                                            GsFilter2d filt) {
-  fused_project_bwd_cam_body<K, DT, true>(GS_PBWD_ARGS, cam_part, filt);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_filt3_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                                             GsFilter2d filt,
-                                                                             const float* __restrict__ f3d) {
-  fused_project_bwd_cam_body<K, DT, true, true>(GS_PBWD_ARGS, cam_part, filt, f3d);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_cam_lens_kernel(GS_PBWD_PARAMS, float* __restrict__ cam_part,
-                                                                            GsFilter2d filt,
-                                                                            const float* __restrict__ f3d, GsLens lens) {
-  fused_project_bwd_cam_body<K, DT, true, true, true>(GS_PBWD_ARGS, cam_part, filt, f3d, lens);
-}
-
-// Camera gradients of a batched frame (gs_render_backward_batch_cam): fused_project_bwd_batch_kernel's parameter
-// gradients, the same bits, plus the camera terms of each view with that view's camera, filter and SH direction.  Per
-// view v the CTA sums its threads' terms in fused_project_bwd_cam_body's order into row blockIdx.x of
-// cam_part[v][gridDim.x][12].  The view loop and the sums are uniform across the CTA: threads past n and Gaussians
-// without a row in view v take part with zeros, and a CTA without a row in view v stores a zero row (the bits the
-// shuffles would give) without reducing.  With the five gradient pointers NULL only cam_part is written.
-template <int K, bool DT, bool F, bool G3, bool L = false>
-__device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_PARAMS, float* __restrict__ cam_part,
-                                                                 const float* __restrict__ f3d,
-                                                                 const GsLens* __restrict__ lenses = nullptr) {
+// Batched frame: K = 0 RGB, 9 / 16 per-Gaussian SH; DT and TIER as above (views[v].filt, lenses[v]).  Thread i loads
+// Gaussian i's parameters once and takes its views in order: view v's share is fused_project_bwd_one over the rows of
+// pair v n + i with view v's camera, and the shares are added in view order with no contraction into their last
+// products: the sum of B single-view backwards accumulated in view order, to within the FMA contractions the compiler
+// chooses differently inside the view loop (measured: 1e-6 relative at most).
+// CG (gs_render_backward_batch_cam): also the camera terms of each view, summed per view v by the CTA in
+// cam_grad_cta_sum's order into row blockIdx.x of cam_part[v][gridDim.x][12].  The view loop and the sums are then
+// uniform across the CTA: threads past n and Gaussians without a row in view v take part with zeros, and a CTA without
+// a row in view v stores a zero row (the bits the shuffles would give) without reducing.  With the five gradient
+// pointers NULL only cam_part is written.
+template <int K, bool DT, int TIER, bool CG>
+__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_kernel(
+    const float* __restrict__ pos, const float* __restrict__ rgb, const float* __restrict__ opa,
+    const float* __restrict__ quat, const float* __restrict__ scale, int n, int n_views, int scale_act,
+    const GsView* __restrict__ views, float near_plane, const uint32_t* __restrict__ offsets_g,
+    const uint32_t* __restrict__ count, const float* __restrict__ grad_inst, const uint32_t* __restrict__ row_epoch,
+    uint32_t epoch, float* __restrict__ g_pos, float* __restrict__ g_rgb, float* __restrict__ g_opa,
+    float* __restrict__ g_quat, float* __restrict__ g_scale, const float* __restrict__ f3d,
+    const GsLens* __restrict__ lenses, float* __restrict__ cam_part) {
   constexpr int D = K ? 3 * K : 3, GW = GS_GREC;
   const int i = blockIdx.x * kBlock + threadIdx.x;
   const bool valid = i < n;
+  if (!CG && !valid && D == 3) return;   // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
   float gp[3] = {0.f, 0.f, 0.f}, gq_raw[4] = {0.f, 0.f, 0.f, 0.f}, gs_raw[3] = {0.f, 0.f, 0.f}, go = 0.f;
   float gcol[D];
 #pragma unroll
   for (int k = 0; k < D; ++k) gcol[k] = 0.f;
   float p[3] = {0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f}, s[3] = {0.f, 0.f, 0.f}, raw_s[3] = {0.f, 0.f, 0.f};
-  float qn = 1.f, opa_raw = 0.f, rgb_raw[3] = {0.f, 0.f, 0.f};
-  float f3 = 0.f;
+  float qn = 1.f, s_act[3], f3 = 0.f, dl2o3, opa_raw = 0.f, rgb_raw[3] = {0.f, 0.f, 0.f};
   float coef[K ? D : 1];
 #pragma unroll
   for (int k = 0; k < (K ? D : 1); ++k) coef[k] = 0.f;
   if (valid) {
-    p[0] = pos[3 * i];
-    p[1] = pos[3 * i + 1];
-    p[2] = pos[3 * i + 2];
-    gs_load_activated(quat, scale, i, scale_act, q, s, raw_s, qn);
-    if constexpr (G3) {
-      float s0[3], dl2o3;
-      f3 = (L && !f3d) ? 0.f : f3d[i];
-      gs_filter3d(f3, s, s0, dl2o3);
-    }
+    fused_project_load<TIER>(pos, quat, scale, f3d, i, scale_act, p, q, s, raw_s, qn, s_act, f3, dl2o3);
     opa_raw = opa[i];
     if constexpr (K > 0) {
 #pragma unroll
@@ -1213,19 +679,20 @@ __device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_P
     if (cnt > 0) {
       const uint32_t o0 = offsets_g[j];
       const GsView vw = views[v];
+      const GsLens ln = TIER == GS_TIER_LENS ? lenses[v] : GsLens{};
+      // the activated scale, formed again from raw_s in each view (gs_load_activated's expression: the same bits):
+      // kept live across the view loop instead, it costs 3-25 registers and a CTA per SM in the RGB kernels
+      float s0[3];
+      if constexpr (TIER >= GS_TIER_FILT3D) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) s0[k] = (scale_act == GS_SCALE_ABS) ? (fabsf(raw_s[k]) + 1e-4f) : expf(raw_s[k]);
+      }
       float acc[GW], gsh[K ? D : 1], vp[3], vq[4], vs[3], vo = 0.f;
 #pragma unroll
       for (int k = 0; k < GW; ++k) acc[k] = 0.f;
-      if constexpr (L) {
-        const GsLens ln = lenses[v];
-        fused_project_bwd_one<D, DT, K, F, true, G3, true>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act,
-                                                           o0, o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn,
-                                                           opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3, ln);
-      } else {
-        fused_project_bwd_one<D, DT, K, F, true, G3>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
-                                                     o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, opa_raw,
-                                                     rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, f3);
-      }
+      fused_project_bwd_one<D, GW, DT, K, TIER, CG>(vw.cam, near_plane, vw.half_w, vw.half_h, vw.filt, scale_act, o0,
+                                                    o0 + cnt, grad_inst, row_epoch, epoch, p, q, s, raw_s, qn, s0, f3,
+                                                    opa_raw, rgb_raw, coef, acc, gsh, vp, vq, vs, vo, cg, ln);
       const float* vc = K ? gsh : acc + 6;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
@@ -1238,41 +705,20 @@ __device__ __forceinline__ void fused_project_bwd_batch_cam_body(GS_PBWD_BATCH_P
 #pragma unroll
       for (int k = 0; k < D; ++k) gcol[k] = __fadd_rn(gcol[k], vc[k]);
     }
-    float* row = cam_part + ((size_t)v * gridDim.x + blockIdx.x) * kCamGrad;
-    // the barrier also keeps the previous view's readers of wsum ahead of this view's writers
-    if (__syncthreads_or(cnt > 0)) {
-      cam_grad_cta_sum(cg, wsum, row);
-    } else if (threadIdx.x < kCamGrad) {
-      row[threadIdx.x] = 0.f;
+    if constexpr (CG) {
+      float* row = cam_part + ((size_t)v * gridDim.x + blockIdx.x) * kCamGrad;
+      // the barrier also keeps the previous view's readers of wsum ahead of this view's writers
+      if (__syncthreads_or(cnt > 0)) {
+        cam_grad_cta_sum(cg, wsum, row);
+      } else if (threadIdx.x < kCamGrad) {
+        row[threadIdx.x] = 0.f;
+      }
     }
   }
-  if (!g_pos) return;                    // camera only (the pointers are all NULL or all set: uniform)
+  if (CG && !g_pos) return;              // camera only (the pointers are all NULL or all set: uniform)
   if (!valid && D == 3) return;          // SH: the whole warp stages its coefficient rows (fused_project_bwd_store)
   fused_project_bwd_store<D>(i, n, valid, gcol, gp, gs_raw, gq_raw, go, g_pos, g_rgb, g_opa, g_quat, g_scale);
 }
-
-template <int K, bool DT, bool F>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_kernel(GS_PBWD_BATCH_PARAMS,
-                                                                             float* __restrict__ cam_part) {
-  fused_project_bwd_batch_cam_body<K, DT, F, false>(GS_PBWD_BATCH_ARGS, cam_part, nullptr);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_filt3_kernel(GS_PBWD_BATCH_PARAMS,
-                                                                                   float* __restrict__ cam_part,
-                                                                                   const float* __restrict__ f3d) {
-  fused_project_bwd_batch_cam_body<K, DT, true, true>(GS_PBWD_BATCH_ARGS, cam_part, f3d);
-}
-
-template <int K, bool DT>
-__global__ void __launch_bounds__(kBlock) fused_project_bwd_batch_cam_lens_kernel(GS_PBWD_BATCH_PARAMS,
-                                                                                  float* __restrict__ cam_part,
-                                                                                  const float* __restrict__ f3d,
-                                                                                  const GsLens* __restrict__ lenses) {
-  fused_project_bwd_batch_cam_body<K, DT, true, true, true>(GS_PBWD_BATCH_ARGS, cam_part, f3d, lenses);
-}
-#undef GS_PBWD_BATCH_PARAMS
-#undef GS_PBWD_PARAMS
 
 // One CTA: grad_cam[k] = sum over the `rows` rows of cam_part[., k] in fp64, in a fixed order (strided per-thread sums,
 // butterfly shuffles, warp sums in warp order).  rows == 0 (no Gaussian) writes zeros.
@@ -1459,6 +905,59 @@ extern "C" int gs_jacobian(const float* pos_cam, int n, float* jac, gs_stream_t 
   return 0;
 }
 
+
+namespace {
+template <int V>
+using Int = std::integral_constant<int, V>;
+
+// The fused projection's one map from a frame's configuration to a kernel instantiation: calls
+// launch(KG, D, GW, TIER, DT, W), each a std::integral_constant, and returns cudaGetLastError(), or
+// cudaErrorInvalidValue for a configuration no instantiation serves.
+//   (d, sh_gaussian) -> (KG, D, GW): per-Gaussian SH d = 27 / 48 -> (9 / 16, d, GS_GREC); otherwise RGB d = 3 ->
+//     (0, 3, GS_GREC) and per-pixel SH d = 27 / other -> (0, 27, 36) / (0, 48, 56)
+//   tier (GsTier) -> TIER; dt -> DT (kDT families, false otherwise); world 0 / 2 / 4 / 8 -> W (kPush families; a lens
+//     frame has no push)
+template <bool kDT, bool kPush, class Launch>
+cudaError_t fused_project_dispatch(int d, bool sh_gaussian, int tier, bool dt, int world, Launch&& launch) {
+  auto by_world = [&](auto kg, auto dd, auto gw, auto t, auto dtc) {
+    if (world == 0) {
+      launch(kg, dd, gw, t, dtc, Int<0>{});
+      return cudaGetLastError();
+    }
+    if constexpr (kPush && t != GS_TIER_LENS) {
+      if (world == 2) launch(kg, dd, gw, t, dtc, Int<2>{});
+      else if (world == 4) launch(kg, dd, gw, t, dtc, Int<4>{});
+      else if (world == 8) launch(kg, dd, gw, t, dtc, Int<8>{});
+      else return cudaErrorInvalidValue;
+      return cudaGetLastError();
+    }
+    return cudaErrorInvalidValue;
+  };
+  auto by_dt = [&](auto kg, auto dd, auto gw, auto t) {
+    if constexpr (kDT) {
+      if (dt) return by_world(kg, dd, gw, t, std::true_type{});
+    }
+    return by_world(kg, dd, gw, t, std::false_type{});
+  };
+  auto by_tier = [&](auto kg, auto dd, auto gw) {
+    switch (tier) {
+      case GS_TIER_NONE: return by_dt(kg, dd, gw, Int<GS_TIER_NONE>{});
+      case GS_TIER_FILT2D: return by_dt(kg, dd, gw, Int<GS_TIER_FILT2D>{});
+      case GS_TIER_FILT3D: return by_dt(kg, dd, gw, Int<GS_TIER_FILT3D>{});
+      default: return by_dt(kg, dd, gw, Int<GS_TIER_LENS>{});
+    }
+  };
+  if (sh_gaussian) {
+    if (d == 27) return by_tier(Int<9>{}, Int<27>{}, Int<GS_GREC>{});
+    if (d == 48) return by_tier(Int<16>{}, Int<48>{}, Int<GS_GREC>{});
+    return cudaErrorInvalidValue;
+  }
+  if (d == 3) return by_tier(Int<0>{}, Int<3>{}, Int<GS_GREC>{});
+  if (d == 27) return by_tier(Int<0>{}, Int<27>{}, Int<36>{});
+  return by_tier(Int<0>{}, Int<48>{}, Int<56>{});
+}
+}  // namespace
+
 cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const float* opa, const float* quat,
                                     const float* scale, int n, int d, int scale_act, const GsCam& cam,
                                     const GsTileGrid& grid, float near_plane, float half_w, float half_h,
@@ -1466,58 +965,14 @@ cudaError_t gs_launch_fused_project(const float* pos, const float* rgb, const fl
                                     unsigned int* n_visible, cudaStream_t st, bool sh_gaussian, const GsFilter2d* filt,
                                     const float* f3d, const GsLens* lens) {
   if (n == 0) return cudaSuccess;
-  if (lens) {
-    const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
-#define GS_LAUNCH_PLENS(K)                                                                                      \
-  fused_project_lens_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
-                                                               grid, near_plane, half_w, half_h, rec, rect, count, \
-                                                               dkey, mask, n_visible, f2, f3d, *lens)
-    if (sh_gaussian && d == 27) GS_LAUNCH_PLENS(9);
-    else if (sh_gaussian && d == 48) GS_LAUNCH_PLENS(16);
-    else if (sh_gaussian) return cudaErrorInvalidValue;
-    else GS_LAUNCH_PLENS(0);
-#undef GS_LAUNCH_PLENS
-    return cudaGetLastError();
-  }
-  if (f3d) {
-    const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
-#define GS_LAUNCH_PFILT3(K)                                                                                      \
-  fused_project_filt3_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
-                                                                grid, near_plane, half_w, half_h, rec, rect, count, \
-                                                                dkey, mask, n_visible, f2, f3d)
-    if (sh_gaussian && d == 27) GS_LAUNCH_PFILT3(9);
-    else if (sh_gaussian && d == 48) GS_LAUNCH_PFILT3(16);
-    else if (sh_gaussian) return cudaErrorInvalidValue;
-    else GS_LAUNCH_PFILT3(0);
-#undef GS_LAUNCH_PFILT3
-    return cudaGetLastError();
-  }
-  if (filt) {
-#define GS_LAUNCH_PFILT(K)                                                                                      \
-  fused_project_filt_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, \
-                                                               grid, near_plane, half_w, half_h, rec, rect, count, \
-                                                               dkey, mask, n_visible, *filt)
-    if (sh_gaussian && d == 27) GS_LAUNCH_PFILT(9);
-    else if (sh_gaussian && d == 48) GS_LAUNCH_PFILT(16);
-    else if (sh_gaussian) return cudaErrorInvalidValue;
-    else GS_LAUNCH_PFILT(0);
-#undef GS_LAUNCH_PFILT
-    return cudaGetLastError();
-  }
-  if (sh_gaussian && d == 27)
-    fused_project_sh_kernel<9><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
-                                                               near_plane, half_w, half_h, rec, rect, count, dkey,
-                                                               mask, n_visible);
-  else if (sh_gaussian && d == 48)
-    fused_project_sh_kernel<16><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, scale_act, cam, grid,
-                                                                near_plane, half_w, half_h, rec, rect, count, dkey,
-                                                                mask, n_visible);
-  else if (sh_gaussian)
-    return cudaErrorInvalidValue;
-  else
-    fused_project_kernel<<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam, grid,
-                                                         near_plane, half_w, half_h, rec, rect, count, dkey, mask, n_visible);
-  return cudaGetLastError();
+  const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
+  const GsLens ln = lens ? *lens : GsLens{};
+  return fused_project_dispatch<false, false>(
+      d, sh_gaussian, gs_tier(filt, f3d, lens), false, 0, [&](auto kg, auto, auto, auto t, auto, auto) {
+        fused_project_kernel<kg, t><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, d, scale_act, cam,
+                                                                    grid, near_plane, half_w, half_h, rec, rect, count,
+                                                                    dkey, mask, n_visible, f2, f3d, ln);
+      });
 }
 
 cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, const float* opa, const float* quat,
@@ -1530,68 +985,13 @@ cudaError_t gs_launch_fused_project_bwd(const float* pos, const float* rgb, cons
                                         const GsLens* lens) {
   if (n == 0) return cudaSuccess;
   const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
-  if (lens) {
-    if (push.world) return cudaErrorInvalidValue;
-#define GS_LAUNCH_PBWD_LENS(D, GW, K)                                                                              \
-  if (depth_grad)                                                                                                  \
-    fused_project_bwd_lens_kernel<D, GW, K, true><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d, *lens);  \
-  else                                                                                                             \
-    fused_project_bwd_lens_kernel<D, GW, K, false><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d, *lens)
-    if (sh_gaussian && d == 27) { GS_LAUNCH_PBWD_LENS(27, GS_GREC, 9); }
-    else if (sh_gaussian && d == 48) { GS_LAUNCH_PBWD_LENS(48, GS_GREC, 16); }
-    else if (sh_gaussian) return cudaErrorInvalidValue;
-    else if (d == 3) { GS_LAUNCH_PBWD_LENS(3, GS_GREC, 0); }
-    else if (d == 27) { GS_LAUNCH_PBWD_LENS(27, 36, 0); }
-    else { GS_LAUNCH_PBWD_LENS(48, 56, 0); }
-#undef GS_LAUNCH_PBWD_LENS
-    return cudaGetLastError();
-  }
-#define GS_LAUNCH_PBWD(D, GW, W, DT)                                                               \
-  if (f3d)                                                                                         \
-    fused_project_bwd_filt3_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d); \
-  else if (filt)                                                                                   \
-    fused_project_bwd_filt_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
-  else                                                                                             \
-    fused_project_bwd_kernel<D, GW, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
-#define GS_LAUNCH_PBWD_W(D, GW, DT)                  \
-  switch (push.world) {                              \
-    case 0: GS_LAUNCH_PBWD(D, GW, 0, DT); break;     \
-    case 2: GS_LAUNCH_PBWD(D, GW, 2, DT); break;     \
-    case 4: GS_LAUNCH_PBWD(D, GW, 4, DT); break;     \
-    case 8: GS_LAUNCH_PBWD(D, GW, 8, DT); break;     \
-    default: return cudaErrorInvalidValue;           \
-  }
-#define GS_LAUNCH_PBWD_SH(K, W, DT)                                                               \
-  if (f3d)                                                                                        \
-    fused_project_bwd_sh_filt3_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, f2, f3d); \
-  else if (filt)                                                                                  \
-    fused_project_bwd_sh_filt_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, *filt); \
-  else                                                                                            \
-    fused_project_bwd_sh_kernel<K, W, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS)
-#define GS_LAUNCH_PBWD_SH_W(K, DT)                   \
-  switch (push.world) {                              \
-    case 0: GS_LAUNCH_PBWD_SH(K, 0, DT); break;      \
-    case 2: GS_LAUNCH_PBWD_SH(K, 2, DT); break;      \
-    case 4: GS_LAUNCH_PBWD_SH(K, 4, DT); break;      \
-    case 8: GS_LAUNCH_PBWD_SH(K, 8, DT); break;      \
-    default: return cudaErrorInvalidValue;           \
-  }
-  if (sh_gaussian && d != 27 && d != 48) return cudaErrorInvalidValue;
-  if (sh_gaussian && d == 27 && depth_grad) { GS_LAUNCH_PBWD_SH_W(9, true) }
-  else if (sh_gaussian && d == 27) { GS_LAUNCH_PBWD_SH_W(9, false) }
-  else if (sh_gaussian && depth_grad) { GS_LAUNCH_PBWD_SH_W(16, true) }
-  else if (sh_gaussian) { GS_LAUNCH_PBWD_SH_W(16, false) }
-  else if (d == 3 && depth_grad) { GS_LAUNCH_PBWD_W(3, GS_GREC, true) }
-  else if (d == 3) { GS_LAUNCH_PBWD_W(3, GS_GREC, false) }
-  else if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_W(27, 36, true) }
-  else if (d == 27) { GS_LAUNCH_PBWD_W(27, 36, false) }
-  else if (depth_grad) { GS_LAUNCH_PBWD_W(48, 56, true) }
-  else { GS_LAUNCH_PBWD_W(48, 56, false) }
-#undef GS_LAUNCH_PBWD_SH_W
-#undef GS_LAUNCH_PBWD_SH
-#undef GS_LAUNCH_PBWD_W
-#undef GS_LAUNCH_PBWD
-  return cudaGetLastError();
+  const GsLens ln = lens ? *lens : GsLens{};
+  return fused_project_dispatch<true, true>(
+      d, sh_gaussian, gs_tier(filt, f3d, lens), depth_grad, push.world, [&](auto kg, auto dd, auto gw, auto t, auto dt, auto w) {
+        fused_project_bwd_kernel<kg, dd, gw, w, dt, t, false><<<grid_for(n), kBlock, 0, st>>>(
+            pos, rgb, opa, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, offsets_g, count, grad_inst,
+            row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, push, f2, f3d, ln, nullptr);
+      });
 }
 
 size_t gs_cam_grad_workspace_bytes(int n) { return (size_t)grid_for(n) * kCamGrad * sizeof(float); }
@@ -1605,31 +1005,20 @@ cudaError_t gs_launch_fused_project_bwd_cam(const float* pos, const float* rgb, 
                                             bool depth_grad, bool sh_gaussian, const GsFilter2d* filt,
                                             const float* f3d, const GsLens* lens) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
-  const GsGradPush push{};
   const GsFilter2d f2 = filt ? *filt : GsFilter2d{};
+  const GsLens ln = lens ? *lens : GsLens{};
   if (n > 0) {
-#define GS_LAUNCH_PBWD_CAM(K, DT)                                                                             \
-  if (lens)                                                                                                   \
-    fused_project_bwd_cam_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, f2, f3d, \
-                                                                             *lens);                          \
-  else if (f3d)                                                                                                    \
-    fused_project_bwd_cam_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, f2, f3d); \
-  else if (filt)                                                                                              \
-    fused_project_bwd_cam_filt_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part, *filt); \
-  else                                                                                                        \
-    fused_project_bwd_cam_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(GS_PBWD_ARGS, cam_part)
-    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_CAM(9, true);
-    else if (d == 27) GS_LAUNCH_PBWD_CAM(9, false);
-    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_CAM(16, true);
-    else if (d == 48) GS_LAUNCH_PBWD_CAM(16, false);
-    else if (depth_grad) GS_LAUNCH_PBWD_CAM(0, true);
-    else GS_LAUNCH_PBWD_CAM(0, false);
-#undef GS_LAUNCH_PBWD_CAM
+    const cudaError_t e = fused_project_dispatch<true, false>(
+        d, d != 3, gs_tier(filt, f3d, lens), depth_grad, 0, [&](auto kg, auto, auto, auto t, auto dt, auto) {
+          fused_project_bwd_kernel<kg, kg ? 3 * kg : 3, GS_GREC, 0, dt, t, true><<<grid_for(n), kBlock, 0, st>>>(
+              pos, rgb, opa, quat, scale, n, scale_act, cam, near_plane, half_w, half_h, offsets_g, count, grad_inst,
+              row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, GsGradPush{}, f2, f3d, ln, cam_part);
+        });
+    if (e != cudaSuccess) return e;
   }
   cam_grad_finish_kernel<<<1, kBlock, 0, st>>>(cam_part, n > 0 ? grid_for(n) : 0, grad_cam);
   return cudaGetLastError();
 }
-#undef GS_PBWD_ARGS
 
 cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
                                           const float* scale, int n, int n_views, int d, int scale_act,
@@ -1639,40 +1028,12 @@ cudaError_t gs_launch_fused_project_batch(const float* pos, const float* rgb, co
                                           const GsLens* lenses) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
-#define GS_LAUNCH_PBATCHL(K)                                                                                     \
-  fused_project_batch_lens_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,  \
-                                                                     scale_act, views, near_plane, rec, rect,     \
-                                                                     count, dkey, mask, n_visible, f3d, lenses)
-  if (lenses) {
-    if (d == 27) GS_LAUNCH_PBATCHL(9);
-    else if (d == 48) GS_LAUNCH_PBATCHL(16);
-    else GS_LAUNCH_PBATCHL(0);
-#undef GS_LAUNCH_PBATCHL
-    return cudaGetLastError();
-  }
-#define GS_LAUNCH_PBATCH(K, F)                                                                                    \
-  fused_project_batch_kernel<K, F><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,     \
-                                                                   scale_act, views, near_plane, rec, rect, count, \
-                                                                   dkey, mask, n_visible)
-#define GS_LAUNCH_PBATCH3(K)                                                                                      \
-  fused_project_batch_filt3_kernel<K><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,  \
-                                                                      scale_act, views, near_plane, rec, rect,     \
-                                                                      count, dkey, mask, n_visible, f3d)
-  const int k = d == 27 ? 9 : (d == 48 ? 16 : 0);
-  if (f3d) {
-    if (k == 9) GS_LAUNCH_PBATCH3(9);
-    else if (k == 16) GS_LAUNCH_PBATCH3(16);
-    else GS_LAUNCH_PBATCH3(0);
-  }
-  else if (k == 9 && filt) GS_LAUNCH_PBATCH(9, true);
-  else if (k == 9) GS_LAUNCH_PBATCH(9, false);
-  else if (k == 16 && filt) GS_LAUNCH_PBATCH(16, true);
-  else if (k == 16) GS_LAUNCH_PBATCH(16, false);
-  else if (filt) GS_LAUNCH_PBATCH(0, true);
-  else GS_LAUNCH_PBATCH(0, false);
-#undef GS_LAUNCH_PBATCH3
-#undef GS_LAUNCH_PBATCH
-  return cudaGetLastError();
+  return fused_project_dispatch<false, false>(
+      d, d != 3, gs_tier(filt, f3d, lenses), false, 0, [&](auto kg, auto, auto, auto t, auto, auto) {
+        fused_project_batch_kernel<kg, t><<<grid_for(n), kBlock, 0, st>>>(pos, rgb, opa, quat, scale, n, n_views, d,
+                                                                          scale_act, views, near_plane, rec, rect,
+                                                                          count, dkey, mask, n_visible, f3d, lenses);
+      });
 }
 
 cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb, const float* opa, const float* quat,
@@ -1684,40 +1045,12 @@ cudaError_t gs_launch_fused_project_bwd_batch(const float* pos, const float* rgb
                                               bool filt, const float* f3d, const GsLens* lenses) {
   if (n == 0) return cudaSuccess;
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
-  if (lenses) {
-#define GS_LAUNCH_PBWD_BATCHL(K, DT)                                                                                \
-  fused_project_bwd_batch_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                       \
-      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
-      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d, lenses)
-    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_BATCHL(9, true);
-    else if (d == 27) GS_LAUNCH_PBWD_BATCHL(9, false);
-    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_BATCHL(16, true);
-    else if (d == 48) GS_LAUNCH_PBWD_BATCHL(16, false);
-    else if (depth_grad) GS_LAUNCH_PBWD_BATCHL(0, true);
-    else GS_LAUNCH_PBWD_BATCHL(0, false);
-#undef GS_LAUNCH_PBWD_BATCHL
-    return cudaGetLastError();
-  }
-#define GS_LAUNCH_PBWD_BATCH(K, DT, F)                                                                              \
-  fused_project_bwd_batch_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                         \
-      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
-      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale)
-#define GS_LAUNCH_PBWD_BATCH_F(K, DT)                                                                             \
-  if (f3d)                                                                                                        \
-    fused_project_bwd_batch_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                  \
-        pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,        \
-        row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d);                                             \
-  else if (filt) GS_LAUNCH_PBWD_BATCH(K, DT, true);                                                               \
-  else GS_LAUNCH_PBWD_BATCH(K, DT, false)
-  if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_F(9, true); }
-  else if (d == 27) { GS_LAUNCH_PBWD_BATCH_F(9, false); }
-  else if (d == 48 && depth_grad) { GS_LAUNCH_PBWD_BATCH_F(16, true); }
-  else if (d == 48) { GS_LAUNCH_PBWD_BATCH_F(16, false); }
-  else if (depth_grad) { GS_LAUNCH_PBWD_BATCH_F(0, true); }
-  else { GS_LAUNCH_PBWD_BATCH_F(0, false); }
-#undef GS_LAUNCH_PBWD_BATCH_F
-#undef GS_LAUNCH_PBWD_BATCH
-  return cudaGetLastError();
+  return fused_project_dispatch<true, false>(
+      d, d != 3, gs_tier(filt, f3d, lenses), depth_grad, 0, [&](auto kg, auto, auto, auto t, auto dt, auto) {
+        fused_project_bwd_batch_kernel<kg, dt, t, false><<<grid_for(n), kBlock, 0, st>>>(
+            pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,
+            row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d, lenses, nullptr);
+      });
 }
 
 cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float* rgb, const float* opa,
@@ -1730,38 +1063,14 @@ cudaError_t gs_launch_fused_project_bwd_batch_cam(const float* pos, const float*
                                                   bool depth_grad, bool sh_gaussian, bool filt, const float* f3d,
                                                   const GsLens* lenses) {
   if (d != 3 && !(sh_gaussian && (d == 27 || d == 48))) return cudaErrorInvalidValue;
-  if (n > 0 && lenses) {
-#define GS_LAUNCH_PBWD_BATCH_CAML(K, DT)                                                                            \
-  fused_project_bwd_batch_cam_lens_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                                   \
-      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
-      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part, f3d, lenses)
-    if (d == 27 && depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(9, true);
-    else if (d == 27) GS_LAUNCH_PBWD_BATCH_CAML(9, false);
-    else if (d == 48 && depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(16, true);
-    else if (d == 48) GS_LAUNCH_PBWD_BATCH_CAML(16, false);
-    else if (depth_grad) GS_LAUNCH_PBWD_BATCH_CAML(0, true);
-    else GS_LAUNCH_PBWD_BATCH_CAML(0, false);
-#undef GS_LAUNCH_PBWD_BATCH_CAML
-  } else if (n > 0) {
-#define GS_LAUNCH_PBWD_BATCH_CAM(K, DT, F)                                                                          \
-  fused_project_bwd_batch_cam_kernel<K, DT, F><<<grid_for(n), kBlock, 0, st>>>(                                     \
-      pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst, row_epoch, \
-      epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part)
-#define GS_LAUNCH_PBWD_BATCH_CAM_F(K, DT)                                                                         \
-  if (f3d)                                                                                                        \
-    fused_project_bwd_batch_cam_filt3_kernel<K, DT><<<grid_for(n), kBlock, 0, st>>>(                              \
-        pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,        \
-        row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, cam_part, f3d);                                   \
-  else if (filt) GS_LAUNCH_PBWD_BATCH_CAM(K, DT, true);                                                           \
-  else GS_LAUNCH_PBWD_BATCH_CAM(K, DT, false)
-    if (d == 27 && depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, true); }
-    else if (d == 27) { GS_LAUNCH_PBWD_BATCH_CAM_F(9, false); }
-    else if (d == 48 && depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(16, true); }
-    else if (d == 48) { GS_LAUNCH_PBWD_BATCH_CAM_F(16, false); }
-    else if (depth_grad) { GS_LAUNCH_PBWD_BATCH_CAM_F(0, true); }
-    else { GS_LAUNCH_PBWD_BATCH_CAM_F(0, false); }
-#undef GS_LAUNCH_PBWD_BATCH_CAM_F
-#undef GS_LAUNCH_PBWD_BATCH_CAM
+  if (n > 0) {
+    const cudaError_t e = fused_project_dispatch<true, false>(
+        d, d != 3, gs_tier(filt, f3d, lenses), depth_grad, 0, [&](auto kg, auto, auto, auto t, auto dt, auto) {
+          fused_project_bwd_batch_kernel<kg, dt, t, true><<<grid_for(n), kBlock, 0, st>>>(
+              pos, rgb, opa, quat, scale, n, n_views, scale_act, views, near_plane, offsets_g, count, grad_inst,
+              row_epoch, epoch, g_pos, g_rgb, g_opa, g_quat, g_scale, f3d, lenses, cam_part);
+        });
+    if (e != cudaSuccess) return e;
   }
   cam_grad_finish_batch_kernel<<<n_views, kBlock, 0, st>>>(cam_part, n > 0 ? grid_for(n) : 0, grad_cams);
   return cudaGetLastError();

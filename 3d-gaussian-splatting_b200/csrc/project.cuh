@@ -302,6 +302,14 @@ struct GsLens {
   float k[4];
 };
 
+// The features a fused-frame projection kernel applies, cumulative: each tier also runs every lower one's arithmetic
+// (a frame without the lower feature passes a zero 2-D filter or a NULL 3-D filter, which give the bits without it).
+enum GsTier { GS_TIER_NONE = 0, GS_TIER_FILT2D, GS_TIER_FILT3D, GS_TIER_LENS };
+
+inline int gs_tier(bool filt2d, const float* f3d, bool lens) {
+  return lens ? GS_TIER_LENS : (f3d ? GS_TIER_FILT3D : (filt2d ? GS_TIER_FILT2D : GS_TIER_NONE));
+}
+
 // (a, b) -> (ad, bd) = D(a, b) and J = dD/d(a, b) row-major {d ad/da, d ad/db, d bd/da, d bd/db}
 __device__ __forceinline__ void gs_lens_map(const GsLens& L, float a, float b, float& ad, float& bd, float J[4]) {
   const float r2 = a * a + b * b;

@@ -133,7 +133,7 @@ def test_single_view(gs, cuda, name):
 
 @pytest.mark.parametrize("name", list(E.BUILDERS))
 def test_batched_equals_single_views(gs, cuda, name):
-    """Family 8: fused_project_one (batched) against fused_project_body (single view) and the oracle."""
+    """Family 8: fused_project_batch_kernel against fused_project_kernel (single view) and the oracle."""
     import renderer
     sc = E.batched(_scene(name))
     singles = _single(gs, sc, cuda, grads=False)

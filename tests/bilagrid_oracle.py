@@ -142,6 +142,51 @@ def slice_backward(image, grids, ids, grad_out):
     return gi, gg
 
 
+def slice_terms(image, grids, ids, grad_out):
+    """Term magnitudes of the slice for per-element error models (fp64, z in fp32 as above), with N the sum of |node|
+    over a pixel's 8 nodes [B, H, W, 12] and u = (r, g, b, 1):
+      out_mag  [B, H, W, 3]       sum_j N_cj |u_j|
+      gi_mag   [B, H, W, 3]       sum_r |go_r| (N_rc + LUM_c (GL - 1) [0 < z < 1] sum_j N_rj |u_j|)
+      gg_mag   [V, GH, GW, GL, 12] sum over the pixels reaching the node of |w_xyz dL/dA|
+      gg_count [V, GH, GW, GL, 1]  the number of (pixel, corner) terms summed into the node"""
+    img = (image if image.dim() == 4 else image[None]).double().detach()
+    go = (grad_out if grad_out.dim() == 4 else grad_out[None]).double()
+    grids = grids.double().detach()
+    bsz, h, w, _ = img.shape
+    nv, gh, gw, gl, _ = grids.shape
+    y0, fy = _cells(h, gh)
+    x0, fx = _cells(w, gw)
+    z = torch.from_numpy(guide_f32(img).astype(np.float64))
+    z0, fz, inside = _zcell(z, gl)
+    idt = torch.as_tensor(list(ids), dtype=torch.long)
+    gsel = grids[idt].abs()
+    bi = torch.arange(bsz)[:, None, None]
+    u = torch.cat([img, torch.ones_like(img[..., :1])], dim=-1).abs()
+    q = (go.abs()[..., :, None] * u[..., None, :]).reshape(bsz, h, w, 12)
+    N = torch.zeros(bsz, h, w, 12, dtype=torch.float64)
+    gg = torch.zeros_like(grids)
+    cnt = torch.zeros(nv * gh * gw * gl, 1, dtype=torch.float64)
+    for a in (0, 1):
+        wx = fx if a else 1 - fx
+        for b in (0, 1):
+            wy = fy if b else 1 - fy
+            wxy = (wy[None, :, None] * wx[None, None, :]).expand(bsz, h, w)
+            for c in (0, 1):
+                wz = fz if c else 1 - fz
+                yy, xx, zz = (y0 + b)[None, :, None].expand(bsz, h, w), (x0 + a)[None, None, :].expand(bsz, h, w), z0 + c
+                N += gsel[bi, yy, xx, zz]
+                flat = (((idt[:, None, None].expand(bsz, h, w) * gh + yy) * gw + xx) * gl + zz).reshape(-1)
+                gg.view(-1, 12).index_add_(0, flat, ((wxy * wz).abs()[..., None] * q).reshape(-1, 12))
+                cnt.index_add_(0, flat, torch.ones(flat.numel(), 1, dtype=torch.float64))
+    Nm = N.reshape(bsz, h, w, 3, 4)
+    out_mag = (Nm * u[..., None, :]).sum(-1)
+    zt = out_mag * (gl - 1) * inside[..., None]                                     # [B, H, W, r]
+    gi_mag = (go.abs()[..., :, None] * (Nm[..., :3] + zt[..., :, None] * torch.tensor(LUM, dtype=torch.float64))).sum(-2)
+    if image.dim() == 3:
+        out_mag, gi_mag = out_mag[0], gi_mag[0]
+    return dict(out_mag=out_mag, gi_mag=gi_mag, gg_mag=gg, gg_count=cnt.view(nv, gh, gw, gl, 1))
+
+
 def tv(grids):
     g = grids.double()
     return sum(float(((g.narrow(d, 1, g.shape[d] - 1) - g.narrow(d, 0, g.shape[d] - 1)) ** 2).mean()) for d in (1, 2, 3))

@@ -39,7 +39,8 @@ def _go(shape, seed, dev):
 CASES = [((1080, 1920), 1, [0]), ((45, 67), 1, [1]), ((8, 5), 1, [1]), ((45, 67), 4, [2, 0, 2, 1])]
 
 
-@pytest.mark.parametrize("shape", [(16, 16, 8), (8, 4, 4), (2, 2, 2), (4, 6, 16), (5, 3, 11)])
+@pytest.mark.parametrize("shape", [(16, 16, 8), (8, 4, 4), (2, 2, 2), (4, 6, 16), (5, 3, 11), (3, 4, 3),
+                                   (6, 5, 5), (4, 3, 9)])
 @pytest.mark.parametrize("hw,b,ids", CASES, ids=["1920x1080", "67x45", "5x8", "67x45-B4-repeat"])
 def test_kernel_matches_oracle(gs, cuda, shape, hw, b, ids):
     gaussian, _ = gs
